@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — coarse-stage training-step throughput of the B200-native hot path (BASELINE.json metric).
+"""bench.py — coarse-stage training-step throughput of the H100-native (sm_90a) hot path (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # this repo (torchrun launches it for N > 1)
   python bench.py --impl reference --gpus N --steps K --warmup W   # CPU arm: the oracle port of the reference path
@@ -8,7 +8,9 @@ One "step" = one full optimiser step of the musiclm_small coarse stage (BASELINE
 token pre-processing -> embedding gather -> 6 x (attention + conv-FFN) -> logit heads -> CE -> backward ->
 gradient all-reduce (N > 1) -> global-norm clip -> AdamW, training semantics (FFN dropout 0.1 and the 15 %
 forgetful mask active), batch 16 per GPU, N = 1024 positions, synthetic uniform token ids, random-init weights.
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR additionally writes what the last timed training step computed
+(its loss, the gradient norm and a fixed sample of the updated parameters) as DIR/<name>.npy, so that two builds can be
+compared output for output: with the same arguments the inputs and the initial weights are identical from run to run.
 """
 import argparse
 import json
@@ -84,12 +86,16 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return dict(hbm_gbs=p["hbm_gbs"], burst=p["bf16_tflops"], sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]), src="measured")
-    return dict(hbm_gbs=6650.0, burst=1590.0, sustained=1400.0, src="fallback")
+        return dict(hbm_gbs=p["hbm_gbs"], burst=p["bf16_tflops"], sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]),
+                    src="MEASURED_PEAKS.json bf16_tflops_sustained (measured)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not a measured rate; a card
+    # with a lower power limit runs below it, so the fractions taken against it are lower bounds
+    return dict(hbm_gbs=3350.0, burst=989.0, sustained=989.0,
+                src="H100 SXM data sheet, 989 TFLOP/s dense bf16 at 700 W (not measured; no MEASURED_PEAKS.json)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -167,8 +173,8 @@ def pick_cpu_threads():
 
 
 def cpu_reference_arm(steps, warmup, budget_s=150.0):
-    """The reference's own CPU path, as restated by the oracle (kind "port": /root/reference cannot travel to the
-    GPU box): full coarse training step (forward, backward, clip 0.5, AdamW) in fp32 on all host cores, on a
+    """The reference's own CPU path, as restated by the oracle (kind "port": the reference package is not a
+    dependency of this project): full coarse training step (forward, backward, clip 0.5, AdamW) in fp32 on all host cores, on a
     bounded sample of the workload (batch 2 instead of 16; CPU throughput is batch-linear)."""
     import numpy as np
     import torch
@@ -288,7 +294,7 @@ def measure(key, args, world, rank, local, inst, full):
     import open_musiclm_b200 as O
     wl = WORKLOADS[key]
     B = args.batch if (full and args.batch) else wl["batch"]
-    steps = args.steps if full else max(5, min(args.steps, 10))
+    steps = args.steps
     torch.manual_seed(0)                                      # identical init on every rank (= the reference's init)
     model = make_model(wl).cuda()
     tr = O.HotPathTrainer(model, cross_entropy_loss_weights=TRAIN["ce_weights"], lr=TRAIN["lr"], lr_warmup=TRAIN["lr_warmup"],
@@ -319,7 +325,10 @@ def measure(key, args, world, rank, local, inst, full):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms) / n
 
-    step_dev = lambda i: tr.train_step([pool_dev[i % len(pool_dev)]])
+    last = {}
+
+    def step_dev(i):
+        last["loss"] = tr.train_step([pool_dev[i % len(pool_dev)]])
     # first step: eager launches, counted (the CUDA graph captured two steps later replays exactly these kernels)
     inst.launches = 0
     step_dev(0)
@@ -379,6 +388,8 @@ def measure(key, args, world, rank, local, inst, full):
         for i in range(2):
             step_dev(i)
         res["ms_step_again"] = timed(step_dev, steps)
+        if args.dump_outputs and rank == 0:      # the parameters are replicated: one rank writes them
+            dump_outputs(args.dump_outputs, tr, last["loss"])
     res["graph"] = tr.use_cuda_graph
     res["overlap"] = getattr(tr, "allreduce_mode", None)
     res["peaks"] = peaks
@@ -459,14 +470,6 @@ def run_b200(args):
         except Exception as e:            # the headline must still be printed
             extras["cfg5"] = {"error": f"{type(e).__name__}: {e}"}
         torch.cuda.empty_cache()
-    gemm_traffic = {}
-    try:   # DRAM bytes of the GEMM family from the committed ncu --set full capture (tools/ncu_summarize.py)
-        gemm_traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_ncu_gemm_traffic.json")))
-    except (OSError, ValueError):
-        try:
-            gemm_traffic = json.load(open(os.path.join(ROOT, "profiles", "r01_ncu_gemm_traffic.json")))
-        except (OSError, ValueError):
-            pass
     cpu = None
     if rank == 0 and world == 1 and not args.no_cpu:
         r = cpu_reference_arm(steps=3, warmup=1, budget_s=60.0)
@@ -482,18 +485,17 @@ def run_b200(args):
             "vs_baseline": None, "dtype": "bf16 (fp16 operands for the forward GEMMs on LayerNorm outputs x weights; fp32 accumulate)", "data": "synthetic",
             "config": {"workload": wl["name"] + ", dropout 0.1 + forgetful mask 0.15, AdamW + clip 0.5",
                        "global_batch": world * B, "per_gpu_batch": B, "seq_len": wl["N"], "parallelism": f"dp{world}",
-                       "l2": "no explicit flush: one step touches > 3 GB of activations/weights, far above the 126 MB L2"},
+                       "l2": "no explicit flush: one step touches > 3 GB of activations/weights, far above the 50 MB L2"},
             "e2e": {"value": tok / (res["ms_e2e"] * 1e-3), "unit": "tokens/s", "ms_per_step": res["ms_e2e"], "h2d_bytes_per_step": res["h2d"],
                     "d2h_bytes_per_step": 4,
                     "api": "HotPathTrainer.train_step_async: batch copied from pinned host memory every step, loss copied "
                            "to pinned host memory every step and read on the host one step later (last one inside the timed region)"},
             "gpu_launches": res["n_launch"] * args.steps, "gpu_launches_per_step": res["n_launch"],
             "launch_mode": ("step replayed from CUDA graphs; gradient all-reduce: " + str(res["overlap"])) if res["graph"] else "eager launches",
-            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel + gemm_ffn_up_kernel (tcgen05; all operand-major variants; FFN-up time includes its fused conv+GEGLU epilogue)", "achieved": ach,
+            "roofline": {"bound": "tensor", "kernel": "gemm_bf16_kernel + gemm_ffn_up_kernel (wgmma; all operand-major variants; FFN-up time includes its fused conv+GEGLU epilogue)", "achieved": ach,
                          "peak": peaks["sustained"], "unit": "TFLOP/s", "frac": ach / peaks["sustained"], "frac_of_burst_peak": ach / peaks["burst"],
                          "flops": "algorithmic (F = 2730, C = 1025; padded tile columns not counted)",
-                         "traffic": gemm_traffic.get("bytes_per_launch"), "traffic_unit": "bytes per launch (family average)", "traffic_source": gemm_traffic.get("source"),
-                         "peak_source": f"MEASURED_PEAKS.json bf16_tflops_sustained ({peaks['src']})",
+                         "peak_source": peaks["src"],
                          "launches_per_step": res["n_gemm"], "gemm_ms_per_step": res["g_ms"] / args.steps,
                          "gemm_share_of_step": (res["g_ms"] / args.steps) / res["ms_instr"], "ms_per_step_instrumented": res["ms_instr"]},
             "step_model_flops": {"tflop_per_step_per_gpu": fl["step"] / 1e12, "achieved_tflops_per_gpu": fl["step"] / (ms_step * 1e-3) / 1e12,
@@ -501,10 +503,11 @@ def run_b200(args):
             "forward_only": {"ms": ms_fwd, "attn_ffn_tflops": fl["fwd_attn_ffn"] / (ms_fwd * 1e-3) / 1e12,
                              "attn_ffn_frac_of_peak": fl["fwd_attn_ffn"] / (ms_fwd * 1e-3) / 1e12 / peaks["sustained"],
                              "attn_ffn_frac_of_burst_peak": fl["fwd_attn_ffn"] / (ms_fwd * 1e-3) / 1e12 / peaks["burst"],
-                             "attn_ffn_frac_of_nominal_2250": fl["fwd_attn_ffn"] / (ms_fwd * 1e-3) / 1e12 / 2250.0},
+                             "attn_ffn_frac_of_datasheet_989": fl["fwd_attn_ffn"] / (ms_fwd * 1e-3) / 1e12 / 989.0},
             "configs": extras,
             "clocks": res["clocks"],
             "cpu_baseline": cpu,
+            "gpu": gpu_info(),
         }
         print(json.dumps(line))
     if world > 1:
@@ -530,6 +533,39 @@ def cpu_cfg1_forward(cores):
     return {"tokens_per_s": 2 * 256 / ts[len(ts) // 2], "ms": ts[len(ts) // 2] * 1e3, "workload": "configs[0]: semantic forward, B=2, N=256, fp32"}
 
 
+DUMP_PARAM_SAMPLE = 4 * 1024 * 1024     # float32 elements of the parameter arena written by --dump-outputs (16 MB)
+
+
+def dump_outputs(out_dir, tr, loss):
+    """What the caller of the timed path receives from its last step: the loss, the global gradient norm that the clip
+    used, and the updated parameters (a fixed, seeded sample of the flat fp32 arena when it is larger than the cap)."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arena = tr.eng.arena_p[:tr.eng.n_params_arena].detach().float()
+    n = arena.numel()
+    if n > DUMP_PARAM_SAMPLE:
+        idx = np.sort(np.random.default_rng(0).choice(n, DUMP_PARAM_SAMPLE, replace=False))
+        params = arena[torch.from_numpy(idx).to(arena.device)]
+    else:
+        params = arena
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    np.save(os.path.join(out_dir, "grad_norm.npy"), np.array([float(tr.grad_norm())], dtype=np.float64))
+    np.save(os.path.join(out_dir, "params.npy"), params.cpu().numpy().astype(np.float32))
+
+
+def gpu_info():
+    """Name and power limit of the card the numbers were measured on (part of every absolute number)."""
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i",
+                            os.environ.get("LOCAL_RANK", "0")], capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception:
+        q = ""
+    import torch
+    return {"name": torch.cuda.get_device_name(), "nvidia_smi": q or None}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -540,6 +576,8 @@ def main():
     ap.add_argument("--config", default="cfg2", choices=sorted(WORKLOADS), help="headline workload (default: BASELINE configs[1])")
     ap.add_argument("--extra", default="cfg3,cfg4", help="other BASELINE configs timed beside it (sub-results under 'configs'); 'none' to skip")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed training step's outputs (loss, gradient norm, parameter sample) as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* libomlm_b200 — C ABI of the B200-native hot path of zhvng/open-musiclm.
+/* libomlm_b200 — C ABI of the H100-native (sm_90a) hot path of zhvng/open-musiclm.
  *
  * The reference has no native code and therefore no FFI of its own: its hot path is the chain of
  * torch calls inside open_musiclm/transformer.py and open_musiclm/open_musiclm.py.  Each entry point
@@ -8,7 +8,7 @@
  *   - are asynchronous (enqueue-only on the given stream) and allocate no persistent memory,
  *   - return 0 on success, 1 on argument errors, 1000+cudaError_t on CUDA errors;
  *     omlm_last_error() returns a thread-local description.
- * There is no CPU fallback: without an sm_100a device every compute entry point fails.
+ * There is no CPU fallback: without an sm_90a device every compute entry point fails.
  */
 #ifndef OMLM_B200_H_
 #define OMLM_B200_H_
@@ -27,7 +27,7 @@ int omlm_device_check(void);
 /* Number of SMs of the current device (the persistent kernels' default grid). */
 int omlm_num_sms(void);
 
-/* bf16 GEMM on tcgen05 tensor cores:  out[m,n] = alpha * sum_k A(m,k) * B(n,k) (+ addend[m,n]).
+/* bf16 / fp16 GEMM on the wgmma tensor cores:  out[m,n] = alpha * sum_k A(m,k) * B(n,k) (+ addend[m,n]).
  *   a_mn_major = 0: A is [M, lda] with k contiguous;  1: A is [K, lda] with m contiguous.
  *   b_mn_major = 0: B is [N, ldb] with k contiguous;  1: B is [K, ldb] with n contiguous.
  *   out_f32: 0 -> bf16 out, 1 -> fp32 out.  addend (fp32, may alias out) gives residual add /
@@ -41,7 +41,7 @@ int omlm_gemm_bf16(const void* A, int a_mn_major, long lda, const void* B, int b
                    long ldadd, float alpha, int splits, int row_split, int row_valid, int n_valid,
                    int block_n, int max_ctas, void* stream);
 /* The same GEMM with the 16-bit operand format selectable: a_f16 = b_f16 = 1 -> IEEE fp16 operands, 0 -> bf16 (same
- * tensor rate, fp32 accumulation).  B200 raises an illegal-instruction fault when the two formats differ (measured), so
+ * tensor rate, fp32 accumulation).  One wgmma instruction takes a single operand format, so
  * a_f16 != b_f16 is rejected.  The hot path uses fp16 for the forward GEMMs whose operands are bounded by
  * construction (LayerNorm outputs x weights, FFN activations) and bf16 wherever a gradient or the raw residual stream
  * is an operand. */
@@ -93,7 +93,7 @@ int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, i
  * Bias-less LayerNorm (transformer.py:24-31).  x fp32 [M,D] -> y [M,D] in fp16 (y_f16 = 1) or bf16 (row m written to row
  * dest_row[m] when given, skipped if negative), optional raw bf16 copy of x (keys/values are
  * projected from the un-normalised stream, transformer.py:228,254), stats[m] = (mean, rstd).  ycopy_bf16 (optional):
- * a bf16 copy of y for the weight-gradient GEMMs (tcgen05 needs both operands in one format; gradients are bf16). */
+ * a bf16 copy of y for the weight-gradient GEMMs (one wgmma takes one operand format; gradients are bf16). */
 int omlm_layernorm_fwd(const float* x, const float* gamma, void* y16, int y_f16, void* ycopy_bf16, void* xraw_bf16,
                        float* stats, const int* dest_row, int M, int D, void* stream);
 /* dx = [dres] + [draw] + LN-backward(dy);  dgamma += sum_rows dy * xhat.  dy row for x row m is
@@ -128,7 +128,7 @@ int omlm_arange_f32(float* out, int n, void* stream);
 int omlm_attn_fwd(const void* qn, const void* kvn, const float* table, int table_ld,
                   const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                   float scale, void* stream);
-/* Same contract on the tcgen05/TMEM/TMA path (two 128-row tiles per CTA, softmax warpgroups ping-ponged). */
+/* Same contract on the wgmma/TMA path (one 128-row tile per CTA, two consumer warpgroups of 64 rows). */
 int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* table, int table_ld,
                      const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                      float scale, void* stream);
@@ -138,9 +138,10 @@ int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* 
                   float* dqn, float* dkvn, float* dtable, int B, int N, int heads, float scale,
                   void* stream);
 
-/* tcgen05/TMEM/TMA backward: dqn and dkvn are OVERWRITTEN (its first kernel clears them, the main kernel reduces into
+/* wgmma/TMA backward: dqn and dkvn are OVERWRITTEN (its first kernel clears them, the main kernel reduces into
  * them), dtable is accumulated (+=: one table gradient over all layers).  The bias gradient -- diagonal sums of dS -- is
- * formed inside the kernel from an fp32-class hi/lo split of dS, no scratch tensor. */
+ * formed inside the kernel from the fp32 dS, summed per CTA in shared memory and added to dtable once; no scratch tensor.
+ * dqn, dkvn and dtable are reduced with floating-point atomics: reproducible up to accumulation order. */
 int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                      const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
                      float* dqn, float* dkvn, float* dtable, int B, int N, int heads,
@@ -149,7 +150,7 @@ int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const voi
 /* ---- ConvFeedForward (transformer.py:122-150) ---------------------------------------------------
  * Interleaved GEGLU layout: Fp = F rounded up to 128; u / W1 rows / conv taps are ordered in groups of 128 channels as
  * [128 value | 128 gate]; h / hn / gamma / W2 columns are in natural channel order (zero padded to Fp).
- * FFN up-projection GEMM (tcgen05) with the causal depthwise conv (k=3), GEGLU (exact erf) and the LayerNorm row
+ * FFN up-projection GEMM (wgmma) with the causal depthwise conv (k=3), GEGLU (exact erf) and the LayerNorm row
  * statistics fused into its epilogue:  u bf16 [M, 2Fp], h bf16 [M, Fp], rowsum fp32 [M, Fp/128, 2] = per-128-channel
  * partial (sum h, sum h^2), plain stores (no zeroing needed; summed in a fixed order by omlm_ffn_norm_fwd).  M = B * Nseq rows, sequences of Nseq consecutive rows.
  * act_f16 = 1: xn, w1 are fp16 operands and the forward activations u, h, hn are fp16 (0: all bf16); the same flag

@@ -1,11 +1,11 @@
-"""open-musiclm hot path, B200-native (sm_100a): package root.
+"""open-musiclm hot path, H100-native (sm_90a): package root.
 
 Only what the TokenConditionedTransformer training path needs lives here:
   csrc/       hand-written CUDA kernels + the C ABI (libomlm_b200.so)
   lib.py      ctypes binding of that ABI (no fallback)
   engine.py   parameter arena, packed weights, kernel sequencing (forward / backward)
   model.py    drop-in `TokenConditionedTransformer`, `create_{semantic,coarse,fine}_transformer`
-  trainer.py  B200-native SingleStageTrainer step loop (`HotPathTrainer`)
+  trainer.py  H100-native SingleStageTrainer step loop (`HotPathTrainer`)
   decode.py   `TokenConditionedTransformerWrapper.generate`: KV-cache autoregressive decoding
   stages.py   `SemanticStage` / `CoarseStage` / `FineStage` and the windowed three-stage `MusicLM` generation
 """

@@ -1,24 +1,16 @@
-// Fused causal multi-query cosine-sim attention, backward, on tcgen05 / TMEM / TMA.
+// Fused causal multi-query cosine-sim attention, backward, on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 // Autograd of transformer.py:304-331.  Folded-row layout: R = N*h query rows per batch element share one K/V head
-// (row r = i*h + head).  Work unit = (batch, 128-key tile, chunk of 128-row query tiles).  512 threads:
+// (row r = i*h + head).  Work unit = (batch, 128-key tile, chunk of 64-row query tiles).  384 threads:
 //
-//   warp 0       TMA producer: K/V tile once, Q/dO tiles through a 2-stage ring
-//   warp 1       tcgen05.mma issuer, five GEMMs per row tile, all M = 128:
-//                   S  = Q K^T          (TMEM cols   0..127)      dP = dO V^T      (128..255)
-//                   dV += P^T dO        (384..447, accumulated over the row tiles, A = P read MN-major)
-//                   dK += dS^T Q        (320..383, accumulated,                    A = dS read MN-major)
-//                   dQ  = dS K          (256..319, per tile,                       A = dS read K-major)
-//   warps 2,3    bias-slice (Toeplitz window, causal -inf folded in) + key-mask builders, one tile ahead
-//   warps 4-11   P / dS: one thread per (query row, 64-key half): S/dP from TMEM, P = exp2(s - lse), dS = P (dP - D).
-//                P and dS are written as bf16 into ONE 128B-swizzled [row][key] smem tile each that serves as K-major and
-//                MN-major MMA operand; the rounding residual dS - bf16(dS) goes to a second bf16 tile (dS_lo).  Two warps
-//                per SM sub-partition hide each other's TMEM / MUFU latencies (one warp per sub-partition did not).
-//   warps 12-15  (a) bias gradient: dTable[hh, i-j] += sum dS is a sum along the diagonals of the dS tile.  It is
-//                formed here from dS_hi + dS_lo (fp32-class: these sums cancel heavily, a bf16-rounded dS shows up
-//                amplified in the rel-pos MLP gradient), each thread owning (head, 8-key chunk) and sliding over the
-//                tile's positions with the diagonal bins in registers, then accumulated in a per-CTA shared table that is
-//                flushed to global once;  (b) drain dQ per tile (TMEM -> red.global.add.v4.f32), dK/dV at the end.
+//   warpgroup 0     TMA producer: the K/V tile once, Q/dO row tiles through a 2-stage ring
+//   warpgroups 1,2  64 keys each, per row tile (all wgmma M = 64, operands in 128B-swizzled smem):
+//                      S  = Q K^T,  dP = dO V^T          (registers)
+//                      P = exp2(s - lse), dS = P (dP - D) in fp32 registers; P, dS -> bf16 [row][key] smem tiles
+//                      dV += P^T dO,  dK += dS^T Q        (A read MN-major; accumulated in registers over the chunk)
+//                      dQ  = dS K                         (per tile, red.global.add.v2.f32 into dqn)
+//                   the bias gradient dTable[hh, i-j] += dS sums the fp32 dS along its diagonals into a per-CTA shared
+//                   table that is flushed to global once.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -26,451 +18,206 @@
 
 namespace omlm {
 
-constexpr int kBtThreads = 512;
-constexpr int kBtBQ = 128, kBtBK = 128;
+constexpr int kBtThreads = 384;
+constexpr int kBtBQ = 64, kBtBK = 128;
 constexpr float kBtL2e = 1.4426950408889634f;
 
-constexpr int kBoK = 0, kBoV = 16384, kBoQ = 32768 /*2 stages x 16K*/, kBoDO = 65536 /*2 x 16K*/;
-constexpr int kBoP = 98304 /*32K*/, kBoDS = 131072 /*32K: bf16(dS)*/, kBoDSL = 163840 /*32K: bf16(dS - bf16(dS))*/;
-constexpr int kBoKneg = 196608 /*512 B*/, kBoBar = 197120 /*256 B*/;
-constexpr int kBoBias = 197376;   // 2 buffers x h*W floats, then the diagonal-sum table h*Wacc floats
+constexpr int kBoK = 0, kBoV = 16384, kBoQ = 32768 /*2 stages x 8K*/, kBoDO = 49152 /*2 x 8K*/;
+constexpr int kBoP = 65536 /*2 wg x 8K*/, kBoDS = 81920 /*2 wg x 8K*/, kBoBar = 98304 /*64 B*/;
+constexpr int kBoAcc = 98368;     // diagonal-sum table: h x Wacc floats
 constexpr int kBtMaxSmem = 232448;
 
-__device__ __forceinline__ void bt_tmem_ld32(uint32_t taddr, float* r) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]),
-        "=r"(u[16]), "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]),
-        "=r"(u[24]), "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-      : "r"(taddr));
-}
 __device__ __forceinline__ float bt_ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void bt_red4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-// byte offset of 16-byte chunk `ch` (8 keys) of row `row` inside a swizzled [128 rows][128 keys] bf16 tile
-__device__ __forceinline__ uint32_t bt_tile_off(int row, int ch) {
-  return static_cast<uint32_t>((ch >> 3) * 16384 + row * 128 + (((ch & 7) ^ (row & 7)) << 4));
-}
-
-// Diagonal sums of one dS tile, fast path for h = 128 / IPT heads (tile rows = IPT positions x h heads).
-// A thread owns (head hh, 8-key chunk ch) and walks the tile's IPT positions; element (il, key c) belongs to the
-// diagonal i - j = const, i.e. to register bin il - (c % 8) + 7: all indices are static after unrolling.
-// Two steps so that the dS tiles are released before the shared table is touched:
-//   bt_diag_gather: tile -> register bins (NU = 16 H / 128 units per thread);
-//   bt_diag_flush : register bins -> per-CTA table.  The strips of chunks ch and ch + 3 of one head do not overlap
-//                   (23 bins, 8 apart), so three rounds of plain read-modify-write separated by the warpgroup's named
-//                   barrier replace the shared-memory float atomics (CAS loops in SASS).
-template <int IPT>
-__device__ __forceinline__ void bt_diag_gather(const uint8_t* ds_hi, const uint8_t* ds_lo, int tid,
-                                               float (&acc)[16 * (128 / IPT) / 128][IPT + 7]) {
-  constexpr int H = 128 / IPT, NU = 16 * H / 128;
-#pragma unroll
-  for (int n = 0; n < NU; ++n) {
-    const int u = tid + n * 128;
-    const int hh = u % H, ch = u / H;
-#pragma unroll
-    for (int k = 0; k < IPT + 7; ++k) acc[n][k] = 0.f;
-#pragma unroll
-    for (int il = 0; il < IPT; ++il) {
-      const uint32_t off = bt_tile_off(il * H + hh, ch);
-      const uint4 a = *reinterpret_cast<const uint4*>(ds_hi + off);
-      const uint4 b = *reinterpret_cast<const uint4*>(ds_lo + off);
-      const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float2 x = unpack_bf16x2(aw[q]), y = unpack_bf16x2(bw[q]);
-        acc[n][il - 2 * q + 7] += x.x + y.x;       // key 8 ch + 2q
-        acc[n][il - 2 * q + 6] += x.y + y.y;       // key 8 ch + 2q + 1
-      }
-    }
-  }
-}
-template <int IPT>
-__device__ __forceinline__ void bt_diag_flush(float* dacc, int Wacc, int tid, int base_t,
-                                              const float (&acc)[16 * (128 / IPT) / 128][IPT + 7]) {
-  constexpr int H = 128 / IPT, NU = 16 * H / 128;
-#pragma unroll
-  for (int phase = 0; phase < 3; ++phase) {
-#pragma unroll
-    for (int n = 0; n < NU; ++n) {
-      const int u = tid + n * 128;
-      const int hh = u % H, ch = u / H;
-      if (ch % 3 == phase) {
-        float* dst = dacc + hh * Wacc + base_t + 120 - ch * 8;
-#pragma unroll
-        for (int k = 0; k < IPT + 7; ++k) dst[k] += acc[n][k];
-      }
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-  }
-}
-
-// Any head count: one thread per tile row, every non-zero element goes to the shared table by itself.
-__device__ __forceinline__ void bt_diag_generic(const uint8_t* ds_hi, const uint8_t* ds_lo, float* dacc, int Wacc, int tid,
-                                                int r0, int R, int h, int i_min0) {
-  const int r = r0 + tid;
-  if (r >= R) return;
-  const int i = r / h, hh = r - i * h;
-  float* dst = dacc + hh * Wacc + (i - i_min0) + 127;
-#pragma unroll 1
-  for (int ch = 0; ch < 16; ++ch) {
-    const uint32_t off = bt_tile_off(tid, ch);
-    const uint4 a = *reinterpret_cast<const uint4*>(ds_hi + off);
-    const uint4 b = *reinterpret_cast<const uint4*>(ds_lo + off);
-    const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float2 x = unpack_bf16x2(aw[q]), y = unpack_bf16x2(bw[q]);
-      const float v0 = x.x + y.x, v1 = x.y + y.y;
-      if (v0 != 0.f) atomicAdd(dst - (ch * 8 + 2 * q), v0);
-      if (v1 != 0.f) atomicAdd(dst - (ch * 8 + 2 * q + 1), v1);
-    }
-  }
+__device__ __forceinline__ void bt_red2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 __global__ void __launch_bounds__(kBtThreads, 1)
 attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
-                   const __grid_constant__ CUtensorMap tmKV,
-                   const float* __restrict__ lse2, const float* __restrict__ dsum, const float* __restrict__ table,
-                   int table_ld, const unsigned char* __restrict__ key_mask, float* __restrict__ dqn,
-                   float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale, int W, int Wd,
-                   int Wacc, int tiles_per_chunk, int units_per_batch) {
+                   const __grid_constant__ CUtensorMap tmKV, const float* __restrict__ lse2, const float* __restrict__ dsum,
+                   const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
+                   float* __restrict__ dqn, float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale,
+                   int Wacc, int tiles_per_chunk, int nbatch) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kBoBar);
   uint64_t* kv_full = bars + 0;
-  uint64_t* qdo_full = bars + 1;    // [2]
-  uint64_t* qdo_empty = bars + 3;   // [2]
-  uint64_t* sd_full = bars + 5;     // S, dP complete in TMEM
-  uint64_t* sd_free = bars + 6;     // S, dP copied to registers (8 warps)
-  uint64_t* pds_full = bars + 7;    // P, dS tiles in smem (8 warps)
-  uint64_t* pds_empty = bars + 8;   // dV/dK/dQ MMAs finished reading P, dS
-  uint64_t* dq_full = bars + 9;     // dQ tile complete in TMEM
-  uint64_t* dq_free = bars + 10;    // dQ tile drained (4 warps)
-  uint64_t* b_full = bars + 11;     // [2]
-  uint64_t* b_empty = bars + 13;    // [2]
-  uint64_t* diag_free = bars + 15;  // diagonal sums of the dS tile taken (4 warps)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  float* kneg = reinterpret_cast<float*>(smem + kBoKneg);
-  float* bias = reinterpret_cast<float*>(smem + kBoBias);
-  const int slice = h * W;
-  float* dacc = bias + 2 * slice;
+  uint64_t* qd_full = bars + 1;    // [2]
+  uint64_t* qd_empty = bars + 3;   // [2]
+  float* dacc = reinterpret_cast<float*>(smem + kBoAcc);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int R = N * h;
-  const int n_row_tiles = (R + kBtBQ - 1) / kBtBQ;
-  // ---- work unit: (b, key tile kt, chunk of row tiles)
-  const int b = blockIdx.x / units_per_batch;
-  int u = blockIdx.x - b * units_per_batch;
-  int kt = 0, rt_begin = 0, rt_end = 0;
-  for (;; ++kt) {
-    const int first = (kt * kBtBK * h) / kBtBQ;
-    const int chunks = (n_row_tiles - first + tiles_per_chunk - 1) / tiles_per_chunk;
-    if (u < chunks) { rt_begin = first + u * tiles_per_chunk; rt_end = min(n_row_tiles, rt_begin + tiles_per_chunk); break; }
-    u -= chunks;
+  const int n_rt = (R + kBtBQ - 1) / kBtBQ;
+  const int n_kt = (N + kBtBK - 1) / kBtBK;
+  // unit -> (batch, key tile, chunk): key tile 0 (the most row tiles) first
+  const int b = blockIdx.x % nbatch;
+  int u = blockIdx.x / nbatch, kt = 0;
+  for (; kt < n_kt; ++kt) {
+    const int cnt = (n_rt - (kt * kBtBK * h) / kBtBQ + tiles_per_chunk - 1) / tiles_per_chunk;
+    if (u < cnt) break;
+    u -= cnt;
   }
   const int j0 = kt * kBtBK;
-  const int T = rt_end - rt_begin;
+  const int rt0 = (j0 * h) / kBtBQ + u * tiles_per_chunk;
+  const int rt1 = min(n_rt, rt0 + tiles_per_chunk);
+  const int T = rt1 - rt0;
+  const int i_lo = (rt0 * kBtBQ) / h, i_hi = min(N - 1, (rt1 * kBtBQ - 1) / h);
+  const int dmin = max(0, i_lo - j0 - (kBtBK - 1));
+  const int wacc_used = i_hi - j0 - dmin + 1;       // <= Wacc (host bound)
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmDO); tma_prefetch_desc(&tmKV);
     mbar_init(kv_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 1);
-      mbar_init(&b_full[i], 2); mbar_init(&b_empty[i], 8);
-    }
-    mbar_init(sd_full, 1); mbar_init(sd_free, 8); mbar_init(pds_full, 8); mbar_init(pds_empty, 1);
-    mbar_init(dq_full, 1); mbar_init(dq_free, 4); mbar_init(diag_free, 4);
+    for (int i = 0; i < 2; ++i) { mbar_init(&qd_full[i], 1); mbar_init(&qd_empty[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
+  for (int x = threadIdx.x; x < h * Wacc; x += blockDim.x) dacc[x] = 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    if (warp == 0) {
-      // ------------------------------------------------------------------ TMA producer
-      if (lane == 0) {
-        mbar_expect_tx(kv_full, 2 * 16384);
-        tma_load_2d(smem + kBoK, &tmKV, kv_full, 0, b * N + j0);
-        tma_load_2d(smem + kBoV, &tmKV, kv_full, 64, b * N + j0);
-        for (int t = 0; t < T; ++t) {
-          const int st = t & 1;
-          mbar_wait(&qdo_empty[st], ((t >> 1) & 1) ^ 1);
-          mbar_expect_tx(&qdo_full[st], 2 * 16384);
-          tma_load_2d(smem + kBoQ + st * 16384, &tmQ, &qdo_full[st], 0, b * R + (rt_begin + t) * kBtBQ);
-          tma_load_2d(smem + kBoDO + st * 16384, &tmDO, &qdo_full[st], 0, b * R + (rt_begin + t) * kBtBQ);
-        }
-      }
-    } else if (warp == 1) {
-      // ------------------------------------------------------------------ MMA issuer
-      if (lane == 0) {
-        constexpr uint32_t id_s = make_idesc_bf16(128, 128, 0, 0);   // S, dP: A and B K-major
-        constexpr uint32_t id_kv = make_idesc_bf16(128, 64, 1, 1);   // dV, dK: A (P / dS) and B (dO / Q) MN-major
-        constexpr uint32_t id_q = make_idesc_bf16(128, 64, 0, 1);    // dQ: A (dS) K-major, B (K) MN-major
-        const uint32_t sk = smem_u32(smem + kBoK), sv = smem_u32(smem + kBoV), sq = smem_u32(smem + kBoQ),
-                       sdo = smem_u32(smem + kBoDO), sp = smem_u32(smem + kBoP), sds = smem_u32(smem + kBoDS);
-        auto issue_s_dp = [&](int st) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_bf16(tmem_base + 0, make_smem_desc(sq + st * 16384 + ks * 32, 16, 1024),
-                      make_smem_desc(sk + ks * 32, 16, 1024), id_s, ks > 0 ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_bf16(tmem_base + 128, make_smem_desc(sdo + st * 16384 + ks * 32, 16, 1024),
-                      make_smem_desc(sv + ks * 32, 16, 1024), id_s, ks > 0 ? 1u : 0u);
-        };
-        mbar_wait(kv_full, 0);
-        mbar_wait(&qdo_full[0], 0);
-        tc_fence_after();
-        issue_s_dp(0);
-        umma_commit(sd_full);
-        for (int t = 0; t < T; ++t) {
-          const int st = t & 1;
-          if (t + 1 < T) {   // next tile's S / dP as soon as this tile's are in registers
-            mbar_wait(sd_free, t & 1);
-            mbar_wait(&qdo_full[(t + 1) & 1], ((t + 1) >> 1) & 1);
-            tc_fence_after();
-            issue_s_dp((t + 1) & 1);
-            umma_commit(sd_full);
-          }
-          mbar_wait(pds_full, t & 1);
-          if (t > 0) mbar_wait(dq_free, (t - 1) & 1);
-          tc_fence_after();
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)   // dV[key, d] += P^T dO   (k = 16 query rows per step)
-            umma_bf16(tmem_base + 384, make_smem_desc(sp + ks * 2048, 16384, 1024),
-                      make_smem_desc(sdo + st * 16384 + ks * 2048, 16384, 1024), id_kv, (t > 0 || ks > 0) ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)   // dK[key, d] += dS^T Q
-            umma_bf16(tmem_base + 320, make_smem_desc(sds + ks * 2048, 16384, 1024),
-                      make_smem_desc(sq + st * 16384 + ks * 2048, 16384, 1024), id_kv, (t > 0 || ks > 0) ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)   // dQ[row, d] = dS K   (k = 16 keys per step)
-            umma_bf16(tmem_base + 256, make_smem_desc(sds + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024),
-                      make_smem_desc(sk + ks * 2048, 16384, 1024), id_q, ks > 0 ? 1u : 0u);
-          umma_commit(dq_full);
-          umma_commit(&qdo_empty[st]);
-          umma_commit(pds_empty);
-        }
-      }
-    } else {
-      // ------------------------------------------------------------------ bias-slice / key-mask builders (64 threads)
-      const int tid = threadIdx.x - 64;
-      for (int c = tid; c < kBtBK; c += 64) {
-        const int j = j0 + c;
-        const bool vis = (j < N) && (key_mask == nullptr || key_mask[static_cast<long long>(b) * N + j] != 0);
-        kneg[c] = vis ? 0.f : -INFINITY;
-      }
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(kv_full, 2 * 16384);
+      tma_load_2d(smem + kBoK, &tmKV, kv_full, 0, b * N + j0);
+      tma_load_2d(smem + kBoV, &tmKV, kv_full, 64, b * N + j0);
       for (int t = 0; t < T; ++t) {
-        const int buf = t & 1;
-        mbar_wait(&b_empty[buf], ((t >> 1) & 1) ^ 1);
-        const int i_min = ((rt_begin + t) * kBtBQ) / h;
-        const int delta_min = i_min - j0 - (kBtBK - 1);
-        float* dst = bias + buf * slice;
-        for (int hh0 = 0; hh0 < h; hh0 += 4) {
-          float v[4][4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float* trow = table + min(hh0 + k, h - 1) * table_ld;
-#pragma unroll
-            for (int uu = 0; uu < 4; ++uu) {
-              const int w = tid + uu * 64;
-              const int delta = delta_min + w;
-              v[k][uu] = (w < Wd && delta >= 0) ? __ldg(trow + min(delta, N - 1)) : -INFINITY;
-            }
-          }
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (hh0 + k < h) {
-#pragma unroll
-              for (int uu = 0; uu < 4; ++uu) {
-                const int w = tid + uu * 64;
-                if (w < Wd) dst[(hh0 + k) * W + w] = v[k][uu] * kBtL2e;
-              }
-            }
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&b_full[buf]);
+        const int st = t & 1;
+        mbar_wait(&qd_empty[st], ((t >> 1) & 1) ^ 1);
+        mbar_expect_tx(&qd_full[st], 2 * 8192);
+        tma_load_2d(smem + kBoQ + st * 8192, &tmQ, &qd_full[st], 0, b * R + (rt0 + t) * kBtBQ);
+        tma_load_2d(smem + kBoDO + st * 8192, &tmDO, &qd_full[st], 0, b * R + (rt0 + t) * kBtBQ);
       }
-    }
-  } else if (warp < 12) {
-    // -------------------------------------------------------------------- P / dS: one thread per (query row, 64-key half)
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
-    const int half = (warp - 4) >> 2;
-    const int quarter = warp & 3;
-    const int row_local = quarter * 32 + lane;
-    const uint32_t t_s = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + half * 64;
-    uint8_t* prow = smem + kBoP + half * 16384 + row_local * 128;
-    uint8_t* dsrow = smem + kBoDS + half * 16384 + row_local * 128;
-    uint8_t* dslrow = smem + kBoDSL + half * 16384 + row_local * 128;
-    const int sw = row_local & 7;
-    const float sc2 = scale * kBtL2e;
-    const float* kn = kneg + half * 64;
-    // per-row softmax statistics: loaded one tile ahead (a dependent global load at the top of every tile stalled the warp)
-    auto row_stats = [&](int t, float& l2v, float& dsmv) {
-      const int rr = (rt_begin + t) * kBtBQ + row_local;
-      const bool ok = t < T && rr < R;
-      l2v = ok ? __ldg(lse2 + static_cast<long long>(b) * R + rr) : INFINITY;
-      dsmv = ok ? __ldg(dsum + static_cast<long long>(b) * R + rr) : 0.f;
-    };
-    float l2_nx, dsm_nx;
-    row_stats(0, l2_nx, dsm_nx);
-    for (int t = 0; t < T; ++t) {
-      const int buf = t & 1;
-      const int r0 = (rt_begin + t) * kBtBQ;
-      const int r = r0 + row_local;
-      const int rc = min(r, R - 1);
-      const int i = rc / h, hh = rc - i * h;
-      const int i_min = r0 / h;
-      const float l2 = l2_nx, dsm = dsm_nx;
-      row_stats(t + 1, l2_nx, dsm_nx);
-      mbar_wait(&b_full[buf], (t >> 1) & 1);
-      mbar_wait(sd_full, t & 1);
-      tc_fence_after();
-      const float* bp = bias + buf * slice + hh * W + (i - i_min) + (kBtBK - 1) - half * 64;
-#pragma unroll 1
-      for (int c2 = 0; c2 < 2; ++c2) {   // 32 keys per step
-        float s[32], dp[32];
-        bt_tmem_ld32(t_s + c2 * 32, s);
-        bt_tmem_ld32(t_s + 128 + c2 * 32, dp);
-        tmem_ld_wait();
-        if (c2 == 1) {   // S and dP fully in registers: the tensor core may start the next tile's S / dP
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(sd_free);
-        }
-        uint32_t pp[16], dh[16], dl[16];
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) {
-          const int c = c2 * 32 + e;
-          // two keys per packed fp32x2 instruction (FADD2 / FFMA2 / FMUL2): same IEEE results, half the issue slots
-          const float2 bk = add2(make_float2(bp[-c], bp[-c - 1]), make_float2(kn[c], kn[c + 1]));
-          const float2 x = add2(fma2(make_float2(s[e], s[e + 1]), splat2(sc2), bk), splat2(-l2));
-          const float p0 = bt_ex2(x.x), p1 = bt_ex2(x.y);
-          pp[e >> 1] = pack_bf16x2(p0, p1);
-          const float2 d = mul2(make_float2(p0, p1), add2(make_float2(dp[e], dp[e + 1]), splat2(-dsm)));
-          const uint32_t hi = pack_bf16x2(d.x, d.y);
-          const float2 hf = unpack_bf16x2(hi);
-          dh[e >> 1] = hi;
-          const float2 lo = add2(d, make_float2(-hf.x, -hf.y));
-          dl[e >> 1] = pack_bf16x2(lo.x, lo.y);
-        }
-        if (c2 == 0 && t > 0) {
-          // the previous tile's MMAs and its diagonal sums must be done with the P / dS buffers
-          mbar_wait(pds_empty, (t - 1) & 1);
-          mbar_wait(diag_free, (t - 1) & 1);
-        }
-#pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4) {   // four 16-byte chunks of 8 keys
-          const int off = ((c2 * 4 + q4) ^ sw) << 4;
-          *reinterpret_cast<uint4*>(prow + off) = make_uint4(pp[q4 * 4], pp[q4 * 4 + 1], pp[q4 * 4 + 2], pp[q4 * 4 + 3]);
-          *reinterpret_cast<uint4*>(dsrow + off) = make_uint4(dh[q4 * 4], dh[q4 * 4 + 1], dh[q4 * 4 + 2], dh[q4 * 4 + 3]);
-          *reinterpret_cast<uint4*>(dslrow + off) = make_uint4(dl[q4 * 4], dl[q4 * 4 + 1], dl[q4 * 4 + 2], dl[q4 * 4 + 3]);
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&b_empty[buf]);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
     }
   } else {
-    // -------------------------------------------------------------------- bias-gradient diagonals + dQ / dK / dV drain
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 112;");
-    const int quarter = warp & 3;
-    const int row_local = quarter * 32 + lane;
-    const int tid = threadIdx.x - 384;
-    const uint32_t t_q = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + 256;
-    const int i_min0 = (rt_begin * kBtBQ) / h;
-    for (int i = tid; i < h * Wacc; i += 128) dacc[i] = 0.f;
-    asm volatile("bar.sync 1, 128;" ::: "memory");
+    // ------------------------------------------------------------------ consumers: 64 keys per warpgroup
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;
+    const int wq = (threadIdx.x >> 5) & 3, qr = lane >> 2, qc = lane & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int kbase = j0 + cw * 64;
+    const uint32_t sk = smem_u32(smem + kBoK) + cw * 8192, sv = smem_u32(smem + kBoV) + cw * 8192;
+    uint8_t* p_tile = smem + kBoP + cw * 8192;
+    uint8_t* ds_tile = smem + kBoDS + cw * 8192;
+    const uint32_t sp = smem_u32(p_tile), sds = smem_u32(ds_tile);
+    const float sc2 = scale * kBtL2e;
+    // key visibility of this thread's 16 columns (8 c + 2 qc + e)
+    uint32_t vis = 0;
+#pragma unroll
+    for (int c = 0; c < 8; ++c)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = kbase + 8 * c + 2 * qc + e;
+        if (j < N && (key_mask == nullptr || key_mask[static_cast<long long>(b) * N + j] != 0)) vis |= 1u << (2 * c + e);
+      }
+    float dv[32], dk[32];
+#pragma unroll
+    for (int x = 0; x < 32; ++x) { dv[x] = 0.f; dk[x] = 0.f; }
+    mbar_wait(kv_full, 0);
     for (int t = 0; t < T; ++t) {
-      const int r0 = (rt_begin + t) * kBtBQ;
-      mbar_wait(pds_full, t & 1);
-      if (h == 8) {
-        float acc[1][23];
-        bt_diag_gather<16>(smem + kBoDS, smem + kBoDSL, tid, acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(diag_free);          // the dS tiles are free again before the table is updated
-        bt_diag_flush<16>(dacc, Wacc, tid, r0 / h - i_min0, acc);
-      } else if (h == 16) {
-        float acc[2][15];
-        bt_diag_gather<8>(smem + kBoDS, smem + kBoDSL, tid, acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(diag_free);
-        bt_diag_flush<8>(dacc, Wacc, tid, r0 / h - i_min0, acc);
-      } else {
-        bt_diag_generic(smem + kBoDS, smem + kBoDSL, dacc, Wacc, tid, r0, R, h, i_min0);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(diag_free);
+      const int st = t & 1;
+      const int rbase = (rt0 + t) * kBtBQ;
+      const uint32_t sq = smem_u32(smem + kBoQ + st * 8192), sdo = smem_u32(smem + kBoDO + st * 8192);
+      mbar_wait(&qd_full[st], (t >> 1) & 1);
+      float s[32], dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        Wgmma<64, false>::ss<0, 0>(s, make_smem_desc(sq + ks * 32, 16, 1024), make_smem_desc(sk + ks * 32, 16, 1024), ks > 0 ? 1u : 0u);
+        Wgmma<64, false>::ss<0, 0>(dp, make_smem_desc(sdo + ks * 32, 16, 1024), make_smem_desc(sv + ks * 32, 16, 1024), ks > 0 ? 1u : 0u);
       }
-      // ---- dQ of this tile
-      const int r = r0 + row_local;
-      mbar_wait(dq_full, t & 1);
-      tc_fence_after();
-      float q[64];
-      bt_tmem_ld32(t_q, q);
-      bt_tmem_ld32(t_q + 32, q + 32);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dq_free);
-      if (r < R) {
-        float* dst = dqn + (static_cast<long long>(b) * R + r) * 64;
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(s);
+      wgmma_reg_fence(dp);
+      // ---- P, dS (fp32), diagonal sums, bf16 tiles
 #pragma unroll
-        for (int c = 0; c < 64; c += 4) bt_red4(dst + c, q[c] * scale, q[c + 1] * scale, q[c + 2] * scale, q[c + 3] * scale);
+      for (int hr = 0; hr < 2; ++hr) {
+        const int lr = wq * 16 + qr + hr * 8;
+        const int r = rbase + lr;
+        const bool row_ok = r < R;
+        const int rc = min(r, R - 1);
+        const int i = rc / h, hh = rc - i * h;
+        const float lse = lse2[static_cast<long long>(b) * R + rc];
+        const float D = dsum[static_cast<long long>(b) * R + rc];
+        const float* trow = table + hh * static_cast<long>(table_ld);
+        float* arow = dacc + hh * Wacc - dmin;
+        uint8_t* prow = p_tile + lr * 128;
+        uint8_t* drow = ds_tile + lr * 128;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          float pp[2], dd[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int j = kbase + 8 * c + 2 * qc + e;
+            const int delta = i - j;
+            const bool live = row_ok && ((vis >> (2 * c + e)) & 1u) && delta >= 0;
+            const float x = s[4 * c + 2 * hr + e];
+            pp[e] = live ? bt_ex2(fmaf(x, sc2, __ldg(trow + (live ? delta : 0)) * kBtL2e) - lse) : 0.f;
+            dd[e] = pp[e] * (dp[4 * c + 2 * hr + e] - D);
+            if (live) atomicAdd(arow + delta, dd[e]);
+          }
+          const uint32_t off = static_cast<uint32_t>(((c ^ (lr & 7)) << 4) + 4 * qc);
+          *reinterpret_cast<uint32_t*>(prow + off) = pack_bf16x2(pp[0], pp[1]);
+          *reinterpret_cast<uint32_t*>(drow + off) = pack_bf16x2(dd[0], dd[1]);
+        }
+      }
+      fence_proxy_async();                                   // P / dS (generic stores) -> visible to wgmma
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+      float dq[32];
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        // rows are the contraction dimension: P^T / dS^T (A) and dO / Q (B) are read MN-major, 16 rows = 2048 bytes
+        Wgmma<64, false>::ss<1, 1>(dv, make_smem_desc(sp + ks * 2048, 8192, 1024), make_smem_desc(sdo + ks * 2048, 8192, 1024), 1u);
+        Wgmma<64, false>::ss<1, 1>(dk, make_smem_desc(sds + ks * 2048, 8192, 1024), make_smem_desc(sq + ks * 2048, 8192, 1024), 1u);
+        // dQ = dS K: keys are the contraction dimension; K [key][dim] is read MN-major
+        Wgmma<64, false>::ss<0, 1>(dq, make_smem_desc(sds + ks * 32, 16, 1024), make_smem_desc(sk + ks * 2048, 8192, 1024), ks > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_reg_fence(dq);
+      wgmma_reg_fence(dv);
+      wgmma_reg_fence(dk);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");   // every thread's wgmma have read the P / dS tiles
+      if (leader) mbar_arrive(&qd_empty[st]);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = rbase + wq * 16 + qr + hr * 8;
+        if (r < R) {
+          float* dst = dqn + (static_cast<long long>(b) * R + r) * 64 + 2 * qc;
+#pragma unroll
+          for (int c = 0; c < 8; ++c) bt_red2(dst + 8 * c, dq[4 * c + 2 * hr] * scale, dq[4 * c + 2 * hr + 1] * scale);
+        }
       }
     }
-    // dq_full(T-1) also covers the last dV / dK MMAs (tcgen05.commit tracks everything issued before it)
-    const int j = j0 + row_local;
-    float a[64];
-    bt_tmem_ld32(t_q + 64, a);         // dK: cols 320..383
-    bt_tmem_ld32(t_q + 96, a + 32);
-    tmem_ld_wait();
-    if (j < N) {
-      float* dst = dkvn + (static_cast<long long>(b) * N + j) * 128;
+    // ---- dK (scaled), dV into dkvn [key][dK 0..63 | dV 64..127]
 #pragma unroll
-      for (int c = 0; c < 64; c += 4) bt_red4(dst + c, a[c] * scale, a[c + 1] * scale, a[c + 2] * scale, a[c + 3] * scale);
-    }
-    bt_tmem_ld32(t_q + 128, a);        // dV: cols 384..447
-    bt_tmem_ld32(t_q + 160, a + 32);
-    tmem_ld_wait();
-    if (j < N) {
-      float* dst = dkvn + (static_cast<long long>(b) * N + j) * 128 + 64;
+    for (int hr = 0; hr < 2; ++hr) {
+      const int j = kbase + wq * 16 + qr + hr * 8;
+      if (j < N) {
+        float* dst = dkvn + (static_cast<long long>(b) * N + j) * 128 + 2 * qc;
 #pragma unroll
-      for (int c = 0; c < 64; c += 4) bt_red4(dst + c, a[c], a[c + 1], a[c + 2], a[c + 3]);
+        for (int c = 0; c < 8; ++c) {
+          bt_red2(dst + 8 * c, dk[4 * c + 2 * hr] * scale, dk[4 * c + 2 * hr + 1] * scale);
+          bt_red2(dst + 64 + 8 * c, dv[4 * c + 2 * hr], dv[4 * c + 2 * hr + 1]);
+        }
+      }
     }
-    tc_fence_before();
-    // ---- flush the CTA's diagonal sums: table index delta = i - j = delta_base + column
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    const int delta_base = i_min0 - j0 - (kBtBK - 1);
-    for (int idx = tid; idx < h * Wacc; idx += 128) {
-      const float v = dacc[idx];
-      const int hh = idx / Wacc, delta = delta_base + (idx - hh * Wacc);
-      if (v != 0.f && delta >= 0 && delta < N) atomicAdd(&dtable[hh * table_ld + delta], v);
+    // ---- flush the diagonal sums of this unit
+    asm volatile("bar.sync 3, 256;" ::: "memory");
+    for (int x = threadIdx.x - 128; x < h * wacc_used; x += 256) {
+      const int hh = x / wacc_used, w = x - hh * wacc_used;
+      const float v = dacc[hh * Wacc + w];
+      if (v != 0.f) atomicAdd(dtable + hh * static_cast<long>(table_ld) + dmin + w, v);
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -517,27 +264,23 @@ extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o
   auto st = reinterpret_cast<cudaStream_t>(stream);
   const long R = static_cast<long>(N) * heads;
   const long rows = static_cast<long>(B) * R;
-  OMLM_KLAUNCH((attn_bwd_tc_dsum_kernel), static_cast<int>((rows * 8 + 255) / 256), 256, 0, st, 
+  OMLM_KLAUNCH((attn_bwd_tc_dsum_kernel), static_cast<int>((rows * 8 + 255) / 256), 256, 0, st,
       reinterpret_cast<const __nv_bfloat16*>(d_o), reinterpret_cast<const __nv_bfloat16*>(o), dsum_scratch, rows,
       dqn, dkvn, static_cast<long>(B) * N * 128 / 4);
   OMLM_LAUNCH_CHECK();
-  const int Wd = (kBtBQ + heads - 1) / heads + 1 + (kBtBK - 1);
-  int W = Wd;
-  const int want = (32 % heads == 0) ? (32 / heads) % 32 : 1;
-  while ((32 % heads == 0) ? (W % 32 != want) : (W % 2 == 0)) ++W;
   CUtensorMap tmQ, tmDO, tmKV;
-  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(rows), 128, 64, 128);
+  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
   if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmDO, d_o, 64, static_cast<uint64_t>(rows), 128, 64, 128);
+  rc = make_tmap_bf16_2d(&tmDO, d_o, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
   if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, 128);
+  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kBtBK);
   if (rc) return rc;
   const int n_row_tiles = static_cast<int>((R + kBtBQ - 1) / kBtBQ);
   const int n_key_tiles = (N + kBtBK - 1) / kBtBK;
-  // chunk length T: as long as the per-CTA diagonal table (heads x (ceil(128 T / heads) + 128) floats) fits in shared
-  // memory, and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
-  auto wacc_of = [&](int T) { int w = (T * kBtBQ + heads - 1) / heads + 128; return w | 1; };
-  auto smem_of = [&](int T) { return kBoBias + (2 * heads * W + heads * wacc_of(T)) * 4 + 1024; };
+  // chunk length T: as long as the per-CTA diagonal table (heads x (64 T / heads + 130) floats) fits in shared memory,
+  // and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
+  auto wacc_of = [&](int T) { return (T * kBtBQ + heads - 1) / heads + kBtBK + 2; };
+  auto smem_of = [&](int T) { return kBoAcc + heads * wacc_of(T) * 4 + 1024; };
   auto units_of = [&](int T) {
     long units = 0;
     for (int kt = 0; kt < n_key_tiles; ++kt) {
@@ -546,19 +289,18 @@ extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o
     }
     return units;
   };
-  OMLM_CHECK_ARG(smem_of(1) <= kBtMaxSmem, "attn_bwd_tc: too many heads (%d) for the shared-memory bias slices", heads);
+  OMLM_CHECK_ARG(smem_of(1) <= kBtMaxSmem, "attn_bwd_tc: too many heads (%d) for the shared-memory diagonal table", heads);
   int tiles_per_chunk = 1;
   for (int cand = 2; cand <= 2 * n_row_tiles; cand *= 2) {
     const int T = cand < n_row_tiles ? cand : n_row_tiles;
     if (smem_of(T) > kBtMaxSmem) break;
     tiles_per_chunk = T;
-    if ((T >= 4 && units_of(T) * B <= 4L * num_sms()) || T == n_row_tiles) break;
+    if ((T >= 8 && units_of(T) * B <= 4L * num_sms()) || T == n_row_tiles) break;
   }
   if (const char* e = getenv("OMLM_ATTN_BWD_T")) {      // diagnostics: force the chunk length
     const int T = atoi(e);
     if (T >= 1 && T <= n_row_tiles && smem_of(T) <= kBtMaxSmem) tiles_per_chunk = T;
   }
-  const int Wacc = wacc_of(tiles_per_chunk);
   const int smem_bytes = smem_of(tiles_per_chunk);
   static int configured = 0;
   if (configured < smem_bytes) {
@@ -566,9 +308,9 @@ extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o
     configured = smem_bytes;
   }
   const int units_per_batch = static_cast<int>(units_of(tiles_per_chunk));
-  OMLM_KLAUNCH((attn_bwd_tc_kernel), B * units_per_batch, kBtThreads, smem_bytes, st, 
-      tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale, W, Wd, Wacc,
-      tiles_per_chunk, units_per_batch);
+  OMLM_KLAUNCH((attn_bwd_tc_kernel), B * units_per_batch, kBtThreads, smem_bytes, st,
+      tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale,
+      wacc_of(tiles_per_chunk), tiles_per_chunk, B);
   OMLM_LAUNCH_CHECK();
   return 0;
 }

@@ -1,21 +1,16 @@
-// Fused causal multi-query cosine-sim attention, forward, on the 5th-gen tensor cores (tcgen05 + TMEM + TMA).
+// Fused causal multi-query cosine-sim attention, forward, on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 //   sim = 8 * qn . kn + table[hh, i-j];  key-padding mask; causal mask; softmax (fp32); out = P v
 //   (transformer.py:304-331; q/k arrive l2-normalised and scaled, transformer.py:269-271)
 //
 // Folded-row layout (attn_common.cuh): per batch element the h heads of MQA are R = N*h query rows,
-// row r = i*h + head, sharing one K/V head.  A CTA owns TWO 128-row query tiles (one per softmax
-// warpgroup) and streams 128-key K/V tiles through a 2-stage TMA ring:
+// row r = i*h + head, sharing one K/V head.  A CTA owns one 128-row query tile and streams 128-key K/V tiles
+// through a 2-stage TMA ring:
 //
-//   warp 0        TMA producer (Q tiles once, K/V ring)
-//   warp 1        tcgen05.mma issuer: S_w = Q_w K^T (128x128x64, TMEM), O_w = P_w V (128x64x128, TMEM),
-//                 ping-ponged between the two warpgroups so that the tensor pipe works on one tile
-//                 while the other warpgroup does softmax
-//   warps 2,3     build the fp32 bias slice (Toeplitz table window, causal -inf folded in) and the key mask
-//                 of the NEXT tile in shared memory
-//   warps 4-7, 8-11  softmax warpgroups: one thread per query row (TMEM lane), S row in registers
-//                 (tcgen05.ld), online softmax in the log2 domain, P -> bf16 -> 128B-swizzled smem (A operand
-//                 of the PV MMA), O accumulated in registers from the per-tile TMEM result.
+//   warpgroup 0     TMA producer (Q tile once, K/V ring)
+//   warpgroups 1,2  64 query rows each: S = Q K^T (wgmma m64n128k16, operands in 128B-swizzled smem, S in registers),
+//                   online softmax in the log2 domain on the accumulator fragment (a row lives in the four lanes of a
+//                   quad), P -> bf16 in registers, O += P V (wgmma m64n64k16 with A from registers, V read MN-major).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -23,41 +18,16 @@
 namespace omlm {
 
 constexpr int kTcThreads = 384;
-constexpr int kTcBQ = 128;      // rows per warpgroup tile
+constexpr int kTcBQ = 128;      // query rows per CTA (64 per consumer warpgroup)
 constexpr int kTcBK = 128;      // keys per tile
 constexpr float kL2e = 1.4426950408889634f;
 
 // smem carve-up (offsets from a 1024-aligned base)
-constexpr int kOffQ = 0;                        // 2 x 16 KB
-constexpr int kOffK = 32768;                    // 2 x 16 KB
-constexpr int kOffV = 65536;                    // 2 x 16 KB
-constexpr int kOffP = 98304;                    // 2 wg x 32 KB
-constexpr int kOffKneg = 163840;                // 2 x 128 floats
-constexpr int kOffBar = 164864;                 // barriers + tmem slot (256 B)
-constexpr int kOffBias = 165120;                // 2 buf x 2 wg x h*W floats
-
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float* r) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]),
-        "=r"(u[16]), "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]),
-        "=r"(u[24]), "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-      : "r"(taddr));
-}
-
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float* r) {
-  uint32_t* u = reinterpret_cast<uint32_t*>(r);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-      : "r"(taddr));
-}
+constexpr int kOffQ = 0;                        // 16 KB
+constexpr int kOffK = 16384;                    // 2 x 16 KB
+constexpr int kOffV = 49152;                    // 2 x 16 KB
+constexpr int kOffBar = 81920;                  // barriers
+constexpr int kTcSmem = kOffBar + 64 + 1024;
 
 __device__ __forceinline__ float ex2_fast(float x) {
   float y;
@@ -68,8 +38,7 @@ __device__ __forceinline__ float ex2_fast(float x) {
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
-                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int W,
-                   int Wd, int nbatch) {
+                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int nbatch) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // pointer arithmetic (not an integer round trip) keeps the shared address space visible to the compiler: LDS/STS, not generic LD/ST
@@ -78,279 +47,151 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;    // [2]
   uint64_t* kv_empty = bars + 3;   // [2]
-  uint64_t* s_full = bars + 5;     // [2 wg]
-  uint64_t* p_full = bars + 7;     // [2 wg]
-  uint64_t* o_full = bars + 9;     // [2 wg]
-  uint64_t* b_full = bars + 11;    // [2 buf]
-  uint64_t* b_empty = bars + 13;   // [2 buf]
-  uint64_t* s_free = bars + 15;    // [2 wg]  S tile copied to registers: the MMA warp may overwrite it
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
-  float* kneg = reinterpret_cast<float*>(smem + kOffKneg);
-  float* bias = reinterpret_cast<float*>(smem + kOffBias);
-  const int slice = h * W;  // floats per (buf, wg) slice
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int R = N * h;
-  const int nblk = (R + 2 * kTcBQ - 1) / (2 * kTcBQ);
+  const int nblk = (R + kTcBQ - 1) / kTcBQ;
   // longest-processing-time-first: all batch elements of the heaviest (latest) row block are scheduled first
   const int b = blockIdx.x % nbatch;
   const int rb = nblk - 1 - blockIdx.x / nbatch;
-  const int r0 = rb * 2 * kTcBQ;
-  const int i_max_cta = min(N - 1, (r0 + 2 * kTcBQ - 1) / h);
+  const int r0 = rb * kTcBQ;
+  const int i_max_cta = min(N - 1, (r0 + kTcBQ - 1) / h);
   const int T = i_max_cta / kTcBK + 1;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmKV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1);
-      mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 4); mbar_init(&o_full[i], 1);
-      mbar_init(&b_full[i], 2); mbar_init(&b_empty[i], 8); mbar_init(&s_free[i], 4);
-    }
+    for (int i = 0; i < 2; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    if (warp == 0) {
-      // ------------------------------------------------------------------ TMA producer
-      if (lane == 0) {
-        mbar_expect_tx(q_full, 2 * 16384);
-        tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, b * R + r0);
-        tma_load_2d(smem + kOffQ + 16384, &tmQ, q_full, 0, b * R + r0 + kTcBQ);
-        for (int t = 0; t < T; ++t) {
-          const int st = t & 1;
-          mbar_wait(&kv_empty[st], ((t >> 1) & 1) ^ 1);
-          mbar_expect_tx(&kv_full[st], 2 * 16384);
-          tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, b * N + t * kTcBK);
-          tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, b * N + t * kTcBK);
-        }
-      }
-    } else if (warp == 1) {
-      // ------------------------------------------------------------------ MMA issuer
-      if (lane == 0) {
-        constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-        constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-        const uint32_t sq = smem_u32(smem + kOffQ), sk = smem_u32(smem + kOffK), sv = smem_u32(smem + kOffV),
-                       sp = smem_u32(smem + kOffP);
-        auto issue_s = [&](int wg, int st) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_bf16(tmem_base + wg * 128, make_smem_desc(sq + wg * 16384 + ks * 32, 16, 1024),
-                      make_smem_desc(sk + st * 16384 + ks * 32, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-        };
-        auto issue_pv = [&](int wg, int st) {
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            umma_bf16(tmem_base + 256 + wg * 64,
-                      make_smem_desc(sp + wg * 32768 + (ks >> 2) * 16384 + (ks & 3) * 32, 16, 1024),
-                      make_smem_desc(sv + st * 16384 + ks * 2048, 8192, 1024), idesc_o, ks > 0 ? 1u : 0u);
-        };
-        mbar_wait(q_full, 0);
-        mbar_wait(&kv_full[0], 0);
-        tc_fence_after();
-        issue_s(0, 0); umma_commit(&s_full[0]);
-        issue_s(1, 0); umma_commit(&s_full[1]);
-        for (int t = 0; t < T; ++t) {
-          const int st = t & 1;
-          if (t + 1 < T) {
-            // S of the next tile as soon as the warpgroup has pulled the current S into registers
-            mbar_wait(&kv_full[(t + 1) & 1], ((t + 1) >> 1) & 1);
-#pragma unroll
-            for (int wg = 0; wg < 2; ++wg) {
-              mbar_wait(&s_free[wg], t & 1);
-              tc_fence_after();
-              issue_s(wg, (t + 1) & 1);
-              umma_commit(&s_full[wg]);
-            }
-          }
-#pragma unroll
-          for (int wg = 0; wg < 2; ++wg) {
-            mbar_wait(&p_full[wg], t & 1);
-            tc_fence_after();
-            issue_pv(wg, st);
-            umma_commit(&o_full[wg]);
-          }
-          umma_commit(&kv_empty[st]);
-        }
-      }
-    } else {
-      // ------------------------------------------------------------------ bias-slice / key-mask builders (64 threads)
-      const int tid = threadIdx.x - 64;
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(q_full, 16384);
+      tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, b * R + r0);
       for (int t = 0; t < T; ++t) {
-        const int buf = t & 1;
-        mbar_wait(&b_empty[buf], ((t >> 1) & 1) ^ 1);
-        const int j0 = t * kTcBK;
-        for (int wg = 0; wg < 2; ++wg) {
-          const int i_min = (r0 + wg * kTcBQ) / h;
-          const int delta_min = i_min - j0 - (kTcBK - 1);
-          float* dst = bias + (buf * 2 + wg) * slice;
-          // all loads of 4 head rows are issued back to back (16 independent L2/L1 requests per thread) before
-          // any store: the slice build must stay well below one tile of softmax time
-          for (int hh0 = 0; hh0 < h; hh0 += 4) {
-            float v[4][4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int hh = min(hh0 + k, h - 1);
-              const float* trow = table + hh * table_ld;
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const int w = tid + u * 64;
-                const int delta = delta_min + w;
-                v[k][u] = (w < Wd && delta >= 0) ? __ldg(trow + min(delta, N - 1)) : -INFINITY;
-              }
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if (hh0 + k < h) {
-                float* drow = dst + (hh0 + k) * W;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                  const int w = tid + u * 64;
-                  if (w < Wd) drow[w] = v[k][u] * kL2e;
-                }
-              }
-            }
-          }
-        }
-        for (int c = tid; c < kTcBK; c += 64) {
-          const int j = j0 + c;
-          const bool vis = (j < N) && (key_mask == nullptr || key_mask[static_cast<long long>(b) * N + j] != 0);
-          kneg[buf * kTcBK + c] = vis ? 0.f : -INFINITY;
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&b_full[buf]);
+        const int st = t & 1;
+        mbar_wait(&kv_empty[st], ((t >> 1) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[st], 2 * 16384);
+        tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, b * N + t * kTcBK);
+        tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, b * N + t * kTcBK);
       }
     }
-  } else {
-    // -------------------------------------------------------------------- softmax warpgroups
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int wg = (warp - 4) >> 2;
-    const int quarter = warp & 3;
-    const int row_local = quarter * 32 + lane;
-    const int r = r0 + wg * kTcBQ + row_local;
-    const int rc = min(r, R - 1);
-    const int i = rc / h, hh = rc - i * h;
-    const int i_min = (r0 + wg * kTcBQ) / h;
-    const uint32_t t_s = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + wg * 128;
-    const uint32_t t_o = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + 256 + wg * 64;
-    uint8_t* prow = smem + kOffP + wg * 32768 + row_local * 128;
-    const int sw = row_local & 7;
-    const float sc2 = scale * kL2e;
-    float m = -INFINITY, l = 0.f;
-    float o_acc[64];
-#pragma unroll
-    for (int c = 0; c < 64; ++c) o_acc[c] = 0.f;
-
-    float alpha_prev = 1.f;
-    for (int t = 0; t < T; ++t) {
-      const int buf = t & 1;
-      mbar_wait(&b_full[buf], (t >> 1) & 1);
-      mbar_wait(&s_full[wg], t & 1);
-      tc_fence_after();
-      float s[128];
-      tmem_ld32_nowait(t_s, s);
-      tmem_ld32_nowait(t_s + 32, s + 32);
-      tmem_ld32_nowait(t_s + 64, s + 64);
-      tmem_ld32_nowait(t_s + 96, s + 96);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_free[wg]);
-      const float* bp = bias + (buf * 2 + wg) * slice + hh * W + (i - i_min) + (kTcBK - 1);
-      const float* kn = kneg + buf * kTcBK;
-      float mx = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 128; c += 4) {
-        const float4 k4 = *reinterpret_cast<const float4*>(kn + c);   // warp-uniform address: one broadcast wavefront
-        {   // two keys per packed fp32x2 instruction (FADD2 / FFMA2): same IEEE results, half the issue slots
-          const float2 a01 = fma2(make_float2(s[c + 0], s[c + 1]), splat2(sc2), add2(make_float2(bp[-c - 0], bp[-c - 1]), make_float2(k4.x, k4.y)));
-          const float2 a23 = fma2(make_float2(s[c + 2], s[c + 3]), splat2(sc2), add2(make_float2(bp[-c - 2], bp[-c - 3]), make_float2(k4.z, k4.w)));
-          s[c + 0] = a01.x; s[c + 1] = a01.y; s[c + 2] = a23.x; s[c + 3] = a23.y;
-        }
-        mx = fmaxf(mx, fmaxf(fmaxf(s[c], s[c + 1]), fmaxf(s[c + 2], s[c + 3])));
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&b_empty[buf]);
-      const float m_new = fmaxf(m, mx);
-      const float ref = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = ex2_fast(m - ref);
-      m = m_new;
-      // ---- O_tile of the PREVIOUS tile first (its PV MMA was issued a whole tile ago): once o_full(t-1) has been
-      //      observed the P buffer is free as well, so the exponentials below stream straight into shared memory
-      //      instead of being parked in 64 registers
-      if (t > 0) {
-        mbar_wait(&o_full[wg], (t - 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int qd = 0; qd < 4; ++qd) {     // 16 columns at a time: the S row (128 registers) is still live here
-          float ot[16];
-          tmem_ld16_nowait(t_o + qd * 16, ot);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 16; ++c) o_acc[qd * 16 + c] = fmaf(o_acc[qd * 16 + c], alpha_prev, ot[c]);
-        }
-      }
-      alpha_prev = alpha;
-      // ---- P = exp2(s - ref) -> bf16 -> smem; four independent partial sums (one serial FADD chain stalled on every MUFU)
-      float sum0 = 0.f, sum1 = 0.f, sum2 = 0.f, sum3 = 0.f;
-#pragma unroll
-      for (int ch = 0; ch < 16; ++ch) {
-        const float2 nref = splat2(-ref);
-        const float2 x01 = add2(make_float2(s[8 * ch + 0], s[8 * ch + 1]), nref), x23 = add2(make_float2(s[8 * ch + 2], s[8 * ch + 3]), nref);
-        const float2 x45 = add2(make_float2(s[8 * ch + 4], s[8 * ch + 5]), nref), x67 = add2(make_float2(s[8 * ch + 6], s[8 * ch + 7]), nref);
-        const float p0 = ex2_fast(x01.x), p1 = ex2_fast(x01.y), p2 = ex2_fast(x23.x), p3 = ex2_fast(x23.y);
-        const float p4 = ex2_fast(x45.x), p5 = ex2_fast(x45.y), p6 = ex2_fast(x67.x), p7 = ex2_fast(x67.y);
-        sum0 += p0 + p1; sum1 += p2 + p3; sum2 += p4 + p5; sum3 += p6 + p7;
-        *reinterpret_cast<uint4*>(prow + (ch >> 3) * 16384 + (((ch & 7) ^ sw) << 4)) =
-            make_uint4(pack_bf16x2(p0, p1), pack_bf16x2(p2, p3), pack_bf16x2(p4, p5), pack_bf16x2(p6, p7));
-      }
-      l = l * alpha + ((sum0 + sum1) + (sum2 + sum3));
-      fence_proxy_async();       // P (generic-proxy stores) must be visible to the tensor core's async proxy
-      tc_fence_before();         // orders this thread's TMEM reads (S, O) before the MMA warp overwrites them
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_full[wg]);
-    }
-    {
-      mbar_wait(&o_full[wg], (T - 1) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int hf = 0; hf < 2; ++hf) {
-        float ot[32];
-        tmem_ld32_nowait(t_o + hf * 32, ot);
-        tmem_ld_wait();
-#pragma unroll
-        for (int c = 0; c < 32; ++c) o_acc[hf * 32 + c] = fmaf(o_acc[hf * 32 + c], alpha_prev, ot[c]);
-      }
-    }
-    tc_fence_before();
-    // ---- finalise
-    if (r < R) {
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      __nv_bfloat16* op = out + (static_cast<long long>(b) * R + r) * 64;
-#pragma unroll
-      for (int ch = 0; ch < 8; ++ch) {
-        uint4 v;
-        v.x = pack_bf16x2(o_acc[ch * 8 + 0] * inv, o_acc[ch * 8 + 1] * inv);
-        v.y = pack_bf16x2(o_acc[ch * 8 + 2] * inv, o_acc[ch * 8 + 3] * inv);
-        v.z = pack_bf16x2(o_acc[ch * 8 + 4] * inv, o_acc[ch * 8 + 5] * inv);
-        v.w = pack_bf16x2(o_acc[ch * 8 + 6] * inv, o_acc[ch * 8 + 7] * inv);
-        reinterpret_cast<uint4*>(op)[ch] = v;
-      }
-      lse2[static_cast<long long>(b) * R + r] = m + log2f(l);
-    }
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // -------------------------------------------------------------------- consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1;
+  const int wq = (threadIdx.x >> 5) & 3, qr = lane >> 2, qc = lane & 3;
+  const bool leader = (threadIdx.x & 127) == 0;
+  int rr[2], ii[2];
+  const float* trow[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    rr[hr] = r0 + cw * 64 + wq * 16 + qr + hr * 8;
+    const int rc = min(rr[hr], R - 1);
+    ii[hr] = rc / h;
+    trow[hr] = table + (rc - ii[hr] * h) * static_cast<long>(table_ld);
+  }
+  const unsigned char* km = key_mask != nullptr ? key_mask + static_cast<long long>(b) * N : nullptr;
+  const float sc2 = scale * kL2e;
+  const uint32_t sq = smem_u32(smem + kOffQ) + cw * 8192, sk = smem_u32(smem + kOffK), sv = smem_u32(smem + kOffV);
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float o[32];
+#pragma unroll
+  for (int c = 0; c < 32; ++c) o[c] = 0.f;
+
+  mbar_wait(q_full, 0);
+  for (int t = 0; t < T; ++t) {
+    const int st = t & 1;
+    mbar_wait(&kv_full[st], (t >> 1) & 1);
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+      Wgmma<128, false>::ss<0, 0>(s, make_smem_desc(sq + ks * 32, 16, 1024), make_smem_desc(sk + st * 16384 + ks * 32, 16, 1024),
+                                  ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(s);
+    // ---- bias, masks, row maxima (columns j = j0 + 8 c + 2 qc + {0,1} of rows ii[0], ii[1])
+    const int j0 = t * kTcBK;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = j0 + 8 * c + 2 * qc + e;
+        const bool vis = j < N && (km == nullptr || km[j] != 0);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int delta = ii[hr] - j;
+          float& x = s[4 * c + 2 * hr + e];
+          x = (vis && delta >= 0) ? fmaf(x, sc2, __ldg(trow[hr] + delta) * kL2e) : -INFINITY;
+          mx[hr] = fmaxf(mx[hr], x);
+        }
+      }
+    }
+    float alpha[2], ref[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+      mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+      const float m_new = fmaxf(m[hr], mx[hr]);
+      ref[hr] = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[hr] = ex2_fast(m[hr] - ref[hr]);
+      m[hr] = m_new;
+    }
+    // ---- P = exp2(s - ref) -> bf16 A fragments (k16 chunk kk = columns 16 kk .. 16 kk + 15)
+    uint32_t pa[8][4];
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      float p[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) p[e] = ex2_fast(s[8 * kk + e] - ref[(e >> 1) & 1]);
+      sum[0] += (p[0] + p[1]) + (p[4] + p[5]);
+      sum[1] += (p[2] + p[3]) + (p[6] + p[7]);
+      pa[kk][0] = pack_bf16x2(p[0], p[1]);
+      pa[kk][1] = pack_bf16x2(p[2], p[3]);
+      pa[kk][2] = pack_bf16x2(p[4], p[5]);
+      pa[kk][3] = pack_bf16x2(p[6], p[7]);
+    }
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) l[hr] = l[hr] * alpha[hr] + sum[hr];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      o[4 * c + 0] *= alpha[0]; o[4 * c + 1] *= alpha[0];
+      o[4 * c + 2] *= alpha[1]; o[4 * c + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      Wgmma<64, false>::rs<1>(o, pa[kk], make_smem_desc(sv + st * 16384 + kk * 2048, 8192, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence(o);
+    if (leader) mbar_arrive(&kv_empty[st]);
+  }
+  // ---- finalise: row sums over the quad, normalise, store
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 1);
+    l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
+    if (rr[hr] < R) {
+      const float inv = l[hr] > 0.f ? 1.f / l[hr] : 0.f;
+      __nv_bfloat16* op = out + (static_cast<long long>(b) * R + rr[hr]) * 64 + 2 * qc;
+#pragma unroll
+      for (int c = 0; c < 8; ++c)
+        *reinterpret_cast<uint32_t*>(op + 8 * c) = pack_bf16x2(o[4 * c + 2 * hr] * inv, o[4 * c + 2 * hr + 1] * inv);
+      if (qc == 0) lse2[static_cast<long long>(b) * R + rr[hr]] = m[hr] + log2f(l[hr]);
+    }
   }
 }
 
@@ -362,29 +203,20 @@ extern "C" int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* ta
   using namespace omlm;
   OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attn_fwd_tc: bad shape");
   OMLM_CHECK_ARG(table_ld >= N, "attn_fwd_tc: bias table shorter than the sequence");
-  // slice row = [positions of the tile] + 127 key offsets; the row pitch W is padded so that the 32 rows of a
-  // warp (32/h positions x h heads) hit 32 distinct banks: W = 32/h (mod 32) when h divides 32, else odd.
-  const int Wd = (kTcBQ + heads - 1) / heads + 1 + (kTcBK - 1);
-  int W = Wd;
-  const int want = (32 % heads == 0) ? (32 / heads) % 32 : 1;
-  while ((32 % heads == 0) ? (W % 32 != want) : (W % 2 == 0)) ++W;
-  const int smem_bytes = kOffBias + 4 * heads * W * 4 + 1024;
-  OMLM_CHECK_ARG(smem_bytes <= 232448, "attn_fwd_tc: too many heads (%d) for the shared-memory bias slices", heads);
   const long R = static_cast<long>(N) * heads;
   CUtensorMap tmQ, tmKV;
-  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(B) * R, 128, 64, 128);
+  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(B) * R, 128, 64, kTcBQ);
   if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, 128);
+  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kTcBK);
   if (rc) return rc;
-  static int configured = 0;
-  if (configured < smem_bytes) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    configured = smem_bytes;
+  static bool configured = false;
+  if (!configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+    configured = true;
   }
-  dim3 grid(static_cast<unsigned>((R + 2 * kTcBQ - 1) / (2 * kTcBQ)) * B, B);   // x: (row block, batch) in LPT order; y only carries B
-  grid.y = 1;
-  OMLM_KLAUNCH((attn_fwd_tc_kernel), grid, kTcThreads, smem_bytes, reinterpret_cast<cudaStream_t>(stream), 
-      tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, W, Wd, B);
+  const unsigned grid = static_cast<unsigned>((R + kTcBQ - 1) / kTcBQ) * B;   // (row block, batch) in LPT order
+  OMLM_KLAUNCH((attn_fwd_tc_kernel), grid, kTcThreads, kTcSmem, reinterpret_cast<cudaStream_t>(stream),
+      tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, B);
   OMLM_LAUNCH_CHECK();
   return 0;
 }

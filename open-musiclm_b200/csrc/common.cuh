@@ -1,4 +1,4 @@
-// Shared host/device helpers for libomlm_b200: error plumbing, TMA descriptor cache, small math.
+// Shared host/device helpers for libomlm_b200 (sm_90a): error plumbing, TMA descriptor cache, small math.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -51,10 +51,9 @@ int num_sms();
 //     this grid's CTAs have all started and resources free up), and
 //   * executes griddepcontrol.wait before its first global-memory access (it blocks until the previous grid has
 //     completed and its writes are visible), after whatever private set-up it can do early.
-// Measured on the cfg2 training step (CUDA-graph replay, same box, A/B): 11.52 ms with PDL against 11.35 ms without --
-// the persistent GEMM CTAs own the whole shared memory of their SM, so a dependent CTA cannot become resident before
-// its predecessor exits, and the programmatic graph edges cost more than the launch gaps they hide.  Hence the default
-// is the plain stream order; without the attribute both instructions are no-ops.
+// The persistent GEMM CTAs own the whole shared memory of their SM, so a dependent CTA cannot become resident before
+// its predecessor exits; the default is therefore the plain stream order.  Without the attribute both instructions
+// are no-ops.
 bool pdl_enabled();
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -103,7 +102,7 @@ __device__ __forceinline__ float bf16_round(float x) {
   return __bfloat162float(__float2bfloat16_rn(x));
 }
 // ---- 16-bit operand formats -------------------------------------------------------------------
-// The tensor-core operands are 16-bit in two flavours (tcgen05 kind::f16 takes either, per operand, at the same rate):
+// The tensor-core operands are 16-bit in two flavours (wgmma takes either at the same rate; both operands of one wgmma share the format):
 //   fp16 (11-bit significand) for tensors that are bounded by construction -- LayerNorm outputs, weights, and the
 //        FFN activations derived from them -- where it cuts the operand rounding error 8x against bf16;
 //   bf16 (8-bit significand, fp32 range) for everything whose range is not bounded: gradients, the raw residual
@@ -128,30 +127,11 @@ __device__ __forceinline__ float2 unpack16x2(uint32_t v) {
   if constexpr (F16) return unpack_f16x2(v); else return unpack_bf16x2(v);
 }
 
-// ---- GELU (exact erf) ------------------------------------------------------------------------
-// Exact-erf GELU pieces from ONE exponential: e = exp(-x^2/2) gives both the normal pdf and, through the
-// ---- packed fp32x2 arithmetic (sm_100 FFMA2 / FMUL2 / FADD2: two independent fp32 operations per issued
-// instruction).  The SIMT kernels here are issue-bound on element-wise fp32 math, so pairing neighbouring channels
-// halves their floating-point instruction count.  Same IEEE round-to-nearest results as the scalar forms.
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rc, rd;\n mov.b64 ra, {%2, %3};\n mov.b64 rb, {%4, %5};\n mov.b64 rc, {%6, %7};\n"
-      " fma.rn.f32x2 rd, ra, rb, rc;\n mov.b64 {%0, %1}, rd;}\n"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(c.x), "f"(c.y));
-  return d;
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd;\n mov.b64 ra, {%2, %3};\n mov.b64 rb, {%4, %5};\n mul.rn.f32x2 rd, ra, rb;\n mov.b64 {%0, %1}, rd;}\n"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  float2 d;
-  asm("{.reg .b64 ra, rb, rd;\n mov.b64 ra, {%2, %3};\n mov.b64 rb, {%4, %5};\n add.rn.f32x2 rd, ra, rb;\n mov.b64 {%0, %1}, rd;}\n"
-      : "=f"(d.x), "=f"(d.y) : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return d;
-}
+// ---- fp32x2 helpers: two neighbouring channels per call, written as two scalar IEEE round-to-nearest operations
+// (sm_90 has no packed fp32 arithmetic; the pairing keeps the element-wise code compact).
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 splat2(float v) { return make_float2(v, v); }
 __device__ __forceinline__ float rcp_approx(float x) {   // MUFU.RCP, <= 1 ulp, no slow path
   float r;
@@ -164,6 +144,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return r;
 }
 
+// ---- GELU (exact erf) ------------------------------------------------------------------------
 // Abramowitz-Stegun 7.1.26 rational form (|error| <= 1.5e-7, below fp32 resolution of the products here),
 // erf(x/sqrt(2)).  cdf = Phi(x), pdf = phi(x);  gelu(x) = x*cdf, gelu'(x) = cdf + x*pdf.
 __device__ __forceinline__ void normal_cdf_pdf(float x, float& cdf, float& pdf) {

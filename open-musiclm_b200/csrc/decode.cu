@@ -7,7 +7,7 @@
 //     conv state   [B, 2, 2 Fp]          the last two pre-conv FFN rows of CausalDSConv (transformer.py:122-131)
 // The bias table [h, Nmax] depends on i - j only (transformer.py:55-67), so one table serves every step.
 //
-// Kernels (M = B <= 16 rows, SIMT: a 128-row tensor-core tile would idle 90 % of its rows and 126 of 148 SMs):
+// Kernels (M = B <= 16 rows, SIMT: a 128-row tensor-core tile would idle 90 % of its rows and most SMs):
 //   skinny_gemm     out[b, n] = A[b, :] . W[n, :] (+ residual), every warp streams two W rows with 16-byte loads; the
 //                   prologue builds A in shared memory: plain 16-bit rows, fp32 rows rounded to bf16 (K/V input),
 //                   LayerNorm of fp32 rows (transformer.py:24-31), or the inner FFN LayerNorm from the fused row sums

@@ -1,7 +1,7 @@
 // One incremental decoding step of the TokenConditionedTransformer as ONE persistent kernel.
 //
 // The per-op decode path (decode.cu) spends a token in 45 launches of a few microseconds of work each: the step is
-// launch/latency bound (0.6 ms per token for 120 MB of weights, 18 us at the HBM rate).  Here the whole step --
+// launch/latency bound (120 MB of weights per token).  Here the whole step --
 // embedding row, L x (q/kv projection, cached attention, out-projection + residual, FFN-up + causal conv + GEGLU,
 // inner LayerNorm + FFN-down + residual), final LayerNorm + logit head -- runs in one launch of one CTA per SM; the
 // stages are separated by a grid-wide barrier (a global arrive counter; every CTA is resident: 1 CTA per SM, launched
@@ -12,10 +12,9 @@
 // products + butterfly, conv / GEGLU, the 4 x 32 tree of the inner-LayerNorm row sums, the attention of
 // attn_decode_kernel), so both paths produce bit-identical logits (tests/test_decode_gpu.py compares them).
 //
-// Status: opt-in (OMLM_DECODE_FUSED=1).  Measured on B200 (10 s three-stage generation, batch 1): 0.68 ms per step
-// against 0.62 ms for the CUDA-graph replay of the per-op kernels -- ncu shows the step waiting at CTA barriers behind
-// single-warp sections (LayerNorm statistics, the row-sum tree, lane-0 epilogues) and instruction-cache misses of the
-// batch-unrolled loops; the launches it saves were not the bound.  Kept as the base for a batched-decode version.
+// Status: opt-in (OMLM_DECODE_FUSED=1); the CUDA-graph replay of the per-op kernels is the default.  The step's
+// stages are each behind single-warp sections (LayerNorm statistics, the row-sum tree, lane-0 epilogues) and a grid
+// barrier, so the launches it saves are not its bound.  Kept as the base for a batched-decode version.
 //
 // Replaces the loop body of TokenConditionedTransformerWrapper.generate (open_musiclm.py:300-319).
 #include "common.cuh"

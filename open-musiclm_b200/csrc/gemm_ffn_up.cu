@@ -1,6 +1,7 @@
-// FFN up-projection as a persistent tcgen05 GEMM whose epilogue does the causal depthwise conv (k=3), GEGLU with
-// exact-erf GELU and the LayerNorm row statistics — the SIMT work runs in the epilogue warps' otherwise idle issue
-// slots while the tensor core computes the next tile (TMEM accumulators are double-buffered).
+// FFN up-projection as a persistent wgmma GEMM whose epilogue does the causal depthwise conv (k=3), GEGLU with
+// exact-erf GELU and the LayerNorm row statistics.  Warpgroup 0 is the TMA producer (it keeps loading the next tile's
+// operands during the epilogue); warpgroups 1 and 2 each own 64 rows of the tile for the wgmma and then share the
+// conv / GEGLU phase.
 //
 //   u = xn @ W1^T                  [M, 2Fp]  (bf16, kept for the backward pass)      transformer.py:144
 //   y[t] = w0 u[t-2] + w1 u[t-1] + w2 u[t]   per channel, zero history at sequence start   transformer.py:122-131
@@ -10,8 +11,7 @@
 // Tiling: 128 x 256 x 64, W1 rows interleaved so that one 256-column tile = [128 value | 128 gate] columns of the same
 // 128 channels.  The conv needs rows t-1, t-2, so M tiles overlap by two rows (tile i covers rows 126 i - 2 ..
 // 126 i + 125 and emits rows 126 i .. 126 i + 125; +1.6 % MMA work, no inter-CTA exchange).  The epilogue first parks
-// the bf16 u tile in shared memory (row pitch 528 B: conflict-free for one-row-per-thread 16-byte accesses), releases
-// TMEM, then every thread reads its own row and the two rows above it.
+// the bf16 u tile in shared memory (row pitch 528 B), then every thread reads its own row and the two rows above it.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -24,7 +24,7 @@ constexpr int kFuUPitch = 528;                                   // bytes per ro
 constexpr int kFuOffU = kFuStages * kFuStage;                    // 147456
 constexpr int kFuOffBar = kFuOffU + kFuBM * kFuUPitch;
 constexpr int kFuSmem = kFuOffBar + 256 + 1024;
-constexpr int kFuThreads = 320;   // TMA warp, MMA warp, 8 epilogue warps (two per TMEM lane quarter / per SM sub-partition)
+constexpr int kFuThreads = 384;   // TMA warpgroup, two wgmma / epilogue warpgroups
 
 // F16: xn, W1 arrive as fp16 and u, h leave as fp16 (all bounded by construction: LayerNorm output x weights);
 // otherwise everything is bf16.
@@ -38,35 +38,25 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kFuOffBar);
   uint64_t* empty_bar = full_bar + kFuStages;
-  uint64_t* tfull_bar = empty_bar + kFuStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
   uint8_t* usm = smem + kFuOffU;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int m_tiles = (M + kFuRowsOut - 1) / kFuRowsOut;
   const int n_tiles = (2 * Fp) / kFuBN;
   const int kb_total = (K + kFuBK - 1) / kFuBK;
   const int work_total = m_tiles * n_tiles;
 
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < kFuStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-      for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 8); }
-      fence_barrier_init();
-    }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
+    for (int i = 0; i < kFuStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
-  if (warp == 0) {
-    if (lane == 0) {   // ---------------------------------------------------------------- TMA producer
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {   // ---------------------------------------------------------------- TMA producer
       int stage = 0; uint32_t phase = 0;
       for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
         const int n_blk = w % n_tiles, m_blk = w / n_tiles;
@@ -80,43 +70,40 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {   // ---------------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc = make_idesc_bf16(kFuBM, kFuBN, 0, 0) & (F16 ? ~((7u << 7) | (7u << 10)) : ~0u);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0;
-      for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * kFuBN;
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kFuStage), sb = sa + kFuA;
-#pragma unroll
-          for (int k = 0; k < kFuBK / 16; ++k)
-            umma_bf16(tmem_d, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024), idesc,
-                      (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == kFuStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // -------------------------------------------------------------------------------------- epilogue warps (256 threads)
-    const int quarter = warp & 3;
-    const int t = quarter * 32 + lane;           // tile row owned by this thread (= TMEM lane)
-    const int et = threadIdx.x - 64;             // 0..255 within the epilogue group
-    const int half = et >> 7;                    // warps 2-5: first 64 channels of the tile, warps 6-9: last 64
-    int acc = 0; uint32_t acc_phase = 0;
+    // -------------------------------------------------------------------------------------- consumers (256 threads)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;                         // 64-row half of the tile for the wgmma
+    const int wq = (threadIdx.x >> 5) & 3, qr = lane >> 2, qc = lane & 3;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int et = threadIdx.x - 128;            // 0..255 within the consumer group
+    int stage = 0; uint32_t phase = 0;
     bool first = true;
     for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
       const int n_blk = w % n_tiles, m_blk = w / n_tiles;
-      if (!first) asm volatile("bar.sync 2, 256;" ::: "memory");   // everyone is done reading the previous u tile
-      first = false;
-      // conv taps of this lane's 4 value + 4 gate channels (phase 2 mapping), fetched under the wait for the MMAs
-      float2 wv[3][2], wg[3][2];                    // taps [k][channel pair]
+      float acc[kFuBN / 2];
+#pragma unroll
+      for (int i = 0; i < kFuBN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < kb_total; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * kFuStage) + cw * 8192, sb = smem_u32(smem + stage * kFuStage + kFuA);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kFuBK / 16; ++k)
+          Wgmma<kFuBN, F16>::template ss<0, 0>(acc, make_smem_desc(sa + k * 32, 16, 1024), make_smem_desc(sb + k * 32, 16, 1024),
+                                               (kb > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kFuStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence(acc);
+      if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+      // conv taps of this lane's 4 value + 4 gate channels (phase 2 mapping)
+      float2 wv[3][2], wg2[3][2];                    // taps [k][channel pair]
       {
         const float4* wp = reinterpret_cast<const float4*>(conv_w + static_cast<long>(n_blk * kFuBN + lane * 4) * 3);
         const float4* gp = reinterpret_cast<const float4*>(conv_w + static_cast<long>(n_blk * kFuBN + 128 + lane * 4) * 3);
@@ -129,33 +116,19 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 #pragma unroll
           for (int q = 0; q < 2; ++q) {
             wv[k][q] = make_float2(fa[(2 * q) * 3 + k], fa[(2 * q + 1) * 3 + k]);
-            wg[k][q] = make_float2(fb[(2 * q) * 3 + k], fb[(2 * q + 1) * 3 + k]);
+            wg2[k][q] = make_float2(fb[(2 * q) * 3 + k], fb[(2 * q + 1) * 3 + k]);
           }
       }
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      // ---- phase 1: accumulators -> bf16 -> parked u tile (this warp: its 32 rows x 128 of the 256 columns)
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * kFuBN + half * 128;
-      uint8_t* urow = usm + t * kFuUPitch;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld32(taddr + c * 32, r);
-        tmem_ld_wait();
+      if (!first) asm volatile("bar.sync 2, 256;" ::: "memory");   // everyone is done reading the previous u tile
+      first = false;
+      // ---- phase 1: accumulator fragment -> 16-bit -> parked u tile
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint4 q;
-          q.x = pack16x2<F16>(__uint_as_float(r[8 * j]), __uint_as_float(r[8 * j + 1]));
-          q.y = pack16x2<F16>(__uint_as_float(r[8 * j + 2]), __uint_as_float(r[8 * j + 3]));
-          q.z = pack16x2<F16>(__uint_as_float(r[8 * j + 4]), __uint_as_float(r[8 * j + 5]));
-          q.w = pack16x2<F16>(__uint_as_float(r[8 * j + 6]), __uint_as_float(r[8 * j + 7]));
-          *reinterpret_cast<uint4*>(urow + half * 256 + c * 64 + j * 16) = q;
-        }
+      for (int hr = 0; hr < 2; ++hr) {
+        uint8_t* urow = usm + (cw * 64 + wq * 16 + qr + hr * 8) * kFuUPitch + qc * 4;
+#pragma unroll
+        for (int i = 0; i < kFuBN / 8; ++i)
+          *reinterpret_cast<uint32_t*>(urow + i * 16) = pack16x2<F16>(acc[4 * i + 2 * hr], acc[4 * i + 2 * hr + 1]);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);   // TMEM buffer free: the next tile's MMAs proceed under phase 2
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       asm volatile("bar.sync 2, 256;" ::: "memory");  // u tile complete
       // ---- phase 2: conv + GEGLU + row statistics.  Warp ew owns tile rows 2+16 ew .. (16 rows), lanes span the 128
       // channels (4 value + 4 gate columns each): every smem read and global store is contiguous across the warp, the
@@ -200,7 +173,7 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
               const float2 yv = fma2(wv[0][q], xv2[q], fma2(wv[1][q], xv1[q], mul2(wv[2][q], xv0[q])));
-              const float2 yg = fma2(wg[0][q], xg2[q], fma2(wg[1][q], xg1[q], mul2(wg[2][q], xg0[q])));
+              const float2 yg = fma2(wg2[0][q], xg2[q], fma2(wg2[1][q], xg1[q], mul2(wg2[2][q], xg0[q])));
               h[q] = mul2(gelu_erf2(yg), yv);
               sm = add2(sm, h[q]);
               sq = fma2(h[q], h[q], sq);
@@ -231,12 +204,6 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         if ((lane >> 1) < nrows) rowsum[(grow0 + (lane >> 1)) * (2L * n_tiles) + 2 * n_blk + (lane & 1)] = st[0];
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -1,14 +1,10 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  C[m,n] = alpha * sum_k A(m,k) * B(n,k) (+ addend)
+// Persistent warp-specialised bf16 / fp16 GEMM for sm_90a:  C[m,n] = alpha * sum_k A(m,k) * B(n,k) (+ addend)
 //
-//   warp 0      : TMA producer  (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
-//   warp 1      : tcgen05.mma issuer (one elected lane), accumulators in TMEM, double-buffered
-//   warps 2..9  : epilogue (tcgen05.ld TMEM -> registers -> fused epilogue -> global); two warps per TMEM lane
-//                 quarter (= per SM sub-partition), each draining one half of the tile's columns.
-//                 Dense outputs (no row remapping, no split-K) leave through shared memory: every warp stages its
-//                 32-row x 128-byte chunk in a 128B-swizzled buffer (bank-conflict free with lane = row) and one lane
-//                 issues a TMA store, so the global writes are whole 128-byte rows instead of 32 scattered 16-byte
-//                 pieces per instruction; a residual / beta = 1 addend arrives the same way (TMA loads into the warp's
-//                 buffers, two chunks ahead, crossing tile boundaries).
+//   warpgroup 0     : TMA producer (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx)
+//   warpgroups 1, 2 : consumers.  Each owns 64 rows of the 128-row tile, issues wgmma (m64 x BN x k16, fp32 accumulators
+//                     in registers) straight from the swizzled ring, keeps one k-block of wgmma in flight and frees the
+//                     previous slot, then runs the fused epilogue from its accumulator fragment (alpha, residual addend,
+//                     row remapping, split-K reductions, bf16 / fp32 stores, LayerNorm-backward row statistics).
 //
 // Operand majors are template parameters so that one kernel serves the forward projections
 // (A K-major, B K-major: nn.Linear weights are [out,in]), the data-gradient GEMMs (B MN-major: the
@@ -25,8 +21,8 @@
 namespace omlm {
 
 constexpr int BM = 128;
-constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle row
-constexpr int kGemmThreads = 320;
+constexpr int BK = 64;  // 64 16-bit elements = 128 bytes = one swizzle row
+constexpr int kGemmThreads = 384;
 
 struct EpiParams {
   void* out;            // bf16 or fp32
@@ -36,16 +32,15 @@ struct EpiParams {
   float alpha;
   int out_f32;    // 0: bf16, 1: fp32
   int atomic;     // 1: red.add into fp32 out (split-K)
-  int vec_ok;     // 16-byte vector stores allowed
+  int vec_ok;     // out / addend rows 16-byte aligned: column pairs move as one vector
   int row_split;  // >0: rows are two halves of row_split, each with row_valid live rows; <0: interleaved GEGLU groups of 128
   int row_valid;
   int n_valid;    // columns >= n_valid are dropped
-  int tma_mode;   // 0: per-thread global stores; 1: TMA store; 2: TMA addend in place + TMA store; 3: TMA addend prefetched (2 buffers) + TMA store;
-                  // 4: TMA store + row statistics against a second [M, N] bf16 tensor (below)
-  // mode 4 (the d_hn data-gradient GEMM of the conv feed-forward): with d = this GEMM's fp32 output row and hn the saved
-  // forward output, every epilogue warp leaves  part[row, 2 n_blk + half] = (sum_c gamma[c] drop(d[c]), sum_c d[c] hn[c])
-  // over its half tile -- the two row sums LayerNorm-backward needs (ffn_mid.cu), which used to cost a separate pass
-  // hn arrives through tmAdd (bf16 boxes of 64 columns x 32 rows) into one staging buffer per warp, one chunk ahead
+  // row statistics (the d_hn data-gradient GEMM of the conv feed-forward): with d = this GEMM's fp32 output row and hn
+  // the saved forward output, part[row, 2 n_blk + half] = (sum_c gamma[c] drop(d[c]), sum_c d[c] hn[c]) over each
+  // 128-column half tile -- the two row sums LayerNorm-backward needs (ffn_mid.cu), without a separate pass
+  const __nv_bfloat16* rs_hn;  // [M, rs_ldhn] bf16
+  long rs_ldhn;
   const float* rs_gamma;       // [N] fp32 (zero in padded columns)
   const uint8_t* rs_keep;      // dropout keep bits [M, N/8] or nullptr
   float2* rs_part;             // [M, rs_parts]
@@ -53,9 +48,6 @@ struct EpiParams {
   int rs_parts;
 };
 
-constexpr int kEpiWarps = 8;
-constexpr int kEpiBuf = 4096;     // one staging buffer: 32 rows x 128 bytes, 128B-swizzled
-__host__ __device__ constexpr int epi_bufs_per_warp(int tma_mode) { return tma_mode == 3 ? 3 : (tma_mode == 4 ? 2 : (tma_mode != 0 ? 1 : 0)); }
 __device__ __forceinline__ float bf16lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
 
@@ -67,26 +59,19 @@ struct GemmSmem {
   static constexpr int kMaxStages = 8;
 };
 
-template <int BN, int A_MN, int B_MN, bool RS = false>
+template <int BN, int A_MN, int B_MN, bool F16, bool RS = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmAdd,
-                 const EpiParams ep, const int M, const int N, const int K, const int splits, const uint32_t idesc,
-                 const int kStages) {
+                 const EpiParams ep, const int M, const int N, const int K, const int splits, const int kStages) {
   pdl_launch_dependents();
   using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atoms.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* staging = smem + kStages * S::kStageBytes;                       // epilogue staging buffers (1024B aligned)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + kEpiWarps * epi_bufs_per_warp(ep.tma_mode) * kEpiBuf);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
   uint64_t* empty_bar = full_bar + S::kMaxStages;
-  uint64_t* tfull_bar = empty_bar + S::kMaxStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* add_bar = tempty_bar + 2;                                       // [kEpiWarps][2] addend chunks landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(add_bar + 2 * kEpiWarps);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
 
   const int m_tiles = (M + BM - 1) / BM;
@@ -96,37 +81,22 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int tiles_total = m_tiles * n_tiles;
   const int work_total = tiles_total * splits;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (ep.tma_mode != 0) tma_prefetch_desc(&tmOut);
-    if (ep.tma_mode >= 2) tma_prefetch_desc(&tmAdd);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int i = 0; i < kStages; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull_bar[i], 1);
-        mbar_init(&tempty_bar[i], 8);
-      }
-      for (int i = 0; i < 2 * kEpiWarps; ++i) mbar_init(&add_bar[i], 1);
-      fence_barrier_init();
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);        // one arrival per consumer warpgroup
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
+    fence_barrier_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
@@ -158,205 +128,57 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
-        const int split = w / tiles_total;
-        const int kb0 = split * kb_per_split;
-        const int kb1 = min(kb_total, kb0 + kb_per_split);
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
-          const uint32_t sb = sa + S::kABytes;
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1;                                   // 64-row half of the tile
+  const int wq = (threadIdx.x >> 5) & 3;                   // warp within the warpgroup: 16 rows each
+  const int qr = lane >> 2, qc = lane & 3;                 // fragment row / column pair within the warp's rows
+  const bool leader = (threadIdx.x & 127) == 0;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
+    const int split = w / tiles_total;
+    const int tile = w - split * tiles_total;
+    const int n_blk = tile % n_tiles, m_blk = tile / n_tiles;
+    const int kb0 = split * kb_per_split;
+    const int kb1 = min(kb_total, kb0 + kb_per_split);
+    float acc[BN / 2];
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // K-major: 16 elements = 32 bytes inside the swizzle row; 8-row groups 1024B apart.
-            // MN-major: 16 k-rows = 2048 bytes; 64-element MN chunks 8192B apart (LBO), 8-row groups 1024B (SBO).
-            const uint64_t ad = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024)
-                                     : make_smem_desc(sa + k * 32, 16, 1024);
-            const uint64_t bd = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024)
-                                     : make_smem_desc(sb + k * 32, 16, 1024);
-            umma_bf16(tmem_d, ad, bd, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * S::kStageBytes) + cw * 8192;   // this warpgroup's 64 rows of A
+      const uint32_t sb = smem_u32(smem + stage * S::kStageBytes + S::kABytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        // K-major: 16 elements = 32 bytes inside the swizzle row; 8-row groups 1024B apart.
+        // MN-major: 16 k-rows = 2048 bytes; 64-element MN chunks 8192B apart (LBO), 8-row groups 1024B (SBO).
+        const uint64_t ad = A_MN ? make_smem_desc(sa + k * 2048, 8192, 1024) : make_smem_desc(sa + k * 32, 16, 1024);
+        const uint64_t bd = B_MN ? make_smem_desc(sb + k * 2048, 8192, 1024) : make_smem_desc(sb + k * 32, 16, 1024);
+        const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
+        Wgmma<BN, F16>::template ss<A_MN, B_MN>(acc, ad, bd, accum);
       }
+      wgmma_commit();
+      wgmma_wait<1>();                                      // the previous k-block's wgmma have read their slot
+      if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-  } else if (ep.tma_mode != 0) {
-    // ------------------------------------------------------------------ epilogue warps, shared-memory staged (TMA)
-    // The warp walks its chunks (32 rows x 128 bytes of output: 32 fp32 or 64 bf16 columns) as ONE sequence across
-    // tiles, so that residual chunks can be requested ahead of the tile they belong to.
-    const int quarter = warp & 3;                 // TMEM lane quarter this warp may read
-    const int ew = warp - 2, half = ew >> 2;      // half: which half of the tile's columns
-    const int n_in = ep.tma_mode == 3 ? 2 : (ep.tma_mode == 2 || ep.tma_mode == 4 ? 1 : 0);
-    const bool inplace = ep.tma_mode == 2;
-    constexpr bool rowstat = RS;       // tma_mode 4 is only ever launched on the RS instantiation
-    float rs1 = 0.f, rs2 = 0.f;
-    uint2 kb_nx = make_uint2(0xffffffffu, 0xffffffffu);
-    uint8_t* my = staging + ew * epi_bufs_per_warp(ep.tma_mode) * kEpiBuf;
-    uint8_t* out_buf = my + (inplace ? 0 : n_in) * kEpiBuf;
-    uint64_t* in_bar = add_bar + ew * 2;
-    const int CW = ep.out_f32 ? 32 : 64;          // columns per chunk
-    const int cpt = (BN / 2) / CW;                // chunks per tile for this warp
-    const int my_tiles = blockIdx.x < work_total ? (work_total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    const int total = my_tiles * cpt;
-    const uint32_t sw = static_cast<uint32_t>(lane & 7) << 4;
-    const uint32_t row_off = static_cast<uint32_t>(lane) * 128;
-    auto coords = [&](int g, int& row0, int& col0) {
-      const int t = g / cpt, c = g - t * cpt;
-      const int tile = blockIdx.x + t * gridDim.x;          // splits == 1 on this path
-      const int n_blk = tile % n_tiles, m_blk = tile / n_tiles;
-      row0 = m_blk * BM + quarter * 32;
-      col0 = n_blk * BN + half * (BN / 2) + c * CW;
-      return row0 < M && col0 < ep.n_valid;
-    };
-    auto issue_load = [&](int g) {                          // lane 0 only
-      int row0, col0;
-      if (g < total && coords(g, row0, col0)) {
-        const int b = g % n_in;
-        mbar_expect_tx(&in_bar[b], kEpiBuf);
-        tma_load_2d(my + b * kEpiBuf, &tmAdd, &in_bar[b], col0, row0);
-      }
-    };
-    auto fetch_keep = [&](int g) {        // this lane's 64 dropout keep bits of chunk g, consumed one chunk later
-      int row0, col0;
-      kb_nx = make_uint2(0xffffffffu, 0xffffffffu);
-      if (ep.rs_keep != nullptr && g < total && coords(g, row0, col0) && row0 + lane < M)
-        kb_nx = __ldg(reinterpret_cast<const uint2*>(ep.rs_keep + static_cast<long>(row0 + lane) * (N >> 3) + (col0 >> 3)));
-    };
-    if constexpr (rowstat) fetch_keep(0);
-    if (!inplace && lane == 0)
-      for (int k = 0; k < n_in; ++k) issue_load(k);
-    int acc = 0;
-    uint32_t acc_phase = 0, in_phase = 0;
-    for (int g = 0; g < total; ++g) {
-      const int c = g % cpt;
-      int row0, col0;
-      const bool live = coords(g, row0, col0);
-      if (c == 0) {
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        tc_fence_after();
-      }
-      const uint8_t* in_buf = my + (n_in ? (g % n_in) : 0) * kEpiBuf;
-      if (n_in != 0) {
-        if (inplace) {        // one buffer: the previous chunk's store must have read it before the addend overwrites it
-          if (lane == 0) { tma_store_wait_read<0>(); issue_load(g); }
-          __syncwarp();
-        }
-        if (live) {
-          const int b = g % n_in;
-          mbar_wait(&in_bar[b], (in_phase >> b) & 1);
-          in_phase ^= 1u << b;
-        }
-      }
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + half * (BN / 2) + c * CW;
-      uint32_t r0[32], r1[32];
-      tmem_ld32(taddr, r0);
-      if (!ep.out_f32) tmem_ld32(taddr + 32, r1);
-      tmem_ld_wait();
-      if (c == cpt - 1) {     // accumulator drained (for this warp): hand the TMEM buffer back to the MMA warp
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-      if (live) {
-        uint4 q[8];
-        if (ep.out_f32) {
+    wgmma_wait<0>();
+    wgmma_reg_fence(acc);
+    if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
+
+    // ------------------------------------------------------------------ epilogue: rows r_lo, r_lo + 8 of the fragment
+    float rs1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][half]
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            float4 v = make_float4(__uint_as_float(r0[4 * j]) * ep.alpha, __uint_as_float(r0[4 * j + 1]) * ep.alpha,
-                                   __uint_as_float(r0[4 * j + 2]) * ep.alpha, __uint_as_float(r0[4 * j + 3]) * ep.alpha);
-            if (n_in != 0) {
-              const float4 a = *reinterpret_cast<const float4*>(in_buf + row_off + ((static_cast<uint32_t>(j) << 4) ^ sw));
-              v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
-            }
-            q[j] = make_uint4(__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w));
-          }
-        } else {
-          if constexpr (rowstat) {     // this thread = one output row, 64 columns
-            const int row = row0 + lane;
-            const uint32_t kb_lo = kb_nx.x, kb_hi = kb_nx.y;
-            fetch_keep(g + 1);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const uint4 hv = *reinterpret_cast<const uint4*>(in_buf + row_off + ((static_cast<uint32_t>(j) << 4) ^ sw));
-              const float4 g0 = __ldg(reinterpret_cast<const float4*>(ep.rs_gamma + col0 + 8 * j));
-              const float4 g1 = __ldg(reinterpret_cast<const float4*>(ep.rs_gamma + col0 + 8 * j + 4));
-              const uint32_t* rr = j < 4 ? r0 + 8 * j : r1 + 8 * (j - 4);
-              const uint32_t kb = ((j < 4 ? kb_lo : kb_hi) >> (8 * (j & 3))) & 0xffu;
-              const float d[8] = {__uint_as_float(rr[0]) * ep.alpha, __uint_as_float(rr[1]) * ep.alpha, __uint_as_float(rr[2]) * ep.alpha,
-                                  __uint_as_float(rr[3]) * ep.alpha, __uint_as_float(rr[4]) * ep.alpha, __uint_as_float(rr[5]) * ep.alpha,
-                                  __uint_as_float(rr[6]) * ep.alpha, __uint_as_float(rr[7]) * ep.alpha};
-              const float hf[8] = {bf16lo(hv.x), bf16hi(hv.x), bf16lo(hv.y), bf16hi(hv.y), bf16lo(hv.z), bf16hi(hv.z), bf16lo(hv.w), bf16hi(hv.w)};
-              const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                rs1 = fmaf(gm[e], ((kb >> e) & 1u) ? d[e] : 0.f, rs1);
-                rs2 = fmaf(d[e], hf[e], rs2);
-              }
-            }
-            if (c == cpt - 1) {
-              if (row < M) ep.rs_part[static_cast<long>(row) * ep.rs_parts + 2 * ((col0 - half * (BN / 2)) / BN) + half] = make_float2(rs1 * ep.rs_keep_scale, rs2);
-              rs1 = 0.f; rs2 = 0.f;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            q[j] = make_uint4(pack_bf16x2(__uint_as_float(r0[8 * j]) * ep.alpha, __uint_as_float(r0[8 * j + 1]) * ep.alpha),
-                              pack_bf16x2(__uint_as_float(r0[8 * j + 2]) * ep.alpha, __uint_as_float(r0[8 * j + 3]) * ep.alpha),
-                              pack_bf16x2(__uint_as_float(r0[8 * j + 4]) * ep.alpha, __uint_as_float(r0[8 * j + 5]) * ep.alpha),
-                              pack_bf16x2(__uint_as_float(r0[8 * j + 6]) * ep.alpha, __uint_as_float(r0[8 * j + 7]) * ep.alpha));
-            q[4 + j] = make_uint4(pack_bf16x2(__uint_as_float(r1[8 * j]) * ep.alpha, __uint_as_float(r1[8 * j + 1]) * ep.alpha),
-                                  pack_bf16x2(__uint_as_float(r1[8 * j + 2]) * ep.alpha, __uint_as_float(r1[8 * j + 3]) * ep.alpha),
-                                  pack_bf16x2(__uint_as_float(r1[8 * j + 4]) * ep.alpha, __uint_as_float(r1[8 * j + 5]) * ep.alpha),
-                                  pack_bf16x2(__uint_as_float(r1[8 * j + 6]) * ep.alpha, __uint_as_float(r1[8 * j + 7]) * ep.alpha));
-          }
-        }
-        if (!inplace) {
-          __syncwarp();       // every lane has read its addend row: the buffer may be refilled, two chunks ahead
-          if (lane == 0) {
-            if (n_in != 0) issue_load(g + n_in);
-            tma_store_wait_read<0>();       // the previous chunk's store has read the staging buffer
-          }
-          __syncwarp();
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<uint4*>(out_buf + row_off + ((static_cast<uint32_t>(j) << 4) ^ sw)) = q[j];
-        fence_proxy_async();   // generic-proxy stores -> visible to the TMA (async proxy)
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmOut, out_buf, col0, row0);
-          tma_store_commit();
-        }
-      } else if (n_in != 0 && !inplace) {
-        if (lane == 0) issue_load(g + n_in);
-      }
-    }
-    if (lane == 0) tma_store_wait_read<0>();   // the staging buffers have been read; the writes themselves complete with the grid
-  } else {
-    // ------------------------------------------------------------------ epilogue warps
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may read
-    const int c_lo = ((warp - 2) >> 2) * (BN / 64), c_hi = c_lo + BN / 64;   // this warp's half of the 32-column chunks
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
-      const int tile = w % tiles_total;
-      const int n_blk = tile % n_tiles, m_blk = tile / n_tiles;
-      int row = m_blk * BM + quarter * 32 + lane;
+    for (int hr = 0; hr < 2; ++hr) {
+      int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
+      const int row_in = row;
       bool row_ok = row < M;
       if (ep.row_split > 0) {
         const int half = row / ep.row_split, r = row - half * ep.row_split;
@@ -367,155 +189,84 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         row_ok = row_ok && ch < ep.row_valid;
         row = (w256 >> 7) * ep.row_valid + ch;
       }
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
-      // residual / beta=1 addend: software-pipelined one 32-column chunk ahead so that its HBM latency overlaps
-      // the TMEM load + store of the previous chunk (and, for chunk 0, the tail of the tile's MMAs)
-      const bool pf = row_ok && ep.addend != nullptr && ep.vec_ok;
-      float4 nxt[8];
-      auto prefetch = [&](int c) {
-        const int col0 = n_blk * BN + c * 32;
-        if (pf && c < c_hi && col0 + 32 <= ep.n_valid) {
-          const float4* ap = reinterpret_cast<const float4*>(ep.addend + static_cast<long>(row) * ep.ldadd + col0);
+      if (!row_ok) continue;
+      const long orow = static_cast<long>(row) * ep.ldo;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) nxt[j] = ap[j];
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = n_blk * BN + 8 * i + 2 * qc;
+        if (col >= ep.n_valid) continue;
+        const bool pair = col + 1 < ep.n_valid && ep.vec_ok;
+        float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
+        if constexpr (RS) {
+          const uint32_t hv = *reinterpret_cast<const uint32_t*>(ep.rs_hn + static_cast<long>(row_in) * ep.rs_ldhn + col);
+          const float2 g = __ldg(reinterpret_cast<const float2*>(ep.rs_gamma + col));
+          uint32_t kb = 0xffu;
+          if (ep.rs_keep != nullptr) kb = ep.rs_keep[static_cast<long>(row_in) * (N >> 3) + (col >> 3)];
+          const int hf = (8 * i) / (BN / 2);
+          rs1[hr][hf] = fmaf(g.x, ((kb >> (col & 7)) & 1u) ? v0 : 0.f, rs1[hr][hf]);
+          rs1[hr][hf] = fmaf(g.y, ((kb >> ((col + 1) & 7)) & 1u) ? v1 : 0.f, rs1[hr][hf]);
+          rs2[hr][hf] = fmaf(v0, bf16lo(hv), rs2[hr][hf]);
+          rs2[hr][hf] = fmaf(v1, bf16hi(hv), rs2[hr][hf]);
         }
-      };
-      prefetch(c_lo);
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = c_lo; c < c_hi; ++c) {
-        uint32_t r[32];
-        tmem_ld32(taddr + c * 32, r);
-        float4 cur[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) cur[j] = nxt[j];
-        prefetch(c + 1);
-        tmem_ld_wait();
-        const int col0 = n_blk * BN + c * 32;
-        if (row_ok && col0 < ep.n_valid) {
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * ep.alpha;
-          const bool full = (col0 + 32 <= ep.n_valid) && ep.vec_ok;
-          if (ep.addend != nullptr) {
-            if (full) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                v[4 * j] += cur[j].x; v[4 * j + 1] += cur[j].y; v[4 * j + 2] += cur[j].z; v[4 * j + 3] += cur[j].w;
-              }
-            } else {
-              const float* ap = ep.addend + static_cast<long>(row) * ep.ldadd + col0;
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < ep.n_valid) v[j] += ap[j];
-            }
-          }
-          if (ep.atomic) {
-            float* op = reinterpret_cast<float*>(ep.out) + static_cast<long>(row) * ep.ldo + col0;
-            if (full) {  // 16-byte aligned: vector reductions (one L2 op per 4 floats)
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(op + 4 * j), "f"(v[4 * j]),
-                             "f"(v[4 * j + 1]), "f"(v[4 * j + 2]), "f"(v[4 * j + 3]) : "memory");
-            } else if ((ep.ldo & 1) == 0 && (reinterpret_cast<uintptr_t>(ep.out) & 7) == 0) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (col0 + 2 * j + 1 < ep.n_valid)
-                  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op + 2 * j), "f"(v[2 * j]), "f"(v[2 * j + 1]) : "memory");
-                else if (col0 + 2 * j < ep.n_valid)
-                  atomicAdd(op + 2 * j, v[2 * j]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < ep.n_valid) atomicAdd(op + j, v[j]);
-            }
-          } else if (ep.out_f32) {
-            float* op = reinterpret_cast<float*>(ep.out) + static_cast<long>(row) * ep.ldo + col0;
-            if (full) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                reinterpret_cast<float4*>(op)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < ep.n_valid) op[j] = v[j];
-            }
-          } else {
-            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + static_cast<long>(row) * ep.ldo + col0;
-            if (full) {
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                uint4 q;
-                q.x = pack_bf16x2(v[8 * j], v[8 * j + 1]);
-                q.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-                q.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-                q.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-                reinterpret_cast<uint4*>(op)[j] = q;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (col0 + j < ep.n_valid) op[j] = __float2bfloat16_rn(v[j]);
-            }
-          }
+        if (ep.addend != nullptr) {
+          const float* ap = ep.addend + static_cast<long>(row) * ep.ldadd + col;
+          if (pair) { const float2 a2 = *reinterpret_cast<const float2*>(ap); v0 += a2.x; v1 += a2.y; }
+          else { v0 += ap[0]; if (col + 1 < ep.n_valid) v1 += ap[1]; }
+        }
+        if (ep.atomic) {
+          float* op = reinterpret_cast<float*>(ep.out) + orow + col;
+          if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
+          else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
+        } else if (ep.out_f32) {
+          float* op = reinterpret_cast<float*>(ep.out) + orow + col;
+          if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+          else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
+        } else {
+          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + orow + col;
+          if (pair) *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
+          else { op[0] = __float2bfloat16_rn(v0); if (col + 1 < ep.n_valid) op[1] = __float2bfloat16_rn(v1); }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    if constexpr (RS) {       // quad reduction: the four lanes of a fragment row hold disjoint column pairs
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          float a1 = rs1[hr][hf], a2 = rs2[hr][hf];
+          a1 += __shfl_xor_sync(0xffffffffu, a1, 1); a1 += __shfl_xor_sync(0xffffffffu, a1, 2);
+          a2 += __shfl_xor_sync(0xffffffffu, a2, 1); a2 += __shfl_xor_sync(0xffffffffu, a2, 2);
+          const int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
+          if (qc == 0 && row < M) ep.rs_part[static_cast<long>(row) * ep.rs_parts + 2 * n_blk + hf] = make_float2(a1 * ep.rs_keep_scale, a2);
+        }
+    }
   }
 }
 
-constexpr int kMaxDynSmem = 232448;      // 227 KB per CTA on sm_100
-constexpr int kBarrierBytes = 512;
+constexpr int kMaxDynSmem = 232448;      // 227 KB per CTA on sm_90
+constexpr int kBarrierBytes = 256;
 
 template <int BN, int A_MN, int B_MN, bool RS = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const CUtensorMap& tmAdd,
-                       const EpiParams& ep, int M, int N, int K, int splits, int max_ctas, int a_f16, int b_f16,
-                       cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& ep, int M, int N, int K, int splits,
+                       int max_ctas, int f16, cudaStream_t stream) {
   using S = GemmSmem<BN>;
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, RS>;
-  // shared memory: operand ring | epilogue staging | barriers.  The ring takes what the staging buffers leave.
-  const int staging = kEpiWarps * epi_bufs_per_warp(ep.tma_mode) * kEpiBuf;
-  int stages = (kMaxDynSmem - 1024 - kBarrierBytes - staging) / S::kStageBytes;
+  auto kern = f16 ? gemm_bf16_kernel<BN, A_MN, B_MN, true, RS> : gemm_bf16_kernel<BN, A_MN, B_MN, false, RS>;
+  int stages = (kMaxDynSmem - 1024 - kBarrierBytes) / S::kStageBytes;
   if (stages > 6) stages = 6;
-  const int smem_bytes = stages * S::kStageBytes + staging + kBarrierBytes + 1024;
-  static bool configured = false;
-  if (!configured) {
+  const int smem_bytes = stages * S::kStageBytes + kBarrierBytes + 1024;
+  static bool configured[2] = {false, false};
+  if (!configured[f16]) {
     OMLM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
-    configured = true;
+    configured[f16] = true;
   }
   const int m_tiles = (M + BM - 1) / BM, n_tiles = (N + BN - 1) / BN;
   const int work = m_tiles * n_tiles * splits;
   int grid = num_sms();
   if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
   if (work < grid) grid = work;
-  // operand formats are instruction-descriptor bits (a_format @7, b_format @10: 0 = fp16, 1 = bf16), set per launch
-  uint32_t idesc = make_idesc_bf16(BM, BN, A_MN, B_MN);
-  if (a_f16) idesc &= ~(7u << 7);
-  if (b_f16) idesc &= ~(7u << 10);
-  OMLM_KLAUNCH((kern), grid, kGemmThreads, smem_bytes, stream, tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, idesc, stages);
+  OMLM_KLAUNCH((kern), grid, kGemmThreads, smem_bytes, stream, tmA, tmB, ep, M, N, K, splits, stages);
   OMLM_LAUNCH_CHECK();
   return 0;
-}
-
-static bool tma_epilogue_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("OMLM_GEMM_TMA_EPI");       // diagnostics: 0 = per-thread global stores everywhere
-    on = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return on == 1;
 }
 
 }  // namespace omlm
@@ -534,7 +285,7 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   OMLM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem %d x %d x %d", M, N, K);
   OMLM_CHECK_ARG(block_n == 128 || block_n == 256, "gemm: block_n must be 128 or 256");
   OMLM_CHECK_ARG(splits >= 1, "gemm: splits must be >= 1");
-  OMLM_CHECK_ARG((a_f16 != 0) == (b_f16 != 0), "gemm: both operands must have the same 16-bit format (tcgen05 kind::f16 faults on fp16 x bf16)");
+  OMLM_CHECK_ARG((a_f16 != 0) == (b_f16 != 0), "gemm: both operands must have the same 16-bit format (one wgmma takes one operand format)");
   OMLM_CHECK_ARG(splits == 1 || (out_f32 && addend == nullptr), "gemm: split-K needs fp32 atomic output and no addend");
   if (n_valid <= 0 || n_valid > N) n_valid = N;
   {  // every split must own at least one k-block (an empty split would publish an unwritten accumulator)
@@ -558,46 +309,27 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   ep.vec_ok = ((ldo * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
               (addend == nullptr || ((ldadd * 4) % 16 == 0 && (reinterpret_cast<uintptr_t>(addend) & 15) == 0));
   ep.row_split = row_split; ep.row_valid = row_valid; ep.n_valid = n_valid;
-  // dense outputs leave through shared memory + TMA (see the kernel header); everything that remaps rows, reduces
-  // atomically or is not 16-byte aligned keeps the per-thread path
-  ep.tma_mode = 0;
-  ep.rs_gamma = nullptr; ep.rs_keep = nullptr; ep.rs_part = nullptr; ep.rs_keep_scale = 1.f; ep.rs_parts = 0;
-  CUtensorMap tmOut = tmA, tmAdd = tmA;     // placeholders when unused (never dereferenced)
+  ep.rs_hn = nullptr; ep.rs_ldhn = 0; ep.rs_gamma = nullptr; ep.rs_keep = nullptr; ep.rs_part = nullptr; ep.rs_keep_scale = 1.f;
+  ep.rs_parts = 0;
+  const int f16 = a_f16 ? 1 : 0;
+  const int key = (block_n == 256 ? 4 : 0) | (a_mn_major ? 2 : 0) | (b_mn_major ? 1 : 0);
   if (rs != nullptr) {
     OMLM_CHECK_ARG(block_n == 256 && N % 256 == 0 && n_valid == N && !out_f32 && addend == nullptr && splits == 1 && row_split == 0 &&
                    ep.vec_ok && rs->parts == 2 * (N / 256) && rs->ldhn % 8 == 0,
                    "gemm row statistics: needs 256-wide tiles, N %% 256 == 0, a dense bf16 output and parts == N / 128");
-    rc = make_tmap_2d(&tmOut, 2, out, (uint64_t)N, (uint64_t)M, (uint64_t)ldo * 2, 64, 32);
-    if (rc) return rc;
-    rc = make_tmap_2d(&tmAdd, 2, rs->hn, (uint64_t)N, (uint64_t)M, (uint64_t)rs->ldhn * 2, 64, 32);
-    if (rc) return rc;
-    ep.tma_mode = 4;
+    OMLM_CHECK_ARG(key == 5, "gemm row statistics: only the A K-major / B MN-major 256-wide instantiation exists");
+    ep.rs_hn = reinterpret_cast<const __nv_bfloat16*>(rs->hn); ep.rs_ldhn = rs->ldhn;
     ep.rs_gamma = rs->gamma; ep.rs_keep = reinterpret_cast<const uint8_t*>(rs->keep_bits);
     ep.rs_part = reinterpret_cast<float2*>(rs->part); ep.rs_keep_scale = rs->keep_scale; ep.rs_parts = rs->parts;
-  } else
-  if (tma_epilogue_enabled() && splits == 1 && row_split == 0 && ep.vec_ok && (addend == nullptr || out_f32)) {
-    const uint32_t cw = out_f32 ? 32 : 64;
-    rc = make_tmap_2d(&tmOut, static_cast<int>(esz), out, (uint64_t)n_valid, (uint64_t)M, (uint64_t)ldo * esz, cw, 32);
-    if (rc) return rc;
-    ep.tma_mode = 1;
-    if (addend != nullptr) {
-      rc = make_tmap_2d(&tmAdd, 4, addend, (uint64_t)n_valid, (uint64_t)M, (uint64_t)ldadd * 4, 32, 32);
-      if (rc) return rc;
-      ep.tma_mode = block_n == 128 ? 3 : 2;   // 128-wide tiles (short K, HBM-bound residual GEMMs): deep prefetch
-    }
-  }
-  const int key = (block_n == 256 ? 4 : 0) | (a_mn_major ? 2 : 0) | (b_mn_major ? 1 : 0);
-  if (ep.tma_mode == 4) {
-    OMLM_CHECK_ARG(key == 5, "gemm row statistics: only the A K-major / B MN-major 256-wide instantiation exists");
-    return launch_gemm<256, 0, 1, true>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
+    return launch_gemm<256, 0, 1, true>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
   }
   switch (key) {
-    case 0: return launch_gemm<128, 0, 0>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
-    case 1: return launch_gemm<128, 0, 1>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
-    case 3: return launch_gemm<128, 1, 1>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
-    case 4: return launch_gemm<256, 0, 0>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
-    case 5: return launch_gemm<256, 0, 1>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
-    case 7: return launch_gemm<256, 1, 1>(tmA, tmB, tmOut, tmAdd, ep, M, N, K, splits, max_ctas, a_f16, b_f16, stream);
+    case 0: return launch_gemm<128, 0, 0>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 1: return launch_gemm<128, 0, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 3: return launch_gemm<128, 1, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 4: return launch_gemm<256, 0, 0>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 5: return launch_gemm<256, 0, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 7: return launch_gemm<256, 1, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
     default:
       set_last_error("gemm: operand majors (a_mn=%d, b_mn=%d) not instantiated", a_mn_major, b_mn_major);
       return 1;

@@ -122,7 +122,7 @@ int omlm_device_check(void) {
   int major = 0, minor = 0;
   OMLM_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   OMLM_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  OMLM_CHECK_ARG(major == 10, "libomlm_b200 is built for sm_100a only; device is sm_%d%d", major, minor);
+  OMLM_CHECK_ARG(major == 9 && minor == 0, "libomlm_b200 is built for sm_90a only; device is sm_%d%d", major, minor);
   return 0;
 }
 

@@ -13,7 +13,7 @@ constexpr int kNormThreads = 256;  // 8 rows per block
 
 // ------------------------------------------------------------------------------------------------
 // LayerNorm forward: y = (x - mean) * rstd * gamma  -> fp16 (y_f16) or bf16;  optional bf16 copy of y (the
-// backward GEMMs pair it with bf16 gradients: tcgen05 wants one format for both operands); optional raw bf16 copy
+// backward GEMMs pair it with bf16 gradients: one wgmma takes one format for both operands); optional raw bf16 copy
 // of x;  stats[m] = (mean, rstd).  NCHUNK * 128 >= D.  (|y| <= sqrt(D) * |gamma|: bounded, hence fp16-safe.)
 template <int NCHUNK>
 __global__ void __launch_bounds__(kNormThreads)
@@ -147,7 +147,7 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restri
       asm volatile("cp.async.wait_group 0;" ::: "memory");
     }
     const uint8_t* sb = wbuf + stage * kStage;
-    // element-wise math on fp32x2 pairs (FFMA2): with 8 warps per SM this kernel is bound by instruction issue
+    // element-wise math on fp32x2 pairs (common.cuh), two channels per call
     float2 hA[NCHUNK], hB[NCHUNK], gA[NCHUNK], gB[NCHUNK];
     float2 s1v = make_float2(0.f, 0.f), s2v = s1v;
     const float2 rs2 = splat2(st.y), nmr = splat2(-st.x * st.y);          // xhat = x * rstd - mean * rstd

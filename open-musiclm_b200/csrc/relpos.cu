@@ -108,7 +108,7 @@ __global__ void colsum_kernel(const float* __restrict__ X, long s_m, long s_n, f
 
 // bf16x3 split for near-fp32 tensor-core products:  x = hi + lo (both bf16).  With
 //   A3 = [a_hi | a_hi | a_lo]  and  W3 = [w_hi | w_lo | w_hi]   (K concatenated),
-// A3 . W3^T = a_hi w_hi + a_hi w_lo + a_lo w_hi  ~  a . w  to ~2^-16 relative, accumulated in fp32 by tcgen05.
+// A3 . W3^T = a_hi w_hi + a_hi w_lo + a_lo w_hi  ~  a . w  to ~2^-16 relative, accumulated in fp32 by wgmma.
 __global__ void split3_kernel(const float* __restrict__ src, long src_ld, __nv_bfloat16* __restrict__ dst, int R,
                               int C, int weight_mode) {
   pdl_prologue();

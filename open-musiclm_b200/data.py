@@ -1,4 +1,4 @@
-"""Token data pipeline for the B200 training path: the reference's pre-tokenised dataset, resident in HBM.
+"""Token data pipeline for the H100 training path: the reference's pre-tokenised dataset, resident in HBM.
 
 The reference trains each stage from `preprocessed.db` (sqlite; one row per audio file with the clap / semantic / coarse /
 fine token arrays, written by open_musiclm/preprocess.py:200,279 with numpy-serialised blobs) through

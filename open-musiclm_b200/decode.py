@@ -1,10 +1,10 @@
-"""KV-cache autoregressive generation for the B200 hot path, behind the reference's wrapper API.
+"""KV-cache autoregressive generation for the H100 hot path, behind the reference's wrapper API.
 
 `TokenConditionedTransformerWrapper.generate` has the signature and the sampling semantics of the reference
 (open_musiclm/open_musiclm.py:253-326, utils.py:71-93): eos appended to the conditioning sequences, no key mask, eos
 forbidden except at the last quantizer of a time step (when allowed), top-k filtering, Gumbel-argmax sampling,
 everything after an eos masked with -1, output folded to [b, n, q].  The reference re-runs the whole prefix through
-the transformer for every sampled token; here the prompt is run once (the regular tcgen05 forward, which also fills the
+the transformer for every sampled token; here the prompt is run once (the regular wgmma forward, which also fills the
 caches) and every further token costs one incremental step over
     per layer:  K/V cache [B, Nmax, 128] bf16  +  the last two pre-conv FFN rows [B, 2, 2Fp]  (CausalDSConv history)
 with the weight-streaming kernels of csrc/decode.cu, replayed from one CUDA graph per quantizer index.
@@ -75,9 +75,9 @@ class DecodeSession:
         self.table = self.rp["table"]
         self._graphs = {}
         # OMLM_DECODE_FUSED=1: the whole step as ONE persistent kernel (csrc/decode_fused.cu; bit-identical to the per-op
-        # sequence in step_ops).  Off by default: measured on the 10 s three-stage generation it is slower than the
-        # graph-replayed per-op launches (5.0 s vs 4.0-4.4 s) -- its 31 stages are each bound by a single-warp prologue
-        # (LayerNorm statistics, row-sum tree) and a grid barrier, not by launch overhead.
+        # sequence in step_ops).  Off by default: on the 10 s three-stage generation it is slower than the graph-replayed
+        # per-op launches (5.41 s vs 4.10 s on an H100 SXM at a 400 W power limit, tools/time_generate.py) -- its 31
+        # stages are each bound by a single-warp prologue (LayerNorm statistics, row-sum tree) and a grid barrier.
         self.fused = os.environ.get("OMLM_DECODE_FUSED", "0") == "1"
         if self.fused:
             pv = eng.pview
@@ -159,7 +159,7 @@ class DecodeSession:
 
 
 class TokenConditionedTransformerWrapper(nn.Module):
-    """open_musiclm.py:219-411 on the B200 path: `generate` (KV-cache decode) and `forward` (loss / logits)."""
+    """open_musiclm.py:219-411 on the H100 path: `generate` (KV-cache decode) and `forward` (loss / logits)."""
 
     def __init__(self, *, transformer: TokenConditionedTransformer, pad_id=-1, unique_consecutive=True,
                  cross_entropy_loss_weights: Optional[List[float]] = None, mask_prob=0.15):

@@ -13,11 +13,11 @@ HBM layout
         w2 [d, Fp], logit heads [q, Cp, d];  conv taps fp32 [2*Fp, 3], inner gamma fp32 [Fp].
   activations: residual stream fp32 [M, d]; GEMM operands 16-bit; attention statistics fp32.
 
-16-bit operand formats (csrc/common.cuh): tcgen05 kind::f16 runs fp16 and bf16 at the same rate, but both operands
-of one MMA must share the format (fp16 x bf16 faults on B200 -- measured).  The FORWARD GEMMs whose operands are bounded
+16-bit operand formats (csrc/common.cuh): wgmma runs fp16 and bf16 at the same rate, but both operands of one
+wgmma must share the format.  The FORWARD GEMMs whose operands are bounded
 by construction -- LayerNorm outputs (xn, xn2, hn, xf) against weights, and the FFN activations between them (u, h) --
-run in fp16 (11-bit significand: 8x less operand rounding than bf16; this is what keeps the logits within 1e-2 of the
-fp32 reference at 24 layers: 3.6e-3 instead of 1.25e-2).  Everything that touches an unbounded range stays bf16: every
+run in fp16 (11-bit significand: 8x less operand rounding than bf16, which is what keeps the logits of deep models within
+1e-2 of the fp32 reference).  Everything that touches an unbounded range stays bf16: every
 BACKWARD GEMM (gradients), the K/V projection of the raw residual stream, attention and its output projection.  So
 the weights are packed twice (fp16 for forward, bf16 for backward) and the saved LayerNorm outputs carry a bf16
 duplicate for the weight-gradient GEMMs.  OMLM_ACT16=bf16 switches the whole path back to bf16 (diagnostics only).
@@ -95,7 +95,7 @@ class Engine:
         self.m = module
         dev = module.device
         if dev.type != "cuda":
-            raise lib.OmlmError("open_musiclm_b200 needs a CUDA (sm_100a) device: move the module with .to('cuda') "
+            raise lib.OmlmError("open_musiclm_b200 needs a CUDA (sm_90a) device: move the module with .to('cuda') "
                                 "before calling it - there is no CPU fallback")
         lib.device_check()
         self.dev = dev
@@ -317,14 +317,24 @@ class Engine:
         return ws
 
     # ------------------------------------------------------------------------------------------ forward
-    # tile / split-K choice: minimise  waves x (k-blocks per unit x tile cost + epilogue)  over the 148 SMs
-    _SMS = 148
+    # tile / split-K choice: minimise  waves x (k-blocks per unit x tile cost + epilogue)  over the device's SMs
+    _sms = None
+    # cost of one k-block of a 128x256 tile in units of a 128x128 one: 256-wide tiles measured ~4 % more efficient per
+    # flop than 128-wide ones at the cfg2 GEMM shapes (tools/bench_gemm.py; H100 SXM, 400 W power limit)
+    KB_COST_256 = 2.0 / 1.04
+
+    @classmethod
+    def _num_sms(cls):
+        if cls._sms is None:
+            cls._sms = lib.num_sms()
+        return cls._sms
 
     @classmethod
     def _tile_cost(cls, m, n, kb, bn, splits, epi):
+        sms = cls._num_sms()
         tiles = ((m + 127) // 128) * ((n + bn - 1) // bn)
-        waves = (tiles * splits + cls._SMS - 1) // cls._SMS
-        per_kb = 1.0 if bn == 128 else 2.0 / 1.2        # measured: 128x256 tiles are ~20 % more efficient per flop
+        waves = (tiles * splits + sms - 1) // sms
+        per_kb = 1.0 if bn == 128 else cls.KB_COST_256
         return waves * (((kb + splits - 1) // splits) * per_kb + epi * (bn / 128.0))
 
     @classmethod
@@ -358,7 +368,7 @@ class Engine:
 
     def _relpos_table(self, ws, N):
         """RelativePositionBias MLP on the causal distances 0..N-1 -> table[h, N] (transformer.py:55-67).
-        The two Hr x Hr layers run on the tcgen05 GEMM with bf16x3-split operands (fp32-class accuracy: the
+        The two Hr x Hr layers run on the wgmma GEMM with bf16x3-split operands (fp32-class accuracy: the
         table reaches |b| ~ 100 and dominates the logits); the rank-1 first layer and the h-wide last layer are SIMT."""
         pv, Hr, h = self.pview, self.Hr, self.h
         pre = "transformer.rel_pos_bias.net."

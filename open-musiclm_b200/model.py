@@ -1,6 +1,6 @@
 """Drop-in boundary: `TokenConditionedTransformer` and the `create_*_transformer` factories with the
 reference's signatures, attributes and state_dict keys/shapes, whose compute runs entirely in
-libomlm_b200 (hand-written sm_100a CUDA behind a C ABI) — no torch ops on the hot path, no fallback.
+libomlm_b200 (hand-written sm_90a CUDA behind a C ABI) — no torch ops on the hot path, no fallback.
 
 Mirrors open_musiclm/open_musiclm.py:23-215, 414-472 (API) and open_musiclm/transformer.py
 (parameter structure).  The module tree below carries parameters only; it exists so that
@@ -135,7 +135,7 @@ class TokenConditionedTransformer(nn.Module):
                  grad_shrink_alpha=0.1, use_absolute_position_embeddings=False,
                  max_absolute_position_embeddings=262, **kwargs):
         super().__init__()
-        # configurations the B200 path does not implement fail loudly (no silent fallback)
+        # configurations the H100 path does not implement fail loudly (no silent fallback)
         unsupported = []
         if has_condition or cond_as_self_attn_prefix:
             unsupported.append("has_condition / cond_as_self_attn_prefix (dead in every shipped config)")

@@ -1,4 +1,4 @@
-"""Stage wrappers and the three-stage windowed generation on top of the B200 TokenConditionedTransformer.
+"""Stage wrappers and the three-stage windowed generation on top of the H100 TokenConditionedTransformer.
 
 Mirrors the orchestration layer of the reference (open_musiclm/open_musiclm.py:514-1035): `SemanticStage`,
 `CoarseStage`, `FineStage` (each a TokenConditionedTransformerWrapper plus the optional tokenizer objects) and
@@ -211,7 +211,7 @@ class MusicLM(nn.Module):
         """open_musiclm.py:860-1035 without the audio-prompt branch: text -> waveform (needs the CLAP quantizer and the codec)."""
         if prime_wave is not None:
             raise NotImplementedError("open_musiclm_b200 MusicLM.forward: audio continuation (prime_wave) needs the wav2vec / codec "
-                                      "tokenizers, which are outside the B200 hot path")
+                                      "tokenizers, which are outside the H100 hot path")
         clap_token_ids = _clap_ids(clap_token_ids, self.clap, None, text)
         acoustic = self.generate_tokens(clap_token_ids=clap_token_ids, **kwargs)
         assert self.neural_codec is not None, "a neural codec is needed to turn acoustic tokens into a waveform"

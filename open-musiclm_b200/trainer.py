@@ -1,4 +1,4 @@
-"""B200-native replacement of the SingleStageTrainer step loop (open_musiclm/trainer.py:415-452) on
+"""H100-native replacement of the SingleStageTrainer step loop (open_musiclm/trainer.py:415-452) on
 top of the engine: per micro-batch  wrapper pre-processing -> forward -> cross entropy -> backward
 (gradients accumulate in the flat fp32 arena), then ONE gradient all-reduce over NCCL, global-norm
 clip, AdamW and the LinearLR warm-up — every arithmetic step a libomlm_b200 kernel.
@@ -83,9 +83,8 @@ class HotPathTrainer:
             prio = -1 if os.environ.get("OMLM_NCCL_PRIO", "1") != "0" else 0
             # sharded update (opt-in, OMLM_SHARD_OPT=1): the buckets are reduce-SCATTERED (half the bytes under the backward
             # pass), every rank runs clip + AdamW on its 1/world of the arena only, then the parameters are all-gathered --
-            # the same bytes on the wire as one all-reduce, but the optimiser pass (0.5 ms of a 11 ms step) shrinks by 1/world.
-            # Measured at 2 GPUs (same box): 11.89 ms against 11.73 ms replicated -- the exposed all-gather of the fp32
-            # parameters costs more than half an AdamW pass saves; not measured at 8 GPUs, hence off by default.
+            # the same bytes on the wire as one all-reduce, but the optimiser pass shrinks by 1/world.  The all-gather of
+            # the fp32 parameters is exposed at the end of the step; off by default (not measured on H100).
             plan = eng.grad_bucket_plan()
             self.shard_opt = os.environ.get("OMLM_SHARD_OPT", "0") == "1" and all((hi - lo) % self.world == 0 for _, sl in plan for lo, hi in sl)
             self.reducer = BucketReducer(eng.arena_g, plan, process_group, side_stream=torch.cuda.Stream(priority=prio), scatter=self.shard_opt)

@@ -1,8 +1,8 @@
 """ORACLE — test infrastructure only.  Generates tests/golden/*.pt from the REAL reference.
 
-Run in the authoring container (needs /root/reference):   python oracle/make_golden.py
+Needs a reference checkout:   OMLM_REFERENCE_ROOT=<checkout> python oracle/make_golden.py
 The fixtures pin oracle/restatement.py (tests/test_oracle_cpu.py) and give the GPU parity tests
-(tests/test_parity_gpu.py) reference outputs that travel to the GPU box.
+(tests/test_parity_gpu.py) reference outputs that the GPU tests compare against.
 
 Each fixture holds: hyper-parameters, the reference model's state_dict, the input token ids, and —
 computed by the reference's own TokenConditionedTransformerWrapper on CPU fp32 in eval mode

@@ -1,7 +1,7 @@
 """ORACLE — test infrastructure only.  Golden token sequences of the REAL reference's autoregressive generate
 (TokenConditionedTransformerWrapper.generate, open_musiclm.py:253-326) under a FIXED Gumbel noise stream.
 
-Run in the authoring container (needs /root/reference):   python oracle/make_golden_generate.py
+Needs a reference checkout:   OMLM_REFERENCE_ROOT=<checkout> python oracle/make_golden_generate.py
 The reference draws its Gumbel noise as torch.zeros_like(logits).uniform_(0, 1) from torch's default CPU generator
 (utils.py:71-73): seeding that generator right before generate() fixes the stream, and the fixture stores the very
 same draws (re-generated with the same seed and shapes) so that the oracle restatement and the CUDA sampler can consume

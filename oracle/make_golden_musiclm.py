@@ -2,7 +2,7 @@
 (MusicLM.forward, open_musiclm.py:860-1035: semantic -> coarse -> fine with sliding windows) on tiny random-weight
 stage transformers, under a fixed Gumbel noise stream.
 
-Run in the authoring container (needs /root/reference):   python oracle/make_golden_musiclm.py
+Needs a reference checkout:   OMLM_REFERENCE_ROOT=<checkout> python oracle/make_golden_musiclm.py
 CLAP and the neural codec do not exist here (SURVEY 8c); they are replaced by stubs that (a) return fixed clap token ids
 for the text and (b) "decode" by returning the acoustic token ids themselves, so the fixture's output is the [b, T, 8]
 token tensor the reference hands to the codec.  The fixture stores the three state_dicts, the clap ids, the windowing

@@ -1,18 +1,18 @@
 """ORACLE — test infrastructure only.
 
-Imports the REAL reference (`/root/reference/open_musiclm`) with the two stub modules SURVEY.md §8c
+Imports the REAL reference (`$OMLM_REFERENCE_ROOT/open_musiclm`, a checkout of zhvng/open-musiclm) with the two stub modules SURVEY.md §8c
 describes, so that its TokenConditionedTransformer / Wrapper / Stage classes run on CPU.  Only
-usable where /root/reference exists (the authoring container); the GPU box never has it.
+usable where that checkout exists; the tests compare against golden data recorded from it (tests/golden/).
 """
 import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("OMLM_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("OMLM_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF_ROOT, "open_musiclm"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "open_musiclm"))
 
 
 def import_reference():

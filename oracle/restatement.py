@@ -3,8 +3,8 @@
 CPU restatement (numpy for the integer/byte path, plain torch fp32 for the floating-point path) of
 the reference's TokenConditionedTransformer training path.  It is written from the reference's
 behaviour, function by function, and every function cites the reference file:line it follows
-(paths relative to /root/reference).  It is pinned against the real reference by
-`oracle/make_golden.py` (run in the authoring container, where /root/reference is importable) and
+(paths relative to the reference checkout).  It is pinned against the real reference by
+`oracle/make_golden.py` (run where a reference checkout is importable) and
 the committed fixtures under tests/golden/ — see tests/test_oracle_cpu.py.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import it.

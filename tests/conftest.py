@@ -9,4 +9,4 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine with one)")

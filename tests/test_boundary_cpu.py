@@ -8,7 +8,7 @@ import torch
 
 import open_musiclm_b200 as O
 from open_musiclm_b200 import lib
-from oracle import ref_harness
+from oracle import make_golden_live as LIVE
 
 GOLD = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "tiny_*.pt")))
 
@@ -45,22 +45,17 @@ def test_state_dict_contract_matches_reference_fixture(path):
 
 
 def test_init_is_bit_identical_to_reference_under_same_seed():
-    if not ref_harness.available():
-        pytest.skip("reference tree not present")
-    ref = ref_harness.import_reference()
-    base = dict(dim=128, depth=2, heads=2, attn_dropout=0.0, ff_dropout=0.1)
-    variants = [dict(), dict(use_conv_ff=False, relative_position_bias_type="t5"),
-                dict(relative_position_bias_type="none", use_absolute_position_embeddings=True)]
-    for extra in variants:
-        kw = dict(base, **extra)
-        for mine, theirs in [(O.create_semantic_transformer, ref.create_semantic_transformer),
-                             (O.create_coarse_transformer, ref.create_coarse_transformer),
-                             (O.create_fine_transformer, ref.create_fine_transformer)]:
+    """Every tensor of the init under seed 0 against the SHA-256 of the reference's (oracle/make_golden_live.py)."""
+    gold = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_live.pt"), weights_only=False)["init_sha"]
+    for vi, extra in enumerate(LIVE.INIT_VARIANTS):
+        kw = dict(LIVE.INIT_BASE, **extra)
+        for stage, mine in [("semantic", O.create_semantic_transformer), ("coarse", O.create_coarse_transformer),
+                            ("fine", O.create_fine_transformer)]:
             torch.manual_seed(0); a = mine(**kw).state_dict()
-            torch.manual_seed(0); b = theirs(**kw).state_dict()
+            b = gold[(vi, stage)]
             assert list(a.keys()) == list(b.keys()), extra
             for k in a:
-                assert torch.equal(a[k], b[k]), (extra, k)
+                assert LIVE.sha(a[k]) == b[k], (extra, k)
 
 
 def test_no_cpu_fallback():

@@ -1,5 +1,5 @@
 """KV-cache decoding (csrc/decode.cu, open_musiclm_b200/decode.py) against (a) torch for the weight-streaming GEMM,
-(b) the full tcgen05 forward for an incremental step, (c) the token sequences the REAL reference's generate produced
+(b) the full wgmma forward for an incremental step, (c) the token sequences the REAL reference's generate produced
 under a fixed Gumbel noise stream (tests/golden/gen_*.pt, oracle/make_golden_generate.py)."""
 import glob
 import os
@@ -154,7 +154,7 @@ def test_fused_decode_step_is_bit_identical_to_the_per_op_path(monkeypatch, B):
 
 
 def test_incremental_step_equals_full_forward_at_model_scale():
-    """musiclm_small coarse stage (d = 1024, L = 6, h = 8): logits of every decode step against the full tcgen05 forward
+    """musiclm_small coarse stage (d = 1024, L = 6, h = 8): logits of every decode step against the full wgmma forward
     over the same prefix (return_only_final_seq_logits, as the reference's generate calls it)."""
     import open_musiclm_b200 as O
     torch.manual_seed(0)
@@ -183,7 +183,7 @@ def test_incremental_step_equals_full_forward_at_model_scale():
 
 
 def test_three_stage_windowed_generation_on_the_decode_path():
-    """stages.MusicLM.generate_tokens with the real B200 wrappers on the reference's weights, clap ids and noise stream
+    """stages.MusicLM.generate_tokens with the real H100 wrappers on the reference's weights, clap ids and noise stream
     (tests/golden/musiclm_windows.pt): same number of sampled tokens (= same window bookkeeping), same output shape, and the
     same tokens as the real reference's MusicLM.forward — up to the first draw where the oracle's best and second-best
     noisy scores are within 5e-2 (from there the cascaded streams legitimately differ)."""

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (csrc/gemm_tc.cu) vs a plain torch fp32 reference of the same contraction."""
+"""wgmma GEMM (csrc/gemm_tc.cu) vs a plain torch fp32 reference of the same contraction."""
 import pytest
 import torch
 
@@ -31,8 +31,8 @@ def test_gemm_majors(a_mn, b_mn, block_n, M, N, K):
 
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, True)])
 def test_gemm_fp16_operands(a_mn, b_mn):
-    """tcgen05 kind::f16 with fp16 operands (instruction-descriptor format bits) — the forward GEMMs of the hot path.
-    Mixed fp16 x bf16 is rejected on the host: B200 raises an illegal-instruction fault for it (measured in round 2)."""
+    """wgmma with fp16 operands (the .f16 instruction form) — the forward GEMMs of the hot path.
+    Mixed fp16 x bf16 is rejected on the host: one wgmma takes a single operand format."""
     from open_musiclm_b200 import lib
     torch.manual_seed(11)
     M, N, K = 384, 640, 520

@@ -229,7 +229,7 @@ def test_attention_fwd_bwd(lib, B, N, h):
     assert rel(dqn, qf.grad) < 1.5e-2
     assert rel(dkvn, kvf.grad) < 1.5e-2
     assert rel(dtab[:, :N], tf.grad[:, :N]) < 1.5e-2
-    # tcgen05 backward
+    # wgmma backward
     # dqn / dkvn are overwritten (cleared inside the call): poison them to pin that contract; dtable accumulates
     dqn2 = torch.full((M, h * 64), float("nan"), device=DEV); dkvn2 = torch.full((M, 128), float("nan"), device=DEV); dtab2 = torch.zeros_like(table)
     lib.attn_bwd_tc(qn, kvn, d_o, out, lse2, table, key_mask, dsum, dqn2, dkvn2, dtab2, B, N, h)
@@ -396,7 +396,7 @@ def test_attention_fwd_speed(lib):
     table = (torch.randn(h, 1, device=DEV) * 0.05 * torch.arange(N, device=DEV)[None]).contiguous()
     key_mask = (torch.rand(B, N, device=DEV) > 0.15).to(torch.uint8); key_mask[:, 0] = 1
     out = torch.empty(M, h * 64, device=DEV, dtype=torch.bfloat16); lse2 = torch.empty(B, N * h, device=DEV)
-    for name, fn in (("mma.sync", lib.attn_fwd), ("tcgen05", lib.attn_fwd_tc)):
+    for name, fn in (("mma.sync", lib.attn_fwd), ("wgmma", lib.attn_fwd_tc)):
         for _ in range(3):
             fn(qn, kvn, table, key_mask, out, lse2, B, N, h)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -1,5 +1,5 @@
 """Pins oracle/restatement.py against the golden fixtures produced by the REAL reference
-(oracle/make_golden.py) and, where /root/reference is importable, against the reference live."""
+(oracle/make_golden.py, oracle/make_golden_live.py)."""
 import glob
 import os
 
@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from oracle import restatement as R
-from oracle import ref_harness
+from oracle import make_golden_live as LIVE
 
 GOLD = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "tiny_*.pt")))
 
@@ -87,54 +87,41 @@ def test_restatement_optimizer_steps():
                 assert rel(params[k], v) < 1e-5, k
 
 
+LIVE_GOLD = os.path.join(os.path.dirname(__file__), "golden", "reference_live.pt")
+
+
 def test_forgetful_mask_matches_reference():
-    if not ref_harness.available():
-        pytest.skip("reference tree not present")
-    ref_harness.import_reference()
-    import sys
-    utils = sys.modules["open_musiclm.utils"]
-    torch.manual_seed(3)
-    shape = (4, 50)
+    m_ref = torch.load(LIVE_GOLD, weights_only=False)["forgetful_mask"]
     torch.manual_seed(11)
-    m_ref = utils.generate_mask_with_prob(shape, 0.15, device="cpu")
-    torch.manual_seed(11)
-    rand = torch.randn(shape)
-    m = R.forgetful_mask(shape, 0.15, rand.numpy())
+    rand = torch.randn((4, 50))
+    m = R.forgetful_mask((4, 50), 0.15, rand.numpy())
     assert np.array_equal(m, m_ref.numpy())
 
 
 @pytest.mark.parametrize("stage", ["semantic", "coarse", "fine"])
 def test_restatement_matches_reference_live(stage):
-    """Authoring-container only: mid-size random config, fresh seeds, straight against the reference."""
-    if not ref_harness.available():
-        pytest.skip("reference tree not present")
-    ref = ref_harness.import_reference()
-    common = dict(attn_dropout=0.0, ff_dropout=0.1, grad_shrink_alpha=0.1, non_causal_prefix_size=0,
-                  relative_position_bias_type="continuous", use_memory_efficient_attention=False)
+    """Mid-size random config against what the reference's wrapper computed on the same weights and tokens
+    (oracle/make_golden_live.py): the weights are this package's init under the reference's seed, pinned to the
+    reference's by the SHA-256 of the state dict."""
+    import open_musiclm_b200 as O
+    gold = torch.load(LIVE_GOLD, weights_only=False)["restatement"][stage]
+    kw, shapes = LIVE.LIVE_STAGES[stage]
     torch.manual_seed(5)
-    if stage == "semantic":
-        model = ref.create_semantic_transformer(dim=192, depth=2, heads=3, **common)
-        cfg = R.semantic_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 1.0])
-        shapes = [(2, 12), (2, 40)]
-    elif stage == "coarse":
-        model = ref.create_coarse_transformer(dim=192, depth=2, heads=3, num_coarse_quantizers=3, **common)
-        cfg = R.coarse_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 0.0, 1.0])
-        shapes = [(2, 12), (2, 20), (2, 9, 3)]
-    else:
-        model = ref.create_fine_transformer(dim=192, depth=2, heads=3, num_coarse_quantizers=3, num_fine_quantizers=5, **common)
-        cfg = R.fine_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 0.0, 1.0])
-        shapes = [(2, 12), (2, 5, 3), (2, 5, 5)]
-    wrapper = ref.TokenConditionedTransformerWrapper(transformer=model, unique_consecutive=False,
-                                                     cross_entropy_loss_weights=cfg.ce_weights).eval()
-    g = torch.Generator().manual_seed(99)
-    toks = [torch.randint(0, 1024, s, generator=g) for s in shapes]
-    with torch.no_grad():
-        loss_ref, logits_ref, _ = wrapper(all_token_ids=[t.clone() for t in toks], return_loss=True)
+    model = getattr(O, f"create_{stage}_transformer")(**kw, **LIVE.LIVE_COMMON)
     sd = {k: v.detach() for k, v in model.state_dict().items()}
-    loss, logits, *_ = R.loss_and_logits(cfg, sd, [t.numpy() for t in toks])
-    assert abs(float(loss) - float(loss_ref)) / float(loss_ref) < 1e-5
-    for a, b in zip(logits, logits_ref):
-        assert rel(a, b.permute(0, 2, 1)) < 2e-5
+    assert LIVE.state_sha(sd) == gold["state_sha"]
+    if stage == "semantic":
+        cfg = R.semantic_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 1.0])
+    elif stage == "coarse":
+        cfg = R.coarse_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 0.0, 1.0])
+    else:
+        cfg = R.fine_cfg(dim=192, depth=2, heads=3, ce_weights=[0.0, 0.0, 1.0])
+    loss, logits, *_ = R.loss_and_logits(cfg, sd, [t.numpy() for t in LIVE.live_tokens(shapes)])
+    assert abs(float(loss) - gold["loss"]) / gold["loss"] < 1e-5
+    assert [int(lg.numel()) for lg in logits] == gold["logit_numel"]
+    for i, (a, b) in enumerate(zip(logits, gold["logits"])):
+        flat = torch.as_tensor(a).reshape(-1)
+        assert rel(flat[LIVE.logit_sample_index(flat.numel(), i)], b) < 2e-5
 
 
 GEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "gen_*.pt")))

@@ -1,7 +1,7 @@
 """The stage wrappers and the three-stage sliding-window generation (open_musiclm_b200/stages.py) against the token
 output of the REAL reference's MusicLM.forward (tests/golden/musiclm_windows.pt, oracle/make_golden_musiclm.py).
 The window bookkeeping is host logic: here it runs on CPU with the oracle's generate() standing in for the CUDA
-wrapper, so the comparison is bit-exact; tests/test_decode_gpu.py runs the same fixture through the B200 decode path."""
+wrapper, so the comparison is bit-exact; tests/test_decode_gpu.py runs the same fixture through the H100 decode path."""
 import os
 from types import SimpleNamespace
 

@@ -3,7 +3,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.ins
 import torch, torch.nn.functional as F
 from open_musiclm_b200 import lib
 h = 8
-for (B, N) in [(16, 1024), (4, 2048), (1, 4096), (64, 512), (16, 2048), (2, 1024), (148, 128), (148, 256), (148,1024)]:
+for (B, N) in [(16, 1024), (4, 2048), (1, 4096), (64, 512), (16, 2048), (2, 1024), (132, 128), (132, 256), (132, 1024)]:
     M = B * N
     qn = F.normalize(torch.randn(M, h, 64, device="cuda"), dim=-1).reshape(M, h * 64).bfloat16()
     kvn = torch.randn(M, 128, device="cuda").bfloat16()

@@ -1,5 +1,5 @@
 """CPU experiment (test tooling, not product): the oracle forward with bf16 rounding inserted at exactly the
-places where the B200 path rounds (GEMM operands and the bf16 activations it stores), each site switchable,
+places where the CUDA path rounds (GEMM operands and the bf16 activations it stores), each site switchable,
 to see which roundings dominate the logits distance to the fp32 oracle at depth."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
