@@ -174,57 +174,92 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
 
     // ------------------------------------------------------------------ epilogue: rows r_lo, r_lo + 8 of the fragment
-    float rs1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][half]
+    int row_in[2];
+    long orow[2], arow[2];
+    bool row_ok[2];
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
-      const int row_in = row;
-      bool row_ok = row < M;
+      row_in[hr] = row;
+      row_ok[hr] = row < M;
       if (ep.row_split > 0) {
         const int half = row / ep.row_split, r = row - half * ep.row_split;
-        row_ok = row_ok && r < ep.row_valid;
+        row_ok[hr] = row_ok[hr] && r < ep.row_valid;
         row = half * ep.row_valid + r;
       } else if (ep.row_split < 0) {   // interleaved GEGLU rows: [128 value | 128 gate] per group of 128 channels
         const int w256 = row & 255, ch = ((row >> 8) << 7) + (w256 & 127);
-        row_ok = row_ok && ch < ep.row_valid;
+        row_ok[hr] = row_ok[hr] && ch < ep.row_valid;
         row = (w256 >> 7) * ep.row_valid + ch;
       }
-      if (!row_ok) continue;
-      const long orow = static_cast<long>(row) * ep.ldo;
+      orow[hr] = static_cast<long>(row) * ep.ldo;
+      arow[hr] = static_cast<long>(row) * ep.ldadd;
+    }
+    // The columns go in batches of kEpiBatch 8-column groups, and every global load of a batch (the addend; hn, keep
+    // bits and gamma for the row statistics) is issued before the batch's first store.  The stores may alias the loads
+    // (a weight gradient without split-K adds into its own output), so the compiler keeps each load behind every earlier
+    // store: loads interleaved with stores each waited a full memory latency, which on H100 cost more than the
+    // mainloop of the addend GEMMs (wo: 153 us with the addend against 58 us without, cfg2 shape, 400 W).
+    constexpr int kEpiBatch = RS ? 4 : 8;   // the row statistics hold three more operands per column pair
+    float rs1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][half]
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
+    for (int i0 = 0; i0 < BN / 8; i0 += kEpiBatch) {
+      float2 add[2][kEpiBatch], gam[kEpiBatch];
+      uint32_t hv[2][kEpiBatch], keep[2][kEpiBatch];
+#pragma unroll
+      for (int j = 0; j < kEpiBatch; ++j) {
+        const int col = n_blk * BN + 8 * (i0 + j) + 2 * qc;
+        const bool c0_ok = col < ep.n_valid, c1_ok = col + 1 < ep.n_valid;
+        if constexpr (RS) gam[j] = c0_ok ? __ldg(reinterpret_cast<const float2*>(ep.rs_gamma + col)) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          add[hr][j] = make_float2(0.f, 0.f);
+          hv[hr][j] = 0u;
+          keep[hr][j] = 0xffu;
+          if (!row_ok[hr] || !c0_ok) continue;
+          if (!RS && ep.addend != nullptr) {   // the row-statistics launch never has an addend (checked on the host)
+            const float* ap = ep.addend + arow[hr] + col;
+            if (c1_ok && ep.vec_ok) add[hr][j] = *reinterpret_cast<const float2*>(ap);
+            else { add[hr][j].x = ap[0]; if (c1_ok) add[hr][j].y = ap[1]; }
+          }
+          if constexpr (RS) {
+            hv[hr][j] = *reinterpret_cast<const uint32_t*>(ep.rs_hn + static_cast<long>(row_in[hr]) * ep.rs_ldhn + col);
+            if (ep.rs_keep != nullptr) keep[hr][j] = ep.rs_keep[static_cast<long>(row_in[hr]) * (N >> 3) + (col >> 3)];
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < kEpiBatch; ++j) {
+        const int i = i0 + j;
         const int col = n_blk * BN + 8 * i + 2 * qc;
         if (col >= ep.n_valid) continue;
         const bool pair = col + 1 < ep.n_valid && ep.vec_ok;
-        float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
-        if constexpr (RS) {
-          const uint32_t hv = *reinterpret_cast<const uint32_t*>(ep.rs_hn + static_cast<long>(row_in) * ep.rs_ldhn + col);
-          const float2 g = __ldg(reinterpret_cast<const float2*>(ep.rs_gamma + col));
-          uint32_t kb = 0xffu;
-          if (ep.rs_keep != nullptr) kb = ep.rs_keep[static_cast<long>(row_in) * (N >> 3) + (col >> 3)];
-          const int hf = (8 * i) / (BN / 2);
-          rs1[hr][hf] = fmaf(g.x, ((kb >> (col & 7)) & 1u) ? v0 : 0.f, rs1[hr][hf]);
-          rs1[hr][hf] = fmaf(g.y, ((kb >> ((col + 1) & 7)) & 1u) ? v1 : 0.f, rs1[hr][hf]);
-          rs2[hr][hf] = fmaf(v0, bf16lo(hv), rs2[hr][hf]);
-          rs2[hr][hf] = fmaf(v1, bf16hi(hv), rs2[hr][hf]);
-        }
-        if (ep.addend != nullptr) {
-          const float* ap = ep.addend + static_cast<long>(row) * ep.ldadd + col;
-          if (pair) { const float2 a2 = *reinterpret_cast<const float2*>(ap); v0 += a2.x; v1 += a2.y; }
-          else { v0 += ap[0]; if (col + 1 < ep.n_valid) v1 += ap[1]; }
-        }
-        if (ep.atomic) {
-          float* op = reinterpret_cast<float*>(ep.out) + orow + col;
-          if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
-          else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
-        } else if (ep.out_f32) {
-          float* op = reinterpret_cast<float*>(ep.out) + orow + col;
-          if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
-          else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
-        } else {
-          __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + orow + col;
-          if (pair) *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
-          else { op[0] = __float2bfloat16_rn(v0); if (col + 1 < ep.n_valid) op[1] = __float2bfloat16_rn(v1); }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          if (!row_ok[hr]) continue;
+          float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
+          if constexpr (RS) {
+            const uint32_t kb = keep[hr][j];
+            const float2 g = gam[j];
+            const int hf = (8 * i) / (BN / 2);
+            rs1[hr][hf] = fmaf(g.x, ((kb >> (col & 7)) & 1u) ? v0 : 0.f, rs1[hr][hf]);
+            rs1[hr][hf] = fmaf(g.y, ((kb >> ((col + 1) & 7)) & 1u) ? v1 : 0.f, rs1[hr][hf]);
+            rs2[hr][hf] = fmaf(v0, bf16lo(hv[hr][j]), rs2[hr][hf]);
+            rs2[hr][hf] = fmaf(v1, bf16hi(hv[hr][j]), rs2[hr][hf]);
+          }
+          if (!RS && ep.addend != nullptr) { v0 += add[hr][j].x; v1 += add[hr][j].y; }
+          if (ep.atomic) {
+            float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
+            if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
+            else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
+          } else if (ep.out_f32) {
+            float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
+            if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+            else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
+          } else {
+            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + orow[hr] + col;
+            if (pair) *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
+            else { op[0] = __float2bfloat16_rn(v0); if (col + 1 < ep.n_valid) op[1] = __float2bfloat16_rn(v1); }
+          }
         }
       }
     }
