@@ -213,7 +213,9 @@ int omlm_gather_windows(const void* src_i16, const long long* start, long long* 
 
 /* ---- incremental (KV-cache) decoding: TokenConditionedTransformerWrapper.generate (open_musiclm.py:253-326) ----------
  * One new position per sequence and step instead of the reference's full-prefix forward per sampled token
- * (open_musiclm.py:303-307).  B <= 16 rows; SIMT weight-streaming kernels (csrc/decode.cu).
+ * (open_musiclm.py:303-307).  Batches of B <= 16 rows run the SIMT weight-streaming kernels of csrc/decode.cu
+ * (omlm_skinny_gemm, omlm_attn_decode); 16 < B <= 256 run the tensor-core GEMM of csrc/decode_gemm.cu (omlm_decode_gemm)
+ * and the cache-sharing attention omlm_attn_decode_mqa.
  * out[b, n] = A[b, :] . W[n, :] (+ addend[b, n]);  W 16-bit [N, ldw] (w_f16: fp16, else bf16).  prologue builds the
  * activation rows in W's format: 0 = A already 16-bit [B, lda];  1 = A fp32, rounded;  2 = LayerNorm(A fp32) * gamma
  * (transformer.py:24-31);  3 = A = h 16-bit [B, K] with the fused per-128-channel sums rowsum [B, K/128, 2]:
@@ -222,6 +224,21 @@ int omlm_gather_windows(const void* src_i16, const long long* start, long long* 
 int omlm_skinny_gemm(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
                      const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
                      int B, int N, int K, void* stream);
+/* The same contract for 1 <= B <= 256 rows on the wgmma tensor cores: the weight rows are the 64-row M operand, the batch
+ * (padded to 64, 128 or 256) the N operand, and the K range is split over CTAs (fp32 partials, summed by a second
+ * kernel in a fixed order) until the grid covers the SMs or the partials' bytes reach 4x the weights'.  Same
+ * prologues with the same rounding points, same output formats and argument checks; the result differs from
+ * omlm_skinny_gemm's only in the fp32 accumulation order.  Deterministic (no floating-point atomics): repeated calls and
+ * CUDA-graph replays give bit-identical outputs.  out must not
+ * overlap A.  Workspaces (device, owned by the caller, reusable by successive calls on one stream):
+ *   a16_ws   16-byte aligned, B * K 16-bit elements: the activation operand (unused when prologue = 0 and A is 16-byte
+ *            aligned with lda % 8 == 0: then A is read in place);
+ *   part_ws  part_ws_bytes >= the part_bytes omlm_decode_gemm_workspace reports (split-K partials, fp32). */
+int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
+                     const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
+                     int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream);
+/* Workspace omlm_decode_gemm needs for a B x N x K call (host-only query; depends on the current device's SM count). */
+int omlm_decode_gemm_workspace(int B, int N, int K, long* part_bytes);
 /* Attention for the new position n = *pos_ptr (device int): q_raw [B, heads*64], kv_raw [B, 128] bf16 are this step's
  * un-normalised projections; they are l2-normalised * scale (transformer.py:269-271), [k | v] is appended to
  * cache [B, cache_ld_b/128 positions, 128] bf16 at n, then softmax(8 q.k_j + table[head, n-j]) V over keys 0..n
@@ -229,6 +246,15 @@ int omlm_skinny_gemm(const void* A, long lda, int prologue, const void* W, long 
 int omlm_attn_decode(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
                      long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
                      int heads, float scale, void* stream);
+/* The same attention with every cached row read once per sequence (omlm_attn_decode reads it once per head): one CTA per
+ * sequence and 128-key slice serves all heads (1 <= heads <= 16), and the slices are combined in a fixed order
+ * (deterministic).  Same rounding points, except that P is rounded to bf16 relative to its slice's maximum: outputs
+ * agree with omlm_attn_decode to bf16 rounding; the appended cache row is bit-identical.  Workspaces (device, owned by
+ * the caller): ws fp32, ws_bytes >= B * ceil(max_pos / 128) * heads * 66 * 4;  counters B ints, ZERO before the first
+ * call (each call leaves them zero). */
+int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                         long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
+                         int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream);
 /* CausalDSConv + GEGLU for one new row (transformer.py:122-137): u_new [B, 2Fp] against state [B, 2, 2Fp] (rows t-2, t-1,
  * shifted in place) -> h [B, Fp], rowsum [B, Fp/128, 2]. */
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,

@@ -253,6 +253,191 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16*
   }
 }
 
+// ------------------------------------------------------------------------------------------------ attention, large batches
+// The same step with every cached row read once per sequence: attn_decode runs one CTA per (sequence, head), so with
+// multi-query attention each row is read `heads` times.  Here grid (splits, B): the CTA of split s serves ALL heads of
+// sequence b over keys [128 s, 128 s + 128) ∩ [0, n] (flash decoding).  It stages those K | V rows in shared memory once,
+// takes row n from this step's projections (and appends it to the cache: exactly one CTA covers n), and leaves per head
+// the split's (max, sum) and unnormalised P V in a workspace.  The last split of a sequence to finish (per-sequence
+// counter) combines the splits in order 0, 1, ... -- fixed order, deterministic -- and writes out.
+// Rounding points of attn_decode: bf16 q / k after l2norm * scale, scores in the exp2 domain, P rounded to bf16 (here
+// relative to the split's own maximum), fp32 normaliser.
+constexpr int kMqThreads = 256, kMqKeys = 128;
+constexpr int kMqRow = 272;                          // bytes per staged K | V row: 256 + 16 of padding (bank spread)
+constexpr int kMqScLd = kMqKeys + 1;                 // score row pitch (floats)
+
+template <int HM>                                    // HM >= heads: 4, 8 or 16
+__global__ void __launch_bounds__(kMqThreads)
+attn_decode_mqa_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16* __restrict__ kv_raw,
+                       const float* __restrict__ q_scale, const float* __restrict__ k_scale,
+                       __nv_bfloat16* __restrict__ cache, long cache_ld_b, const float* __restrict__ table, int table_ld,
+                       const int* __restrict__ pos_ptr, __nv_bfloat16* __restrict__ out, int h, float scale,
+                       float* __restrict__ part_o, float2* __restrict__ part_ml, int* __restrict__ counters, int max_splits) {
+  pdl_prologue();
+  extern __shared__ __align__(16) uint8_t mq_smem[];
+  uint8_t* skv = mq_smem;                                                      // [kMqKeys][kMqRow]
+  float* sc = reinterpret_cast<float*>(mq_smem + kMqKeys * kMqRow);            // [HM][kMqScLd] scores, then P
+  constexpr int G = kMqThreads / (HM * 8);                                     // key groups of the P V product
+  __shared__ float sq[HM][64], sk[64];
+  __shared__ float so[G][HM * 64];
+  __shared__ float s_m[HM], s_l[HM];
+  __shared__ int s_last;
+  const int split = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int n = *pos_ptr;
+  const int j0 = split * kMqKeys;
+  if (j0 > n) return;                                // beyond this step's keys (the grid covers max_pos)
+  const int nk = min(kMqKeys, n + 1 - j0), active = n / kMqKeys + 1;
+  // ---- l2norm * scale of every head's query and of the new key, rounded to bf16 (warp w: heads w, w + 8, then k)
+  for (int t = warp; t <= h; t += kMqThreads / 32) {
+    const __nv_bfloat16* src = t < h ? q_raw + static_cast<long>(b) * h * 64 + t * 64 : kv_raw + static_cast<long>(b) * 128;
+    const float x0 = __bfloat162float(src[lane]), x1 = __bfloat162float(src[lane + 32]);
+    const float inv = 1.f / fmaxf(sqrtf(warp_sum(x0 * x0 + x1 * x1)), 1e-12f);
+    const float* s = t < h ? q_scale : k_scale;
+    float* dst = t < h ? sq[t] : sk;
+    dst[lane] = bf16_round(x0 * inv * s[lane]);
+    dst[lane + 32] = bf16_round(x1 * inv * s[lane + 32]);
+  }
+  __nv_bfloat16* crow = cache + static_cast<long>(b) * cache_ld_b;
+  for (int i = tid; i < nk * 16; i += kMqThreads) {  // cached rows j < n, 16 bytes per thread
+    const int r = i >> 4, c = i & 15, j = j0 + r;
+    if (j < n) *reinterpret_cast<uint4*>(skv + r * kMqRow + c * 16) = __ldg(reinterpret_cast<const uint4*>(crow + static_cast<long>(j) * 128) + c);
+  }
+  __syncthreads();
+  if (n - j0 < kMqKeys && tid < 128) {               // row n: this step's [k | v], staged and appended to the cache
+    const __nv_bfloat16 v = tid < 64 ? __float2bfloat16_rn(sk[tid]) : kv_raw[static_cast<long>(b) * 128 + tid];
+    reinterpret_cast<__nv_bfloat16*>(skv + (n - j0) * kMqRow)[tid] = v;
+    crow[static_cast<long>(n) * 128 + tid] = v;
+  }
+  __syncthreads();
+  // ---- scores (log2 domain): 8 q.k_j + bias[head, n - j]; thread = key r, heads of parity tid / 128
+  const float l2e = 1.4426950408889634f;
+  {
+    const int r = tid & (kMqKeys - 1), hp = tid >> 7;
+    float dot[HM / 2];
+#pragma unroll
+    for (int u = 0; u < HM / 2; ++u) dot[u] = 0.f;
+    if (r < nk) {
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(skv + r * kMqRow + c * 16);
+        const uint32_t rw[4] = {raw.x, raw.y, raw.z, raw.w};
+        float kf[8];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { const float2 t = unpack_bf16x2(rw[q]); kf[2 * q] = t.x; kf[2 * q + 1] = t.y; }
+#pragma unroll
+        for (int u = 0; u < HM / 2; ++u) {
+          if (hp + 2 * u < h) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e) dot[u] = fmaf(sq[hp + 2 * u][c * 8 + e], kf[e], dot[u]);
+          }
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < HM / 2; ++u) {
+        const int hh = hp + 2 * u;
+        if (hh < h) sc[hh * kMqScLd + r] = (dot[u] * scale + table[hh * table_ld + (n - j0 - r)]) * l2e;
+      }
+    }
+  }
+  __syncthreads();
+  // ---- per head: the split's max and sum; P rounded to bf16 (warp w: heads w, w + 8)
+  for (int hh = warp; hh < h; hh += kMqThreads / 32) {
+    float* s = sc + hh * kMqScLd;
+    float mx = -INFINITY;
+    for (int r = lane; r < nk; r += 32) mx = fmaxf(mx, s[r]);
+    mx = warp_max(mx);
+    float sum = 0.f;
+    for (int r = lane; r < nk; r += 32) {
+      const float p = exp2f(s[r] - mx);
+      sum += p;
+      s[r] = bf16_round(p);
+    }
+    sum = warp_sum(sum);
+    if (lane == 0) { s_m[hh] = mx; s_l[hh] = sum; }
+  }
+  __syncthreads();
+  // ---- P V: thread = (key group g, head, 8-dim chunk)
+  {
+    const int g = tid / (HM * 8), hh = (tid >> 3) % HM, ch = tid & 7;
+    float o[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[e] = 0.f;
+    if (hh < h) {
+      for (int r = g; r < nk; r += G) {
+        const float p = sc[hh * kMqScLd + r];
+        const uint4 raw = *reinterpret_cast<const uint4*>(skv + r * kMqRow + 128 + ch * 16);
+        const uint32_t rw[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 t = unpack_bf16x2(rw[q]);
+          o[2 * q] = fmaf(p, t.x, o[2 * q]);
+          o[2 * q + 1] = fmaf(p, t.y, o[2 * q + 1]);
+        }
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) so[g][hh * 64 + ch * 8 + e] = o[e];
+  }
+  __syncthreads();
+  if (active == 1) {                                 // a single split: normalise and write out directly
+    for (int i = tid; i < h * 64; i += kMqThreads) {
+      float acc = 0.f;
+#pragma unroll
+      for (int g = 0; g < G; ++g) acc += so[g][i];
+      out[static_cast<long>(b) * h * 64 + i] = __float2bfloat16_rn(acc / s_l[i >> 6]);
+    }
+    return;
+  }
+  const long base = static_cast<long>(b) * max_splits;
+  for (int i = tid; i < h * 64; i += kMqThreads) {
+    float acc = 0.f;
+#pragma unroll
+    for (int g = 0; g < G; ++g) acc += so[g][i];
+    __stcg(part_o + (base + split) * h * 64 + i, acc);
+  }
+  if (tid < h) __stcg(part_ml + (base + split) * h + tid, make_float2(s_m[tid], s_l[tid]));
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(counters + b, 1) == active - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  // ---- last split of this sequence: combine the splits in order (rescaled to the common maximum)
+  for (int i = tid; i < h * 64; i += kMqThreads) {
+    const int hh = i >> 6;
+    float mx = -INFINITY;
+    for (int s = 0; s < active; ++s) mx = fmaxf(mx, __ldcg(part_ml + (base + s) * h + hh).x);
+    float l = 0.f, acc = 0.f;
+    for (int s = 0; s < active; ++s) {
+      const float2 ml = __ldcg(part_ml + (base + s) * h + hh);
+      const float f = exp2f(ml.x - mx);
+      l = fmaf(f, ml.y, l);
+      acc = fmaf(f, __ldcg(part_o + (base + s) * h * 64 + i), acc);
+    }
+    out[static_cast<long>(b) * h * 64 + i] = __float2bfloat16_rn(acc / l);
+  }
+  if (tid == 0) counters[b] = 0;                     // ready for the next step (or graph replay)
+}
+
+template <int HM>
+static int launch_attn_decode_mqa(dim3 grid, cudaStream_t st, const void* q_raw, const void* kv_raw, const float* q_scale,
+                                  const float* k_scale, void* cache, long cache_ld_b, const float* table, int table_ld,
+                                  const int* pos_ptr, void* out, int heads, float scale, float* part_o, float2* part_ml,
+                                  int* counters, int max_splits) {
+  constexpr int smem = kMqKeys * kMqRow + HM * kMqScLd * 4;
+  static bool configured = false;
+  if (!configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(attn_decode_mqa_kernel<HM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = true;
+  }
+  OMLM_KLAUNCH((attn_decode_mqa_kernel<HM>), grid, kMqThreads, smem, st,
+      reinterpret_cast<const __nv_bfloat16*>(q_raw), reinterpret_cast<const __nv_bfloat16*>(kv_raw), q_scale, k_scale,
+      reinterpret_cast<__nv_bfloat16*>(cache), cache_ld_b, table, table_ld, pos_ptr, reinterpret_cast<__nv_bfloat16*>(out), heads,
+      scale, part_o, part_ml, counters, max_splits);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------ conv + GEGLU, one new row
 // u_new [B, 2Fp] (interleaved GEGLU layout), state [B, 2, 2Fp] = rows t-2, t-1 -> h [B, Fp], rowsum [B, Fp/128, 2];
 // the state is shifted in place.  grid (Fp/128, B), 128 threads (one per channel of the group).
@@ -444,6 +629,26 @@ int omlm_attn_decode(const void* q_raw, const void* kv_raw, const float* q_scale
       reinterpret_cast<__nv_bfloat16*>(cache), cache_ld_b, table, table_ld, pos_ptr, reinterpret_cast<__nv_bfloat16*>(out), heads, scale);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                         long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
+                         int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(B >= 1 && heads >= 1 && heads <= 16 && max_pos >= 1 && table_ld >= max_pos, "attn_decode_mqa: bad shape");
+  const int max_splits = (max_pos + kMqKeys - 1) / kMqKeys;
+  const long need = static_cast<long>(B) * max_splits * heads * (64 + 2) * 4;
+  OMLM_CHECK_ARG(ws != nullptr && counters != nullptr && ws_bytes >= need, "attn_decode_mqa: workspace of %ld bytes, %ld needed", ws_bytes, need);
+  float* part_o = ws;
+  float2* part_ml = reinterpret_cast<float2*>(ws + static_cast<long>(B) * max_splits * heads * 64);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(max_splits, B);
+  if (heads <= 4) return launch_attn_decode_mqa<4>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
+                                                   pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+  if (heads <= 8) return launch_attn_decode_mqa<8>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
+                                                   pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+  return launch_attn_decode_mqa<16>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
+                                    pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
 }
 
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,

@@ -8,6 +8,9 @@ the transformer for every sampled token; here the prompt is run once (the regula
 caches) and every further token costs one incremental step over
     per layer:  K/V cache [B, Nmax, 128] bf16  +  the last two pre-conv FFN rows [B, 2, 2Fp]  (CausalDSConv history)
 with the weight-streaming kernels of csrc/decode.cu, replayed from one CUDA graph per quantizer index.
+Up to 16 sequences per call run the SIMT kernels (skinny_gemm, attn_decode); 17 to 256 run the wgmma GEMM of
+csrc/decode_gemm.cu, whose batch is the tensor cores' N operand, and attn_decode_mqa, which reads every cached row once
+per sequence instead of once per head.  The choice follows from the batch size; it is not an option.
 """
 import os
 from typing import List, Optional, Sequence
@@ -17,6 +20,9 @@ from torch import nn
 
 from . import lib
 from .model import TokenConditionedTransformer
+
+SKINNY_MAX_BATCH = 16      # up to here the SIMT kernels (skinny_gemm, attn_decode); above, the tensor-core path
+MAX_BATCH = 256            # sequences per generate() call
 
 
 class _Capture:
@@ -43,8 +49,11 @@ class DecodeSession:
     def __init__(self, eng, B: int, n_prompt: int, n_new: int):
         if eng.abs_pos:
             raise NotImplementedError("open_musiclm_b200 generate: absolute position embeddings are not supported by the decode path")
-        if B > 16:
-            raise lib.OmlmError("open_musiclm_b200 generate: batch sizes above 16 are not supported by the decode kernels")
+        if B > MAX_BATCH:
+            raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
+        if B > SKINNY_MAX_BATCH and os.environ.get("OMLM_DECODE_FUSED", "0") == "1":
+            raise lib.OmlmError(f"open_musiclm_b200 generate: the fused decode step (OMLM_DECODE_FUSED=1) supports at most "
+                                f"{SKINNY_MAX_BATCH} sequences (got {B})")
         self.eng, self.B, self.n_prompt, self.n_new = eng, B, n_prompt, n_new
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
         d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
@@ -79,6 +88,12 @@ class DecodeSession:
         # per-op launches (5.41 s vs 4.10 s on an H100 SXM at a 400 W power limit, tools/time_generate.py) -- its 31
         # stages are each bound by a single-warp prologue (LayerNorm statistics, row-sum tree) and a grid barrier.
         self.fused = os.environ.get("OMLM_DECODE_FUSED", "0") == "1"
+        # more than 16 sequences: tensor-core GEMMs and the cache-sharing attention, with their scratch allocated here so
+        # that graph capture allocates nothing
+        self.batched = B > SKINNY_MAX_BATCH
+        if self.batched:
+            shapes = [(HD, d), (128, d), (d, HD), (2 * Fp, d), (d, Fp)] + [(cp, d) for cp in eng.Cp]
+            self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h)
         if self.fused:
             pv = eng.pview
             layers = []
@@ -111,6 +126,8 @@ class DecodeSession:
 
     def step_ops(self, qi_next: int):
         """The same step as separate launches (one per operation)."""
+        if self.batched:
+            return self.step_batched(qi_next)
         eng, B = self.eng, self.B
         pv, d, HD, F, Fp, h = eng.pview, eng.d, eng.HD, eng.F, eng.Fp, eng.h
         xa, xm = self.x
@@ -127,6 +144,26 @@ class DecodeSession:
             lib.skinny_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm)
         S = len(eng.seqs) - 1
         lib.skinny_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"])
+
+    def step_batched(self, qi_next: int):
+        """step_ops for more than 16 sequences: the same operations on the tensor-core GEMM and the cache-sharing
+        attention (same rounding points; fp32 sums in another order)."""
+        eng, ws = self.eng, self.ws
+        pv, F, h = eng.pview, eng.F, eng.h
+        xa, xm = self.x
+        lib.embed_gather(eng.table, self.next_row, xa)
+        for l in range(eng.L):
+            p, pk = f"transformer.layers.{l}.", eng.pk[l]
+            lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws)
+            lib.decode_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1, ws=ws)
+            lib.attn_decode_mqa(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
+                                self.n_max, self.o, h, ws=ws)
+            lib.decode_gemm(self.o, pk["wo_b"], xm, addend=xa, ws=ws)
+            lib.decode_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]], ws=ws)
+            lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
+            lib.decode_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm, ws=ws)
+        S = len(eng.seqs) - 1
+        lib.decode_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"], ws=ws)
 
     def sample(self, qi: int, top_k: int, temperature: float, allow_eos: bool, uniform, seed, bump_pos: bool):
         eng = self.eng

@@ -342,6 +342,53 @@ def skinny_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, add
          _I(FMT[out.dtype]), _L(out.stride(0)), _I(B), _I(N), _I(K), _stream())
 
 
+def decode_gemm_workspace(B, N, K):
+    """Bytes of split-K partials omlm_decode_gemm needs for a B x N x K call on the current device."""
+    part = _L(0)
+    call("omlm_decode_gemm_workspace", _I(B), _I(N), _I(K), ctypes.byref(part))
+    return part.value
+
+
+class DecodeWorkspace:
+    """Scratch of the large-batch decode kernels, allocated once so that CUDA-graph capture allocates nothing:
+    the 16-bit activation operand [B, max K], the split-K partials, the attention's per-slice partials and its
+    per-sequence counters (zero; every call leaves them zero).  shapes: the (N, K) of every decode_gemm call; max_pos /
+    heads: attention."""
+
+    def __init__(self, device, B, shapes, max_pos=0, heads=0):
+        part = max(decode_gemm_workspace(B, N, K) for N, K in shapes)
+        attn = B * -(-max_pos // 128) * heads * 66 if max_pos else 0
+        self.a16 = torch.empty(B * max(K for _, K in shapes), device=device, dtype=torch.int16)
+        self.part = torch.empty(max(part // 4, 1), device=device, dtype=torch.float32)
+        self.attn = torch.empty(max(attn, 1), device=device, dtype=torch.float32)
+        self.counters = torch.zeros(B, device=device, dtype=torch.int32)
+
+
+def decode_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, addend=None, ws=None):
+    """skinny_gemm's contract for 1 <= B <= 256 rows on the tensor cores (omlm_decode_gemm).  ws: a DecodeWorkspace
+    covering this shape (None: a fresh one, which is not CUDA-graph capturable)."""
+    B = A.shape[0]
+    N, K = W.shape
+    assert W.dtype in _T16 and W.stride(1) == 1 and out.stride(-1) == 1 and A.stride(-1) == 1
+    assert (prologue in (0, 3) and A.dtype == W.dtype) or (prologue in (1, 2) and A.dtype == torch.float32)
+    if ws is None:
+        ws = DecodeWorkspace(A.device, B, [(N, K)])
+    call("omlm_decode_gemm", _p(A), _L(A.stride(0)), _I(prologue), _p(W), _L(W.stride(0)), _I(int(W.dtype == torch.float16)),
+         _p(gamma), _p(rowsum), _I(n_real), _p(addend), _L(addend.stride(0) if addend is not None else 0), _p(out),
+         _I(FMT[out.dtype]), _L(out.stride(0)), _I(B), _I(N), _I(K), _p(ws.a16), _p(ws.part), _L(ws.part.numel() * 4),
+         _stream())
+
+
+def attn_decode_mqa(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, ws=None, scale=8.0):
+    """attn_decode's contract with every cached row read once per sequence (omlm_attn_decode_mqa), 1 <= heads <= 16."""
+    B = q_raw.shape[0]
+    if ws is None:
+        ws = DecodeWorkspace(q_raw.device, B, [(1, 8)], max_pos=max_pos, heads=heads)
+    call("omlm_attn_decode_mqa", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(cache), _L(cache.stride(0)), _p(table),
+         _I(table.stride(0)), _p(pos), _I(max_pos), _p(out), _I(B), _I(heads), _F(scale), _p(ws.attn), _L(ws.attn.numel() * 4),
+         _p(ws.counters), _stream())
+
+
 class _DecodeLayer(ctypes.Structure):
     """omlm_decode_layer (include/omlm_b200.h): the per-layer pointers of the fused decode step."""
     _fields_ = [(n, ctypes.c_void_p) for n in ("wq", "wkv", "wo", "w1", "w2", "conv", "gin", "g_attn", "g_ff", "q_scale", "k_scale",
