@@ -60,6 +60,67 @@ int omlm_gemm16_rowstat(const void* A, int a_f16, int a_mn_major, long lda, cons
                         int M, int N, int K, void* out_bf16, long ldo, const void* hn_bf16, long ldhn, const void* keep_bits,
                         const float* gamma, float keep_scale, float* part, int parts, int max_ctas, void* stream);
 
+/* ---- deterministic variants -------------------------------------------------------------------------------------
+ * The training path's float reductions that the entry points above perform with atomics (so their results depend on
+ * the order in which CTAs finish) have variants with the suffix _det.  Each keeps its default's contract and
+ * arithmetic and fixes the order of every float sum, so repeated calls and CUDA-graph replays on one GPU model (same
+ * SM count: tile and split choices depend on it) give bit-identical results.  Partial sums go to scratch the caller
+ * owns (part_ws, part_ws_bytes: too small is an argument error); the library allocates nothing.
+ *
+ * Split-K GEMM, out fp32 += A B (the weight gradients): split s writes its fp32 partial [rows_out, ceil4(n_valid)] to
+ * part_ws (no atomics) and a second kernel adds the partials to out in split order.  rows_out is the number of output
+ * rows the row remap reaches (row_split > 0: M / row_split * row_valid, M must be a multiple of row_split; < 0:
+ * 2 * row_valid; 0: M).  splits is
+ * clamped as in omlm_gemm16; with one split the call is the in-place addend GEMM (no scratch used).
+ * omlm_gemm16_splitk_det_workspace reports the bytes of part_ws (0 for one split). */
+int omlm_gemm16_splitk_det(const void* A, int a_f16, int a_mn_major, long lda, const void* B, int b_f16, int b_mn_major, long ldb,
+                           int M, int N, int K, float* out, long ldo, int splits, int row_split, int row_valid, int n_valid,
+                           int block_n, int max_ctas, float* part_ws, long part_ws_bytes, void* stream);
+int omlm_gemm16_splitk_det_workspace(int M, int N, int K, int splits, int row_split, int row_valid, int n_valid, long* part_bytes);
+/* omlm_layernorm_bwd: each CTA writes its dgamma sum as one row of part_ws (>= 4 * SMs * D floats), omlm_colsum adds
+ * the rows to dgamma in CTA order. */
+int omlm_layernorm_bwd_det(const void* dy_bf16, const float* x, const float* stats, const float* gamma,
+                           const float* dres, const void* draw_bf16, const int* src_row, float* dx,
+                           void* dx_bf16, float* dgamma, int M, int D, float* part_ws, long part_ws_bytes, void* stream);
+/* omlm_qk_l2norm_bwd: per-CTA rows of (q scale | k scale) sums in part_ws (>= 8 * SMs * 128 floats), then omlm_colsum. */
+int omlm_qk_l2norm_bwd_det(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
+                           const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
+                           float* dq_scale, float* dk_scale, int M, int heads, float* part_ws, long part_ws_bytes, void* stream);
+/* omlm_ffn_mid_bwd: per-CTA rows [B * ceil(N / 128), 7F] of (dgamma [F] | dconv_w [2F, 3]) sums in part_ws, then
+ * omlm_colsum. */
+int omlm_ffn_mid_bwd_det(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
+                         const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
+                         float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, float* part_ws, long part_ws_bytes,
+                         void* stream);
+/* omlm_sgemm_small without the split of K over CTAs (each output element is one CTA's in-order sum). */
+int omlm_sgemm_small_det(const float* A, long sa_m, long sa_k, const float* B, long sb_k, long sb_n, float* C,
+                         long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
+                         int accumulate, void* stream);
+/* omlm_embed_scatter_add: each destination row is summed by one warp over its positions in ascending order
+ * (dtable row + scale * dx rows, each add rounded).  first_ws: table_rows ints, INT_MAX before the first call (each call
+ * leaves them so); rows outside [0, table_rows) are skipped. */
+int omlm_embed_scatter_add_det(float* dtable, const int* src_row, const float* dx, int M, int D, float scale, int* first_ws,
+                               int table_rows, void* stream);
+/* omlm_cross_entropy: per-CTA (loss, rows) pairs in part_ws (>= ceil(rows / 8) * 8 bytes), added to loss_acc in CTA order
+ * by omlm_colsum. */
+int omlm_cross_entropy_det(const float* logits, long ld, const int* labels, int label_stride, int rows_per_batch,
+                           long batch_stride, int rows, int C, int ignore_index, float grad_scale, float loss_scale,
+                           void* dlogits_bf16, long ldd, int Cp, float* loss_acc, float* part_ws, long part_ws_bytes, void* stream);
+/* omlm_grad_sumsq: per-CTA double sums in part_ws (>= 4 * SMs doubles), added to acc in CTA order. */
+int omlm_grad_sumsq_det(const float* g, long n, float prescale, double* acc, double* part_ws, long part_ws_bytes, void* stream);
+/* omlm_attn_bwd_tc with a fixed order for dQ, dK|dV and the bias gradient: dQ of a row tile and dK|dV of a key tile are
+ * added in turns (key tile, warpgroup) and (row chunk) kept by counters in iws; each CTA's diagonal sums go to its own
+ * partial table in ws and a second kernel adds the tables to dtable in CTA order.  ws (ws_bytes) and iws (iws_count
+ * ints) are sized by omlm_attn_bwd_tc_det_workspace (iws_count may be larger).  iws[iws_count - 1] is an error word that
+ * must be zero before the first call.  It is set to 1 if a turn was not granted within seconds: the kernel never hangs,
+ * and that call's sums -- and those of every later call until the caller clears the word -- are added in arrival order,
+ * correct up to rounding like omlm_attn_bwd_tc's but not reproducible. */
+int omlm_attn_bwd_tc_det(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
+                         const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
+                         float* dqn, float* dkvn, float* dtable, int B, int N, int heads, float scale,
+                         float* ws, long ws_bytes, int* iws, long iws_count, void* stream);
+int omlm_attn_bwd_tc_det_workspace(int B, int N, int heads, long* ws_bytes, long* iws_count);
+
 /* ---- integer token path (bit-exact) ------------------------------------------------------------
  * One pass over the raw ids of all sequences of a TokenConditionedTransformer batch.
  * Wrapper mode (append_eos=1): eos (= codebook size) appended to every sequence
@@ -141,7 +202,8 @@ int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* 
 /* wgmma/TMA backward: dqn and dkvn are OVERWRITTEN (its first kernel clears them, the main kernel reduces into
  * them), dtable is accumulated (+=: one table gradient over all layers).  The bias gradient -- diagonal sums of dS -- is
  * formed inside the kernel from the fp32 dS, summed per CTA in shared memory and added to dtable once; no scratch tensor.
- * dqn, dkvn and dtable are reduced with floating-point atomics: reproducible up to accumulation order. */
+ * dqn, dkvn and dtable are reduced with floating-point atomics: reproducible up to accumulation order
+ * (omlm_attn_bwd_tc_det fixes the order). */
 int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                      const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
                      float* dqn, float* dkvn, float* dtable, int B, int N, int heads,

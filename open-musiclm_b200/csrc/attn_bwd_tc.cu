@@ -11,6 +11,17 @@
 //                      dQ  = dS K                         (per tile, red.global.add.v2.f32 into dqn)
 //                   the bias gradient dTable[hh, i-j] += dS sums the fp32 dS along its diagonals into a per-CTA shared
 //                   table that is flushed to global once.
+//
+// Deterministic variant (DET, omlm_attn_bwd_tc_det): the same work units and arithmetic, with every float reduction in a
+// fixed order.  dQ of a row tile and dK|dV of a key tile are still added with red.global.add, but in turns enforced by
+// per-tile counters (the deterministic backward of FlashAttention-3): row tile rt takes the (key tile, warpgroup) pairs
+// in the order (0,0), (0,1), (1,0), ...; key tile kt takes its row chunks in chunk order.  A turn only ever waits for
+// a CTA with a lower block index, which the hardware dispatched first, so the waits cannot deadlock; a wait that does not
+// end within seconds sets an error word and gives up instead of hanging.  The bias gradient stages the fp32 dS tile in
+// shared memory; each thread then owns (head, diagonal) pairs and sums them in row order into its warpgroup's table, the
+// two tables are added per unit into a partial table in global memory, and a second kernel adds the partial tables to
+// dtable in unit order.  After a time-out the error word stays set and later calls skip their waits, until the caller
+// clears it: their sums are then added in arrival order (correct up to rounding, not reproducible).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -26,6 +37,9 @@ constexpr int kBoK = 0, kBoV = 16384, kBoQ = 32768 /*2 stages x 8K*/, kBoDO = 49
 constexpr int kBoP = 65536 /*2 wg x 8K*/, kBoDS = 81920 /*2 wg x 8K*/, kBoBar = 98304 /*64 B*/;
 constexpr int kBoAcc = 98368;     // diagonal-sum table: h x Wacc floats
 constexpr int kBtMaxSmem = 232448;
+// DET: fp32 dS tiles [2 wg][64 rows][kBtSdsLd] at kBoAcc, then one diagonal table per warpgroup (2 x h x Wacc floats)
+constexpr int kBtSdsLd = 72;      // padded row: the fragment stores of the 8 rows of a quad land in different banks
+constexpr int kBoAccDet = kBoAcc + 2 * 64 * kBtSdsLd * 4;
 
 __device__ __forceinline__ float bt_ex2(float x) {
   float y;
@@ -36,12 +50,44 @@ __device__ __forceinline__ void bt_red2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
+// ---- DET turn counters.  One thread of a warpgroup waits for the turn, the warpgroup adds, fences and signals.
+__device__ __forceinline__ int bt_ld_acquire(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ unsigned long long bt_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __noinline__ void bt_wait_turn(const int* ctr, int turn, int* err) {
+  const unsigned long long t0 = bt_globaltimer();
+  while (bt_ld_acquire(ctr) != turn) {
+    if (*reinterpret_cast<volatile int*>(err) != 0) return;
+    if (bt_globaltimer() - t0 > 4000000000ull) { atomicExch(err, 1); return; }   // 4 s: report, never hang
+    __nanosleep(64);
+  }
+}
+__device__ __forceinline__ void bt_pass_turn(int* ctr) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(ctr) : "memory");
+}
+
+struct BtDet {
+  int* turn_dq;     // [B, row tiles]
+  int* turn_kv;     // [B, key tiles, 2]
+  int* meta;        // [units, 2]: (dmin, used width) of each unit's partial table
+  int* err;
+  float* dpart;     // [units, h, Wacc]
+};
+
+template <bool DET>
 __global__ void __launch_bounds__(kBtThreads, 1)
 attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                    const __grid_constant__ CUtensorMap tmKV, const float* __restrict__ lse2, const float* __restrict__ dsum,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                    float* __restrict__ dqn, float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale,
-                   int Wacc, int tiles_per_chunk, int nbatch) {
+                   int Wacc, int tiles_per_chunk, int nbatch, const BtDet det) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -49,7 +95,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* kv_full = bars + 0;
   uint64_t* qd_full = bars + 1;    // [2]
   uint64_t* qd_empty = bars + 3;   // [2]
-  float* dacc = reinterpret_cast<float*>(smem + kBoAcc);
+  float* dacc = reinterpret_cast<float*>(smem + (DET ? kBoAccDet : kBoAcc));
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int R = N * h;
@@ -77,7 +123,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int i = 0; i < 2; ++i) { mbar_init(&qd_full[i], 1); mbar_init(&qd_empty[i], 2); }
     fence_barrier_init();
   }
-  for (int x = threadIdx.x; x < h * Wacc; x += blockDim.x) dacc[x] = 0.f;
+  for (int x = threadIdx.x; x < (DET ? 2 : 1) * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
   __syncthreads();
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
@@ -106,6 +152,9 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const uint32_t sk = smem_u32(smem + kBoK) + cw * 8192, sv = smem_u32(smem + kBoV) + cw * 8192;
     uint8_t* p_tile = smem + kBoP + cw * 8192;
     uint8_t* ds_tile = smem + kBoDS + cw * 8192;
+    float* sdsf = reinterpret_cast<float*>(smem + kBoAcc) + cw * 64 * kBtSdsLd;    // DET: this warpgroup's fp32 dS tile
+    float* wacc = dacc + (DET ? cw * h * Wacc : 0);                                 // DET: this warpgroup's diagonal table
+    const int tid128 = threadIdx.x & 127;
     const uint32_t sp = smem_u32(p_tile), sds = smem_u32(ds_tile);
     const float sc2 = scale * kBtL2e;
     // key visibility of this thread's 16 columns (8 c + 2 qc + e)
@@ -162,8 +211,9 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             const float x = s[4 * c + 2 * hr + e];
             pp[e] = live ? bt_ex2(fmaf(x, sc2, __ldg(trow + (live ? delta : 0)) * kBtL2e) - lse) : 0.f;
             dd[e] = pp[e] * (dp[4 * c + 2 * hr + e] - D);
-            if (live) atomicAdd(arow + delta, dd[e]);
+            if (!DET && live) atomicAdd(arow + delta, dd[e]);
           }
+          if (DET) *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
           const uint32_t off = static_cast<uint32_t>(((c ^ (lr & 7)) << 4) + 4 * qc);
           *reinterpret_cast<uint32_t*>(prow + off) = pack_bf16x2(pp[0], pp[1]);
           *reinterpret_cast<uint32_t*>(drow + off) = pack_bf16x2(dd[0], dd[1]);
@@ -182,12 +232,31 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Wgmma<64, false>::ss<0, 1>(dq, make_smem_desc(sds + ks * 32, 16, 1024), make_smem_desc(sk + ks * 2048, 8192, 1024), ks > 0 ? 1u : 0u);
       }
       wgmma_commit();
+      if constexpr (DET) {
+        // diagonal sums of the fp32 dS tile while the tensor cores run: thread-owned (head, diagonal) pairs, rows in order
+        const int it_lo = rbase / h, it_hi = min((rbase + kBtBQ - 1) / h, N - 1);
+        const int dlo = max(0, it_lo - kbase - 63), dhi = it_hi - kbase;
+        const int W = dhi - dlo + 1;
+        for (int p = tid128; p < h * W; p += 128) {
+          const int hh = p / W, dl = dlo + (p - hh * W);
+          const int i0 = max((rbase - hh + h - 1) / h, kbase + dl);
+          const int i1 = min(min((rbase + kBtBQ - 1 - hh) / h, N - 1), kbase + dl + 63);
+          float sum = 0.f;
+          for (int i = i0; i <= i1; ++i) sum += sdsf[(i * h + hh - rbase) * kBtSdsLd + (i - dl - kbase)];
+          wacc[hh * Wacc + dl - dmin] += sum;
+        }
+      }
       wgmma_wait<0>();
       wgmma_reg_fence(dq);
       wgmma_reg_fence(dv);
       wgmma_reg_fence(dk);
       asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");   // every thread's wgmma have read the P / dS tiles
       if (leader) mbar_arrive(&qd_empty[st]);
+      int* turn = DET ? det.turn_dq + static_cast<long>(b) * n_rt + rt0 + t : nullptr;
+      if constexpr (DET) {
+        if (leader) bt_wait_turn(turn, 2 * kt + cw, det.err);
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+      }
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int r = rbase + wq * 16 + qr + hr * 8;
@@ -197,8 +266,18 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           for (int c = 0; c < 8; ++c) bt_red2(dst + 8 * c, dq[4 * c + 2 * hr] * scale, dq[4 * c + 2 * hr + 1] * scale);
         }
       }
+      if constexpr (DET) {
+        __threadfence();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+        if (leader) bt_pass_turn(turn);
+      }
     }
     // ---- dK (scaled), dV into dkvn [key][dK 0..63 | dV 64..127]
+    int* kv_turn = DET ? det.turn_kv + (static_cast<long>(b) * n_kt + kt) * 2 + cw : nullptr;
+    if constexpr (DET) {
+      if (leader) bt_wait_turn(kv_turn, u, det.err);
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+    }
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       const int j = kbase + wq * 16 + qr + hr * 8;
@@ -211,14 +290,45 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         }
       }
     }
+    if constexpr (DET) {
+      __threadfence();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+      if (leader) bt_pass_turn(kv_turn);
+    }
     // ---- flush the diagonal sums of this unit
     asm volatile("bar.sync 3, 256;" ::: "memory");
-    for (int x = threadIdx.x - 128; x < h * wacc_used; x += 256) {
-      const int hh = x / wacc_used, w = x - hh * wacc_used;
-      const float v = dacc[hh * Wacc + w];
-      if (v != 0.f) atomicAdd(dtable + hh * static_cast<long>(table_ld) + dmin + w, v);
+    if constexpr (DET) {       // (warpgroup 1 + warpgroup 2) -> this unit's partial table; summed in unit order later
+      float* up = det.dpart + static_cast<long>(blockIdx.x) * h * Wacc;
+      for (int x = threadIdx.x - 128; x < h * wacc_used; x += 256) {
+        const int hh = x / wacc_used, w = x - hh * wacc_used;
+        up[hh * Wacc + w] = dacc[hh * Wacc + w] + dacc[(h + hh) * Wacc + w];
+      }
+      if (threadIdx.x == 128) { det.meta[2 * blockIdx.x] = dmin; det.meta[2 * blockIdx.x + 1] = wacc_used; }
+    } else {
+      for (int x = threadIdx.x - 128; x < h * wacc_used; x += 256) {
+        const int hh = x / wacc_used, w = x - hh * wacc_used;
+        const float v = dacc[hh * Wacc + w];
+        if (v != 0.f) atomicAdd(dtable + hh * static_cast<long>(table_ld) + dmin + w, v);
+      }
     }
   }
+}
+
+// DET: dtable[hh, d] += the partial tables of all units, in unit order
+__global__ void __launch_bounds__(256)
+attn_bwd_dtable_reduce_kernel(const float* __restrict__ dpart, const int* __restrict__ meta, int units, int h, int Wacc,
+                              float* __restrict__ dtable, int table_ld, int N) {
+  pdl_prologue();
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= h * N) return;
+  const int hh = x / N, d = x - hh * N;
+  float* dst = dtable + hh * static_cast<long>(table_ld) + d;
+  float acc = *dst;
+  for (int u = 0; u < units; ++u) {
+    const int w = d - __ldg(meta + 2 * u);
+    if (w >= 0 && w < __ldg(meta + 2 * u + 1)) acc += dpart[(static_cast<long>(u) * h + hh) * Wacc + w];
+  }
+  *dst = acc;
 }
 
 // D[r] = sum_d dO[r, d] * O[r, d];  also clears the dQ / dK|dV accumulators the main kernel reduces into
@@ -254,33 +364,21 @@ attn_bwd_tc_dsum_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat
 
 }  // namespace omlm
 
-extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
-                                const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
-                                float* dqn, float* dkvn, float* dtable, int B, int N, int heads,
-                                float scale, void* stream) {
-  using namespace omlm;
-  OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attn_bwd_tc: bad shape");
-  OMLM_CHECK_ARG(table_ld >= N, "attn_bwd_tc: bias table shorter than the sequence");
-  auto st = reinterpret_cast<cudaStream_t>(stream);
+namespace omlm {
+
+// Launch geometry shared by the launch and the workspace query.
+struct BtConfig {
+  int tiles_per_chunk, wacc, smem_bytes, units_per_batch, n_row_tiles, n_key_tiles;
+};
+
+static int bt_config(int B, int N, int heads, bool det, BtConfig* cfg) {
   const long R = static_cast<long>(N) * heads;
-  const long rows = static_cast<long>(B) * R;
-  OMLM_KLAUNCH((attn_bwd_tc_dsum_kernel), static_cast<int>((rows * 8 + 255) / 256), 256, 0, st,
-      reinterpret_cast<const __nv_bfloat16*>(d_o), reinterpret_cast<const __nv_bfloat16*>(o), dsum_scratch, rows,
-      dqn, dkvn, static_cast<long>(B) * N * 128 / 4);
-  OMLM_LAUNCH_CHECK();
-  CUtensorMap tmQ, tmDO, tmKV;
-  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
-  if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmDO, d_o, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
-  if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kBtBK);
-  if (rc) return rc;
   const int n_row_tiles = static_cast<int>((R + kBtBQ - 1) / kBtBQ);
   const int n_key_tiles = (N + kBtBK - 1) / kBtBK;
   // chunk length T: as long as the per-CTA diagonal table (heads x (64 T / heads + 130) floats) fits in shared memory,
   // and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
   auto wacc_of = [&](int T) { return (T * kBtBQ + heads - 1) / heads + kBtBK + 2; };
-  auto smem_of = [&](int T) { return kBoAcc + heads * wacc_of(T) * 4 + 1024; };
+  auto smem_of = [&](int T) { return det ? kBoAccDet + 2 * heads * wacc_of(T) * 4 + 1024 : kBoAcc + heads * wacc_of(T) * 4 + 1024; };
   auto units_of = [&](int T) {
     long units = 0;
     for (int kt = 0; kt < n_key_tiles; ++kt) {
@@ -301,16 +399,97 @@ extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o
     const int T = atoi(e);
     if (T >= 1 && T <= n_row_tiles && smem_of(T) <= kBtMaxSmem) tiles_per_chunk = T;
   }
-  const int smem_bytes = smem_of(tiles_per_chunk);
-  static int configured = 0;
-  if (configured < smem_bytes) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    configured = smem_bytes;
+  cfg->tiles_per_chunk = tiles_per_chunk;
+  cfg->wacc = wacc_of(tiles_per_chunk);
+  cfg->smem_bytes = smem_of(tiles_per_chunk);
+  cfg->units_per_batch = static_cast<int>(units_of(tiles_per_chunk));
+  cfg->n_row_tiles = n_row_tiles;
+  cfg->n_key_tiles = n_key_tiles;
+  return 0;
+}
+
+static int bt_ints(int B, const BtConfig& c) {     // turn counters, then the units' (dmin, width), then the error word
+  return B * c.n_row_tiles + 2 * B * c.n_key_tiles + 2 * B * c.units_per_batch + 1;
+}
+
+static int attn_bwd_tc_impl(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
+                            const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
+                            float* dqn, float* dkvn, float* dtable, int B, int N, int heads, float scale, bool det,
+                            float* ws, long ws_bytes, int* iws, long iws_count, void* stream) {
+  OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attn_bwd_tc: bad shape");
+  OMLM_CHECK_ARG(table_ld >= N, "attn_bwd_tc: bias table shorter than the sequence");
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  const long R = static_cast<long>(N) * heads;
+  const long rows = static_cast<long>(B) * R;
+  BtConfig cfg;
+  int rc = bt_config(B, N, heads, det, &cfg);
+  if (rc) return rc;
+  const int units = B * cfg.units_per_batch;
+  BtDet dp{nullptr, nullptr, nullptr, nullptr, nullptr};
+  if (det) {
+    OMLM_CHECK_ARG(ws != nullptr && iws != nullptr && ws_bytes >= static_cast<long>(units) * heads * cfg.wacc * 4 &&
+                   iws_count >= bt_ints(B, cfg), "attn_bwd_tc_det: workspace too small (see omlm_attn_bwd_tc_det_workspace)");
+    dp.turn_dq = iws;
+    dp.turn_kv = iws + static_cast<long>(B) * cfg.n_row_tiles;
+    dp.meta = dp.turn_kv + 2L * B * cfg.n_key_tiles;
+    dp.err = iws + iws_count - 1;      // the caller's last int, whatever the buffer's size
+    dp.dpart = ws;
+    OMLM_CUDA(cudaMemsetAsync(iws, 0, (static_cast<long>(B) * cfg.n_row_tiles + 2L * B * cfg.n_key_tiles) * sizeof(int), st));
   }
-  const int units_per_batch = static_cast<int>(units_of(tiles_per_chunk));
-  OMLM_KLAUNCH((attn_bwd_tc_kernel), B * units_per_batch, kBtThreads, smem_bytes, st,
-      tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale,
-      wacc_of(tiles_per_chunk), tiles_per_chunk, B);
+  OMLM_KLAUNCH((attn_bwd_tc_dsum_kernel), static_cast<int>((rows * 8 + 255) / 256), 256, 0, st,
+      reinterpret_cast<const __nv_bfloat16*>(d_o), reinterpret_cast<const __nv_bfloat16*>(o), dsum_scratch, rows,
+      dqn, dkvn, static_cast<long>(B) * N * 128 / 4);
   OMLM_LAUNCH_CHECK();
+  CUtensorMap tmQ, tmDO, tmKV;
+  rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tmDO, d_o, 64, static_cast<uint64_t>(rows), 128, 64, kBtBQ);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kBtBK);
+  if (rc) return rc;
+  auto kern = det ? attn_bwd_tc_kernel<true> : attn_bwd_tc_kernel<false>;
+  static int configured[2] = {0, 0};
+  if (configured[det] < cfg.smem_bytes) {
+    OMLM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.smem_bytes));
+    configured[det] = cfg.smem_bytes;
+  }
+  OMLM_KLAUNCH((kern), units, kBtThreads, cfg.smem_bytes, st,
+      tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale,
+      cfg.wacc, cfg.tiles_per_chunk, B, dp);
+  OMLM_LAUNCH_CHECK();
+  if (det) {
+    OMLM_KLAUNCH((attn_bwd_dtable_reduce_kernel), (heads * N + 255) / 256, 256, 0, st,
+        static_cast<const float*>(dp.dpart), static_cast<const int*>(dp.meta), units, heads, cfg.wacc, dtable, table_ld, N);
+    OMLM_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+}  // namespace omlm
+
+extern "C" int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
+                                const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
+                                float* dqn, float* dkvn, float* dtable, int B, int N, int heads,
+                                float scale, void* stream) {
+  return omlm::attn_bwd_tc_impl(qn, kvn, d_o, o, lse2, table, table_ld, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads,
+                                scale, false, nullptr, 0, nullptr, 0, stream);
+}
+
+extern "C" int omlm_attn_bwd_tc_det(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
+                                    const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
+                                    float* dqn, float* dkvn, float* dtable, int B, int N, int heads, float scale,
+                                    float* ws, long ws_bytes, int* iws, long iws_count, void* stream) {
+  return omlm::attn_bwd_tc_impl(qn, kvn, d_o, o, lse2, table, table_ld, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads,
+                                scale, true, ws, ws_bytes, iws, iws_count, stream);
+}
+
+extern "C" int omlm_attn_bwd_tc_det_workspace(int B, int N, int heads, long* ws_bytes, long* iws_count) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0 && ws_bytes != nullptr && iws_count != nullptr, "attn_bwd_tc_det_workspace: bad arguments");
+  BtConfig cfg;
+  const int rc = bt_config(B, N, heads, true, &cfg);
+  if (rc) return rc;
+  *ws_bytes = static_cast<long>(B) * cfg.units_per_batch * heads * cfg.wacc * 4;
+  *iws_count = bt_ints(B, cfg);
   return 0;
 }

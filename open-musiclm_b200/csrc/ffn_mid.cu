@@ -179,11 +179,13 @@ __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc, bool
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(n) : "memory");
 }
 
-template <bool F16>
+// DET: no atomics -- the warps' sums are combined in warp order and written to this CTA's row blockIdx.x of part
+// [gridDim.x, 7F] in the parameters' layouts (dgamma [F] | dconv_w [2F, 3]); omlm_colsum adds the rows in order.
+template <bool F16, bool DET>
 __global__ void __launch_bounds__(kTileThreads, 2)
 ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, const float2* __restrict__ stats,
                         const float2* __restrict__ rowstat, const int parts, __nv_bfloat16* __restrict__ du,
-                        float* __restrict__ dgamma, float* __restrict__ dconv_w) {
+                        float* __restrict__ dgamma, float* __restrict__ dconv_w, float* __restrict__ part) {
   pdl_prologue();
   extern __shared__ __align__(16) uint8_t tsm[];
   uint8_t* su = tsm + kTOffU;
@@ -340,30 +342,60 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
       da2[q] = da1[q]; da1[q] = da0[q]; dg2[q] = dg1[q]; dg1[q] = dg0[q];
     }
   }
-  // ---- weight gradients: warps combine in shared memory, one global atomic per (channel, tap) and CTA
+  if constexpr (DET) {
+    __syncthreads();                                      // every warp is done with the u tile: reuse it
+    float* wsum = reinterpret_cast<float*>(su);           // [warps][7][128]
+    float* ws = wsum + warp * 7 * 128;
 #pragma unroll
-  for (int q = 0; q < 2; ++q) {
-    atomicAdd(&sacc[lane * 4 + 2 * q], dgam[q].x);
-    atomicAdd(&sacc[lane * 4 + 2 * q + 1], dgam[q].y);
+    for (int q = 0; q < 2; ++q) {
+      ws[lane * 4 + 2 * q] = dgam[q].x;
+      ws[lane * 4 + 2 * q + 1] = dgam[q].y;
 #pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      atomicAdd(&sacc[(1 + k) * 128 + lane * 4 + 2 * q], dwa[k][q].x);
-      atomicAdd(&sacc[(1 + k) * 128 + lane * 4 + 2 * q + 1], dwa[k][q].y);
-      atomicAdd(&sacc[(4 + k) * 128 + lane * 4 + 2 * q], dwg[k][q].x);
-      atomicAdd(&sacc[(4 + k) * 128 + lane * 4 + 2 * q + 1], dwg[k][q].y);
+      for (int k = 0; k < 3; ++k) {
+        ws[(1 + k) * 128 + lane * 4 + 2 * q] = dwa[k][q].x;
+        ws[(1 + k) * 128 + lane * 4 + 2 * q + 1] = dwa[k][q].y;
+        ws[(4 + k) * 128 + lane * 4 + 2 * q] = dwg[k][q].x;
+        ws[(4 + k) * 128 + lane * 4 + 2 * q + 1] = dwg[k][q].y;
+      }
     }
-  }
-  __syncthreads();
-  // parameter gradients in the parameters' own layout: inner gamma [F]; conv taps [2F, 3] with the value half in rows
-  // [0, F) and the gate half in rows [F, 2F) (transformer.py:122-137) -- accumulated (+=), padded channels dropped
-  for (int i = tid; i < 7 * 128; i += kTileThreads) {
-    const int q = i >> 7, ch = g * 128 + (i & 127);
-    if (ch >= a.F) continue;
-    const float v = sacc[i];
-    if (q == 0) atomicAdd(&dgamma[ch], v);
-    else if (dconv_w != nullptr) {
-      if (q < 4) atomicAdd(&dconv_w[static_cast<long>(ch) * 3 + (q - 1)], v);
-      else atomicAdd(&dconv_w[(static_cast<long>(a.F) + ch) * 3 + (q - 4)], v);
+    __syncthreads();
+    float* prow = part + static_cast<long>(blockIdx.x) * 7 * a.F;
+    for (int i = tid; i < 7 * 128; i += kTileThreads) {
+      const int q = i >> 7, ch = g * 128 + (i & 127);
+      if (ch >= a.F) continue;
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < kTileWarps; ++w) v += wsum[w * 7 * 128 + i];
+      if (q == 0) prow[ch] = v;
+      else if (q < 4) prow[a.F + static_cast<long>(ch) * 3 + (q - 1)] = v;
+      else prow[a.F + (static_cast<long>(a.F) + ch) * 3 + (q - 4)] = v;
+    }
+  } else {
+    // ---- weight gradients: warps combine in shared memory, one global atomic per (channel, tap) and CTA
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      atomicAdd(&sacc[lane * 4 + 2 * q], dgam[q].x);
+      atomicAdd(&sacc[lane * 4 + 2 * q + 1], dgam[q].y);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        atomicAdd(&sacc[(1 + k) * 128 + lane * 4 + 2 * q], dwa[k][q].x);
+        atomicAdd(&sacc[(1 + k) * 128 + lane * 4 + 2 * q + 1], dwa[k][q].y);
+        atomicAdd(&sacc[(4 + k) * 128 + lane * 4 + 2 * q], dwg[k][q].x);
+        atomicAdd(&sacc[(4 + k) * 128 + lane * 4 + 2 * q + 1], dwg[k][q].y);
+      }
+    }
+    __syncthreads();
+    // parameter gradients in the parameters' own layout: inner gamma [F]; conv taps [2F, 3] with the value half in rows
+    // [0, F) and the gate half in rows [F, 2F) (transformer.py:122-137) -- accumulated (+=), padded channels dropped
+    for (int i = tid; i < 7 * 128; i += kTileThreads) {
+      const int q = i >> 7, ch = g * 128 + (i & 127);
+      if (ch >= a.F) continue;
+      const float v = sacc[i];
+      if (q == 0) atomicAdd(&dgamma[ch], v);
+      else if (dconv_w != nullptr) {
+        if (q < 4) atomicAdd(&dconv_w[static_cast<long>(ch) * 3 + (q - 1)], v);
+        else atomicAdd(&dconv_w[(static_cast<long>(a.F) + ch) * 3 + (q - 4)], v);
+      }
     }
   }
 }
@@ -389,9 +421,10 @@ int omlm_ffn_norm_fwd(const void* h, const float* rowsum, const float* gamma, vo
   return 0;
 }
 
-int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
-                     const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
-                     float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, void* stream) {
+static int ffn_mid_bwd_impl(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
+                            const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
+                            float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, float* part, long part_bytes,
+                            void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(B > 0 && N > 0 && F > 0 && Fp >= F && Fp % 128 == 0, "ffn_mid_bwd: bad shape F=%d Fp=%d", F, Fp);
   OMLM_CHECK_ARG(drop_p >= 0.f && drop_p < 1.f && (drop_p == 0.f || keep_bits != nullptr), "ffn_mid_bwd: dropout needs keep_bits");
@@ -399,7 +432,12 @@ int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float
   MidArgs a{reinterpret_cast<const __nv_bfloat16*>(u), conv_w, gamma, N, F, Fp, drop_p, reinterpret_cast<const uint8_t*>(keep_bits)};
   const long M = static_cast<long>(B) * N;
   auto stats_kern = ffn_mid_bwd_stats_kernel;
-  auto walk_kern = act_f16 ? ffn_mid_bwd_walk_kernel<true> : ffn_mid_bwd_walk_kernel<false>;
+  const bool det = part != nullptr;
+  auto walk_kern = act_f16 ? (det ? ffn_mid_bwd_walk_kernel<true, true> : ffn_mid_bwd_walk_kernel<true, false>)
+                           : (det ? ffn_mid_bwd_walk_kernel<false, true> : ffn_mid_bwd_walk_kernel<false, false>);
+  const int row_blocks = B * ((N + kTileRows - 1) / kTileRows);
+  if (det) OMLM_CHECK_ARG(part_bytes >= static_cast<long>(row_blocks) * 7 * F * 4, "ffn_mid_bwd_det: partials need %ld bytes",
+                          static_cast<long>(row_blocks) * 7 * F * 4);
   OMLM_CHECK_ARG(rowstat_parts >= 0 && rowstat != nullptr, "ffn_mid_bwd: rowstat buffer / parts");
   if (rowstat_parts == 0) {      // no partial sums from the d_hn GEMM: one pass over (dhn, hn) here
     OMLM_KLAUNCH((stats_kern), static_cast<int>((M + 7) / 8), 256, 0, st,
@@ -410,17 +448,41 @@ int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float
   }
   static bool configured = false;
   if (!configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
-    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
+    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
+    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
+    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
+    OMLM_CUDA(cudaFuncSetAttribute(ffn_mid_bwd_walk_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileSmem));
     configured = true;
   }
-  dim3 grid(B * ((N + kTileRows - 1) / kTileRows), Fp / 128);
+  dim3 grid(row_blocks, Fp / 128);
   OMLM_KLAUNCH((walk_kern), grid, kTileThreads, kTileSmem, st, a, reinterpret_cast<const __nv_bfloat16*>(dhn),
                                                                 reinterpret_cast<const float2*>(stats),
                                                                 reinterpret_cast<const float2*>(rowstat), rowstat_parts,
-                                                                reinterpret_cast<__nv_bfloat16*>(du), dgamma, dconv_w);
+                                                                reinterpret_cast<__nv_bfloat16*>(du), dgamma, dconv_w, part);
   OMLM_LAUNCH_CHECK();
+  if (det) {
+    const int rc = omlm_colsum(part, 7L * F, 1, dgamma, row_blocks, F, 1, stream);
+    if (rc || dconv_w == nullptr) return rc;
+    return omlm_colsum(part + F, 7L * F, 1, dconv_w, row_blocks, 6 * F, 1, stream);
+  }
   return 0;
+}
+
+int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
+                     const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
+                     float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, void* stream) {
+  return ffn_mid_bwd_impl(dhn, hn, u, stats, conv_w, gamma, keep_bits, rowstat, rowstat_parts, du, dgamma, dconv_w, B, N, F, Fp,
+                          drop_p, act_f16, nullptr, 0, stream);
+}
+
+int omlm_ffn_mid_bwd_det(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
+                         const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
+                         float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, float* part_ws, long part_ws_bytes,
+                         void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(part_ws != nullptr, "ffn_mid_bwd_det: no partials buffer");
+  return ffn_mid_bwd_impl(dhn, hn, u, stats, conv_w, gamma, keep_bits, rowstat, rowstat_parts, du, dgamma, dconv_w, B, N, F, Fp,
+                          drop_p, act_f16, part_ws, part_ws_bytes, stream);
 }
 
 }  // extern "C"

@@ -17,6 +17,7 @@
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
 #include <stdlib.h>
+#include <algorithm>
 
 namespace omlm {
 
@@ -32,6 +33,7 @@ struct EpiParams {
   float alpha;
   int out_f32;    // 0: bf16, 1: fp32
   int atomic;     // 1: red.add into fp32 out (split-K)
+  long split_stride;   // > 0 (deterministic split-K): split s stores its fp32 partial at out + s * split_stride, no atomics
   int vec_ok;     // out / addend rows 16-byte aligned: column pairs move as one vector
   int row_split;  // >0: rows are two halves of row_split, each with row_valid live rows; <0: interleaved GEGLU groups of 128
   int row_valid;
@@ -252,7 +254,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
             else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
           } else if (ep.out_f32) {
-            float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
+            float* op = reinterpret_cast<float*>(ep.out) + split * ep.split_stride + orow[hr] + col;
             if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
             else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
           } else {
@@ -314,7 +316,7 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
                        long ldb, int M, int N, int K, void* out, int out_f32, long ldo,
                        const float* addend, long ldadd, float alpha, int splits,
                        int row_split, int row_valid, int n_valid, int block_n, int max_ctas,
-                       void* stream_, const omlm::RowStatArgs* rs) {
+                       void* stream_, const omlm::RowStatArgs* rs, long split_stride = 0) {
   using namespace omlm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   OMLM_CHECK_ARG(M > 0 && N > 0 && K > 0, "gemm: empty problem %d x %d x %d", M, N, K);
@@ -322,6 +324,7 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   OMLM_CHECK_ARG(splits >= 1, "gemm: splits must be >= 1");
   OMLM_CHECK_ARG((a_f16 != 0) == (b_f16 != 0), "gemm: both operands must have the same 16-bit format (one wgmma takes one operand format)");
   OMLM_CHECK_ARG(splits == 1 || (out_f32 && addend == nullptr), "gemm: split-K needs fp32 atomic output and no addend");
+  OMLM_CHECK_ARG(split_stride == 0 || (out_f32 && addend == nullptr && rs == nullptr), "gemm: partial slices need fp32 output");
   if (n_valid <= 0 || n_valid > N) n_valid = N;
   {  // every split must own at least one k-block (an empty split would publish an unwritten accumulator)
     const int kb_total = (K + BK - 1) / BK;
@@ -339,7 +342,7 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   if (rc) return rc;
   EpiParams ep;
   ep.out = out; ep.addend = addend; ep.ldo = ldo; ep.ldadd = ldadd; ep.alpha = alpha;
-  ep.out_f32 = out_f32; ep.atomic = splits > 1 ? 1 : 0;
+  ep.out_f32 = out_f32; ep.atomic = (splits > 1 && split_stride == 0) ? 1 : 0; ep.split_stride = split_stride;
   const long esz = out_f32 ? 4 : 2;
   ep.vec_ok = ((ldo * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
               (addend == nullptr || ((ldadd * 4) % 16 == 0 && (reinterpret_cast<uintptr_t>(addend) & 15) == 0));
@@ -378,6 +381,77 @@ extern "C" int omlm_gemm16(const void* A, int a_f16, int a_mn_major, long lda, c
                            void* stream_) {
   return gemm16_impl(A, a_f16, a_mn_major, lda, B, b_f16, b_mn_major, ldb, M, N, K, out, out_f32, ldo, addend, ldadd, alpha, splits,
                      row_split, row_valid, n_valid, block_n, max_ctas, stream_, nullptr);
+}
+
+namespace omlm {
+// out[r, c] = out[r, c] + part[0][r, c] + part[1][r, c] + ... (split order) over rows_out x n_valid
+__global__ void __launch_bounds__(256)
+splitk_reduce_kernel(float* __restrict__ out, long ldo, const float* __restrict__ part, long slice, long ldp, int splits,
+                     int rows_out, int n_valid) {
+  pdl_prologue();
+  const long total = static_cast<long>(rows_out) * n_valid;
+  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
+    const long r = i / n_valid, c = i - r * n_valid;
+    float v = out[r * ldo + c];
+    for (int s = 0; s < splits; ++s) v += part[s * slice + r * ldp + c];
+    out[r * ldo + c] = v;
+  }
+}
+
+// rows of the output a GEMM with this row remap writes (row_split > 0: whole halves of row_split rows, row_valid live
+// rows each; < 0: value and gate halves of row_valid channels; 0: M)
+static int gemm_rows_out(int M, int row_split, int row_valid) {
+  if (row_split > 0) return (M + row_split - 1) / row_split * row_valid;
+  if (row_split < 0) return 2 * row_valid;
+  return M;
+}
+
+static int gemm_splits_effective(int K, int splits) {   // the clamp of gemm16_impl: every split owns >= 1 k-block
+  const int kb_total = (K + BK - 1) / BK;
+  if (splits > kb_total) splits = kb_total;
+  if (splits < 1) splits = 1;
+  const int per = (kb_total + splits - 1) / splits;
+  return (kb_total + per - 1) / per;
+}
+}  // namespace omlm
+
+extern "C" int omlm_gemm16_splitk_det_workspace(int M, int N, int K, int splits, int row_split, int row_valid, int n_valid,
+                                                long* part_bytes) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && N > 0 && K > 0 && splits >= 1 && part_bytes != nullptr, "gemm16_splitk_det_workspace: bad arguments");
+  if (n_valid <= 0 || n_valid > N) n_valid = N;
+  OMLM_CHECK_ARG(row_split <= 0 || M % row_split == 0, "gemm16_splitk_det: M (%d) must be whole halves of row_split (%d)", M, row_split);
+  const int s = gemm_splits_effective(K, splits);
+  *part_bytes = s > 1 ? static_cast<long>(s) * gemm_rows_out(M, row_split, row_valid) * ((n_valid + 3) / 4 * 4) * 4 : 0;
+  return 0;
+}
+
+extern "C" int omlm_gemm16_splitk_det(const void* A, int a_f16, int a_mn_major, long lda, const void* B, int b_f16, int b_mn_major,
+                                      long ldb, int M, int N, int K, float* out, long ldo, int splits, int row_split, int row_valid,
+                                      int n_valid, int block_n, int max_ctas, float* part_ws, long part_ws_bytes, void* stream_) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && N > 0 && K > 0 && splits >= 1, "gemm16_splitk_det: empty problem %d x %d x %d", M, N, K);
+  if (n_valid <= 0 || n_valid > N) n_valid = N;
+  const int s = gemm_splits_effective(K, splits);
+  // every partial row the reduction reads must be written by some split: a remap of row_split > 0 needs whole halves
+  OMLM_CHECK_ARG(row_split <= 0 || M % row_split == 0, "gemm16_splitk_det: M (%d) must be whole halves of row_split (%d)", M, row_split);
+  if (s == 1)         // one split: the plain in-place accumulation (out += A B through the addend)
+    return gemm16_impl(A, a_f16, a_mn_major, lda, B, b_f16, b_mn_major, ldb, M, N, K, out, 1, ldo, out, ldo, 1.f, 1,
+                       row_split, row_valid, n_valid, block_n, max_ctas, stream_, nullptr);
+  const int rows_out = gemm_rows_out(M, row_split, row_valid);
+  const long ldp = (n_valid + 3) / 4 * 4;
+  const long slice = static_cast<long>(rows_out) * ldp;
+  OMLM_CHECK_ARG(part_ws != nullptr && part_ws_bytes >= s * slice * 4 && (reinterpret_cast<uintptr_t>(part_ws) & 15) == 0,
+                 "gemm16_splitk_det: partials need %ld bytes (16-byte aligned), got %ld", s * slice * 4, part_ws_bytes);
+  int rc = gemm16_impl(A, a_f16, a_mn_major, lda, B, b_f16, b_mn_major, ldb, M, N, K, part_ws, 1, ldp, nullptr, 0, 1.f, s,
+                       row_split, row_valid, n_valid, block_n, max_ctas, stream_, nullptr, slice);
+  if (rc) return rc;
+  const long total = static_cast<long>(rows_out) * n_valid;
+  const int grid = static_cast<int>(std::min<long>((total + 255) / 256, static_cast<long>(num_sms()) * 8));
+  OMLM_KLAUNCH((splitk_reduce_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream_), out, ldo,
+               static_cast<const float*>(part_ws), slice, ldp, s, rows_out, n_valid);
+  OMLM_LAUNCH_CHECK();
+  return 0;
 }
 
 extern "C" int omlm_gemm16_rowstat(const void* A, int a_f16, int a_mn_major, long lda, const void* B, int b_f16, int b_mn_major,

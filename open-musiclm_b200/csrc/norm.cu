@@ -89,14 +89,16 @@ __device__ __forceinline__ void ln_cp8(void* dst, const void* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(dst))), "l"(src) : "memory");
 }
 
-template <int NCHUNK, int WARPS>
+// DET: no atomics -- the warps' dgamma sums are combined in warp order and written as this block's row of part
+// [gridDim.x, D]; omlm_colsum then adds the rows to dgamma in block order.
+template <int NCHUNK, int WARPS, bool DET>
 __global__ void __launch_bounds__(WARPS * 32)
 layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restrict__ x,
                      const float2* __restrict__ stats, const float* __restrict__ gamma,
                      const float* __restrict__ dres, const __nv_bfloat16* __restrict__ draw,
                      const int* __restrict__ src_row, float* __restrict__ dx,
                      __nv_bfloat16* __restrict__ dx_bf16, float* __restrict__ dgamma, int M, int D,
-                     int rows_per_block) {
+                     int rows_per_block, float* __restrict__ part) {
   pdl_prologue();
   constexpr int kRow = NCHUNK * 128;                 // padded row length in elements
   constexpr int kStage = kRow * 12;                  // x fp32 | dres fp32 | dy bf16 | draw bf16
@@ -200,16 +202,30 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restri
     }
     d_cur = d_nxt; d_nxt = d_nn;
   }
+  if constexpr (DET) {
+    __syncthreads();                                  // every warp is done with its stage buffers: reuse them
+    float* wdg = reinterpret_cast<float*>(lsm);       // [WARPS][kRow]
 #pragma unroll
-  for (int c = 0; c < NCHUNK; ++c) {
-    const int col = (c * 32 + lane) * 4;
-    atomicAdd(&sdg[col + 0], dg[c].x);
-    atomicAdd(&sdg[col + 1], dg[c].y);
-    atomicAdd(&sdg[col + 2], dg[c].z);
-    atomicAdd(&sdg[col + 3], dg[c].w);
+    for (int c = 0; c < NCHUNK; ++c) *reinterpret_cast<float4*>(wdg + warp * kRow + (c * 32 + lane) * 4) = dg[c];
+    __syncthreads();
+    for (int i = threadIdx.x; i < D; i += WARPS * 32) {
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < WARPS; ++w) v += wdg[w * kRow + i];
+      part[static_cast<long>(blockIdx.x) * D + i] = v;
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < NCHUNK; ++c) {
+      const int col = (c * 32 + lane) * 4;
+      atomicAdd(&sdg[col + 0], dg[c].x);
+      atomicAdd(&sdg[col + 1], dg[c].y);
+      atomicAdd(&sdg[col + 2], dg[c].z);
+      atomicAdd(&sdg[col + 3], dg[c].w);
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < D; i += WARPS * 32) atomicAdd(&dgamma[i], sdg[i]);
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < D; i += WARPS * 32) atomicAdd(&dgamma[i], sdg[i]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -267,14 +283,18 @@ qk_l2norm_fwd_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat1
 // l2norm * scale backward.  y = s * x/|x|.  dx = (s*dy - xh * (xh . s*dy)) / |x| ;  ds += dy * xh.
 // dqn: fp32 [M, h*64] (atomically accumulated by the attention backward); dkvn: fp32 [M, 128].
 // Outputs bf16 dq_raw [M, h*64], dkv_raw [M, 128] (value gradient passes through).
+// DET: the 32 vector slots of a block are combined in slot order and written as this block's row of part [gridDim.x,
+// 128] (q scale | k scale); omlm_colsum adds the rows in block order.
+template <bool DET>
 __global__ void __launch_bounds__(256)
 qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dkvn,
                      const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16* __restrict__ kv_raw,
                      const float* __restrict__ q_scale, const float* __restrict__ k_scale,
                      __nv_bfloat16* __restrict__ dq_raw, __nv_bfloat16* __restrict__ dkv_raw,
-                     float* __restrict__ dq_scale, float* __restrict__ dk_scale, int M, int h) {
+                     float* __restrict__ dq_scale, float* __restrict__ dk_scale, int M, int h, float* __restrict__ part) {
   pdl_prologue();
   __shared__ float sds[2][64];
+  __shared__ float sslot[DET ? 2 * 32 * 64 : 1];
   if (threadIdx.x < 128) sds[threadIdx.x >> 6][threadIdx.x & 63] = 0.f;
   __syncthreads();
   const int sub = threadIdx.x & 7;
@@ -354,14 +374,27 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
       *reinterpret_cast<uint4*>(dst + sub * 8) = ov;
     }
   }
+  if constexpr (DET) {
+    const int slot = threadIdx.x >> 3;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    atomicAdd(&sds[0][sub * 8 + i], dsq[i]);
-    atomicAdd(&sds[1][sub * 8 + i], dsk[i]);
+    for (int i = 0; i < 8; ++i) { sslot[slot * 64 + sub * 8 + i] = dsq[i]; sslot[(32 + slot) * 64 + sub * 8 + i] = dsk[i]; }
+    __syncthreads();
+    if (threadIdx.x < 128) {
+      const int k = threadIdx.x >> 6, c = threadIdx.x & 63;
+      float v = 0.f;
+      for (int sl = 0; sl < 32; ++sl) v += sslot[(k * 32 + sl) * 64 + c];
+      part[static_cast<long>(blockIdx.x) * 128 + threadIdx.x] = v;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      atomicAdd(&sds[0][sub * 8 + i], dsq[i]);
+      atomicAdd(&sds[1][sub * 8 + i], dsk[i]);
+    }
+    __syncthreads();
+    if (threadIdx.x < 64) atomicAdd(&dq_scale[threadIdx.x], sds[0][threadIdx.x]);
+    else if (threadIdx.x < 128) atomicAdd(&dk_scale[threadIdx.x - 64], sds[1][threadIdx.x - 64]);
   }
-  __syncthreads();
-  if (threadIdx.x < 64) atomicAdd(&dq_scale[threadIdx.x], sds[0][threadIdx.x]);
-  else if (threadIdx.x < 128) atomicAdd(&dk_scale[threadIdx.x - 64], sds[1][threadIdx.x - 64]);
 }
 
 template <int NCHUNK>
@@ -374,16 +407,17 @@ static int launch_ln_fwd(const float* x, const float* gamma, __nv_bfloat16* y, _
   return 0;
 }
 
-template <int NCHUNK>
+template <int NCHUNK, bool DET = false>
 static int launch_ln_bwd(const __nv_bfloat16* dy, const float* x, const float2* stats, const float* gamma,
                          const float* dres, const __nv_bfloat16* draw, const int* src_row, float* dx,
-                         __nv_bfloat16* dx_bf16, float* dgamma, int M, int D, cudaStream_t st) {
+                         __nv_bfloat16* dx_bf16, float* dgamma, int M, int D, cudaStream_t st, float* part = nullptr,
+                         long part_bytes = 0) {
   // shared memory (2 stages of 12 B/element per warp) decides residency: 8 warps up to D = 1024, 4 above
   constexpr int WARPS = NCHUNK <= 8 ? 8 : 4;
   constexpr int smem = WARPS * 2 * NCHUNK * 128 * 12 + NCHUNK * 128 * 4;
   static bool configured = false;
   if (!configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(layernorm_bwd_kernel<NCHUNK, WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    OMLM_CUDA(cudaFuncSetAttribute(layernorm_bwd_kernel<NCHUNK, WARPS, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
   const int per_sm = std::max(1, std::min(4, (220 * 1024) / smem));
@@ -391,9 +425,12 @@ static int launch_ln_bwd(const __nv_bfloat16* dy, const float* x, const float2* 
   int rows_per_block = (M + blocks - 1) / blocks;
   if (rows_per_block < WARPS) rows_per_block = WARPS;
   blocks = (M + rows_per_block - 1) / rows_per_block;
-  OMLM_KLAUNCH((layernorm_bwd_kernel<NCHUNK, WARPS>), blocks, WARPS * 32, smem, st, dy, x, stats, gamma, dres, draw, src_row, dx,
-                                                                       dx_bf16, dgamma, M, D, rows_per_block);
+  if (DET) OMLM_CHECK_ARG(part != nullptr && part_bytes >= static_cast<long>(blocks) * D * 4,
+                          "layernorm_bwd_det: partials need %ld bytes", static_cast<long>(blocks) * D * 4);
+  OMLM_KLAUNCH((layernorm_bwd_kernel<NCHUNK, WARPS, DET>), blocks, WARPS * 32, smem, st, dy, x, stats, gamma, dres, draw, src_row, dx,
+                                                                       dx_bf16, dgamma, M, D, rows_per_block, part);
   OMLM_LAUNCH_CHECK();
+  if (DET) return omlm_colsum(part, D, 1, dgamma, blocks, D, 1, st);
   return 0;
 }
 
@@ -436,6 +473,24 @@ int omlm_layernorm_bwd(const void* dy_bf16, const float* x, const float* stats, 
   return launch_ln_bwd<16>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st);
 }
 
+int omlm_layernorm_bwd_det(const void* dy_bf16, const float* x, const float* stats, const float* gamma,
+                           const float* dres, const void* draw_bf16, const int* src_row, float* dx,
+                           void* dx_bf16, float* dgamma, int M, int D, float* part_ws, long part_ws_bytes, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0 && D <= 2048, "layernorm_bwd_det: unsupported shape %d x %d", M, D);
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  auto dy = reinterpret_cast<const __nv_bfloat16*>(dy_bf16);
+  auto dr = reinterpret_cast<const __nv_bfloat16*>(draw_bf16);
+  auto s2 = reinterpret_cast<const float2*>(stats);
+  auto dxb = reinterpret_cast<__nv_bfloat16*>(dx_bf16);
+  const int nchunk = (D + 127) / 128;
+  if (nchunk <= 1) return launch_ln_bwd<1, true>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st, part_ws, part_ws_bytes);
+  if (nchunk <= 2) return launch_ln_bwd<2, true>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st, part_ws, part_ws_bytes);
+  if (nchunk <= 4) return launch_ln_bwd<4, true>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st, part_ws, part_ws_bytes);
+  if (nchunk <= 8) return launch_ln_bwd<8, true>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st, part_ws, part_ws_bytes);
+  return launch_ln_bwd<16, true>(dy, x, s2, gamma, dres, dr, src_row, dx, dxb, dgamma, M, D, st, part_ws, part_ws_bytes);
+}
+
 int omlm_qk_l2norm_fwd(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale,
                        void* qn, void* kvn, int M, int heads, void* stream) {
   using namespace omlm;
@@ -449,21 +504,45 @@ int omlm_qk_l2norm_fwd(const void* q_raw, const void* kv_raw, const float* q_sca
   return 0;
 }
 
-int omlm_qk_l2norm_bwd(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
-                       const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
-                       float* dq_scale, float* dk_scale, int M, int heads, void* stream) {
+static int qk_l2norm_bwd_impl(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
+                              const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
+                              float* dq_scale, float* dk_scale, int M, int heads, float* part, long part_bytes, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(M > 0 && heads > 0, "qk_l2norm_bwd: bad shape");
   const long long total = static_cast<long long>(M) * (heads + 2);
   long long blocks = (total + 31) / 32;
   const long long cap = static_cast<long long>(num_sms()) * 8;
   if (blocks > cap) blocks = cap;
-  OMLM_KLAUNCH((qk_l2norm_bwd_kernel), static_cast<int>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream), 
+  const bool det = part != nullptr;
+  if (det) OMLM_CHECK_ARG(part_bytes >= blocks * 128 * 4, "qk_l2norm_bwd_det: partials need %lld bytes", blocks * 128 * 4);
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  OMLM_KLAUNCH((det ? qk_l2norm_bwd_kernel<true> : qk_l2norm_bwd_kernel<false>), static_cast<int>(blocks), 256, 0, st,
       dqn, dkvn, reinterpret_cast<const __nv_bfloat16*>(q_raw), reinterpret_cast<const __nv_bfloat16*>(kv_raw),
       q_scale, k_scale, reinterpret_cast<__nv_bfloat16*>(dq_raw), reinterpret_cast<__nv_bfloat16*>(dkv_raw),
-      dq_scale, dk_scale, M, heads);
+      dq_scale, dk_scale, M, heads, part);
   OMLM_LAUNCH_CHECK();
+  if (det) {
+    const int rc = omlm_colsum(part, 128, 1, dq_scale, static_cast<int>(blocks), 64, 1, stream);
+    if (rc) return rc;
+    return omlm_colsum(part + 64, 128, 1, dk_scale, static_cast<int>(blocks), 64, 1, stream);
+  }
   return 0;
+}
+
+int omlm_qk_l2norm_bwd(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
+                       const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
+                       float* dq_scale, float* dk_scale, int M, int heads, void* stream) {
+  return qk_l2norm_bwd_impl(dqn, dkvn, q_raw, kv_raw, q_scale, k_scale, dq_raw, dkv_raw, dq_scale, dk_scale, M, heads,
+                            nullptr, 0, stream);
+}
+
+int omlm_qk_l2norm_bwd_det(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
+                           const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
+                           float* dq_scale, float* dk_scale, int M, int heads, float* part_ws, long part_ws_bytes, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(part_ws != nullptr, "qk_l2norm_bwd_det: no partials buffer");
+  return qk_l2norm_bwd_impl(dqn, dkvn, q_raw, kv_raw, q_scale, k_scale, dq_raw, dkv_raw, dq_scale, dk_scale, M, heads,
+                            part_ws, part_ws_bytes, stream);
 }
 
 }  // extern "C"

@@ -11,9 +11,10 @@
 
 namespace omlm {
 
-// acc[0] (double) += sum (g * prescale)^2
+// acc[0] (double) += sum (g * prescale)^2.  part != nullptr (deterministic): the block's sum goes to part[blockIdx.x]
+// instead, and sumsq_finish_kernel adds the blocks' sums to acc in block order.
 __global__ void __launch_bounds__(512)
-sumsq_kernel(const float* __restrict__ g, long n, float prescale, double* __restrict__ acc) {
+sumsq_kernel(const float* __restrict__ g, long n, float prescale, double* __restrict__ acc, double* __restrict__ part) {
   pdl_prologue();
   float s = 0.f;
   const long n4 = n >> 2;
@@ -30,8 +31,20 @@ sumsq_kernel(const float* __restrict__ g, long n, float prescale, double* __rest
   if (threadIdx.x < 32) {
     float v = threadIdx.x < 16 ? red[threadIdx.x] : 0.f;
     v = warp_sum(v);
-    if (threadIdx.x == 0) atomicAdd(acc, static_cast<double>(v) * prescale * prescale);
+    if (threadIdx.x == 0) {
+      if (part != nullptr) part[blockIdx.x] = static_cast<double>(v) * prescale * prescale;
+      else atomicAdd(acc, static_cast<double>(v) * prescale * prescale);
+    }
   }
+}
+
+__global__ void __launch_bounds__(32) sumsq_finish_kernel(const double* __restrict__ part, int n, double* __restrict__ acc) {
+  pdl_prologue();
+  double s = 0.0;
+  for (int i = threadIdx.x; i < n; i += 32) s += part[i];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (threadIdx.x == 0) acc[0] += s;
 }
 
 // hyper: [0] lr  [1] beta1  [2] beta2  [3] eps  [4] weight_decay  [5] 1-beta1^t  [6] 1-beta2^t
@@ -231,7 +244,21 @@ int omlm_grad_sumsq(const float* g, long n, float prescale, double* acc, void* s
   OMLM_CHECK_ARG(n > 0, "grad_sumsq: empty");
   OMLM_CHECK_ARG((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grad_sumsq: arena must be 16B aligned");
   const int blocks = static_cast<int>(std::min<long>((n / 4 + 511) / 512 + 1, static_cast<long>(num_sms()) * 4));
-  OMLM_KLAUNCH((sumsq_kernel), blocks, 512, 0, reinterpret_cast<cudaStream_t>(stream), g, n, prescale, acc);
+  OMLM_KLAUNCH((sumsq_kernel), blocks, 512, 0, reinterpret_cast<cudaStream_t>(stream), g, n, prescale, acc, nullptr);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+
+int omlm_grad_sumsq_det(const float* g, long n, float prescale, double* acc, double* part_ws, long part_ws_bytes, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(n > 0, "grad_sumsq_det: empty");
+  OMLM_CHECK_ARG((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grad_sumsq_det: arena must be 16B aligned");
+  const int blocks = static_cast<int>(std::min<long>((n / 4 + 511) / 512 + 1, static_cast<long>(num_sms()) * 4));
+  OMLM_CHECK_ARG(part_ws != nullptr && part_ws_bytes >= blocks * 8L, "grad_sumsq_det: partials need %ld bytes", blocks * 8L);
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  OMLM_KLAUNCH((sumsq_kernel), blocks, 512, 0, st, g, n, prescale, acc, part_ws);
+  OMLM_LAUNCH_CHECK();
+  OMLM_KLAUNCH((sumsq_finish_kernel), 1, 32, 0, st, static_cast<const double*>(part_ws), blocks, acc);
   OMLM_LAUNCH_CHECK();
   return 0;
 }

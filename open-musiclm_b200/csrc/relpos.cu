@@ -147,14 +147,14 @@ __global__ void arange_kernel(float* out, int n) {
 
 extern "C" {
 
-int omlm_sgemm_small(const float* A, long sa_m, long sa_k, const float* B, long sb_k, long sb_n, float* C,
-                     long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
-                     int accumulate, void* stream) {
+static int sgemm_small_impl(const float* A, long sa_m, long sa_k, const float* B, long sb_k, long sb_n, float* C,
+                            long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
+                            int accumulate, bool allow_split, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(M > 0 && N > 0 && K > 0, "sgemm_small: empty problem");
   dim3 grid((N + 63) / 64, (M + 63) / 64);
   // skinny problems with a long reduction (dW of the rel-pos MLP, the h-column table): split K over up to ~256 CTAs
-  if (accumulate && act == 0 && Z == nullptr && K >= 128) {
+  if (allow_split && accumulate && act == 0 && Z == nullptr && K >= 128) {
     const int ctas = static_cast<int>(grid.x * grid.y);
     if (ctas < 64) grid.z = static_cast<unsigned>(std::max(1, std::min((K + 31) / 32, 256 / ctas)));
   }
@@ -162,6 +162,18 @@ int omlm_sgemm_small(const float* A, long sa_m, long sa_k, const float* B, long 
       A, sa_m, sa_k, B, sb_k, sb_n, C, sc_m, sc_n, Z, bias, M, N, K, act, accumulate);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+int omlm_sgemm_small(const float* A, long sa_m, long sa_k, const float* B, long sb_k, long sb_n, float* C,
+                     long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
+                     int accumulate, void* stream) {
+  return sgemm_small_impl(A, sa_m, sa_k, B, sb_k, sb_n, C, sc_m, sc_n, Z, bias, M, N, K, act, accumulate, true, stream);
+}
+
+int omlm_sgemm_small_det(const float* A, long sa_m, long sa_k, const float* B, long sb_k, long sb_n, float* C,
+                         long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
+                         int accumulate, void* stream) {
+  return sgemm_small_impl(A, sa_m, sa_k, B, sb_k, sb_n, C, sc_m, sc_n, Z, bias, M, N, K, act, accumulate, false, stream);
 }
 
 int omlm_silu_bwd(const float* dA, const float* Z, float* dZ, void* dZ_bf16, long n, void* stream) {

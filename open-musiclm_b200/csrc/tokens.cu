@@ -151,6 +151,71 @@ __global__ void embed_scatter_kernel(float* __restrict__ dtable, const int* __re
   }
 }
 
+// Deterministic scatter-add: every destination row is summed by one warp, over its positions in ascending order.
+// Pass 1 records the first position of every row (integer atomicMin: order-independent); in pass 2 the warp of that
+// first position walks the remaining positions, adds the matching dx rows in order onto the table row and restores the
+// row's marker to INT_MAX.  The adds are the default kernel's (dst + dx * scale, each rounded), in position order.
+__global__ void embed_first_kernel(const int* __restrict__ src_row, int M, int rows, int* __restrict__ first) {
+  pdl_prologue();
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  const int r = src_row[m];
+  if (r >= 0 && r < rows) atomicMin(first + r, m);
+}
+
+template <int NCH>
+__global__ void __launch_bounds__(256)
+embed_scatter_det_kernel(float* __restrict__ dtable, const int* __restrict__ src_row, const float* __restrict__ dx, int M, int D,
+                         int rows, float scale, int* __restrict__ first) {
+  pdl_prologue();
+  const int lane = threadIdx.x & 31;
+  const int m = blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (m >= M) return;
+  const int r = src_row[m];
+  if (r < 0 || r >= rows || __ldcg(first + r) != m) return;
+  float* trow = dtable + static_cast<long long>(r) * D;
+  float4 acc[NCH];
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const int col = (c * 32 + lane) * 4;
+    acc[c] = col < D ? *reinterpret_cast<const float4*>(trow + col) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  for (int base = m; base < M; base += 32) {
+    const int idx = base + lane;
+    unsigned hit = __ballot_sync(0xffffffffu, idx < M && src_row[idx] == r);
+    while (hit) {
+      const int mm = base + __ffs(hit) - 1;
+      hit &= hit - 1;
+      const float* g = dx + static_cast<long long>(mm) * D;
+#pragma unroll
+      for (int c = 0; c < NCH; ++c) {
+        const int col = (c * 32 + lane) * 4;
+        if (col < D) {
+          const float4 v = *reinterpret_cast<const float4*>(g + col);
+          acc[c].x = __fadd_rn(acc[c].x, __fmul_rn(v.x, scale));
+          acc[c].y = __fadd_rn(acc[c].y, __fmul_rn(v.y, scale));
+          acc[c].z = __fadd_rn(acc[c].z, __fmul_rn(v.z, scale));
+          acc[c].w = __fadd_rn(acc[c].w, __fmul_rn(v.w, scale));
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const int col = (c * 32 + lane) * 4;
+    if (col < D) *reinterpret_cast<float4*>(trow + col) = acc[c];
+  }
+  if (lane == 0) first[r] = 0x7fffffff;
+}
+
+template <int NCH>
+static int launch_scatter_det(float* dtable, const int* src_row, const float* dx, int M, int D, int rows, float scale, int* first,
+                              cudaStream_t st) {
+  OMLM_KLAUNCH((embed_scatter_det_kernel<NCH>), (M + 7) / 8, 256, 0, st, dtable, src_row, dx, M, D, rows, scale, first);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace omlm
 
 extern "C" {
@@ -212,6 +277,22 @@ int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, i
   OMLM_KLAUNCH((embed_scatter_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), dtable, src_row, dx, M, D, scale);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+int omlm_embed_scatter_add_det(float* dtable, const int* src_row, const float* dx, int M, int D, float scale, int* first_ws,
+                               int table_rows, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0 && D <= 2048, "embed_scatter_det: bad shape %d x %d", M, D);
+  OMLM_CHECK_ARG(first_ws != nullptr && table_rows > 0, "embed_scatter_det: no row-marker workspace");
+  auto st = reinterpret_cast<cudaStream_t>(stream);
+  OMLM_KLAUNCH((embed_first_kernel), (M + 255) / 256, 256, 0, st, src_row, M, table_rows, first_ws);
+  OMLM_LAUNCH_CHECK();
+  const int nch = (D + 127) / 128;
+  if (nch <= 1) return launch_scatter_det<1>(dtable, src_row, dx, M, D, table_rows, scale, first_ws, st);
+  if (nch <= 2) return launch_scatter_det<2>(dtable, src_row, dx, M, D, table_rows, scale, first_ws, st);
+  if (nch <= 4) return launch_scatter_det<4>(dtable, src_row, dx, M, D, table_rows, scale, first_ws, st);
+  if (nch <= 8) return launch_scatter_det<8>(dtable, src_row, dx, M, D, table_rows, scale, first_ws, st);
+  return launch_scatter_det<16>(dtable, src_row, dx, M, D, table_rows, scale, first_ws, st);
 }
 
 }  // extern "C"

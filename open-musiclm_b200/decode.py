@@ -304,7 +304,8 @@ class TokenConditionedTransformerWrapper(nn.Module):
             if self._trainer is None:
                 self._trainer = HotPathTrainer(m, cross_entropy_loss_weights=self.cross_entropy_loss_weights, mask_prob=self.mask_prob,
                                                pad_id=self.pad_id, use_cuda_graph=False)
-            return self._trainer._micro_batch(all_token_ids, m.training, 0, False), None, None
+            return self._trainer._micro_batch(all_token_ids, m.training, 0, False,
+                                             det=torch.are_deterministic_algorithms_enabled()), None, None
         dev = m.device
         ids = [t.to(dev, torch.int64).reshape(t.shape[0], -1) for t in all_token_ids]
         ids = [torch.cat([t, torch.full((t.shape[0], 1), e, device=dev, dtype=torch.int64)], 1) for t, e in zip(ids, self.eos_ids)]

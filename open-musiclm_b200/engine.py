@@ -24,6 +24,7 @@ duplicate for the weight-gradient GEMMs.  OMLM_ACT16=bf16 switches the whole pat
 """
 import math
 import os
+import weakref
 from typing import List, Optional
 
 import torch
@@ -134,6 +135,9 @@ class Engine:
         self.err_flag = torch.zeros(1, dtype=torch.int32, device=dev)  # latched by omlm_token_plan (token id out of range)
         self.loss_acc = torch.zeros(2, device=dev)
         self.sumsq = torch.zeros(1, device=dev, dtype=torch.float64)
+        self.det_sumsq_part = None      # deterministic mode (see workspace()): per-CTA partials of grad_sumsq
+        self.det_rows = None            #   and the row markers of the embedding scatter-add
+        self._det_attn = weakref.WeakSet()   # every live attention-backward workspace (also those kept by captured graphs)
 
     # ------------------------------------------------------------------------------------------ arena
     def _build_arena(self):
@@ -247,13 +251,22 @@ class Engine:
 
     def check_errors(self):
         """Raises if a token id outside an embedding table was seen since the last check (nn.Embedding's IndexError;
-        asynchronous like the reference's device-side assert on CUDA: this call synchronises)."""
+        asynchronous like the reference's device-side assert on CUDA: this call synchronises).  Also raises if, in
+        deterministic mode, the attention backward's ordered accumulation gave up waiting for a turn: those steps summed
+        in arrival order (correct up to rounding) and are not reproducible.  Both flags are cleared by the raise."""
         bits = int(self.err_flag.item())
         if bits:
             self.err_flag.zero_()
             bad = [s for s in range(len(self.seqs)) if bits >> s & 1]
             raise lib.OmlmError(f"token id out of range for the embedding table of sequence(s) {bad} "
                                 f"(valid ids: 0..codebook_size, or the pad id at quantizer-0 positions)")
+        late = [w for w in list(self._det_attn) if w.error()]
+        if late:
+            for w in late:
+                w.clear_error()
+            raise lib.OmlmError("deterministic mode: the attention backward timed out waiting for an accumulation turn; "
+                                "the steps since the last check summed dQ / dK|dV in arrival order (correct up to rounding, "
+                                "not reproducible)")
 
     # ------------------------------------------------------------------------------------------ plans / workspaces
     _MAX_SHAPES = 8       # plans / workspaces kept (least recently used shapes are dropped: their HBM returns to torch)
@@ -268,8 +281,13 @@ class Engine:
             self._plans.pop(next(iter(self._plans)))
         return pl
 
-    def workspace(self, pl: _Plan, train: bool):
-        key = (pl.B, tuple(pl.n_tok), train)
+    # deterministic mode: bytes of split-K partials the weight-gradient GEMMs may use (the split count is capped to fit)
+    DET_WGRAD_PART_BYTES = 64 << 20
+
+    def workspace(self, pl: _Plan, train: bool, det: bool = False):
+        """Activation buffers of one shape.  det (torch.are_deterministic_algorithms_enabled() when the step is issued):
+        a separate set that also holds the scratch of the fixed-order kernel variants (add_det_scratch)."""
+        key = (pl.B, tuple(pl.n_tok), train, det)
         if key in self._ws:
             ws = self._ws.pop(key)
             self._ws[key] = ws                      # most recently used
@@ -313,8 +331,36 @@ class Engine:
                 dq_raw=E(M, HD), dkv_raw=E(M, 128), dtable=E(h, pl.N, dt=f32),
                 rp_d0=E(pl.N, self.Hr, dt=f32), rp_d1=E(pl.N, self.Hr, dt=f32), rp_dz3=E(pl.N, 3 * self.Hr),
             )
+        if det:
+            self.add_det_scratch(pl, ws, train)
         self._ws[key] = ws
         return ws
+
+    def add_det_scratch(self, pl: _Plan, ws, train: bool):
+        """Scratch of the deterministic kernel variants (include/omlm_b200.h, *_det): one fp32 buffer for the per-CTA
+        partial sums (the kernels run one after another on the stream and share it), the attention backward's workspace,
+        the split-K partials of the weight gradients, and, once per engine, the grad_sumsq partials and the embedding
+        row markers.  Allocated only in deterministic mode, before any graph capture."""
+        if "det_part" in ws and (ws.get("det_train") or not train):
+            return
+        dev, sms, d, B, N = self.dev, self._num_sms(), self.d, pl.B, pl.N
+        rows_ce = max(pl.B * c for (_, _, c, _) in pl.groups)
+        floats = max(2 * ((rows_ce + 7) // 8), 64)                              # cross-entropy (loss, rows) pairs
+        if train:
+            floats = max(floats, 4 * sms * max(d, 128),                         # layernorm_bwd dgamma rows
+                         8 * sms * 128,                                         # qk_l2norm_bwd scale rows
+                         B * ((N + 127) // 128) * 7 * self.F)                   # ffn_mid_bwd gamma / conv rows
+            ws["det_attn"] = lib.AttnBwdDetWorkspace(dev, B, N, self.h)
+            self._det_attn.add(ws["det_attn"])
+            shapes = [(cp, d) for cp in self.Cp] + [(d, self.F), (2 * self.F, d), (d, self.HD), (self.HD, d), (128, d)]
+            need = max(48 * m * _round_up(n, 4) * 4 for m, n in shapes)
+            ws["det_wgrad"] = torch.empty(min(need, self.DET_WGRAD_PART_BYTES) // 4, device=dev, dtype=torch.float32)
+            if self.det_sumsq_part is None:
+                self.det_sumsq_part = torch.empty(4 * sms, device=dev, dtype=torch.float64)
+            if self.det_rows is None:
+                self.det_rows = lib.embed_row_markers(self.table.numel() // d, dev)
+        ws["det_part"] = torch.empty(floats, device=dev, dtype=torch.float32)
+        ws["det_train"] = train
 
     # ------------------------------------------------------------------------------------------ forward
     # tile / split-K choice: minimise  waves x (k-blocks per unit x tile cost + epilogue)  over the device's SMs
@@ -359,9 +405,9 @@ class Engine:
             lib.sgemm_small(w, (1, 1), ws["ones"], (1, 1), ws["table"], (ws["table"].stride(0), 1), self.h, N, 1)
         # 'none': the table stays zero
 
-    def bias_table_backward(self, ws, N):
+    def bias_table_backward(self, ws, N, det=False):
         if self.bias_type == "continuous":
-            self._relpos_backward(ws, N)
+            self._relpos_backward(ws, N, det)
         elif self.bias_type == "t5":
             gw = self.gview["transformer.rel_pos_bias.relative_attention_bias.weight"]      # bucket 0 collects every delta
             lib.colsum(ws["dtable"], 1, ws["dtable"].stride(0), gw[0], N, self.h, accumulate=True)
@@ -425,27 +471,41 @@ class Engine:
             lib.gemm(xf[base:base + rows], self.pk_logit[s][qi], ws["logits"][gi], block_n=128)
 
     # ------------------------------------------------------------------------------------------ backward
-    def _wgrad(self, dy, x, gout, m, n, **kw):
-        """gout[m, n] += dy[rows, m]^T x[rows, n]   (both operands MN-major, fp32 accumulate into the grad arena)."""
+    def _wgrad(self, dy, x, gout, m, n, det_part=None, **kw):
+        """gout[m, n] += dy[rows, m]^T x[rows, n]   (both operands MN-major, fp32 accumulate into the grad arena).
+        det_part (deterministic mode): split-K partials go to this scratch and are summed in split order; the split
+        count is capped so that they fit."""
         k = dy.shape[0]
         kb = (k + 63) // 64
+        s_max = max(1, min(kb // 8, 48))
+        if det_part is not None:
+            rs, rv, nv = kw.get("row_split", 0), kw.get("row_valid", 0), kw.get("n_valid", 0) or n
+            rows_out = (m + rs - 1) // rs * rv if rs > 0 else (2 * rv if rs < 0 else m)
+            s_max = max(1, min(s_max, det_part.numel() // (rows_out * _round_up(nv, 4))))
         best = None
         for bn in (128, 256):
-            for s in range(1, max(1, min(kb // 8, 48)) + 1):
+            for s in range(1, s_max + 1):
                 c = self._tile_cost(m, n, kb, bn, s, 14.0 if s > 1 else 10.0)
                 if best is None or c < best[0]:
                     best = (c, bn, s)
         _, bn, s = best
-        if s > 1:
+        if det_part is not None:
+            lib.gemm_splitk_det(dy, x, gout, det_part, a_mn=True, b_mn=True, M=m, N=n, K=k, splits=s, block_n=bn,
+                                max_ctas=self.bwd_max_ctas, **kw)
+        elif s > 1:
             lib.gemm(dy, x, gout, a_mn=True, b_mn=True, M=m, N=n, K=k, splits=s, block_n=bn, max_ctas=self.bwd_max_ctas, **kw)
         else:
             lib.gemm(dy, x, gout, a_mn=True, b_mn=True, M=m, N=n, K=k, addend=gout, block_n=bn, max_ctas=self.bwd_max_ctas, **kw)
 
-    def backward_core(self, pl: _Plan, ws, src_row, key_mask, groups_with_grad, drop: bool = False, on_ready=None):
+    def backward_core(self, pl: _Plan, ws, src_row, key_mask, groups_with_grad, drop: bool = False, on_ready=None, det: bool = False):
         """Consumes ws['dlogits'] (bf16, permuted rows) and accumulates every parameter gradient into arena_g.
         on_ready(trigger): called when a group of gradients is final -- 'heads', 'layer<l>' (matrices of layer l), 'tail'
-        (everything else) -- so that a data-parallel caller can start reducing it underneath the rest of the pass."""
+        (everything else) -- so that a data-parallel caller can start reducing it underneath the rest of the pass.
+        det: the fixed-order kernel variants (ws must hold their scratch, see add_det_scratch): bit-identical gradients
+        for identical inputs on the same GPU model."""
         ready = on_ready if on_ready is not None else (lambda trigger: None)
+        part = ws["det_part"] if det else None
+        wpart = ws["det_wgrad"] if det else None
         B, N, M, d, h, HD, F, Fp = pl.B, pl.N, pl.M, self.d, self.h, self.HD, self.F, self.Fp
         pv, gv = self.pview, self.gview
         x = ws["x"]
@@ -461,11 +521,12 @@ class Engine:
             rows = B * cnt
             dl = ws["dlogits"][gi]
             lib.gemm(dl, self.pk_logit_b[s][qi], ws["dxf"][base:base + rows], b_mn=True, M=rows, N=d, K=self.Cp[s], block_n=128, max_ctas=self.bwd_max_ctas)
-            self._wgrad(dl, ws["xf"][base:base + rows], gv[f"logit_weights.{s}"][qi], self.Cp[s], d, row_split=self.Cp[s], row_valid=self.C[s])
+            self._wgrad(dl, ws["xf"][base:base + rows], gv[f"logit_weights.{s}"][qi], self.Cp[s], d, det_part=wpart, row_split=self.Cp[s],
+                        row_valid=self.C[s])
         ready("heads")
         dxa, dxb = ws["dx"]
         lib.layernorm_bwd(ws["dxf"], x[2 * self.L], ws["st_o"], pv["transformer.norm.gamma"], dxa, gv["transformer.norm.gamma"],
-                          src_row=pl.dest_row, dx_bf16=ws["dx_bf"])
+                          src_row=pl.dest_row, dx_bf16=ws["dx_bf"], part=part)
         ws["dtable"].zero_()
         for l in reversed(range(self.L)):
             p, pk = f"transformer.layers.{l}.", self.pk[l]
@@ -484,38 +545,39 @@ class Engine:
             # (the tile kernel runs right behind the GEMM that wrote dhn, while dhn is still in L2; the weight gradient after it)
             lib.ffn_mid_bwd(ws["dhn"], ws["hn"][l], ws["u"][l], ws["st_i"][l], pk["conv"], pk["gin"], ws["rowstat"], ws["du"],
                             gv[p + fk["gin"]], gv[p + fk["conv"]] if fk["conv"] is not None else None, B, N, F, Fp, drop_p,
-                            keep_bits=keep, rowstat_parts=parts)
-            self._wgrad(ws["dx_bf"], ws["hn"][l], gv[p + fk["w2"]], d, Fp, n_valid=F)
+                            keep_bits=keep, rowstat_parts=parts, part=part)
+            self._wgrad(ws["dx_bf"], ws["hn"][l], gv[p + fk["w2"]], d, Fp, det_part=wpart, n_valid=F)
             lib.gemm(ws["du"], pk["w1_b"], ws["dxn"], b_mn=True, M=M, N=d, K=2 * Fp, block_n=self._bn_for(M, d, 2 * Fp), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["du"], ws["xn2"][l], gv[p + fk["w1"]], 2 * Fp, d, row_split=-1, row_valid=F)
-            lib.layernorm_bwd(ws["dxn"], xm, ws["st_f"][l], pv[p + fk["g1"]], dxb, gv[p + fk["g1"]], dres=dxa, dx_bf16=ws["dx_bf"])
+            self._wgrad(ws["du"], ws["xn2"][l], gv[p + fk["w1"]], 2 * Fp, d, det_part=wpart, row_split=-1, row_valid=F)
+            lib.layernorm_bwd(ws["dxn"], xm, ws["st_f"][l], pv[p + fk["g1"]], dxb, gv[p + fk["g1"]], dres=dxa, dx_bf16=ws["dx_bf"], part=part)
             # ---- attention
             lib.gemm(ws["dx_bf"], pk["wo_b"], ws["d_o"], b_mn=True, M=M, N=HD, K=d, block_n=self._bn_for(M, HD, d), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["dx_bf"], ws["o"][l], gv[p + "0.to_out.0.weight"], d, HD)
+            self._wgrad(ws["dx_bf"], ws["o"][l], gv[p + "0.to_out.0.weight"], d, HD, det_part=wpart)
             lib.attn_bwd_tc(ws["qn"][l], ws["kvn"][l], ws["d_o"], ws["o"][l], ws["lse"][l], ws["table"], key_mask, ws["dsum"],
-                            ws["dqn"], ws["dkvn"], ws["dtable"], B, N, h)
+                            ws["dqn"], ws["dkvn"], ws["dtable"], B, N, h, det=ws["det_attn"] if det else None)
             lib.qk_l2norm_bwd(ws["dqn"], ws["dkvn"], ws["q_raw"][l], ws["kv_raw"][l], pv[p + "0.q_scale"], pv[p + "0.k_scale"],
-                              ws["dq_raw"], ws["dkv_raw"], gv[p + "0.q_scale"], gv[p + "0.k_scale"], h)
+                              ws["dq_raw"], ws["dkv_raw"], gv[p + "0.q_scale"], gv[p + "0.k_scale"], h, part=part)
             lib.gemm(ws["dq_raw"], pk["wq_b"], ws["dxn"], b_mn=True, M=M, N=d, K=HD, block_n=self._bn_for(M, d, HD), max_ctas=self.bwd_max_ctas)
             lib.gemm(ws["dkv_raw"], pk["wkv_b"], ws["dxraw"], b_mn=True, M=M, N=d, K=128, block_n=self._bn_for(M, d, 128), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["dq_raw"], ws["xn"][l], gv[p + "0.to_q.weight"], HD, d)
-            self._wgrad(ws["dkv_raw"], ws["xraw"][l], gv[p + "0.to_kv.weight"], 128, d)
+            self._wgrad(ws["dq_raw"], ws["xn"][l], gv[p + "0.to_q.weight"], HD, d, det_part=wpart)
+            self._wgrad(ws["dkv_raw"], ws["xraw"][l], gv[p + "0.to_kv.weight"], 128, d, det_part=wpart)
             ready(f"layer{l}")
             lib.layernorm_bwd(ws["dxn"], xa, ws["st_a"][l], pv[p + "0.norm.gamma"], dxa, gv[p + "0.norm.gamma"], dres=dxb, draw=ws["dxraw"],
-                              dx_bf16=ws["dx_bf"])
+                              dx_bf16=ws["dx_bf"], part=part)
         # ---- embeddings + start tokens (grad_shrink: utils.py:60-61)
-        lib.embed_scatter_add(self.dtable_emb, src_row, dxa, self.alpha)
+        rows = self.det_rows if det else None
+        lib.embed_scatter_add(self.dtable_emb, src_row, dxa, self.alpha, first=rows)
         if pl.src_row2 is not None:
-            lib.embed_scatter_add(self.dtable_emb, pl.src_row2, dxa, self.alpha)
-        self.bias_table_backward(ws, N)
+            lib.embed_scatter_add(self.dtable_emb, pl.src_row2, dxa, self.alpha, first=rows)
+        self.bias_table_backward(ws, N, det)
         ready("tail")
 
-    def _relpos_backward(self, ws, N):
+    def _relpos_backward(self, ws, N, det=False):
         pv, gv, Hr, h = self.pview, self.gview, self.Hr, self.h
         pre = "transformer.rel_pos_bias.net."
         dT = ws["dtable"]                                   # [h, N]: dY[n, hh] = dT[hh, n]
         a3 = ws["rp_a"][2]
-        lib.sgemm_small(dT, (N, 1), a3, (Hr, 1), gv[pre + "3.weight"], (Hr, 1), h, Hr, N, accumulate=True)      # dW4 = dY^T a3
+        lib.sgemm_small(dT, (N, 1), a3, (Hr, 1), gv[pre + "3.weight"], (Hr, 1), h, Hr, N, accumulate=True, det=det)   # dW4 = dY^T a3
         lib.colsum(dT, 1, N, gv[pre + "3.bias"], N, h, accumulate=True)
         d_cur, d_nxt = ws["rp_d0"], ws["rp_d1"]
         lib.sgemm_small(dT, (1, N), pv[pre + "3.weight"], (Hr, 1), d_cur, (Hr, 1), N, Hr, h)                      # da3 = dY W4
@@ -537,7 +599,7 @@ class Engine:
                 lib.gemm(dz_lo, w_hi, d_nxt, b_mn=True, M=N, N=Hr, K=Hr, addend=d_nxt, block_n=128)
                 d_cur, d_nxt = d_nxt, d_cur
             else:
-                lib.sgemm_small(d_cur, (1, Hr), ws["rp_in"], (1, 1), gv[f"{pre}0.0.weight"], (1, 1), Hr, 1, N, accumulate=True)
+                lib.sgemm_small(d_cur, (1, Hr), ws["rp_in"], (1, 1), gv[f"{pre}0.0.weight"], (1, 1), Hr, 1, N, accumulate=True, det=det)
 
     # ------------------------------------------------------------------------------------------ reference-API path
     def api_forward(self, all_token_ids, self_attn_mask, only_final):
@@ -557,7 +619,8 @@ class Engine:
         drop = self.m.training and self.drop_p > 0
         if drop:
             self.seed += 1
-        outs = _ApiFunction.apply(self, pl, src_row, key_mask, need_grad, wanted, drop, *self._param_list)
+        outs = _ApiFunction.apply(self, pl, src_row, key_mask, need_grad, wanted, drop, torch.are_deterministic_algorithms_enabled(),
+                                  *self._param_list)
         res, k = [], 0
         for s in range(len(self.seqs)):
             if s in wanted:
@@ -591,8 +654,8 @@ class _ApiFunction(torch.autograd.Function):
     forward(), libomlm_b200 backward in backward(); gradients are returned per parameter."""
 
     @staticmethod
-    def forward(ctx, eng: Engine, pl, src_row, key_mask, need_grad, wanted, drop, *params):
-        ws = eng.workspace(pl, need_grad)
+    def forward(ctx, eng: Engine, pl, src_row, key_mask, need_grad, wanted, drop, det, *params):
+        ws = eng.workspace(pl, need_grad, det)
         eng.forward_core(pl, ws, src_row, key_mask, need_grad, wanted, drop)
         ctx.eng, ctx.pl, ctx.src_row, ctx.key_mask, ctx.wanted, ctx.drop = eng, pl, src_row, key_mask, sorted(wanted), drop
         ctx.need_grad = need_grad
@@ -618,14 +681,18 @@ class _ApiFunction(torch.autograd.Function):
             if g is not None:
                 eng.scatter_dlogits(pl, ws, s, g)
                 with_grad.add(s)
+        # the switch is read again here: a backward issued in deterministic mode runs the fixed-order kernels
+        det = torch.are_deterministic_algorithms_enabled()
+        if det:
+            eng.add_det_scratch(pl, ws, True)
         # gradients are produced in a scratch copy of the arena so that autograd can accumulate them itself
         saved = eng.arena_g.clone()
         eng.arena_g.zero_()
-        eng.backward_core(pl, ws, ctx.src_row, ctx.key_mask, with_grad, ctx.drop)
+        eng.backward_core(pl, ws, ctx.src_row, ctx.key_mask, with_grad, ctx.drop, det=det)
         fresh = eng.arena_g.clone()
         eng.arena_g.copy_(saved)
         outs = []
         for n, p in eng.m.named_parameters():
             o = eng.layout[n]
             outs.append(fresh[o:o + p.numel()].view(p.shape))
-        return (None, None, None, None, None, None, None, *outs)
+        return (None, None, None, None, None, None, None, None, *outs)

@@ -102,6 +102,23 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, M=None, N=None, K=None, addend=No
     return out
 
 
+def gemm_splitk_det_workspace(M, N, K, splits, row_split=0, row_valid=0, n_valid=0):
+    """Bytes of fp32 partials gemm_splitk_det needs (0 when the clamped split count is 1)."""
+    out = _L(0)
+    call("omlm_gemm16_splitk_det_workspace", _I(M), _I(N), _I(K), _I(splits), _I(row_split), _I(row_valid), _I(n_valid), ctypes.byref(out))
+    return out.value
+
+
+def gemm_splitk_det(a, b, out, part, *, a_mn=False, b_mn=False, M, N, K, splits, row_split=0, row_valid=0, n_valid=0,
+                    block_n=128, max_ctas=0):
+    """out (fp32) += A B with split-K partials summed in split order (omlm_gemm16_splitk_det); part: fp32 scratch."""
+    assert a.dtype in _T16 and b.dtype in _T16 and out.dtype == torch.float32 and part.dtype == torch.float32
+    call("omlm_gemm16_splitk_det", _p(a), _I(int(a.dtype == torch.float16)), _I(int(a_mn)), _L(a.stride(0)),
+         _p(b), _I(int(b.dtype == torch.float16)), _I(int(b_mn)), _L(b.stride(0)), _I(M), _I(N), _I(K), _p(out), _L(out.stride(0)),
+         _I(splits), _I(row_split), _I(row_valid), _I(n_valid), _I(block_n), _I(max_ctas), _p(part), _L(part.numel() * 4), _stream())
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # thin tensor-level wrappers (tensors in, raw pointers out); shapes are validated on the C side
 # ------------------------------------------------------------------------------------------------
@@ -144,9 +161,19 @@ def embed_gather(table, src_row, x, src_row2=None):
     call("omlm_embed_gather", _p(table), _p(src_row), _p(src_row2), _p(x), _I(M), _I(D), _stream())
 
 
-def embed_scatter_add(dtable, src_row, dx, scale):
+def embed_scatter_add(dtable, src_row, dx, scale, first=None):
+    """first: int32 row markers (INT_MAX, one per table row) -> the deterministic variant (omlm_embed_scatter_add_det)."""
     M, D = dx.shape
-    call("omlm_embed_scatter_add", _p(dtable), _p(src_row), _p(dx), _I(M), _I(D), _F(scale), _stream())
+    if first is None:
+        call("omlm_embed_scatter_add", _p(dtable), _p(src_row), _p(dx), _I(M), _I(D), _F(scale), _stream())
+    else:
+        call("omlm_embed_scatter_add_det", _p(dtable), _p(src_row), _p(dx), _I(M), _I(D), _F(scale), _p(first),
+             _I(first.numel()), _stream())
+
+
+def embed_row_markers(rows, device):
+    """The row markers embed_scatter_add's deterministic variant needs (every call leaves them as made here)."""
+    return torch.full((rows,), 0x7FFFFFFF, dtype=torch.int32, device=device)
 
 
 def layernorm_fwd(x, gamma, y, xraw=None, stats=None, dest_row=None, ycopy=None):
@@ -157,10 +184,14 @@ def layernorm_fwd(x, gamma, y, xraw=None, stats=None, dest_row=None, ycopy=None)
          _p(dest_row), _I(M), _I(D), _stream())
 
 
-def layernorm_bwd(dy, x, stats, gamma, dx, dgamma, dres=None, draw=None, src_row=None, dx_bf16=None):
+def layernorm_bwd(dy, x, stats, gamma, dx, dgamma, dres=None, draw=None, src_row=None, dx_bf16=None, part=None):
+    """part: fp32 scratch -> the deterministic variant (omlm_layernorm_bwd_det)."""
     M, D = x.shape
-    call("omlm_layernorm_bwd", _p(dy), _p(x), _p(stats), _p(gamma), _p(dres), _p(draw), _p(src_row), _p(dx),
-         _p(dx_bf16), _p(dgamma), _I(M), _I(D), _stream())
+    args = (_p(dy), _p(x), _p(stats), _p(gamma), _p(dres), _p(draw), _p(src_row), _p(dx), _p(dx_bf16), _p(dgamma), _I(M), _I(D))
+    if part is None:
+        call("omlm_layernorm_bwd", *args, _stream())
+    else:
+        call("omlm_layernorm_bwd_det", *args, _p(part), _L(part.numel() * 4), _stream())
 
 
 def qk_l2norm_fwd(q_raw, kv_raw, q_scale, k_scale, qn, kvn, heads):
@@ -168,13 +199,17 @@ def qk_l2norm_fwd(q_raw, kv_raw, q_scale, k_scale, qn, kvn, heads):
          _I(q_raw.shape[0]), _I(heads), _stream())
 
 
-def qk_l2norm_bwd(dqn, dkvn, q_raw, kv_raw, q_scale, k_scale, dq_raw, dkv_raw, dq_scale, dk_scale, heads):
-    call("omlm_qk_l2norm_bwd", _p(dqn), _p(dkvn), _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(dq_raw),
-         _p(dkv_raw), _p(dq_scale), _p(dk_scale), _I(q_raw.shape[0]), _I(heads), _stream())
+def qk_l2norm_bwd(dqn, dkvn, q_raw, kv_raw, q_scale, k_scale, dq_raw, dkv_raw, dq_scale, dk_scale, heads, part=None):
+    args = (_p(dqn), _p(dkvn), _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(dq_raw), _p(dkv_raw), _p(dq_scale), _p(dk_scale),
+            _I(q_raw.shape[0]), _I(heads))
+    if part is None:
+        call("omlm_qk_l2norm_bwd", *args, _stream())
+    else:
+        call("omlm_qk_l2norm_bwd_det", *args, _p(part), _L(part.numel() * 4), _stream())
 
 
-def sgemm_small(A, sa, B, sb, C, sc, M, N, K, *, Z=None, bias=None, act=0, accumulate=False):
-    call("omlm_sgemm_small", _p(A), _L(sa[0]), _L(sa[1]), _p(B), _L(sb[0]), _L(sb[1]), _p(C), _L(sc[0]), _L(sc[1]),
+def sgemm_small(A, sa, B, sb, C, sc, M, N, K, *, Z=None, bias=None, act=0, accumulate=False, det=False):
+    call("omlm_sgemm_small_det" if det else "omlm_sgemm_small", _p(A), _L(sa[0]), _L(sa[1]), _p(B), _L(sb[0]), _L(sb[1]), _p(C), _L(sc[0]), _L(sc[1]),
          _p(Z), _p(bias), _I(M), _I(N), _I(K), _I(act), _I(int(accumulate)), _stream())
 
 
@@ -215,9 +250,33 @@ def attn_bwd(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dt
          _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale), _stream())
 
 
-def attn_bwd_tc(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads, scale=8.0):
-    call("omlm_attn_bwd_tc", _p(qn), _p(kvn), _p(d_o), _p(o), _p(lse2), _p(table), _I(table.stride(0)), _p(key_mask),
-         _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale), _stream())
+def attn_bwd_tc(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads, scale=8.0, det=None):
+    """det: an AttnBwdDetWorkspace for this (B, N, heads) -> the fixed-order variant (omlm_attn_bwd_tc_det)."""
+    args = (_p(qn), _p(kvn), _p(d_o), _p(o), _p(lse2), _p(table), _I(table.stride(0)), _p(key_mask),
+            _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale))
+    if det is None:
+        call("omlm_attn_bwd_tc", *args, _stream())
+    else:
+        call("omlm_attn_bwd_tc_det", *args, _p(det.ws), _L(det.ws.numel() * 4), _p(det.iws), _L(det.iws.numel()), _stream())
+
+
+class AttnBwdDetWorkspace:
+    """Scratch of omlm_attn_bwd_tc_det for one (B, N, heads): the units' partial bias-gradient tables and the int words
+    (turn counters, table windows, error word -- allocated zero)."""
+
+    def __init__(self, device, B, N, heads):
+        ws, iws = _L(0), _L(0)
+        call("omlm_attn_bwd_tc_det_workspace", _I(B), _I(N), _I(heads), ctypes.byref(ws), ctypes.byref(iws))
+        self.ws = torch.empty(max(ws.value // 4, 1), device=device, dtype=torch.float32)
+        self.iws = torch.zeros(iws.value, device=device, dtype=torch.int32)
+
+    def error(self):
+        """True if a turn was not granted in time since the word was last cleared: those calls summed in arrival order
+        (correct up to rounding, not reproducible).  Synchronises."""
+        return bool(int(self.iws[-1].item()))
+
+    def clear_error(self):
+        self.iws[-1].zero_()
 
 
 def gemm_ffn_up(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, Nseq, Fp, max_ctas=0):
@@ -233,13 +292,18 @@ def ffn_norm_fwd(h, rowsum, gamma, hn, stats, F, Fp, drop_p=0.0, seed=None, laye
          _I(F), _I(Fp), _F(drop_p), _p(seed), _I(layer), _I(int(h.dtype == torch.float16)), _stream())
 
 
-def ffn_mid_bwd(dhn, hn, u, stats, conv_w, gamma, rowstat, du, dgamma, dconv_w, B, N, F, Fp, drop_p=0.0, keep_bits=None, rowstat_parts=0):
+def ffn_mid_bwd(dhn, hn, u, stats, conv_w, gamma, rowstat, du, dgamma, dconv_w, B, N, F, Fp, drop_p=0.0, keep_bits=None, rowstat_parts=0,
+                part=None):
     """dgamma [F] / dconv_w [2F, 3] (or None) are accumulated in the parameters' own layouts; rowstat_parts > 0: rowstat
     holds the partial row sums written by gemm_rowstat, else it is a [M, 2] scratch."""
     assert u.dtype in _T16 and hn.dtype == dhn.dtype == du.dtype == torch.bfloat16
     assert dgamma.numel() == F and (dconv_w is None or dconv_w.numel() == 6 * F)
-    call("omlm_ffn_mid_bwd", _p(dhn), _p(hn), _p(u), _p(stats), _p(conv_w), _p(gamma), _p(keep_bits), _p(rowstat), _I(rowstat_parts), _p(du),
-         _p(dgamma), _p(dconv_w), _I(B), _I(N), _I(F), _I(Fp), _F(drop_p), _I(int(u.dtype == torch.float16)), _stream())
+    args = (_p(dhn), _p(hn), _p(u), _p(stats), _p(conv_w), _p(gamma), _p(keep_bits), _p(rowstat), _I(rowstat_parts), _p(du),
+            _p(dgamma), _p(dconv_w), _I(B), _I(N), _I(F), _I(Fp), _F(drop_p), _I(int(u.dtype == torch.float16)))
+    if part is None:
+        call("omlm_ffn_mid_bwd", *args, _stream())
+    else:
+        call("omlm_ffn_mid_bwd_det", *args, _p(part), _L(part.numel() * 4), _stream())
 
 
 def gemm_rowstat(a, b, out, hn, gamma, part, *, b_mn=False, M=None, N=None, K=None, keep_bits=None, keep_scale=1.0, max_ctas=0):
@@ -256,17 +320,25 @@ def gemm_rowstat(a, b, out, hn, gamma, part, *, b_mn=False, M=None, N=None, K=No
 
 
 def cross_entropy(logits, labels, C, loss_acc, *, grad_scale=0.0, dlogits=None, ignore_index=-100, label_stride=1, rows=None,
-                  rows_per_batch=0, batch_stride=0, loss_scale=1.0):
+                  rows_per_batch=0, batch_stride=0, loss_scale=1.0, part=None):
     """labels: int32; flat (rows_per_batch = 0) or the strided view described in include/omlm_b200.h (pass the tensor whose
     data_ptr is the first label of the group)."""
     rows = logits.shape[0] if rows is None else rows
-    call("omlm_cross_entropy", _p(logits), _L(logits.stride(0)), _p(labels), _I(label_stride), _I(rows_per_batch), _L(batch_stride),
-         _I(rows), _I(C), _I(ignore_index), _F(grad_scale), _F(loss_scale), _p(dlogits),
-         _L(dlogits.stride(0) if dlogits is not None else 0), _I(dlogits.shape[1] if dlogits is not None else 0), _p(loss_acc), _stream())
+    args = (_p(logits), _L(logits.stride(0)), _p(labels), _I(label_stride), _I(rows_per_batch), _L(batch_stride),
+            _I(rows), _I(C), _I(ignore_index), _F(grad_scale), _F(loss_scale), _p(dlogits),
+            _L(dlogits.stride(0) if dlogits is not None else 0), _I(dlogits.shape[1] if dlogits is not None else 0), _p(loss_acc))
+    if part is None:
+        call("omlm_cross_entropy", *args, _stream())
+    else:
+        call("omlm_cross_entropy_det", *args, _p(part), _L(part.numel() * 4), _stream())
 
 
-def grad_sumsq(g, acc, prescale=1.0):
-    call("omlm_grad_sumsq", _p(g), _L(g.numel()), _F(prescale), _p(acc), _stream())
+def grad_sumsq(g, acc, prescale=1.0, part=None):
+    """part: float64 scratch (>= 4 * SMs) -> the deterministic variant (omlm_grad_sumsq_det)."""
+    if part is None:
+        call("omlm_grad_sumsq", _p(g), _L(g.numel()), _F(prescale), _p(acc), _stream())
+    else:
+        call("omlm_grad_sumsq_det", _p(g), _L(g.numel()), _F(prescale), _p(acc), _p(part), _L(part.numel() * 8), _stream())
 
 
 def adamw_step(p, g, m, v, n_decay, hyper, sumsq):

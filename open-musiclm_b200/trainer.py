@@ -98,7 +98,7 @@ class HotPathTrainer:
         eng.arena_g.zero_()
 
     # -------------------------------------------------------------------------------------------
-    def _micro_batch(self, token_ids: Sequence[torch.Tensor], train: bool, slot: int, backward: bool, reducer=None):
+    def _micro_batch(self, token_ids: Sequence[torch.Tensor], train: bool, slot: int, backward: bool, reducer=None, det: bool = False):
         eng = self.eng
         dev = eng.dev
         ids = [t.reshape(t.shape[0], -1).to(dev, torch.int64, non_blocking=True) for t in token_ids]
@@ -118,7 +118,7 @@ class HotPathTrainer:
             ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base,
             eng.start_row, append_eos=True, drop_last=True, mask_cond=True, pad_id=self.pad_id, forget_keep=forget,
             err_flag=eng.err_flag)
-        ws = eng.workspace(pl, backward)
+        ws = eng.workspace(pl, backward, det)
         weighted = {s for s in range(S) if self.ce_weights[s] > 0}
         drop = train and eng.drop_p > 0
         eng.forward_core(pl, ws, src_row, key_mask, backward, weighted, drop)
@@ -140,10 +140,11 @@ class HotPathTrainer:
                 scale = self.ce_weights[s] / total_n / self.grad_accum_every
                 lib.cross_entropy(ws["logits"][gi], labels[0, lab_off[s] + qi:], eng.C[s], acc, grad_scale=scale,
                                   dlogits=ws["dlogits"][gi] if backward else None, rows=B * cnt, label_stride=q, rows_per_batch=cnt,
-                                  batch_stride=labels.stride(0), loss_scale=self.ce_weights[s] / total_n)
+                                  batch_stride=labels.stride(0), loss_scale=self.ce_weights[s] / total_n,
+                                  part=ws["det_part"] if det else None)
         loss = acc[0]
         if backward:
-            eng.backward_core(pl, ws, src_row, key_mask, weighted, drop, on_ready=reducer.fire if reducer is not None else None)
+            eng.backward_core(pl, ws, src_row, key_mask, weighted, drop, on_ready=reducer.fire if reducer is not None else None, det=det)
         return loss
 
     def _set_hyper(self):
@@ -159,7 +160,7 @@ class HotPathTrainer:
         h[8] = grad_prescale(self.pg)
         self.hyper.copy_(h, non_blocking=True)
 
-    def _fwd_bwd_body(self, micro_batches, overlap=True):
+    def _fwd_bwd_body(self, micro_batches, det, overlap=True):
         """Device work of one optimiser step up to the reduced gradient arena (capturable in a CUDA graph).  With several
         ranks the last micro-batch's backward pass fires the bucketed all-reduces (the reference reduces on every
         micro-batch, trainer.py:439; the reduced sum is the same)."""
@@ -167,34 +168,35 @@ class HotPathTrainer:
         if red is not None:
             red.begin()
         for i, mb in enumerate(micro_batches):
-            self._micro_batch(mb, True, i, True, reducer=red if i == len(micro_batches) - 1 else None)
+            self._micro_batch(mb, True, i, True, reducer=red if i == len(micro_batches) - 1 else None, det=det)
         if red is not None:
             red.join()
         elif self.world > 1:
             allreduce_sum_(self.eng.arena_g, self.pg)
 
-    def _update_body(self):
-        """Clip + AdamW + re-pack on the reduced gradient arena (capturable in a CUDA graph)."""
+    def _update_body(self, det):
+        """Clip + AdamW + re-pack on the reduced gradient arena (capturable in a CUDA graph).  det: the gradient norm is
+        summed in a fixed order."""
         eng = self.eng
         eng.sumsq.zero_()
         if self.shard_opt:
-            self._sharded_update()
+            self._sharded_update(det)
         else:
             if self.max_grad_norm is not None:
-                lib.grad_sumsq(eng.arena_g, eng.sumsq, prescale=grad_prescale(self.pg))
+                lib.grad_sumsq(eng.arena_g, eng.sumsq, prescale=grad_prescale(self.pg), part=eng.det_sumsq_part if det else None)
             lib.adamw_step(eng.arena_p, eng.arena_g, eng.adam_m, eng.adam_v, eng.n_decay, self.hyper, eng.sumsq)
         eng.arena_g.zero_()
         eng.refresh_packed(force=True)
         self.loss_out.copy_(self.loss_buf.sum() / self.grad_accum_every)
 
-    def _sharded_update(self):
+    def _sharded_update(self, det):
         """After the reduce-scatter this rank holds the summed gradient of ITS part of every arena slice: global norm from
         the parts (one 8-byte all-reduce), AdamW on the parts, all-gather of the updated parameters."""
         eng, W, r = self.eng, self.world, self.rank
         parts = [shard_of(lo, hi, W, r) for lo, hi in self.reducer.slices()]
         if self.max_grad_norm is not None:
             for a, b in parts:
-                lib.grad_sumsq(eng.arena_g[a:b], eng.sumsq, prescale=grad_prescale(self.pg))
+                lib.grad_sumsq(eng.arena_g[a:b], eng.sumsq, prescale=grad_prescale(self.pg), part=eng.det_sumsq_part if det else None)
             dist.all_reduce(eng.sumsq, op=dist.ReduceOp.SUM, group=self.pg)
         for a, b in parts:
             lib.adamw_step(eng.arena_p[a:b], eng.arena_g[a:b], eng.adam_m[a:b], eng.adam_v[a:b], max(0, min(b - a, eng.n_decay - a)),
@@ -209,11 +211,11 @@ class HotPathTrainer:
                 all_gather_(self.eng.adam_m[lo:hi], self.world, self.rank, self.pg)
                 all_gather_(self.eng.adam_v[lo:hi], self.world, self.rank, self.pg)
 
-    def _step_body(self, micro_batches):
-        self._fwd_bwd_body(micro_batches)
-        self._update_body()
+    def _step_body(self, micro_batches, det):
+        self._fwd_bwd_body(micro_batches, det)
+        self._update_body(det)
 
-    def _capture(self, st):
+    def _capture(self, st, det):
         """One CUDA graph for the whole step.  With several ranks the NCCL all-reduces are captured too (fork / join on
         the side stream; thread-local capture mode keeps NCCL's watchdog thread out of it).  If that capture is refused,
         fall back to two graphs around ONE eager all-reduce of the arena (no overlap)."""
@@ -223,7 +225,7 @@ class HotPathTrainer:
         try:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, capture_error_mode="thread_local"):
-                self._step_body(st["static"])
+                self._step_body(st["static"], det)
             return ("one", g)
         except Exception as e:
             import warnings
@@ -237,9 +239,9 @@ class HotPathTrainer:
             ga, gb = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
             with torch.cuda.graph(ga):
                 for i, mb in enumerate(st["static"]):
-                    self._micro_batch(mb, True, i, True)
+                    self._micro_batch(mb, True, i, True, det=det)
             with torch.cuda.graph(gb, pool=ga.pool()):
-                self._update_body()
+                self._update_body(det)
             return ("two", ga, gb)
         except Exception as e:
             import warnings
@@ -260,17 +262,23 @@ class HotPathTrainer:
         the stage's order, e.g. (clap, semantic, coarse); host or device).  Returns the mean loss as a device
         scalar.  After two eager steps per input shape the step is replayed from ONE CUDA graph (forward, backward, the
         bucketed NCCL all-reduces on their side stream, clip, AdamW, re-pack); inputs are copied into static device
-        buffers, hyper-parameters live in device memory."""
+        buffers, hyper-parameters live in device memory.
+        With torch.use_deterministic_algorithms(True) the step runs the fixed-order kernel variants: the same inputs,
+        build, world size and GPU model (SM count) give bit-identical losses, gradient norms, parameters and Adam
+        moments, eagerly and under graph replay.  The mode is part of the graph key: toggling it re-captures.
+        transformer.engine.check_errors() raises if a deterministic step could not keep its order (never expected; the
+        attention backward gives up waiting for an accumulation turn after seconds instead of hanging)."""
         assert len(micro_batches) == self.grad_accum_every
         eng = self.eng
+        det = torch.are_deterministic_algorithms_enabled()
         self.transformer.train()
         eng.refresh_packed()        # no-op unless the parameters were written from outside (load_state_dict, manual edits):
         self._set_hyper()           # the captured graph re-packs only after its own optimiser update
         if not self.use_cuda_graph:
-            self._step_body(micro_batches)
+            self._step_body(micro_batches, det)
             self.steps += 1
             return self.loss_out
-        key = tuple(tuple(t.shape) for mb in micro_batches for t in mb)
+        key = (det,) + tuple(tuple(t.shape) for mb in micro_batches for t in mb)
         st = self._graphs.pop(key, None)
         if st is not None:
             self._graphs[key] = st                   # most recently used
@@ -285,16 +293,16 @@ class HotPathTrainer:
         if st["graphs"] is not None:
             self._replay(st["graphs"])
         elif st["count"] < 2:
-            self._step_body(st["static"])
+            self._step_body(st["static"], det)
             st["count"] += 1
         else:
-            st["graphs"] = self._capture(st)
+            st["graphs"] = self._capture(st, det)
             # a captured graph addresses the engine's plan / workspace buffers directly: keep them alive with the graph
             # even if the engine's own shape cache evicts them
             st["keepalive"] = (dict(eng._plans), dict(eng._ws))
             if st["graphs"] is None:
                 self.use_cuda_graph = False
-                self._step_body(st["static"])
+                self._step_body(st["static"], det)
             else:
                 self._replay(st["graphs"])
         self.steps += 1
@@ -318,7 +326,7 @@ class HotPathTrainer:
     def eval_loss(self, token_ids: Sequence[torch.Tensor]):
         """Wrapper forward in eval mode (no forgetful mask, no dropout): the parity configuration."""
         self.transformer.eval()
-        return self._micro_batch(token_ids, False, 0, False)
+        return self._micro_batch(token_ids, False, 0, False, det=torch.are_deterministic_algorithms_enabled())
 
     def grad_norm(self):
         return torch.sqrt(self.eng.sumsq).float()
