@@ -189,7 +189,8 @@ int omlm_arange_f32(float* out, int n, void* stream);
 int omlm_attn_fwd(const void* qn, const void* kvn, const float* table, int table_ld,
                   const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                   float scale, void* stream);
-/* Same contract on the wgmma/TMA path (one 128-row tile per CTA, two consumer warpgroups of 64 rows). */
+/* Same contract on the wgmma/TMA path (one 128-row tile per CTA, two consumer warpgroups of 64 rows; each reads the
+ * bias from a per-tile window of the table staged in shared memory, so heads is limited to 68). */
 int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* table, int table_ld,
                      const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                      float scale, void* stream);
@@ -201,7 +202,9 @@ int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* 
 
 /* wgmma/TMA backward: dqn and dkvn are OVERWRITTEN (its first kernel clears them, the main kernel reduces into
  * them), dtable is accumulated (+=: one table gradient over all layers).  The bias gradient -- diagonal sums of dS -- is
- * formed inside the kernel from the fp32 dS, summed per CTA in shared memory and added to dtable once; no scratch tensor.
+ * formed inside the kernel from the fp32 dS staged in shared memory (each thread sums its (head, diagonal) pairs in row
+ * order, no shared-memory atomics), summed per CTA and added to dtable once; no scratch tensor.  The bias is read from a
+ * per-tile window of the table in shared memory; the windows and diagonal tables limit heads to 58.
  * dqn, dkvn and dtable are reduced with floating-point atomics: reproducible up to accumulation order
  * (omlm_attn_bwd_tc_det fixes the order). */
 int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,

@@ -9,19 +9,22 @@
 //                      P = exp2(s - lse), dS = P (dP - D) in fp32 registers; P, dS -> bf16 [row][key] smem tiles
 //                      dV += P^T dO,  dK += dS^T Q        (A read MN-major; accumulated in registers over the chunk)
 //                      dQ  = dS K                         (per tile, red.global.add.v2.f32 into dqn)
-//                   the bias gradient dTable[hh, i-j] += dS sums the fp32 dS along its diagonals into a per-CTA shared
-//                   table that is flushed to global once.
+//                   the bias enters from a per-tile Toeplitz window in shared memory (per head, pre-scaled by log2 e),
+//                   staged while S and dP run.
+//                   The bias gradient dTable[hh, i-j] += dS: the fp32 dS tile is staged in shared memory and, while dV,
+//                   dK and dQ run, each thread owns (head, diagonal) pairs and sums them in row order into its
+//                   warpgroup's table (no shared-memory float atomics); the two tables are flushed once per unit.
 //
 // Deterministic variant (DET, omlm_attn_bwd_tc_det): the same work units and arithmetic, with every float reduction in a
 // fixed order.  dQ of a row tile and dK|dV of a key tile are still added with red.global.add, but in turns enforced by
 // per-tile counters (the deterministic backward of FlashAttention-3): row tile rt takes the (key tile, warpgroup) pairs
 // in the order (0,0), (0,1), (1,0), ...; key tile kt takes its row chunks in chunk order.  A turn only ever waits for
 // a CTA with a lower block index, which the hardware dispatched first, so the waits cannot deadlock; a wait that does not
-// end within seconds sets an error word and gives up instead of hanging.  The bias gradient stages the fp32 dS tile in
-// shared memory; each thread then owns (head, diagonal) pairs and sums them in row order into its warpgroup's table, the
-// two tables are added per unit into a partial table in global memory, and a second kernel adds the partial tables to
-// dtable in unit order.  After a time-out the error word stays set and later calls skip their waits, until the caller
-// clears it: their sums are then added in arrival order (correct up to rounding, not reproducible).
+// end within seconds sets an error word and gives up instead of hanging.  The two diagonal tables of a unit are added
+// into a partial table in global memory (the default adds them to dtable with one atomic per entry), and a second
+// kernel adds the partial tables to dtable in unit order.  After a time-out the error word stays set and later calls
+// skip their waits, until the caller clears it: their sums are then added in arrival order (correct up to rounding, not
+// reproducible).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -35,11 +38,15 @@ constexpr float kBtL2e = 1.4426950408889634f;
 
 constexpr int kBoK = 0, kBoV = 16384, kBoQ = 32768 /*2 stages x 8K*/, kBoDO = 49152 /*2 x 8K*/;
 constexpr int kBoP = 65536 /*2 wg x 8K*/, kBoDS = 81920 /*2 wg x 8K*/, kBoBar = 98304 /*64 B*/;
-constexpr int kBoAcc = 98368;     // diagonal-sum table: h x Wacc floats
+constexpr int kBoSds = 98368;     // fp32 dS tiles [2 wg][64 rows][kBtSdsLd]
 constexpr int kBtMaxSmem = 232448;
-// DET: fp32 dS tiles [2 wg][64 rows][kBtSdsLd] at kBoAcc, then one diagonal table per warpgroup (2 x h x Wacc floats)
 constexpr int kBtSdsLd = 72;      // padded row: the fragment stores of the 8 rows of a quad land in different banks
-constexpr int kBoAccDet = kBoAcc + 2 * 64 * kBtSdsLd * 4;
+// then the bias windows [2 wg][h][win_ld] floats, then one diagonal-sum table per warpgroup [2][h][Wacc] floats
+constexpr int kBoWin = kBoSds + 2 * 64 * kBtSdsLd * 4;
+
+// Row stride of a bias window: a row tile spans at most ceil(63 / h) + 1 positions, so a warpgroup's window (64 keys)
+// holds at most ceil(63 / h) + 64 deltas; 8 mod 32 floats, so the eight rows of a quad column hit at most two per bank.
+static int bt_win_ld(int h) { return ((62 + h) / h + 64 + 23) / 32 * 32 + 8; }
 
 __device__ __forceinline__ float bt_ex2(float x) {
   float y;
@@ -87,7 +94,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                    const __grid_constant__ CUtensorMap tmKV, const float* __restrict__ lse2, const float* __restrict__ dsum,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                    float* __restrict__ dqn, float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale,
-                   int Wacc, int tiles_per_chunk, int nbatch, const BtDet det) {
+                   int Wacc, int win_ld, int tiles_per_chunk, int nbatch, const BtDet det) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -95,7 +102,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* kv_full = bars + 0;
   uint64_t* qd_full = bars + 1;    // [2]
   uint64_t* qd_empty = bars + 3;   // [2]
-  float* dacc = reinterpret_cast<float*>(smem + (DET ? kBoAccDet : kBoAcc));
+  float* dacc = reinterpret_cast<float*>(smem + kBoWin) + 2 * h * win_ld;
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
   const int R = N * h;
@@ -123,7 +130,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int i = 0; i < 2; ++i) { mbar_init(&qd_full[i], 1); mbar_init(&qd_empty[i], 2); }
     fence_barrier_init();
   }
-  for (int x = threadIdx.x; x < (DET ? 2 : 1) * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
+  for (int x = threadIdx.x; x < 2 * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
   __syncthreads();
   pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
@@ -152,8 +159,9 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const uint32_t sk = smem_u32(smem + kBoK) + cw * 8192, sv = smem_u32(smem + kBoV) + cw * 8192;
     uint8_t* p_tile = smem + kBoP + cw * 8192;
     uint8_t* ds_tile = smem + kBoDS + cw * 8192;
-    float* sdsf = reinterpret_cast<float*>(smem + kBoAcc) + cw * 64 * kBtSdsLd;    // DET: this warpgroup's fp32 dS tile
-    float* wacc = dacc + (DET ? cw * h * Wacc : 0);                                 // DET: this warpgroup's diagonal table
+    float* sdsf = reinterpret_cast<float*>(smem + kBoSds) + cw * 64 * kBtSdsLd;    // this warpgroup's fp32 dS tile
+    float* win = reinterpret_cast<float*>(smem + kBoWin) + cw * h * win_ld;        // this warpgroup's bias window
+    float* wacc = dacc + cw * h * Wacc;                                             // this warpgroup's diagonal table
     const int tid128 = threadIdx.x & 127;
     const uint32_t sp = smem_u32(p_tile), sds = smem_u32(ds_tile);
     const float sc2 = scale * kBtL2e;
@@ -183,10 +191,22 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Wgmma<64, false>::ss<0, 0>(dp, make_smem_desc(sdo + ks * 32, 16, 1024), make_smem_desc(sv + ks * 32, 16, 1024), ks > 0 ? 1u : 0u);
       }
       wgmma_commit();
+      // ---- while S / dP run: the tile's bias window (per head, deltas it_lo - kbase - 63 .. it_hi - kbase, pre-scaled
+      // by log2 e; entries for delta < 0 are never read).  The previous tile's reads of the window ended before every
+      // thread's first barrier of that tile.
+      const int it_lo = min(rbase, R - 1) / h, it_hi = min(rbase + kBtBQ - 1, R - 1) / h;
+      {
+        const int win_w = it_hi - it_lo + 64, dlo = it_lo - kbase - 63;
+        for (int x = tid128; x < h * win_w; x += 128) {
+          const int hh = x / win_w, w = x - hh * win_w, d = dlo + w;
+          win[hh * win_ld + w] = d >= 0 ? __ldg(table + hh * static_cast<long>(table_ld) + d) * kBtL2e : 0.f;
+        }
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
       wgmma_wait<0>();
       wgmma_reg_fence(s);
       wgmma_reg_fence(dp);
-      // ---- P, dS (fp32), diagonal sums, bf16 tiles
+      // ---- P, dS (fp32 staged for the diagonal sums), bf16 tiles
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int lr = wq * 16 + qr + hr * 8;
@@ -196,8 +216,8 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const int i = rc / h, hh = rc - i * h;
         const float lse = lse2[static_cast<long long>(b) * R + rc];
         const float D = dsum[static_cast<long long>(b) * R + rc];
-        const float* trow = table + hh * static_cast<long>(table_ld);
-        float* arow = dacc + hh * Wacc - dmin;
+        const float* wrow = win + hh * win_ld + i - it_lo + 63 - 2 * qc;   // column 8 c + e at wrow[-8 c - e]
+        const int dcol = i - kbase - 2 * qc;                                 // delta of column 8 c + e is dcol - 8 c - e
         uint8_t* prow = p_tile + lr * 128;
         uint8_t* drow = ds_tile + lr * 128;
 #pragma unroll
@@ -205,15 +225,14 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           float pp[2], dd[2];
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const int j = kbase + 8 * c + 2 * qc + e;
-            const int delta = i - j;
-            const bool live = row_ok && ((vis >> (2 * c + e)) & 1u) && delta >= 0;
+            // the causal compare stays: a row whose visible keys all lie in the future has lse2 = -inf, and
+            // exp2(-inf - -inf) would turn its P into NaN instead of 0
+            const bool live = row_ok && ((vis >> (2 * c + e)) & 1u) && dcol >= 8 * c + e;
             const float x = s[4 * c + 2 * hr + e];
-            pp[e] = live ? bt_ex2(fmaf(x, sc2, __ldg(trow + (live ? delta : 0)) * kBtL2e) - lse) : 0.f;
+            pp[e] = live ? bt_ex2(fmaf(x, sc2, wrow[-8 * c - e]) - lse) : 0.f;
             dd[e] = pp[e] * (dp[4 * c + 2 * hr + e] - D);
-            if (!DET && live) atomicAdd(arow + delta, dd[e]);
           }
-          if (DET) *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
+          *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
           const uint32_t off = static_cast<uint32_t>(((c ^ (lr & 7)) << 4) + 4 * qc);
           *reinterpret_cast<uint32_t*>(prow + off) = pack_bf16x2(pp[0], pp[1]);
           *reinterpret_cast<uint32_t*>(drow + off) = pack_bf16x2(dd[0], dd[1]);
@@ -232,9 +251,8 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Wgmma<64, false>::ss<0, 1>(dq, make_smem_desc(sds + ks * 32, 16, 1024), make_smem_desc(sk + ks * 2048, 8192, 1024), ks > 0 ? 1u : 0u);
       }
       wgmma_commit();
-      if constexpr (DET) {
+      {
         // diagonal sums of the fp32 dS tile while the tensor cores run: thread-owned (head, diagonal) pairs, rows in order
-        const int it_lo = rbase / h, it_hi = min((rbase + kBtBQ - 1) / h, N - 1);
         const int dlo = max(0, it_lo - kbase - 63), dhi = it_hi - kbase;
         const int W = dhi - dlo + 1;
         for (int p = tid128; p < h * W; p += 128) {
@@ -307,7 +325,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     } else {
       for (int x = threadIdx.x - 128; x < h * wacc_used; x += 256) {
         const int hh = x / wacc_used, w = x - hh * wacc_used;
-        const float v = dacc[hh * Wacc + w];
+        const float v = dacc[hh * Wacc + w] + dacc[(h + hh) * Wacc + w];
         if (v != 0.f) atomicAdd(dtable + hh * static_cast<long>(table_ld) + dmin + w, v);
       }
     }
@@ -368,17 +386,18 @@ namespace omlm {
 
 // Launch geometry shared by the launch and the workspace query.
 struct BtConfig {
-  int tiles_per_chunk, wacc, smem_bytes, units_per_batch, n_row_tiles, n_key_tiles;
+  int tiles_per_chunk, wacc, win_ld, smem_bytes, units_per_batch, n_row_tiles, n_key_tiles;
 };
 
-static int bt_config(int B, int N, int heads, bool det, BtConfig* cfg) {
+static int bt_config(int B, int N, int heads, BtConfig* cfg) {
   const long R = static_cast<long>(N) * heads;
   const int n_row_tiles = static_cast<int>((R + kBtBQ - 1) / kBtBQ);
   const int n_key_tiles = (N + kBtBK - 1) / kBtBK;
-  // chunk length T: as long as the per-CTA diagonal table (heads x (64 T / heads + 130) floats) fits in shared memory,
-  // and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
+  // chunk length T: as long as the per-CTA diagonal tables (2 x heads x (64 T / heads + 130) floats) fit in shared
+  // memory, and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
+  const int win_ld = bt_win_ld(heads);
   auto wacc_of = [&](int T) { return (T * kBtBQ + heads - 1) / heads + kBtBK + 2; };
-  auto smem_of = [&](int T) { return det ? kBoAccDet + 2 * heads * wacc_of(T) * 4 + 1024 : kBoAcc + heads * wacc_of(T) * 4 + 1024; };
+  auto smem_of = [&](int T) { return kBoWin + 2 * heads * (win_ld + wacc_of(T)) * 4 + 1024; };
   auto units_of = [&](int T) {
     long units = 0;
     for (int kt = 0; kt < n_key_tiles; ++kt) {
@@ -387,7 +406,7 @@ static int bt_config(int B, int N, int heads, bool det, BtConfig* cfg) {
     }
     return units;
   };
-  OMLM_CHECK_ARG(smem_of(1) <= kBtMaxSmem, "attn_bwd_tc: too many heads (%d) for the shared-memory diagonal table", heads);
+  OMLM_CHECK_ARG(smem_of(1) <= kBtMaxSmem, "attn_bwd_tc: too many heads (%d) for the shared-memory bias tables", heads);
   int tiles_per_chunk = 1;
   for (int cand = 2; cand <= 2 * n_row_tiles; cand *= 2) {
     const int T = cand < n_row_tiles ? cand : n_row_tiles;
@@ -401,6 +420,7 @@ static int bt_config(int B, int N, int heads, bool det, BtConfig* cfg) {
   }
   cfg->tiles_per_chunk = tiles_per_chunk;
   cfg->wacc = wacc_of(tiles_per_chunk);
+  cfg->win_ld = win_ld;
   cfg->smem_bytes = smem_of(tiles_per_chunk);
   cfg->units_per_batch = static_cast<int>(units_of(tiles_per_chunk));
   cfg->n_row_tiles = n_row_tiles;
@@ -422,7 +442,7 @@ static int attn_bwd_tc_impl(const void* qn, const void* kvn, const void* d_o, co
   const long R = static_cast<long>(N) * heads;
   const long rows = static_cast<long>(B) * R;
   BtConfig cfg;
-  int rc = bt_config(B, N, heads, det, &cfg);
+  int rc = bt_config(B, N, heads, &cfg);
   if (rc) return rc;
   const int units = B * cfg.units_per_batch;
   BtDet dp{nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -455,7 +475,7 @@ static int attn_bwd_tc_impl(const void* qn, const void* kvn, const void* d_o, co
   }
   OMLM_KLAUNCH((kern), units, kBtThreads, cfg.smem_bytes, st,
       tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale,
-      cfg.wacc, cfg.tiles_per_chunk, B, dp);
+      cfg.wacc, cfg.win_ld, cfg.tiles_per_chunk, B, dp);
   OMLM_LAUNCH_CHECK();
   if (det) {
     OMLM_KLAUNCH((attn_bwd_dtable_reduce_kernel), (heads * N + 255) / 256, 256, 0, st,
@@ -487,7 +507,7 @@ extern "C" int omlm_attn_bwd_tc_det_workspace(int B, int N, int heads, long* ws_
   using namespace omlm;
   OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0 && ws_bytes != nullptr && iws_count != nullptr, "attn_bwd_tc_det_workspace: bad arguments");
   BtConfig cfg;
-  const int rc = bt_config(B, N, heads, true, &cfg);
+  const int rc = bt_config(B, N, heads, &cfg);
   if (rc) return rc;
   *ws_bytes = static_cast<long>(B) * cfg.units_per_batch * heads * cfg.wacc * 4;
   *iws_count = bt_ints(B, cfg);

@@ -11,6 +11,10 @@
 //   warpgroups 1,2  64 query rows each: S = Q K^T (wgmma m64n128k16, operands in 128B-swizzled smem, S in registers),
 //                   online softmax in the log2 domain on the accumulator fragment (a row lives in the four lanes of a
 //                   quad), P -> bf16 in registers, O += P V (wgmma m64n64k16 with A from registers, V read MN-major).
+//                   While S is in flight each warpgroup stages the Toeplitz bias window of its 64 rows and the key tile
+//                   (per head, deltas i_lo - j0 - 127 .. i_hi - j0, pre-scaled by log2 e, -inf for delta < 0 so the
+//                   causal mask costs nothing) in shared memory and ballots the tile's key mask into four words; the
+//                   softmax then reads the bias with LDS instead of one gathered global load per score.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -27,7 +31,14 @@ constexpr int kOffQ = 0;                        // 16 KB
 constexpr int kOffK = 16384;                    // 2 x 16 KB
 constexpr int kOffV = 49152;                    // 2 x 16 KB
 constexpr int kOffBar = 81920;                  // barriers
-constexpr int kTcSmem = kOffBar + 64 + 1024;
+constexpr int kOffWin = kOffBar + 64;           // bias windows: [2 warpgroups][2 buffers][h][win_ld] floats
+constexpr int kTcMaxSmem = 232448;
+
+// Row stride of a bias window: a warpgroup's 64 rows span at most ceil(63 / h) + 1 positions, so a window holds at most
+// ceil(63 / h) + 128 deltas.  The stride is 8 mod 32 floats so the eight rows of a quad column (eight heads at h = 8)
+// read from at most two rows per bank.
+static int fwd_win_ld(int h) { return ((62 + h) / h + 128 + 23) / 32 * 32 + 8; }
+static int fwd_smem(int h) { return kOffWin + 4 * h * fwd_win_ld(h) * 4 + 1024; }
 
 __device__ __forceinline__ float ex2_fast(float x) {
   float y;
@@ -38,7 +49,8 @@ __device__ __forceinline__ float ex2_fast(float x) {
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
-                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int nbatch) {
+                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int nbatch,
+                   int win_ld) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // pointer arithmetic (not an integer round trip) keeps the shared address space visible to the compiler: LDS/STS, not generic LD/ST
@@ -89,15 +101,19 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
   const int cw = wg - 1;
   const int wq = (threadIdx.x >> 5) & 3, qr = lane >> 2, qc = lane & 3;
-  const bool leader = (threadIdx.x & 127) == 0;
-  int rr[2], ii[2];
-  const float* trow[2];
+  const int tid128 = threadIdx.x & 127;
+  const bool leader = tid128 == 0;
+  // this warpgroup's rows span positions i_lo .. i_hi; a tile's window starts at delta i_lo - j0 - 127
+  const int i_lo = min(r0 + cw * 64, R - 1) / h, i_hi = min(r0 + cw * 64 + 63, R - 1) / h;
+  const int win_w = i_hi - i_lo + kTcBK;
+  float* win = reinterpret_cast<float*>(smem + kOffWin) + cw * 2 * h * win_ld;   // [2 buffers][h][win_ld]
+  int rr[2], woff[2];    // woff: window offset of (row, column 2 qc) in a buffer; column 8 c + e is woff - 8 c - e
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     rr[hr] = r0 + cw * 64 + wq * 16 + qr + hr * 8;
     const int rc = min(rr[hr], R - 1);
-    ii[hr] = rc / h;
-    trow[hr] = table + (rc - ii[hr] * h) * static_cast<long>(table_ld);
+    const int i = rc / h;
+    woff[hr] = (rc - i * h) * win_ld + i - i_lo + kTcBK - 1 - 2 * qc;
   }
   const unsigned char* km = key_mask != nullptr ? key_mask + static_cast<long long>(b) * N : nullptr;
   const float sc2 = scale * kL2e;
@@ -118,22 +134,37 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       Wgmma<128, false>::ss<0, 0>(s, make_smem_desc(sq + ks * 32, 16, 1024), make_smem_desc(sk + st * 16384 + ks * 32, 16, 1024),
                                   ks > 0 ? 1u : 0u);
     wgmma_commit();
+    // ---- while S runs: the tile's bias window (buffer t & 1) and key-visibility words (bit l of word k = column 32 k + l)
+    const int j0 = t * kTcBK;
+    float* wt = win + (t & 1) * h * win_ld;
+    {
+      const int dlo = i_lo - j0 - (kTcBK - 1);
+      for (int x = tid128; x < h * win_w; x += 128) {
+        const int hh = x / win_w, w = x - hh * win_w, d = dlo + w;
+        wt[hh * win_ld + w] = d >= 0 ? __ldg(table + hh * static_cast<long>(table_ld) + d) * kL2e : -INFINITY;
+      }
+    }
+    uint32_t visw[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int j = j0 + 32 * k + lane;
+      visw[k] = __ballot_sync(0xffffffffu, j < N && (km == nullptr || km[j] != 0));
+    }
+    // the buffer written here was last read in tile t - 2, before every thread's barrier of tile t - 1
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
     wgmma_wait<0>();
     wgmma_reg_fence(s);
-    // ---- bias, masks, row maxima (columns j = j0 + 8 c + 2 qc + {0,1} of rows ii[0], ii[1])
-    const int j0 = t * kTcBK;
+    // ---- bias, masks, row maxima (columns j = j0 + 8 c + 2 qc + {0,1} of this thread's two rows)
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int c = 0; c < 16; ++c) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int j = j0 + 8 * c + 2 * qc + e;
-        const bool vis = j < N && (km == nullptr || km[j] != 0);
+        const bool vis = (visw[c >> 2] >> (8 * (c & 3) + 2 * qc + e)) & 1u;
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
-          const int delta = ii[hr] - j;
           float& x = s[4 * c + 2 * hr + e];
-          x = (vis && delta >= 0) ? fmaf(x, sc2, __ldg(trow[hr] + delta) * kL2e) : -INFINITY;
+          x = vis ? fmaf(x, sc2, wt[woff[hr] - 8 * c - e]) : -INFINITY;   // delta < 0: the window holds -inf
           mx[hr] = fmaxf(mx[hr], x);
         }
       }
@@ -203,20 +234,23 @@ extern "C" int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* ta
   using namespace omlm;
   OMLM_CHECK_ARG(B > 0 && N > 0 && heads > 0, "attn_fwd_tc: bad shape");
   OMLM_CHECK_ARG(table_ld >= N, "attn_fwd_tc: bias table shorter than the sequence");
+  const int smem = fwd_smem(heads);
+  OMLM_CHECK_ARG(smem <= kTcMaxSmem, "attn_fwd_tc: too many heads (%d) for the shared-memory bias windows", heads);
   const long R = static_cast<long>(N) * heads;
   CUtensorMap tmQ, tmKV;
   int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(B) * R, 128, 64, kTcBQ);
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kTcBK);
   if (rc) return rc;
-  static bool configured = false;
-  if (!configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
-    configured = true;
+  static int configured = 0;
+  if (configured < smem) {
+    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = smem;
   }
   const unsigned grid = static_cast<unsigned>((R + kTcBQ - 1) / kTcBQ) * B;   // (row block, batch) in LPT order
-  OMLM_KLAUNCH((attn_fwd_tc_kernel), grid, kTcThreads, kTcSmem, reinterpret_cast<cudaStream_t>(stream),
-      tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, B);
+  OMLM_KLAUNCH((attn_fwd_tc_kernel), grid, kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
+      tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, B,
+      fwd_win_ld(heads));
   OMLM_LAUNCH_CHECK();
   return 0;
 }

@@ -27,7 +27,11 @@ def run(B, N, h, tag):
         return e0.elapsed_time(e1) / n * 1e3
     us_f = t(lambda: lib.attn_fwd_tc(qn, kvn, table, km, out, lse, B, N, h))
     us_b = t(lambda: lib.attn_bwd_tc(qn, kvn, d_o, out, lse, table, km, dsum, dqn, dkvn, dtab, B, N, h))
-    print(f"{tag}: B={B} N={N} h={h}  fwd {us_f:.1f} us ({fl / us_f / 1e6:.0f} TF/s)   bwd {us_b:.1f} us ({2.5 * fl / us_b / 1e6:.0f} TF/s)", flush=True)
+    det = lib.AttnBwdDetWorkspace("cuda", B, N, h)
+    us_d = t(lambda: lib.attn_bwd_tc(qn, kvn, d_o, out, lse, table, km, dsum, dqn, dkvn, dtab, B, N, h, det=det))
+    assert not det.error()
+    print(f"{tag}: B={B} N={N} h={h}  fwd {us_f:.1f} us ({fl / us_f / 1e6:.0f} TF/s)   bwd {us_b:.1f} us ({2.5 * fl / us_b / 1e6:.0f} TF/s)"
+          f"   bwd det {us_d:.1f} us ({2.5 * fl / us_d / 1e6:.0f} TF/s)", flush=True)
 
 
 if __name__ == "__main__":
