@@ -17,12 +17,12 @@
 extern "C" {
 #endif
 
-#define OMLM_B200_ABI_VERSION 2
+#define OMLM_B200_ABI_VERSION 3
 #define OMLM_MAX_SEQS 4
 
 const char* omlm_last_error(void);
 int omlm_abi_version(void);
-/* 0 iff the current CUDA device is compute capability 10.x. */
+/* 0 iff the current CUDA device is compute capability 9.0. */
 int omlm_device_check(void);
 /* Number of SMs of the current device (the persistent kernels' default grid). */
 int omlm_num_sms(void);
@@ -324,24 +324,6 @@ int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_s
  * shifted in place) -> h [B, Fp], rowsum [B, Fp/128, 2]. */
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,
                            int act_f16, void* stream);
-/* The whole incremental step in ONE launch (csrc/decode_fused.cu): embedding row, L x (q/kv projection, cached attention,
- * out-projection + residual, FFN-up + conv + GEGLU, inner LayerNorm + FFN-down + residual), final LayerNorm + the logit
- * head `w_logit` [C_pad, d] -> logits [B, ld_logits] fp32.  One CTA per SM with grid-wide barriers between the stages;
- * bit-identical to the sequence of omlm_embed_gather / omlm_skinny_gemm / omlm_attn_decode / omlm_decode_conv_geglu calls.
- * layers_device: DEVICE array of L records.  barrier: one device uint (zeroed by the call); err_flag is set to 1 if a
- * barrier times out (never hangs).  x0 (result), x1: fp32 [B, d] scratch; q_raw [B, heads*64], kv_raw [B, 128], o [B, heads*64]
- * bf16 scratch; hbuf [B, Fp] 16-bit and hf32 [B, Fp] fp32 scratch. */
-typedef struct {
-  const void *wq, *wkv, *wo, *w1, *w2;
-  const float *conv, *gin, *g_attn, *g_ff, *q_scale, *k_scale;
-  void* cache;
-  void* conv_state;
-} omlm_decode_layer;
-int omlm_decode_step(const omlm_decode_layer* layers_device, int L, int B, int d, int heads, int F, int Fp, int n_max, int act_f16,
-                     const float* emb_table, const int* next_row, const float* table, int table_ld, const int* pos_ptr,
-                     float* x0, float* x1, void* q_raw, void* kv_raw, void* o, void* hbuf, float* hf32, const void* w_logit,
-                     int C_pad, const float* g_final, float* logits, long ld_logits, unsigned int* barrier, int* err_flag,
-                     float scale, void* stream);
 /* Sampling of one token per sequence (open_musiclm.py:309-319, utils.py:71-84): eos (class C-1) forbidden unless
  * allow_eos, top-k with the given k, Gumbel-argmax at `temperature`.  uniform: optional [steps, B, C] uniform(0,1) draws
  * (slice *step_ptr is used; reproduces a given torch stream), else a Philox stream keyed by *seed.  Writes

@@ -44,7 +44,6 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
 __global__ void __launch_bounds__(256)
 attn_bwd_dsum_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat16* __restrict__ o,
                      float* __restrict__ dsum, long rows) {
-  pdl_prologue();
   const long r = (static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 3;
   const int sub = threadIdx.x & 7;
   float s = 0.f;
@@ -71,7 +70,6 @@ attn_bwd_kernel(const __nv_bfloat16* __restrict__ qn, const __nv_bfloat16* __res
                 const unsigned char* __restrict__ key_mask, float* __restrict__ dqn,
                 float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale,
                 int tiles_per_chunk, int units_per_batch) {
-  pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem_raw[];
   AttnBwdSmem& sm = *reinterpret_cast<AttnBwdSmem*>(smem_raw);
   const int R = N * h;

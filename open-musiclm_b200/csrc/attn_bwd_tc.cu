@@ -95,7 +95,6 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                    float* __restrict__ dqn, float* __restrict__ dkvn, float* __restrict__ dtable, int N, int h, float scale,
                    int Wacc, int win_ld, int tiles_per_chunk, int nbatch, const BtDet det) {
-  pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kBoBar);
@@ -132,7 +131,6 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   }
   for (int x = threadIdx.x; x < 2 * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
   __syncthreads();
-  pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
@@ -336,7 +334,6 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 __global__ void __launch_bounds__(256)
 attn_bwd_dtable_reduce_kernel(const float* __restrict__ dpart, const int* __restrict__ meta, int units, int h, int Wacc,
                               float* __restrict__ dtable, int table_ld, int N) {
-  pdl_prologue();
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= h * N) return;
   const int hh = x / N, d = x - hh * N;
@@ -354,7 +351,6 @@ attn_bwd_dtable_reduce_kernel(const float* __restrict__ dpart, const int* __rest
 __global__ void __launch_bounds__(256)
 attn_bwd_tc_dsum_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat16* __restrict__ o,
                         float* __restrict__ dsum, long rows, float* __restrict__ dqn, float* __restrict__ dkvn, long kv_vec4) {
-  pdl_prologue();
   const long tid = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long r = tid >> 3;
   const int sub = threadIdx.x & 7;

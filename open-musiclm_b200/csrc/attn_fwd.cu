@@ -30,7 +30,6 @@ __global__ void __launch_bounds__(kAttnThreads, 2)
 attn_fwd_kernel(const __nv_bfloat16* __restrict__ qn, const __nv_bfloat16* __restrict__ kvn,
                 const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                 __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale) {
-  pdl_prologue();
   extern __shared__ __align__(128) uint8_t smem_raw[];
   AttnFwdSmem& sm = *reinterpret_cast<AttnFwdSmem*>(smem_raw);
   const int b = blockIdx.y;

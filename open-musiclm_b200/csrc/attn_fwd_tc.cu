@@ -51,7 +51,6 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                    __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int nbatch,
                    int win_ld) {
-  pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // pointer arithmetic (not an integer round trip) keeps the shared address space visible to the compiler: LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -78,7 +77,6 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer

@@ -45,29 +45,12 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* gptr, uint64_t dim0, uint64_
 
 int num_sms();
 
-// ---- kernel launches: programmatic dependent launch (PDL), OFF by default ---------------------------------------------
-// Every kernel of the library can be launched with the programmatic-stream-serialization attribute (OMLM_PDL=1); it then
-//   * executes griddepcontrol.launch_dependents first thing (the next kernel's CTAs may become resident as soon as
-//     this grid's CTAs have all started and resources free up), and
-//   * executes griddepcontrol.wait before its first global-memory access (it blocks until the previous grid has
-//     completed and its writes are visible), after whatever private set-up it can do early.
-// The persistent GEMM CTAs own the whole shared memory of their SM, so a dependent CTA cannot become resident before
-// its predecessor exits; the default is therefore the plain stream order.  Without the attribute both instructions
-// are no-ops.
-bool pdl_enabled();
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_prologue() { pdl_launch_dependents(); pdl_wait(); }
-
+// ---- kernel launches ----------------------------------------------------------------------------------------------------
+// cudaLaunchKernelEx returns the launch's own error, so a failure is reported at the launch that caused it.
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 #define OMLM_KLAUNCH(kern, grid, block, smem, stream, ...)                                                   \

@@ -43,7 +43,6 @@ constexpr int kSkWarps = 8, kSkRowsPerWarp = 2;
 
 __global__ void __launch_bounds__(kSkWarps * 32)
 skinny_gemm_kernel(const SkinnyArgs a) {
-  pdl_prologue();
   extern __shared__ __align__(16) uint8_t sk_smem[];
   uint16_t* sA = reinterpret_cast<uint16_t*>(sk_smem);              // [B][K] in the operand format
   __shared__ float s_mean[kDecMaxB], s_rstd[kDecMaxB];
@@ -153,7 +152,6 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16*
                    const float* __restrict__ q_scale, const float* __restrict__ k_scale,
                    __nv_bfloat16* __restrict__ cache, long cache_ld_b, const float* __restrict__ table, int table_ld,
                    const int* __restrict__ pos_ptr, __nv_bfloat16* __restrict__ out, int h, float scale) {
-  pdl_prologue();
   extern __shared__ __align__(16) float ad_smem[];
   float* sc = ad_smem;                       // [n + 1] scores, then probabilities
   __shared__ float sq[64], sk[64], sv[64];
@@ -273,7 +271,6 @@ attn_decode_mqa_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloa
                        __nv_bfloat16* __restrict__ cache, long cache_ld_b, const float* __restrict__ table, int table_ld,
                        const int* __restrict__ pos_ptr, __nv_bfloat16* __restrict__ out, int h, float scale,
                        float* __restrict__ part_o, float2* __restrict__ part_ml, int* __restrict__ counters, int max_splits) {
-  pdl_prologue();
   extern __shared__ __align__(16) uint8_t mq_smem[];
   uint8_t* skv = mq_smem;                                                      // [kMqKeys][kMqRow]
   float* sc = reinterpret_cast<float*>(mq_smem + kMqKeys * kMqRow);            // [HM][kMqScLd] scores, then P
@@ -444,7 +441,6 @@ static int launch_attn_decode_mqa(dim3 grid, cudaStream_t st, const void* q_raw,
 __global__ void __launch_bounds__(128)
 decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restrict__ state, const float* __restrict__ conv_w,
                          uint16_t* __restrict__ h_out, float* __restrict__ rowsum, int Fp, int f16) {
-  pdl_prologue();
   const int grp = blockIdx.x, b = blockIdx.y, c = threadIdx.x;
   const long col_v = static_cast<long>(grp) * 256 + c, col_g = col_v + 128;
   const long ld = 2L * Fp;
@@ -488,7 +484,6 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
               long long* __restrict__ tokens, long tokens_ld, int* __restrict__ next_row, int row_offset,
               int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B) {
-  pdl_prologue();
   extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys
   float* lg = sm_l;
   uint32_t* key = reinterpret_cast<uint32_t*>(sm_l + C);

@@ -32,7 +32,6 @@ template <bool F16>
 __global__ void __launch_bounds__(128)
 decode_gemm_prologue_kernel(const void* __restrict__ A, long lda, int prologue, const float* __restrict__ gamma,
                             const float* __restrict__ rowsum, int n_real, uint16_t* __restrict__ a16, int K) {
-  pdl_prologue();
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
   __shared__ float s_mean, s_rstd;
   if (prologue >= 2) {
@@ -109,7 +108,6 @@ template <int BN, int WGS, bool F16>
 __global__ void __launch_bounds__(WGS * 128 + 32, 1)
 decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmA, const DgEpi ep,
                    const int B, const int N, const int K, const int kb_per_split, const int stages) {
-  pdl_launch_dependents();
   using S = DgSmem<BN, WGS>;
   constexpr int kConsumers = WGS * 128;
   extern __shared__ uint8_t dg_smem_raw[];
@@ -131,7 +129,6 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (threadIdx.x >= kConsumers) {
     // ------------------------------------------------------------------ TMA producer (one thread)
@@ -193,7 +190,6 @@ decode_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constan
 template <int BN, int WGS>
 __global__ void __launch_bounds__(256)
 decode_gemm_reduce_kernel(const DgEpi ep, const int B, const int N, const int tiles, const int splits) {
-  pdl_prologue();
   constexpr int kConsumers = WGS * 128;
   const long per_split = static_cast<long>(tiles) * (BN / 2) * kConsumers;
   const long idx = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x;

@@ -73,7 +73,6 @@ ffn_norm_fwd_kernel(const __nv_bfloat16* __restrict__ h, const float2* __restric
                     const float* __restrict__ gamma, __nv_bfloat16* __restrict__ hn, __nv_bfloat16* __restrict__ hn_copy, float2* __restrict__ stats,
                     uint8_t* __restrict__ keep_bits, long M, int F, int Fp, float drop_p,
                     const unsigned long long* __restrict__ seed_ptr, uint32_t layer) {
-  pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long row = static_cast<long>(blockIdx.x) * 8 + warp;
   if (row >= M) return;
@@ -129,7 +128,6 @@ __global__ void __launch_bounds__(256)
 ffn_mid_bwd_stats_kernel(const __nv_bfloat16* __restrict__ dhn, const __nv_bfloat16* __restrict__ hn,
                          const float* __restrict__ gamma, float2* __restrict__ rowstat, long M, int F, int Fp,
                          float drop_p, const uint8_t* __restrict__ keep_bits) {
-  pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long row = static_cast<long>(blockIdx.x) * 8 + warp;
   if (row >= M) return;
@@ -186,7 +184,6 @@ __global__ void __launch_bounds__(kTileThreads, 2)
 ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, const float2* __restrict__ stats,
                         const float2* __restrict__ rowstat, const int parts, __nv_bfloat16* __restrict__ du,
                         float* __restrict__ dgamma, float* __restrict__ dconv_w, float* __restrict__ part) {
-  pdl_prologue();
   extern __shared__ __align__(16) uint8_t tsm[];
   uint8_t* su = tsm + kTOffU;
   uint8_t* sd = tsm + kTOffD;

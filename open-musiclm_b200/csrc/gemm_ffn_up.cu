@@ -33,7 +33,6 @@ __global__ void __launch_bounds__(kFuThreads, 1)
 gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    __nv_bfloat16* __restrict__ u_out, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rowsum,
                    const float* __restrict__ conv_w, int M, int Nseq, int K, int Fp) {
-  pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kFuOffBar);
@@ -52,7 +51,6 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");

@@ -65,7 +65,6 @@ template <int BN, int A_MN, int B_MN, bool F16, bool RS = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const EpiParams ep, const int M, const int N, const int K, const int splits, const int kStages) {
-  pdl_launch_dependents();
   using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atoms.
@@ -93,7 +92,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();   // private set-up done: from here on global memory written by the previous kernel is touched
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
@@ -388,7 +386,6 @@ namespace omlm {
 __global__ void __launch_bounds__(256)
 splitk_reduce_kernel(float* __restrict__ out, long ldo, const float* __restrict__ part, long slice, long ldp, int splits,
                      int rows_out, int n_valid) {
-  pdl_prologue();
   const long total = static_cast<long>(rows_out) * n_valid;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const long r = i / n_valid, c = i - r * n_valid;

@@ -5,7 +5,6 @@
 #include <cudaTypedefs.h>
 #include <stdarg.h>
 #include <string.h>
-#include <stdlib.h>
 #include <mutex>
 
 namespace omlm {
@@ -85,15 +84,6 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* gptr, uint64_t dim0, uint64_
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   OMLM_CHECK_ARG(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (3-D) failed with CUresult %d", (int)r);
   return 0;
-}
-
-bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char* e = getenv("OMLM_PDL");       // OMLM_PDL=1 turns programmatic dependent launch on (see common.cuh)
-    on = (e != nullptr && e[0] == '1') ? 1 : 0;
-  }
-  return on == 1;
 }
 
 int num_sms() {

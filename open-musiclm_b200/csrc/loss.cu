@@ -20,7 +20,6 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long ld, const int* __restri
                   int rows_per_batch, long batch_stride,
                   int rows, int C, int ignore_index, float grad_scale, float loss_scale, __nv_bfloat16* __restrict__ dlogits,
                   long ldd, int Cp, float* __restrict__ loss_acc, float2* __restrict__ part) {
-  pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * 8 + warp;
   float my_loss = 0.f, my_cnt = 0.f;

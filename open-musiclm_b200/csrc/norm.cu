@@ -20,7 +20,6 @@ __global__ void __launch_bounds__(kNormThreads)
 layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                      __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ ycopy, __nv_bfloat16* __restrict__ xraw,
                      float2* __restrict__ stats, const int* __restrict__ dest_row, int M, int D, int y_f16) {
-  pdl_prologue();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * (kNormThreads / 32) + warp;
   if (row >= M) return;
@@ -99,7 +98,6 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restri
                      const int* __restrict__ src_row, float* __restrict__ dx,
                      __nv_bfloat16* __restrict__ dx_bf16, float* __restrict__ dgamma, int M, int D,
                      int rows_per_block, float* __restrict__ part) {
-  pdl_prologue();
   constexpr int kRow = NCHUNK * 128;                 // padded row length in elements
   constexpr int kStage = kRow * 12;                  // x fp32 | dres fp32 | dy bf16 | draw bf16
   extern __shared__ __align__(16) uint8_t lsm[];
@@ -235,7 +233,6 @@ __global__ void __launch_bounds__(256)
 qk_l2norm_fwd_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16* __restrict__ kv_raw,
                      const float* __restrict__ q_scale, const float* __restrict__ k_scale,
                      __nv_bfloat16* __restrict__ qn, __nv_bfloat16* __restrict__ kvn, int M, int h) {
-  pdl_prologue();
   const long long gvec = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 3;
   const int sub = threadIdx.x & 7;
   const int per_row = h + 2;
@@ -292,7 +289,6 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
                      const float* __restrict__ q_scale, const float* __restrict__ k_scale,
                      __nv_bfloat16* __restrict__ dq_raw, __nv_bfloat16* __restrict__ dkv_raw,
                      float* __restrict__ dq_scale, float* __restrict__ dk_scale, int M, int h, float* __restrict__ part) {
-  pdl_prologue();
   __shared__ float sds[2][64];
   __shared__ float sslot[DET ? 2 * 32 * 64 : 1];
   if (threadIdx.x < 128) sds[threadIdx.x >> 6][threadIdx.x & 63] = 0.f;

@@ -15,7 +15,6 @@ namespace omlm {
 // instead, and sumsq_finish_kernel adds the blocks' sums to acc in block order.
 __global__ void __launch_bounds__(512)
 sumsq_kernel(const float* __restrict__ g, long n, float prescale, double* __restrict__ acc, double* __restrict__ part) {
-  pdl_prologue();
   float s = 0.f;
   const long n4 = n >> 2;
   const float4* g4 = reinterpret_cast<const float4*>(g);
@@ -39,7 +38,6 @@ sumsq_kernel(const float* __restrict__ g, long n, float prescale, double* __rest
 }
 
 __global__ void __launch_bounds__(32) sumsq_finish_kernel(const double* __restrict__ part, int n, double* __restrict__ acc) {
-  pdl_prologue();
   double s = 0.0;
   for (int i = threadIdx.x; i < n; i += 32) s += part[i];
 #pragma unroll
@@ -52,7 +50,6 @@ __global__ void __launch_bounds__(32) sumsq_finish_kernel(const double* __restri
 __global__ void __launch_bounds__(512)
 adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              long n, long n_decay, const float* __restrict__ hyper, const double* __restrict__ sumsq) {
-  pdl_prologue();
   const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4];
   const float bc1 = hyper[5], bc2 = hyper[6], max_norm = hyper[7], prescale = hyper[8];
   float coef = prescale;
@@ -175,7 +172,6 @@ __device__ __forceinline__ void pack_quad(long i, const float* __restrict__ src,
 template <typename OutT>
 __global__ void pack_kernel(const float* __restrict__ src, long src_ld, int rows_valid, int cols_valid,
                             OutT* __restrict__ dst, long dst_ld, int rows_p, int cols_p, int split_dst, int split_src) {
-  pdl_prologue();
   const long total = static_cast<long>(rows_p) * ((cols_p + 3) >> 2);
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x)
     pack_quad<OutT>(i, src, src_ld, rows_valid, cols_valid, dst, dst_ld, cols_p, split_dst, split_src);
@@ -186,7 +182,6 @@ __global__ void pack_kernel(const float* __restrict__ src, long src_ld, int rows
 constexpr int kPackMaxJobs = 512;
 constexpr int kPackUnit = 1024;      // quads per unit: 4 per thread, 256 apart (coalesced), all four loads in flight together
 __global__ void __launch_bounds__(256) pack_multi_kernel(const omlm_pack_job* __restrict__ jobs, int njobs, long total_units) {
-  pdl_prologue();
   __shared__ long starts[kPackMaxJobs + 1];
   __shared__ omlm_pack_job s_job;
   for (int j = threadIdx.x; j < njobs; j += blockDim.x) starts[j] = jobs[j].unit_start;
@@ -224,7 +219,6 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const omlm_pack_job* __
 __global__ void unpack_add_kernel(const float* __restrict__ packed, long p_ld, int rows_p, int cols_p,
                                   float* __restrict__ dst, long dst_ld, int rows_valid, int cols_valid,
                                   int split_dst, int split_src) {
-  pdl_prologue();
   const long total = static_cast<long>(rows_p) * cols_p;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int r = static_cast<int>(i / cols_p), c = static_cast<int>(i - static_cast<long>(r) * cols_p);

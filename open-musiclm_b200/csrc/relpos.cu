@@ -16,7 +16,6 @@ sgemm_small_kernel(const float* __restrict__ A, long sa_m, long sa_k, const floa
                    long sb_k, long sb_n, float* __restrict__ C, long sc_m, long sc_n,
                    float* __restrict__ Z, const float* __restrict__ bias, int M, int N, int K, int act,
                    int accumulate) {
-  pdl_prologue();
   __shared__ float As[16][64 + 4];
   __shared__ float Bs[16][64 + 4];
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
@@ -77,7 +76,6 @@ sgemm_small_kernel(const float* __restrict__ A, long sa_m, long sa_k, const floa
 // dZ = dA * silu'(z),  silu'(z) = s + z*s*(1-s), s = sigmoid(z)
 __global__ void silu_bwd_kernel(const float* __restrict__ dA, const float* __restrict__ Zp,
                                 float* __restrict__ dZ, __nv_bfloat16* __restrict__ dZ_bf16, long n) {
-  pdl_prologue();
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long>(gridDim.x) * blockDim.x) {
     const float z = Zp[i];
@@ -91,7 +89,6 @@ __global__ void silu_bwd_kernel(const float* __restrict__ dA, const float* __res
 // out[n] (+)= sum_m X[m*s_m + n*s_n]
 __global__ void colsum_kernel(const float* __restrict__ X, long s_m, long s_n, float* __restrict__ out,
                               int M, int N, int accumulate) {
-  pdl_prologue();
   const int n = blockIdx.x;
   float s = 0.f;
   for (int m = threadIdx.x; m < M; m += blockDim.x) s += X[m * s_m + n * s_n];
@@ -111,7 +108,6 @@ __global__ void colsum_kernel(const float* __restrict__ X, long s_m, long s_n, f
 // A3 . W3^T = a_hi w_hi + a_hi w_lo + a_lo w_hi  ~  a . w  to ~2^-16 relative, accumulated in fp32 by wgmma.
 __global__ void split3_kernel(const float* __restrict__ src, long src_ld, __nv_bfloat16* __restrict__ dst, int R,
                               int C, int weight_mode) {
-  pdl_prologue();
   const long total = static_cast<long>(R) * C;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int r = static_cast<int>(i / C), c = static_cast<int>(i - static_cast<long>(r) * C);
@@ -127,7 +123,6 @@ __global__ void split3_kernel(const float* __restrict__ src, long src_ld, __nv_b
 
 // z += bias (in place);  a = silu(z)
 __global__ void bias_silu_kernel(float* __restrict__ z, const float* __restrict__ bias, float* __restrict__ a, int R, int C) {
-  pdl_prologue();
   const long total = static_cast<long>(R) * C;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % C);
@@ -138,7 +133,6 @@ __global__ void bias_silu_kernel(float* __restrict__ z, const float* __restrict_
 }
 
 __global__ void arange_kernel(float* out, int n) {
-  pdl_prologue();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out[i] = static_cast<float>(i);
 }

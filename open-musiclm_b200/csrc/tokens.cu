@@ -29,7 +29,6 @@ __global__ void token_plan_kernel(const TokenPlanArgs a, const unsigned char* __
                                   long long* __restrict__ ids_out, int* __restrict__ src_row,
                                   unsigned char* __restrict__ key_mask, int* __restrict__ labels,
                                   int* __restrict__ err_flag, int N, int n_ids_total, int n_labels_total) {
-  pdl_prologue();
   const int b = blockIdx.x;
   int pos = 0, id_off = 0, lab_off = 0;
   for (int s = 0; s < a.n_seqs; ++s) {
@@ -85,7 +84,6 @@ __global__ void token_plan_kernel(const TokenPlanArgs a, const unsigned char* __
 __global__ void forgetful_mask_kernel(unsigned char* __restrict__ keep, int N, int num_drop,
                                       const unsigned long long* __restrict__ seed_ptr,
                                       unsigned long long stream_id) {
-  pdl_prologue();
   extern __shared__ unsigned int keys[];
   const int b = blockIdx.x;
   const unsigned long long seed = *seed_ptr;
@@ -111,7 +109,6 @@ __global__ void forgetful_mask_kernel(unsigned char* __restrict__ keep, int N, i
 // a negative row contributes zero.  fp32 table, fp32 out; 128-bit copies.
 __global__ void embed_gather_kernel(const float* __restrict__ table, const int* __restrict__ src_row,
                                     const int* __restrict__ src_row2, float* __restrict__ x, int M, int D) {
-  pdl_prologue();
   const int vec_per_row = D >> 2;
   const long long total = static_cast<long long>(M) * vec_per_row;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -134,7 +131,6 @@ __global__ void embed_gather_kernel(const float* __restrict__ table, const int* 
 // dtable[src_row[m], :] += scale * dx[m, :]   (scale = grad_shrink alpha, utils.py:60-61).
 __global__ void embed_scatter_kernel(float* __restrict__ dtable, const int* __restrict__ src_row,
                                      const float* __restrict__ dx, int M, int D, float scale) {
-  pdl_prologue();
   const int vec_per_row = D >> 2;
   const long long total = static_cast<long long>(M) * vec_per_row;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
@@ -156,7 +152,6 @@ __global__ void embed_scatter_kernel(float* __restrict__ dtable, const int* __re
 // first position walks the remaining positions, adds the matching dx rows in order onto the table row and restores the
 // row's marker to INT_MAX.  The adds are the default kernel's (dst + dx * scale, each rounded), in position order.
 __global__ void embed_first_kernel(const int* __restrict__ src_row, int M, int rows, int* __restrict__ first) {
-  pdl_prologue();
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= M) return;
   const int r = src_row[m];
@@ -167,7 +162,6 @@ template <int NCH>
 __global__ void __launch_bounds__(256)
 embed_scatter_det_kernel(float* __restrict__ dtable, const int* __restrict__ src_row, const float* __restrict__ dx, int M, int D,
                          int rows, float scale, int* __restrict__ first) {
-  pdl_prologue();
   const int lane = threadIdx.x & 31;
   const int m = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (m >= M) return;
@@ -304,7 +298,6 @@ int omlm_embed_scatter_add_det(float* dtable, const int* src_row, const float* d
 namespace omlm {
 __global__ void gather_windows_kernel(const short* __restrict__ src, const long long* __restrict__ start, long long* __restrict__ out,
                                       int len, int width, int B) {
-  pdl_prologue();
   const long long per_row = static_cast<long long>(len) * width;
   const long long total = per_row * B;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {

@@ -12,7 +12,6 @@ Up to 16 sequences per call run the SIMT kernels (skinny_gemm, attn_decode); 17 
 csrc/decode_gemm.cu, whose batch is the tensor cores' N operand, and attn_decode_mqa, which reads every cached row once
 per sequence instead of once per head.  The choice follows from the batch size; it is not an option.
 """
-import os
 from typing import List, Optional, Sequence
 
 import torch
@@ -51,9 +50,6 @@ class DecodeSession:
             raise NotImplementedError("open_musiclm_b200 generate: absolute position embeddings are not supported by the decode path")
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
-        if B > SKINNY_MAX_BATCH and os.environ.get("OMLM_DECODE_FUSED", "0") == "1":
-            raise lib.OmlmError(f"open_musiclm_b200 generate: the fused decode step (OMLM_DECODE_FUSED=1) supports at most "
-                                f"{SKINNY_MAX_BATCH} sequences (got {B})")
         self.eng, self.B, self.n_prompt, self.n_new = eng, B, n_prompt, n_new
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
         d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
@@ -83,49 +79,17 @@ class DecodeSession:
         eng.build_bias_table(self.rp, N)
         self.table = self.rp["table"]
         self._graphs = {}
-        # OMLM_DECODE_FUSED=1: the whole step as ONE persistent kernel (csrc/decode_fused.cu; bit-identical to the per-op
-        # sequence in step_ops).  Off by default: on the 10 s three-stage generation it is slower than the graph-replayed
-        # per-op launches (5.41 s vs 4.10 s on an H100 SXM at a 400 W power limit, tools/time_generate.py) -- its 31
-        # stages are each bound by a single-warp prologue (LayerNorm statistics, row-sum tree) and a grid barrier.
-        self.fused = os.environ.get("OMLM_DECODE_FUSED", "0") == "1"
         # more than 16 sequences: tensor-core GEMMs and the cache-sharing attention, with their scratch allocated here so
         # that graph capture allocates nothing
         self.batched = B > SKINNY_MAX_BATCH
         if self.batched:
             shapes = [(HD, d), (128, d), (d, HD), (2 * Fp, d), (d, Fp)] + [(cp, d) for cp in eng.Cp]
             self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h)
-        if self.fused:
-            pv = eng.pview
-            layers = []
-            for l in range(eng.L):
-                p, pk = f"transformer.layers.{l}.", eng.pk[l]
-                layers.append(dict(wq=pk["wq"], wkv=pk["wkv_b"], wo=pk["wo_b"], w1=pk["w1"], w2=pk["w2"], conv=pk["conv"], gin=pk["gin"],
-                                   g_attn=pv[p + "0.norm.gamma"], g_ff=pv[p + eng.ffk["g1"]], q_scale=pv[p + "0.q_scale"],
-                                   k_scale=pv[p + "0.k_scale"], cache=self.cache[l], conv_state=self.conv[l]))
-            self.layer_table, self._keep = lib.decode_layer_table(layers, dev)
-            self.hf32 = E(B, Fp, dt=f32)
-            self.barrier = torch.zeros(1, device=dev, dtype=torch.int32)
-            self.err_flag = torch.zeros(1, device=dev, dtype=torch.int32)
 
     # ------------------------------------------------------------------------------------------ one incremental step
     def step(self, qi_next: int):
         """Processes the position self.pos (embedding row self.next_row) through all layers and leaves the logits of
-        head qi_next in self.logits."""
-        if not self.fused:
-            return self.step_ops(qi_next)
-        eng = self.eng
-        S = len(eng.seqs) - 1
-        lib.decode_step(self.layer_table, eng.L, self.B, eng.d, eng.h, eng.F, eng.Fp, self.n_max, eng.a16 == torch.float16, eng.table,
-                        self.next_row, self.table, self.pos, self.x[0], self.x[1], self.q_raw, self.kv_raw, self.o, self.h, self.hf32,
-                        eng.pk_logit[S][qi_next], eng.pview["transformer.norm.gamma"], self.logits, self.barrier, self.err_flag)
-
-    def check(self):
-        """Raises if a grid-wide barrier of the fused step timed out (synchronises)."""
-        if self.fused and int(self.err_flag.item()):
-            raise lib.OmlmError("open_musiclm_b200 generate: the fused decode step timed out at a grid barrier")
-
-    def step_ops(self, qi_next: int):
-        """The same step as separate launches (one per operation)."""
+        head qi_next in self.logits (one launch per operation)."""
         if self.batched:
             return self.step_batched(qi_next)
         eng, B = self.eng, self.B
@@ -146,7 +110,7 @@ class DecodeSession:
         lib.skinny_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"])
 
     def step_batched(self, qi_next: int):
-        """step_ops for more than 16 sequences: the same operations on the tensor-core GEMM and the cache-sharing
+        """step for more than 16 sequences: the same operations on the tensor-core GEMM and the cache-sharing
         attention (same rounding points; fp32 sums in another order)."""
         eng, ws = self.eng, self.ws
         pv, F, h = eng.pview, eng.F, eng.h
@@ -284,7 +248,6 @@ class TokenConditionedTransformerWrapper(nn.Module):
                     sess.step_and_sample((p - 1) % q, p % q, top_k, temperature, allow(p), uni, eng.seed, use_graph=use_cuda_graph)
             eng.seed += 1
             sampled = torch.cat([prefix, sess.tokens[:, :n_new]], 1)
-            sess.check()
         else:
             sampled = prefix
         eos_mask = (sampled == eos).float()                                                         # utils.py:86-93

@@ -461,27 +461,6 @@ def attn_decode_mqa(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos,
          _p(ws.counters), _stream())
 
 
-class _DecodeLayer(ctypes.Structure):
-    """omlm_decode_layer (include/omlm_b200.h): the per-layer pointers of the fused decode step."""
-    _fields_ = [(n, ctypes.c_void_p) for n in ("wq", "wkv", "wo", "w1", "w2", "conv", "gin", "g_attn", "g_ff", "q_scale", "k_scale",
-                                                "cache", "conv_state")]
-
-
-def decode_layer_table(layers, device):
-    """layers: list of dicts of tensors keyed like _DecodeLayer's fields -> (device table, keep-alive list)."""
-    arr = (_DecodeLayer * len(layers))(*[_DecodeLayer(*[ly[n].data_ptr() for n, _ in _DecodeLayer._fields_]) for ly in layers])
-    host = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-    return host.to(device), [t for ly in layers for t in ly.values()]
-
-
-def decode_step(table_dev, L, B, d, heads, F, Fp, n_max, act_f16, emb_table, next_row, bias_table, pos, x0, x1, q_raw, kv_raw, o,
-                hbuf, hf32, w_logit, g_final, logits, barrier, err_flag, scale=8.0):
-    call("omlm_decode_step", ctypes.c_void_p(table_dev.data_ptr()), _I(L), _I(B), _I(d), _I(heads), _I(F), _I(Fp), _I(n_max), _I(int(act_f16)),
-         _p(emb_table), _p(next_row), _p(bias_table), _I(bias_table.stride(0)), _p(pos), _p(x0), _p(x1), _p(q_raw), _p(kv_raw), _p(o),
-         _p(hbuf), _p(hf32), _p(w_logit), _I(w_logit.shape[0]), _p(g_final), _p(logits), _L(logits.stride(0)), _p(barrier), _p(err_flag),
-         _F(scale), _stream())
-
-
 def attn_decode(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, scale=8.0):
     call("omlm_attn_decode", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(cache), _L(cache.stride(0)), _p(table),
          _I(table.stride(0)), _p(pos), _I(max_pos), _p(out), _I(q_raw.shape[0]), _I(heads), _F(scale), _stream())

@@ -128,9 +128,9 @@ def test_generate_matches_reference_tokens_under_fixed_noise(path):
 
 
 @pytest.mark.parametrize("B", [1, 3])
-def test_fused_decode_step_is_bit_identical_to_the_per_op_path(monkeypatch, B):
-    """The one-launch decode step (csrc/decode_fused.cu) against the per-op launches on a model-scale stage (d = 1024, conv
-    FFN, 8 heads, 2 layers): same sampled tokens and bit-identical logits at every step, eager and from CUDA graphs."""
+def test_graph_replay_samples_the_eager_tokens_at_model_scale(B):
+    """Eager launches against CUDA-graph replay of the decode step on a model-scale stage (d = 1024, conv FFN, 8 heads,
+    2 layers): the same tokens under the same noise stream."""
     import open_musiclm_b200 as O
     torch.manual_seed(0)
     m = O.create_coarse_transformer(dim=1024, depth=2, heads=8, num_coarse_quantizers=3, attn_dropout=0.0, ff_dropout=0.1).cuda().eval()
@@ -139,18 +139,11 @@ def test_fused_decode_step_is_bit_identical_to_the_per_op_path(monkeypatch, B):
     cond = [torch.randint(0, 1024, (B, 12), generator=g).cuda(), torch.randint(0, 1024, (B, 20), generator=g).cuda()]
     n_new = 8 * 3
     uni = torch.rand(n_new, B, 1025, generator=g).clamp_(1e-6, 1 - 1e-6)
-    outs, traces = {}, {}
-    for fused in ("1", "0"):
-        monkeypatch.setenv("OMLM_DECODE_FUSED", fused)
-        tr = []
-        outs[fused, "eager"] = w.generate(conditioning_token_ids=cond, max_time_steps=8, uniform_noise=uni, trace_logits=tr)
-        outs[fused, "graph"] = w.generate(conditioning_token_ids=cond, max_time_steps=8, uniform_noise=uni)
-        traces[fused] = tr
-    assert torch.equal(outs["1", "eager"], outs["0", "eager"]) and torch.equal(outs["1", "graph"], outs["0", "graph"])
-    assert torch.equal(outs["1", "eager"], outs["1", "graph"])
-    assert len(traces["1"]) == len(traces["0"]) == n_new
-    for s_, (a, b) in enumerate(zip(traces["1"], traces["0"])):
-        assert torch.equal(a, b), (s_, float((a - b).abs().max()))
+    trace = []
+    eager = w.generate(conditioning_token_ids=cond, max_time_steps=8, uniform_noise=uni, trace_logits=trace)
+    graph = w.generate(conditioning_token_ids=cond, max_time_steps=8, uniform_noise=uni)
+    assert len(trace) == n_new
+    assert torch.equal(eager, graph)
 
 
 def test_incremental_step_equals_full_forward_at_model_scale():

@@ -1,8 +1,6 @@
-"""BASELINE configs[4]: 10 s three-stage generation on the KV-cache decode path (bench.measure_generation), fused and per-op."""
+"""BASELINE configs[4]: 10 s three-stage generation on the KV-cache decode path (bench.measure_generation)."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import bench
-for fused in (sys.argv[1:] or ["1", "0"]):
-    os.environ["OMLM_DECODE_FUSED"] = fused
-    r = bench.measure_generation()
-    print("fused=" + fused, json.dumps({k: r[k] for k in ("tokens_in_output", "ms_device", "ms_wall", "tokens_per_s", "audio_seconds_per_second")}), flush=True)
+r = bench.measure_generation()
+print(json.dumps({k: r[k] for k in ("tokens_in_output", "ms_device", "ms_wall", "tokens_per_s", "audio_seconds_per_second")}), flush=True)

@@ -88,7 +88,7 @@ def main():
         for c in sess.conv:
             c.zero_()
         sess.pos.fill_(n)                    # every replay processes position n: keys 0..n
-        ms = time_graph(lambda: sess.step_ops(0), args.reps)
+        ms = time_graph(lambda: sess.step(0), args.reps)
         med, spread = stat(ms)
         kv_bytes = L * B * (n + 1) * 128 * 2
         byts = w_bytes + kv_bytes
@@ -133,12 +133,12 @@ def main():
         for c in sess.cache + sess.conv:
             c.zero_()
         sess.pos.fill_(n)
-        sess.step_ops(0)
+        sess.step(0)
         torch.cuda.synchronize()
         steps = 5
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
             for _ in range(steps):
-                sess.step_ops(0)
+                sess.step(0)
             torch.cuda.synchronize()
         per = {}
         for e in prof.events():
