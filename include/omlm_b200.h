@@ -325,7 +325,8 @@ int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_s
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,
                            int act_f16, void* stream);
 /* Sampling of one token per sequence (open_musiclm.py:309-319, utils.py:71-84): eos (class C-1) forbidden unless
- * allow_eos, top-k with the given k, Gumbel-argmax at `temperature`.  uniform: optional [steps, B, C] uniform(0,1) draws
+ * allow_eos, top-k with the given k (exactly k kept: among values equal to the k-th largest the lower indices win, and
+ * -0.0 equals +0.0), Gumbel-argmax at `temperature`; 2 <= C <= 16384.  uniform: optional [steps, B, C] uniform(0,1) draws
  * (slice *step_ptr is used; reproduces a given torch stream), else a Philox stream keyed by *seed.  Writes
  * tokens[b, *step_ptr] and next_row[b] = row_offset + token (embedding-table row for the next step), then advances
  * step_ptr[0] (step_ptr[1] is scratch) and, when given, pos_ptr[0]. */

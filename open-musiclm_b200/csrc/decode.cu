@@ -492,15 +492,21 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   __shared__ uint32_t s_thr;
   const int b = blockIdx.x, tid = threadIdx.x;
   const int step = *step_ptr;
+  // Sort keys: an order-preserving map float -> uint, with -0.0 mapped like +0.0 so that the two zeros are equal values
+  // and the tie rule below (lower index wins) applies between them, as it does in torch.topk's comparison.
+  // A NaN logit maps above +inf (or below -inf for a negative NaN), so it can take a top-k slot, but its noisy score
+  // is NaN, which never compares greater than the running best: the kernel never samples a NaN entry (torch's argmax
+  // would).
   for (int c = tid; c < C; c += 256) {
     float v = logits[b * ld + c];
     if (c == C - 1 && !allow_eos) v = -INFINITY;
     lg[c] = v;
-    const uint32_t u = __float_as_uint(v);
-    key[c] = (u & 0x80000000u) ? ~u : (u | 0x80000000u);       // order-preserving map float -> uint
+    uint32_t u = __float_as_uint(v);
+    if (u == 0x80000000u) u = 0u;
+    key[c] = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
   }
   __syncthreads();
-  // ---- k-th largest key by bitwise bisection (32 counting passes over C <= a few thousand values)
+  // ---- k-th largest key by bitwise bisection (32 counting passes over C <= 16384 values)
   if (tid < 32) {
     uint32_t thr = 0;
     for (int bit = 31; bit >= 0; --bit) {
@@ -661,7 +667,13 @@ int omlm_sample(const float* logits, long ld, int C, int top_k, float temperatur
                 int* pos_ptr, int B, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384 && temperature > 0.f && top_k >= 1 && top_k <= C, "sample: bad arguments");
-  OMLM_KLAUNCH((sample_kernel), B, 256, 2 * C * 4, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature, allow_eos, uniform, seed, tokens,
+  const int smem = 2 * C * 4;                     // 128 KB at C = 16384: above the 48 KB a launch gets without the opt-in
+  static int configured = 0;
+  if (smem > configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = smem;
+  }
+  OMLM_KLAUNCH((sample_kernel), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature, allow_eos, uniform, seed, tokens,
                                                                             tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B);
   OMLM_LAUNCH_CHECK();
   return 0;
