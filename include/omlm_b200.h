@@ -304,6 +304,15 @@ int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long 
                      int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream);
 /* Workspace omlm_decode_gemm needs for a B x N x K call (host-only query; depends on the current device's SM count). */
 int omlm_decode_gemm_workspace(int B, int N, int K, long* part_bytes);
+/* omlm_decode_gemm's contract with a K split that does not depend on B: the k-blocks per split are the ones
+ * omlm_decode_gemm picks for a batch padded to 64 (a function of N, K and the SM count).  Row b of the output is then
+ * bit-identical to the same row computed in a call of any other batch size, 1 to 256, on the same GPU model (seeded
+ * generation relies on it).  Above 64 rows the split-K partials are up to 4x larger than omlm_decode_gemm's;
+ * omlm_decode_gemm_invariant_workspace reports their bytes. */
+int omlm_decode_gemm_invariant(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
+                               const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
+                               int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream);
+int omlm_decode_gemm_invariant_workspace(int B, int N, int K, long* part_bytes);
 /* Attention for the new position n = *pos_ptr (device int): q_raw [B, heads*64], kv_raw [B, 128] bf16 are this step's
  * un-normalised projections; they are l2-normalised * scale (transformer.py:269-271), [k | v] is appended to
  * cache [B, cache_ld_b/128 positions, 128] bf16 at n, then softmax(8 q.k_j + table[head, n-j]) V over keys 0..n
@@ -333,6 +342,13 @@ int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, 
 int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                 const unsigned long long* seed, long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_ptr,
                 int* pos_ptr, int B, void* stream);
+/* omlm_sample with per-sequence seeds (device, B unsigned 64-bit values; NULL: omlm_sample).  The uniform of class c at
+ * sample index t = *step_ptr of sequence b is word x0 of Philox-4x32-7 on the counter (c, t, 0, 0x5eed) under the key
+ * seeds[b] (low word first), as (x0 >> 8) / 2^24: it does not depend on b or B.  seeds and uniform exclude each other;
+ * seed is then unused. */
+int omlm_sample_seeded(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
+                       const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                       int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
 
 #ifdef __cplusplus
 }

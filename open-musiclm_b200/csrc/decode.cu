@@ -475,13 +475,15 @@ decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restric
 // ------------------------------------------------------------------------------------------------ sampling
 // logits [B, ld] fp32, C classes.  eos (= class C-1) is forbidden unless allow_eos (open_musiclm.py:311-313); top-k with
 // k = max(int((1 - thres) C), 1) (utils.py:78-84); Gumbel-argmax at temperature T (utils.py:71-76) with the uniform
-// draw either supplied (uniform [steps, B, C], slice *step_ptr: parity runs reproduce torch's stream) or generated
-// (Philox keyed by seed, step).
+// draw either supplied (uniform [steps, B, C], slice *step_ptr: parity runs reproduce torch's stream) or generated:
+// Philox keyed by *seed_ptr on the counter (c, b, step, 0x5a17), or, when per-sequence seeds are given, keyed by
+// seeds[b] on the counter (c, step, 0, 0x5eed) -- a stream that depends neither on the row b nor on the batch.
 // Writes tokens[b, t] (t = *step_ptr), the embedding-table row of the sampled token for the next step, and advances
 // the device-side counters (*step_ptr, *pos_ptr) once per launch.  grid B, 256 threads.
 __global__ void __launch_bounds__(256)
 sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float temperature, int allow_eos,
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
+              const unsigned long long* __restrict__ seeds,
               long long* __restrict__ tokens, long tokens_ld, int* __restrict__ next_row, int row_offset,
               int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B) {
   extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys
@@ -530,7 +532,7 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   __syncthreads();
   float best = -INFINITY;
   int best_i = 0x7fffffff;
-  const unsigned long long seed = seed_ptr != nullptr ? *seed_ptr : 0ull;
+  const unsigned long long seed = seeds != nullptr ? seeds[b] : (seed_ptr != nullptr ? *seed_ptr : 0ull);
   for (int c = tid; c < C; c += 256) {
     bool keep = key[c] > thr;
     if (!keep && key[c] == thr) {
@@ -542,6 +544,10 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     float u;
     if (uniform != nullptr) {
       u = uniform[(static_cast<long>(step) * B + b) * C + c];
+    } else if (seeds != nullptr) {
+      const uint4 r = philox4x32(static_cast<uint32_t>(c), static_cast<uint32_t>(step), 0u, 0x5eedu,
+                                 static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+      u = (r.x >> 8) * (1.0f / 16777216.0f);
     } else {
       const uint4 r = philox4x32(static_cast<uint32_t>(c), static_cast<uint32_t>(b), static_cast<uint32_t>(step), 0x5a17u,
                                  static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
@@ -662,21 +668,29 @@ int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, 
   return 0;
 }
 
-int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
-                const unsigned long long* seed, long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_ptr,
-                int* pos_ptr, int B, void* stream) {
+int omlm_sample_seeded(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
+                       const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                       int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384 && temperature > 0.f && top_k >= 1 && top_k <= C, "sample: bad arguments");
+  OMLM_CHECK_ARG(seeds == nullptr || uniform == nullptr, "sample: per-sequence seeds and supplied uniforms exclude each other");
   const int smem = 2 * C * 4;                     // 128 KB at C = 16384: above the 48 KB a launch gets without the opt-in
   static int configured = 0;
   if (smem > configured) {
     OMLM_CUDA(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
-  OMLM_KLAUNCH((sample_kernel), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature, allow_eos, uniform, seed, tokens,
-                                                                            tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B);
+  OMLM_KLAUNCH((sample_kernel), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature, allow_eos, uniform, seed,
+               seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
+                const unsigned long long* seed, long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_ptr,
+                int* pos_ptr, int B, void* stream) {
+  return omlm_sample_seeded(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, nullptr, tokens, tokens_ld, next_row,
+                            row_offset, step_ptr, pos_ptr, B, stream);
 }
 
 }  // extern "C"

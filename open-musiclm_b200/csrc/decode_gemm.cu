@@ -209,20 +209,29 @@ struct DgPlan {
   long part_floats;
 };
 
-// Batch padding, tile height and K split of one call: enough CTAs to cover the SMs, every split non-empty, and at most
-// K / Bp splits, so that the partials (written and read: 8 Bp bytes per output row and split) stay within 4x the
+// K-blocks per split for `tiles` tiles and batch padding bn: enough CTAs to cover the SMs, every split non-empty, and at
+// most K / bn splits, so that the partials (written and read: 8 bn bytes per output row and split) stay within 4x the
 // weight bytes (2 K per row) -- they live in L2, the weights come from HBM.
-static DgPlan dg_plan(int B, int N, int K) {
+static int dg_kb_per_split(int tiles, int bn, int K) {
+  const int kb = (K + kDgBK - 1) / kDgBK;
+  int splits = (num_sms() + tiles - 1) / tiles;
+  const int cap = K / bn;
+  splits = splits > cap ? cap : splits;
+  splits = splits < 1 ? 1 : (splits > kb ? kb : splits);
+  return (kb + splits - 1) / splits;
+}
+
+// Batch padding, tile height and K split of one call.  invariant: the split is the one the policy picks at Bp = 64
+// (64-row tiles), whatever B is, so that every output element sums the same k-blocks in the same order for every batch
+// size (the tile height and the batch padding change which CTA computes an element, not its sum).  Above 64 rows the
+// partials then exceed the 4x budget by up to Bp / 64.
+static DgPlan dg_plan(int B, int N, int K, bool invariant = false) {
   DgPlan p;
   p.bn = B <= 64 ? 64 : (B <= 128 ? 128 : 256);
   p.wgs = p.bn >= 128 ? 2 : 1;                    // wider batches: 128-row tiles halve the re-reads of the activations
   p.tiles = (N + 64 * p.wgs - 1) / (64 * p.wgs);
   const int kb = (K + kDgBK - 1) / kDgBK;
-  int splits = (num_sms() + p.tiles - 1) / p.tiles;
-  const int cap = K / p.bn;
-  splits = splits > cap ? cap : splits;
-  splits = splits < 1 ? 1 : (splits > kb ? kb : splits);
-  p.kb_per_split = (kb + splits - 1) / splits;
+  p.kb_per_split = invariant ? dg_kb_per_split((N + 63) / 64, 64, K) : dg_kb_per_split(p.tiles, p.bn, K);
   p.splits = (kb + p.kb_per_split - 1) / p.kb_per_split;
   p.part_floats = p.splits > 1 ? static_cast<long>(p.splits) * p.tiles * 64 * p.wgs * p.bn : 0;
   return p;
@@ -250,22 +259,16 @@ static int dg_launch(const CUtensorMap& tmW, const CUtensorMap& tmA, const DgEpi
   return 0;
 }
 
-}  // namespace omlm
-
-extern "C" {
-
-int omlm_decode_gemm_workspace(int B, int N, int K, long* part_bytes) {
-  using namespace omlm;
+static int dg_workspace(int B, int N, int K, bool invariant, long* part_bytes) {
   OMLM_CHECK_ARG(B >= 1 && B <= kDgMaxB && N > 0 && K > 0, "decode_gemm_workspace: bad shape B=%d N=%d K=%d", B, N, K);
-  const DgPlan p = dg_plan(B, N, K);
+  const DgPlan p = dg_plan(B, N, K, invariant);
   if (part_bytes != nullptr) *part_bytes = p.part_floats * 4;
   return 0;
 }
 
-int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
-                     const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
-                     int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream) {
-  using namespace omlm;
+static int dg_run(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
+                  const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
+                  int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, bool invariant, void* stream) {
   OMLM_CHECK_ARG(B >= 1 && B <= kDgMaxB, "decode_gemm: batch %d out of range (1..%d)", B, kDgMaxB);
   OMLM_CHECK_ARG(N > 0 && K > 0 && K % 8 == 0 && ldw % 8 == 0, "decode_gemm: K and ldw must be multiples of 8 (K=%d ldw=%ld)", K, ldw);
   OMLM_CHECK_ARG(prologue >= 0 && prologue <= 3, "decode_gemm: prologue %d", prologue);
@@ -273,7 +276,7 @@ int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long 
   OMLM_CHECK_ARG(prologue != 3 || (rowsum != nullptr && K % 128 == 0 && n_real > 0), "decode_gemm: inner-norm prologue needs rowsum and K % 128 == 0");
   OMLM_CHECK_ARG(out_fmt == kFmtBF16 || out_fmt == kFmtF32 || out_fmt == kFmtF16, "decode_gemm: out_fmt");
   OMLM_CHECK_ARG((reinterpret_cast<uintptr_t>(W) & 15) == 0, "decode_gemm: W must be 16-byte aligned");
-  const DgPlan p = dg_plan(B, N, K);
+  const DgPlan p = dg_plan(B, N, K, invariant);
   OMLM_CHECK_ARG(part_ws_bytes >= p.part_floats * 4 && (p.part_floats == 0 || part_ws != nullptr),
                  "decode_gemm: split-K workspace of %ld bytes, %ld needed", part_ws_bytes, p.part_floats * 4);
   const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -299,6 +302,32 @@ int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long 
   if (p.bn == 64)  return w_f16 ? dg_launch<64, 1, true>(tmW, tmA, ep, p, B, N, K, st) : dg_launch<64, 1, false>(tmW, tmA, ep, p, B, N, K, st);
   if (p.bn == 128) return w_f16 ? dg_launch<128, 2, true>(tmW, tmA, ep, p, B, N, K, st) : dg_launch<128, 2, false>(tmW, tmA, ep, p, B, N, K, st);
   return w_f16 ? dg_launch<256, 2, true>(tmW, tmA, ep, p, B, N, K, st) : dg_launch<256, 2, false>(tmW, tmA, ep, p, B, N, K, st);
+}
+
+}  // namespace omlm
+
+extern "C" {
+
+int omlm_decode_gemm_workspace(int B, int N, int K, long* part_bytes) {
+  return omlm::dg_workspace(B, N, K, false, part_bytes);
+}
+
+int omlm_decode_gemm(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
+                     const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
+                     int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream) {
+  return omlm::dg_run(A, lda, prologue, W, ldw, w_f16, gamma, rowsum, n_real, addend, ldadd, out, out_fmt, ldo, B, N, K, a16_ws,
+                      part_ws, part_ws_bytes, false, stream);
+}
+
+int omlm_decode_gemm_invariant_workspace(int B, int N, int K, long* part_bytes) {
+  return omlm::dg_workspace(B, N, K, true, part_bytes);
+}
+
+int omlm_decode_gemm_invariant(const void* A, long lda, int prologue, const void* W, long ldw, int w_f16, const float* gamma,
+                               const float* rowsum, int n_real, const float* addend, long ldadd, void* out, int out_fmt, long ldo,
+                               int B, int N, int K, void* a16_ws, float* part_ws, long part_ws_bytes, void* stream) {
+  return omlm::dg_run(A, lda, prologue, W, ldw, w_f16, gamma, rowsum, n_real, addend, ldadd, out, out_fmt, ldo, B, N, K, a16_ws,
+                      part_ws, part_ws_bytes, true, stream);
 }
 
 }  // extern "C"

@@ -11,6 +11,10 @@ with the weight-streaming kernels of csrc/decode.cu, replayed from one CUDA grap
 Up to 16 sequences per call run the SIMT kernels (skinny_gemm, attn_decode); 17 to 256 run the wgmma GEMM of
 csrc/decode_gemm.cu, whose batch is the tensor cores' N operand, and attn_decode_mqa, which reads every cached row once
 per sequence instead of once per head.  The choice follows from the batch size; it is not an option.
+
+Seeded generation (`generate(seeds=...)`) takes the tensor-core path at every batch size, with the GEMM's K split fixed
+independently of B (omlm_decode_gemm_invariant), and draws each sequence's noise from its own seed: the tokens of a
+sequence are then a function of its own inputs and seed, not of the batch it runs in (DESIGN section 4).
 """
 from typing import List, Optional, Sequence
 
@@ -42,15 +46,34 @@ class _Capture:
         s.conv[l][:, 2 - k:].copy_(rows[:, s.n_prompt - k:])
 
 
-class DecodeSession:
-    """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens."""
+def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
+    """B per-sequence seeds (ints, taken modulo 2^64, or an int64 tensor read as raw 64-bit patterns) as an int64
+    device tensor of those bit patterns."""
+    if isinstance(seeds, torch.Tensor):
+        if seeds.dtype != torch.int64:
+            raise ValueError(f"open_musiclm_b200 generate: seeds must be an int64 tensor or a list of ints, not {seeds.dtype}")
+        vals = seeds.reshape(-1).tolist()
+    else:
+        vals = [int(s) for s in seeds]
+    if len(vals) != B:
+        raise ValueError(f"open_musiclm_b200 generate: {len(vals)} seeds for {B} sequences")
+    vals = [v & 0xFFFFFFFFFFFFFFFF for v in vals]
+    return torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in vals], dtype=torch.int64, device=device)
 
-    def __init__(self, eng, B: int, n_prompt: int, n_new: int):
+
+class DecodeSession:
+    """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens.
+    seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
+    self.seeds)."""
+
+    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False):
         if eng.abs_pos:
             raise NotImplementedError("open_musiclm_b200 generate: absolute position embeddings are not supported by the decode path")
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
-        self.eng, self.B, self.n_prompt, self.n_new = eng, B, n_prompt, n_new
+        if seeded and eng.h > 16:
+            raise lib.OmlmError(f"open_musiclm_b200 generate: seeded generation supports at most 16 heads ({eng.h} given)")
+        self.eng, self.B, self.n_prompt, self.n_new, self.seeded = eng, B, n_prompt, n_new, seeded
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
         d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
         self.n_max = n_prompt + n_new
@@ -79,12 +102,13 @@ class DecodeSession:
         eng.build_bias_table(self.rp, N)
         self.table = self.rp["table"]
         self._graphs = {}
-        # more than 16 sequences: tensor-core GEMMs and the cache-sharing attention, with their scratch allocated here so
-        # that graph capture allocates nothing
-        self.batched = B > SKINNY_MAX_BATCH
+        # more than 16 sequences, or seeded mode: tensor-core GEMMs and the cache-sharing attention, with their scratch
+        # allocated here so that graph capture allocates nothing
+        self.batched = B > SKINNY_MAX_BATCH or seeded
+        self.seeds = torch.zeros(B, device=dev, dtype=torch.int64) if seeded else None
         if self.batched:
             shapes = [(HD, d), (128, d), (d, HD), (2 * Fp, d), (d, Fp)] + [(cp, d) for cp in eng.Cp]
-            self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h)
+            self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h, invariant=seeded)
 
     # ------------------------------------------------------------------------------------------ one incremental step
     def step(self, qi_next: int):
@@ -110,24 +134,26 @@ class DecodeSession:
         lib.skinny_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"])
 
     def step_batched(self, qi_next: int):
-        """step for more than 16 sequences: the same operations on the tensor-core GEMM and the cache-sharing
-        attention (same rounding points; fp32 sums in another order)."""
-        eng, ws = self.eng, self.ws
+        """step for more than 16 sequences (or seeded mode): the same operations on the tensor-core GEMM and the
+        cache-sharing attention (same rounding points; fp32 sums in another order).  Seeded mode fixes the GEMMs' K split
+        independently of B; attn_decode_mqa's per-sequence CTAs already are."""
+        eng, ws, inv = self.eng, self.ws, self.seeded
         pv, F, h = eng.pview, eng.F, eng.h
         xa, xm = self.x
         lib.embed_gather(eng.table, self.next_row, xa)
         for l in range(eng.L):
             p, pk = f"transformer.layers.{l}.", eng.pk[l]
-            lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws)
-            lib.decode_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1, ws=ws)
+            lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws, invariant=inv)
+            lib.decode_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1, ws=ws, invariant=inv)
             lib.attn_decode_mqa(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
                                 self.n_max, self.o, h, ws=ws)
-            lib.decode_gemm(self.o, pk["wo_b"], xm, addend=xa, ws=ws)
-            lib.decode_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]], ws=ws)
+            lib.decode_gemm(self.o, pk["wo_b"], xm, addend=xa, ws=ws, invariant=inv)
+            lib.decode_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]], ws=ws, invariant=inv)
             lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
-            lib.decode_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm, ws=ws)
+            lib.decode_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm, ws=ws, invariant=inv)
         S = len(eng.seqs) - 1
-        lib.decode_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"], ws=ws)
+        lib.decode_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"], ws=ws,
+                        invariant=inv)
 
     def sample(self, qi: int, top_k: int, temperature: float, allow_eos: bool, uniform, seed, bump_pos: bool):
         eng = self.eng
@@ -135,11 +161,11 @@ class DecodeSession:
         q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
         row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
         lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                   self.counters, self.pos if bump_pos else None, self.B)
+                   self.counters, self.pos if bump_pos else None, self.B, seeds=self.seeds)
 
     def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True):
         """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
-        key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None)
+        key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded)
         g = self._graphs.get(key)
         if g is None or not use_graph:
             body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True))
@@ -185,13 +211,22 @@ class TokenConditionedTransformerWrapper(nn.Module):
     def generate(self, *, conditioning_token_ids: List[torch.Tensor], pred_token_ids: Optional[torch.Tensor] = None,
                  max_time_steps=512, filter_thres=0.9, temperature=1., include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, allow_eos_in_output=False, uniform_noise: Optional[torch.Tensor] = None,
-                 use_cuda_graph=True, trace_logits: Optional[list] = None, **kwargs):
+                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, **kwargs):
         """Same contract as open_musiclm.py:253-326.  uniform_noise (optional, [n_sampled, b, codebook+1] in (0, 1)):
         the uniform draws behind the Gumbel noise, one slice per sampled token in order — parity runs pass the stream
-        torch's default CPU generator would have produced; by default the noise comes from a device Philox stream.
+        torch's default CPU generator would have produced; by default the noise comes from a device Philox stream keyed
+        by Engine.seed, which every unseeded call advances.
+        seeds (optional): one unsigned 64-bit seed per sequence (a list of ints, or an int64 tensor read as raw bits).
+        The tokens of sequence b, and the logits they were sampled from, are then a function only of the weights, that
+        sequence's conditioning and prefix, seeds[b] and the sampling arguments: not of the batch size, the row, the other
+        rows, CUDA-graph or eager execution, or earlier calls (on one GPU model and build; DESIGN section 4).  Engine.seed
+        is left untouched.  seeds=torch.randint(2**62, (b,)) puts generation under torch.manual_seed.  Excludes
+        uniform_noise.
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
+        if seeds is not None and uniform_noise is not None:
+            raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
         m, eng = self.transformer, self.transformer.engine
         was_training = m.training
         m.eval()
@@ -212,13 +247,16 @@ class TokenConditionedTransformerWrapper(nn.Module):
             init_step = 0
             prefix = torch.empty(B, 0, device=dev, dtype=torch.int64)
         n_new = max(0, (max_time_steps - init_step) * q)
+        seed_vals = seeds_tensor(seeds, B, dev) if seeds is not None else None
         if n_new > 0:
             ids = cond + [prefix]
             _, src_row, key_mask, _, n_tok = lib.token_plan(
                 ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
                 append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
             pl = eng.plan(B, n_tok)
-            sess = DecodeSession(eng, B, pl.N, n_new)
+            sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None)
+            if seed_vals is not None:
+                sess.seeds.copy_(seed_vals)
             ws = eng.workspace(pl, False)
             eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_Capture(sess))
             # logits of the prompt's last position: final sequence, position p_last = its token count, head p_last mod q
@@ -246,7 +284,8 @@ class TokenConditionedTransformerWrapper(nn.Module):
                     sess.sample(p % q, top_k, temperature, allow(p), uni, eng.seed, True)
                 else:
                     sess.step_and_sample((p - 1) % q, p % q, top_k, temperature, allow(p), uni, eng.seed, use_graph=use_cuda_graph)
-            eng.seed += 1
+            if seed_vals is None:
+                eng.seed += 1
             sampled = torch.cat([prefix, sess.tokens[:, :n_new]], 1)
         else:
             sampled = prefix

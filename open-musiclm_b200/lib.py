@@ -414,10 +414,11 @@ def skinny_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, add
          _I(FMT[out.dtype]), _L(out.stride(0)), _I(B), _I(N), _I(K), _stream())
 
 
-def decode_gemm_workspace(B, N, K):
-    """Bytes of split-K partials omlm_decode_gemm needs for a B x N x K call on the current device."""
+def decode_gemm_workspace(B, N, K, invariant=False):
+    """Bytes of split-K partials omlm_decode_gemm (invariant: omlm_decode_gemm_invariant) needs for a B x N x K call on
+    the current device."""
     part = _L(0)
-    call("omlm_decode_gemm_workspace", _I(B), _I(N), _I(K), ctypes.byref(part))
+    call("omlm_decode_gemm_invariant_workspace" if invariant else "omlm_decode_gemm_workspace", _I(B), _I(N), _I(K), ctypes.byref(part))
     return part.value
 
 
@@ -425,10 +426,10 @@ class DecodeWorkspace:
     """Scratch of the large-batch decode kernels, allocated once so that CUDA-graph capture allocates nothing:
     the 16-bit activation operand [B, max K], the split-K partials, the attention's per-slice partials and its
     per-sequence counters (zero; every call leaves them zero).  shapes: the (N, K) of every decode_gemm call; max_pos /
-    heads: attention."""
+    heads: attention; invariant: also large enough for decode_gemm(..., invariant=True)."""
 
-    def __init__(self, device, B, shapes, max_pos=0, heads=0):
-        part = max(decode_gemm_workspace(B, N, K) for N, K in shapes)
+    def __init__(self, device, B, shapes, max_pos=0, heads=0, invariant=False):
+        part = max(decode_gemm_workspace(B, N, K, inv) for N, K in shapes for inv in ((False, True) if invariant else (False,)))
         attn = B * -(-max_pos // 128) * heads * 66 if max_pos else 0
         self.a16 = torch.empty(B * max(K for _, K in shapes), device=device, dtype=torch.int16)
         self.part = torch.empty(max(part // 4, 1), device=device, dtype=torch.float32)
@@ -436,16 +437,17 @@ class DecodeWorkspace:
         self.counters = torch.zeros(B, device=device, dtype=torch.int32)
 
 
-def decode_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, addend=None, ws=None):
+def decode_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, addend=None, ws=None, invariant=False):
     """skinny_gemm's contract for 1 <= B <= 256 rows on the tensor cores (omlm_decode_gemm).  ws: a DecodeWorkspace
-    covering this shape (None: a fresh one, which is not CUDA-graph capturable)."""
+    covering this shape (None: a fresh one, which is not CUDA-graph capturable).  invariant: the K split does not depend
+    on B, so each output row is bit-identical for every batch size (omlm_decode_gemm_invariant)."""
     B = A.shape[0]
     N, K = W.shape
     assert W.dtype in _T16 and W.stride(1) == 1 and out.stride(-1) == 1 and A.stride(-1) == 1
     assert (prologue in (0, 3) and A.dtype == W.dtype) or (prologue in (1, 2) and A.dtype == torch.float32)
     if ws is None:
-        ws = DecodeWorkspace(A.device, B, [(N, K)])
-    call("omlm_decode_gemm", _p(A), _L(A.stride(0)), _I(prologue), _p(W), _L(W.stride(0)), _I(int(W.dtype == torch.float16)),
+        ws = DecodeWorkspace(A.device, B, [(N, K)], invariant=invariant)
+    call("omlm_decode_gemm_invariant" if invariant else "omlm_decode_gemm", _p(A), _L(A.stride(0)), _I(prologue), _p(W), _L(W.stride(0)), _I(int(W.dtype == torch.float16)),
          _p(gamma), _p(rowsum), _I(n_real), _p(addend), _L(addend.stride(0) if addend is not None else 0), _p(out),
          _I(FMT[out.dtype]), _L(out.stride(0)), _I(B), _I(N), _I(K), _p(ws.a16), _p(ws.part), _L(ws.part.numel() * 4),
          _stream())
@@ -473,9 +475,15 @@ def decode_conv_geglu(u_new, state, conv_w, h_out, rowsum):
          _I(int(u_new.dtype == torch.float16)), _stream())
 
 
-def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B):
-    call("omlm_sample", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _I(int(allow_eos)), _p(uniform),
-         _p(seed), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
+def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B, seeds=None):
+    """seeds: int64 [B] device tensor of per-sequence seeds (raw 64-bit patterns) -> omlm_sample_seeded."""
+    if seeds is None:
+        call("omlm_sample", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _I(int(allow_eos)), _p(uniform),
+             _p(seed), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
+        return
+    assert seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B
+    call("omlm_sample_seeded", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _I(int(allow_eos)), _p(uniform),
+         _p(seed), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
 
 
 def gather_windows(src_i16, start, out):

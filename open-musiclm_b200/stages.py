@@ -33,6 +33,26 @@ class NoiseStream:
         return out
 
 
+_MASK64 = (1 << 64) - 1
+SEMANTIC, COARSE, FINE = 0, 1, 2       # stage numbers of window_seed
+
+
+def splitmix64(x: int) -> int:
+    """The splitmix64 output function (Steele, Lea and Flood, "Fast splittable pseudorandom number generators", 2014)
+    of the 64-bit value x: x + 0x9E3779B97F4A7C15, then two xor-shift-multiply rounds and a final xor-shift."""
+    z = (x + 0x9E3779B97F4A7C15) & _MASK64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _MASK64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _MASK64
+    return z ^ (z >> 31)
+
+
+def window_seed(seed: int, stage: int, window: int) -> int:
+    """The seed MusicLM.generate_tokens hands one sequence's generate call for window `window` (0, 1, ... in the order
+    of generation) of stage `stage` (SEMANTIC, COARSE, FINE), given that sequence's seed:
+        splitmix64(seed ^ splitmix64(stage << 32 | window))   (all values unsigned 64-bit)."""
+    return splitmix64((int(seed) & _MASK64) ^ splitmix64((stage << 32) | window))
+
+
 def _n_new(pred_token_ids, max_time_steps: int, q: int) -> int:
     init = 0 if pred_token_ids is None else pred_token_ids.shape[1]
     return max(0, (max_time_steps - init) * q)
@@ -178,30 +198,51 @@ class MusicLM(nn.Module):
     def generate_tokens(self, *, clap_token_ids, output_seconds=8, semantic_window_seconds=10, coarse_window_seconds=4,
                         fine_window_seconds=2, semantic_steps_per_second=50, acoustic_steps_per_second=75,
                         semantic_sliding_window_step_percent=0.5, coarse_sliding_window_step_percent=0.5,
-                        fine_sliding_window_step_percent=1, noise: Optional[NoiseStream] = None, return_all=False):
+                        fine_sliding_window_step_percent=1, noise: Optional[NoiseStream] = None, return_all=False, seeds=None):
         """The token-level body of MusicLM.forward (open_musiclm.py:925-1031, no audio prompt): returns the acoustic tokens
-        [b, T, coarse + fine quantizers] the reference would hand to the codec (return_all: also the three streams)."""
+        [b, T, coarse + fine quantizers] the reference would hand to the codec (return_all: also the three streams).
+        seeds (optional): one unsigned 64-bit seed per prompt (list of ints or int64 tensor).  Every generate call then gets
+        the per-sequence seeds window_seed(seeds[b], stage, window index), so the whole song of prompt b is a function
+        of (prompt b, seeds[b]), whatever else is in the batch.  Excludes noise."""
+        if seeds is not None and noise is not None:
+            raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: seeds and noise exclude each other")
+        if seeds is not None:
+            seeds = seeds.reshape(-1).tolist() if isinstance(seeds, torch.Tensor) else [int(s) for s in seeds]
+            if len(seeds) != clap_token_ids.shape[0]:
+                raise ValueError(f"open_musiclm_b200 MusicLM.generate_tokens: {len(seeds)} seeds for {clap_token_ids.shape[0]} prompts")
+        counter = {}
+
+        def seeded(stage):             # the per-sequence seeds of this stage's next window (none when unseeded)
+            if seeds is None:
+                return {}
+            w = counter.get(stage, 0)
+            counter[stage] = w + 1
+            return dict(seeds=[window_seed(s, stage, w) for s in seeds])
+
         sps, aps = semantic_steps_per_second, acoustic_steps_per_second
         common = dict(clap_token_ids=clap_token_ids, include_eos_in_output=False, append_eos_to_conditioning_tokens=True, noise=noise)
         # ---- semantic stream: first window from scratch, then windows conditioned on the tail of the stream (:930-949)
-        sem = self.semantic.generate(semantic_token_ids=None, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps), **common)
+        sem = self.semantic.generate(semantic_token_ids=None, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps),
+                                     **common, **seeded(SEMANTIC))
         keep = int(semantic_window_seconds * sps * (1 - semantic_sliding_window_step_percent))
         while sem.shape[1] < int(output_seconds * sps):
-            nxt = self.semantic.generate(semantic_token_ids=sem[:, -keep:], max_time_steps=int(semantic_window_seconds * sps), **common)
+            nxt = self.semantic.generate(semantic_token_ids=sem[:, -keep:], max_time_steps=int(semantic_window_seconds * sps), **common,
+                                         **seeded(SEMANTIC))
             sem = torch.cat([sem, nxt[:, keep:]], 1)
         # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail (:956-985)
         win = int(coarse_window_seconds * sps - 1)
         coarse, keep = None, int(coarse_window_seconds * aps * (1 - coarse_sliding_window_step_percent))
         for sem_win in _windows(sem, win, int(win * coarse_sliding_window_step_percent)):
             pred = self.coarse.generate(semantic_token_ids=sem_win, coarse_token_ids=None if coarse is None else coarse[:, -keep:],
-                                        max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common)
+                                        max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common, **seeded(COARSE))
             coarse = pred if coarse is None else torch.cat([coarse, pred[:, keep:]], 1)
         # ---- fine stream: one window of coarse tokens per generate (:995-1024)
         fwin = int(fine_window_seconds * aps)
         fine, keep = None, int(fwin * (1 - fine_sliding_window_step_percent))
         for coarse_win in _windows(coarse, fwin, int(fwin * fine_sliding_window_step_percent)):
             cond = fine[:, -keep:] if (fine is not None and keep > 0) else None
-            pred = self.fine.generate(coarse_token_ids=coarse_win, fine_token_ids=cond, max_time_steps=fwin, temperature=0.4, **common)
+            pred = self.fine.generate(coarse_token_ids=coarse_win, fine_token_ids=cond, max_time_steps=fwin, temperature=0.4, **common,
+                                      **seeded(FINE))
             fine = pred if fine is None else torch.cat([fine, pred[:, keep:]], 1)
         acoustic = torch.cat([coarse, fine], -1)                                                       # :1032
         return (acoustic, sem, coarse, fine) if return_all else acoustic
