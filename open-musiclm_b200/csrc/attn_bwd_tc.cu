@@ -9,8 +9,8 @@
 //                      P = exp2(s - lse), dS = P (dP - D) in fp32 registers; P, dS -> bf16 [row][key] smem tiles
 //                      dV += P^T dO,  dK += dS^T Q        (A read MN-major; accumulated in registers over the chunk)
 //                      dQ  = dS K                         (per tile, red.global.add.v2.f32 into dqn)
-//                   the bias enters from a per-tile Toeplitz window in shared memory (per head, pre-scaled by log2 e),
-//                   staged while S and dP run.
+//                   the bias enters from a per-tile Toeplitz window in shared memory (per head), copied by cp.async
+//                   one tile ahead, while the previous tile's dV, dK and dQ run; lse2 and D are loaded as far ahead.
 //                   The bias gradient dTable[hh, i-j] += dS: the fp32 dS tile is staged in shared memory and, while dV,
 //                   dK and dQ run, each thread owns (head, diagonal) pairs and sums them in row order into its
 //                   warpgroup's table (no shared-memory float atomics); the two tables are flushed once per unit.
@@ -29,6 +29,12 @@
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
 #include <stdlib.h>
+#include <algorithm>
+#include <array>
+#include <functional>
+#include <map>
+#include <mutex>
+#include <vector>
 
 namespace omlm {
 
@@ -55,6 +61,9 @@ __device__ __forceinline__ float bt_ex2(float x) {
 }
 __device__ __forceinline__ void bt_red2(float* addr, float a, float b) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void bt_cp_async4(float* dst, const float* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 
 // ---- DET turn counters.  One thread of a warpgroup waits for the turn, the warpgroup adds, fences and signals.
@@ -172,6 +181,27 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const int j = kbase + 8 * c + 2 * qc + e;
         if (j < N && (key_mask == nullptr || key_mask[static_cast<long long>(b) * N + j] != 0)) vis |= 1u << (2 * c + e);
       }
+    // A row tile's operands from global memory are fetched one tile ahead, while the previous tile's GEMMs run:
+    //  - its bias window (per head, deltas it_lo - kbase - 63 .. it_hi - kbase) by cp.async; the raw table values are
+    //    scaled by log2 e where they are read.  Entries for delta < 0 are never read and are not copied.
+    //  - lse2 and D of this thread's two rows, into registers.
+    auto fetch_tile = [&](int rb, float (&lse)[2], float (&D)[2]) {
+      const int it_lo = min(rb, R - 1) / h, it_hi = min(rb + kBtBQ - 1, R - 1) / h;
+      const int win_w = it_hi - it_lo + 64, dlo = it_lo - kbase - 63;
+      for (int hh = tid128 / win_w, w = tid128 - hh * win_w; hh < h;) {      // entry (hh, w); win_w >= 64
+        if (dlo + w >= 0) bt_cp_async4(win + hh * win_ld + w, table + hh * static_cast<long>(table_ld) + dlo + w);
+        for (w += 128; w >= win_w; ++hh) w -= win_w;
+      }
+      asm volatile("cp.async.commit_group;" ::: "memory");
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int rc = min(rb + wq * 16 + qr + hr * 8, R - 1);
+        lse[hr] = lse2[static_cast<long long>(b) * R + rc];
+        D[hr] = dsum[static_cast<long long>(b) * R + rc];
+      }
+    };
+    float lse_t[2], D_t[2];
+    fetch_tile(rt0 * kBtBQ, lse_t, D_t);
     float dv[32], dk[32];
 #pragma unroll
     for (int x = 0; x < 32; ++x) { dv[x] = 0.f; dk[x] = 0.f; }
@@ -189,17 +219,8 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Wgmma<64, false>::ss<0, 0>(dp, make_smem_desc(sdo + ks * 32, 16, 1024), make_smem_desc(sv + ks * 32, 16, 1024), ks > 0 ? 1u : 0u);
       }
       wgmma_commit();
-      // ---- while S / dP run: the tile's bias window (per head, deltas it_lo - kbase - 63 .. it_hi - kbase, pre-scaled
-      // by log2 e; entries for delta < 0 are never read).  The previous tile's reads of the window ended before every
-      // thread's first barrier of that tile.
       const int it_lo = min(rbase, R - 1) / h, it_hi = min(rbase + kBtBQ - 1, R - 1) / h;
-      {
-        const int win_w = it_hi - it_lo + 64, dlo = it_lo - kbase - 63;
-        for (int x = tid128; x < h * win_w; x += 128) {
-          const int hh = x / win_w, w = x - hh * win_w, d = dlo + w;
-          win[hh * win_ld + w] = d >= 0 ? __ldg(table + hh * static_cast<long>(table_ld) + d) * kBtL2e : 0.f;
-        }
-      }
+      asm volatile("cp.async.wait_all;" ::: "memory");                // this thread's part of the tile's bias window
       asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
       wgmma_wait<0>();
       wgmma_reg_fence(s);
@@ -212,12 +233,16 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         const bool row_ok = r < R;
         const int rc = min(r, R - 1);
         const int i = rc / h, hh = rc - i * h;
-        const float lse = lse2[static_cast<long long>(b) * R + rc];
-        const float D = dsum[static_cast<long long>(b) * R + rc];
+        const float lse = lse_t[hr], D = D_t[hr];
         const float* wrow = win + hh * win_ld + i - it_lo + 63 - 2 * qc;   // column 8 c + e at wrow[-8 c - e]
         const int dcol = i - kbase - 2 * qc;                                 // delta of column 8 c + e is dcol - 8 c - e
         uint8_t* prow = p_tile + lr * 128;
         uint8_t* drow = ds_tile + lr * 128;
+        // the row's 16 window entries, loaded together (always inside the window; those of masked columns may be
+        // stale and are discarded below)
+        float wv[16];
+#pragma unroll
+        for (int x = 0; x < 16; ++x) wv[x] = wrow[-8 * (x >> 1) - (x & 1)];
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
           float pp[2], dd[2];
@@ -227,7 +252,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             // exp2(-inf - -inf) would turn its P into NaN instead of 0
             const bool live = row_ok && ((vis >> (2 * c + e)) & 1u) && dcol >= 8 * c + e;
             const float x = s[4 * c + 2 * hr + e];
-            pp[e] = live ? bt_ex2(fmaf(x, sc2, wrow[-8 * c - e]) - lse) : 0.f;
+            pp[e] = live ? bt_ex2(fmaf(x, sc2, wv[2 * c + e] * kBtL2e) - lse) : 0.f;
             dd[e] = pp[e] * (dp[4 * c + 2 * hr + e] - D);
           }
           *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
@@ -237,7 +262,8 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         }
       }
       fence_proxy_async();                                   // P / dS (generic stores) -> visible to wgmma
-      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");   // also: every thread is done with the window
+      if (t + 1 < T) fetch_tile(rbase + kBtBQ, lse_t, D_t);
       float dq[32];
       wgmma_fence();
 #pragma unroll
@@ -253,13 +279,28 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         // diagonal sums of the fp32 dS tile while the tensor cores run: thread-owned (head, diagonal) pairs, rows in order
         const int dlo = max(0, it_lo - kbase - 63), dhi = it_hi - kbase;
         const int W = dhi - dlo + 1;
-        for (int p = tid128; p < h * W; p += 128) {
-          const int hh = p / W, dl = dlo + (p - hh * W);
-          const int i0 = max((rbase - hh + h - 1) / h, kbase + dl);
-          const int i1 = min(min((rbase + kBtBQ - 1 - hh) / h, N - 1), kbase + dl + 63);
+        // head hh has the tile's rows at positions ceil((rbase - hh) / h) .. floor((rbase + 63 - hh) / h)
+        const int q0 = rbase / h, r0 = rbase - q0 * h;
+        const int q1 = (rbase + kBtBQ - 1) / h, r1 = rbase + kBtBQ - 1 - q1 * h;
+        // W <= 0: this warpgroup's keys all lie after the tile's last position, no pairs
+        for (int hh = W > 0 ? tid128 / W : h, w = W > 0 ? tid128 - hh * W : 0; hh < h;) {   // pair (hh, dlo + w)
+          const int dl = dlo + w;
+          const int i0 = max(q0 + (hh < r0 ? 1 : 0), kbase + dl);
+          const int i1 = min(min(q1 - (hh > r1 ? 1 : 0), N - 1), kbase + dl + 63);
+          // eight rows' loads in flight at once; the adds stay in row order
+          const float* src = sdsf + (i0 * h + hh - rbase) * kBtSdsLd + (i0 - dl - kbase);
+          const int stride = h * kBtSdsLd + 1;
           float sum = 0.f;
-          for (int i = i0; i <= i1; ++i) sum += sdsf[(i * h + hh - rbase) * kBtSdsLd + (i - dl - kbase)];
+          for (int i = i0; i <= i1; i += 8, src += 8 * stride) {
+            float x[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] = i + k <= i1 ? src[k * stride] : 0.f;
+#pragma unroll
+            for (int k = 0; k < 8; ++k)
+              if (i + k <= i1) sum += x[k];
+          }
           wacc[hh * Wacc + dl - dmin] += sum;
+          for (w += 128; w >= W && hh < h; ++hh) w -= W;
         }
       }
       wgmma_wait<0>();
@@ -385,12 +426,51 @@ struct BtConfig {
   int tiles_per_chunk, wacc, win_ld, smem_bytes, units_per_batch, n_row_tiles, n_key_tiles;
 };
 
+// Chunk length T (row tiles per unit).  One CTA runs per SM and the units differ in length (the row tiles of key tile
+// kt start at 2 kt h, and a unit's last chunk may be short), so T is picked by replaying the hardware's dispatch: units
+// in block order, each to the SM that frees first, a unit costing its row tiles plus about one tile for its K/V load
+// and dK/dV flush.  T is at most 16: longer chunks leave few units to fill the last wave, and in the deterministic mode
+// a row tile's later key tiles wait for the earlier ones, so long chunks serialise the turns.  Among equal makespans
+// the longer chunk wins (fewer K/V loads and dK/dV flushes).  Memoised: the replay costs up to a millisecond.
+template <class Fits>
+static int bt_pick_chunk(int B, int n_row_tiles, int n_key_tiles, int heads, Fits fits) {
+  static std::mutex mu;
+  static std::map<std::array<int, 5>, int> memo;
+  const int sms = num_sms();
+  const std::array<int, 5> key{B, n_row_tiles, n_key_tiles, heads, sms};
+  std::lock_guard<std::mutex> lock(mu);
+  const auto hit = memo.find(key);
+  if (hit != memo.end()) return hit->second;
+  int best_T = 1;
+  long best = -1;
+  std::vector<long> busy(sms);
+  for (int T = 1; T <= std::min(16, n_row_tiles); ++T) {
+    if (!fits(T)) break;
+    std::fill(busy.begin(), busy.end(), 0L);      // a min-heap of the SMs' busy-until times
+    for (int kt = 0; kt < n_key_tiles; ++kt) {
+      const int first = (kt * kBtBK * heads) / kBtBQ;
+      for (int rt = first; rt < n_row_tiles; rt += T) {
+        const long cost = std::min(T, n_row_tiles - rt) + 1;
+        for (int b = 0; b < B; ++b) {
+          std::pop_heap(busy.begin(), busy.end(), std::greater<long>());
+          busy.back() += cost;
+          std::push_heap(busy.begin(), busy.end(), std::greater<long>());
+        }
+      }
+    }
+    const long makespan = *std::max_element(busy.begin(), busy.end());
+    if (best < 0 || makespan <= best) { best = makespan; best_T = T; }
+  }
+  memo[key] = best_T;
+  return best_T;
+}
+
 static int bt_config(int B, int N, int heads, BtConfig* cfg) {
   const long R = static_cast<long>(N) * heads;
   const int n_row_tiles = static_cast<int>((R + kBtBQ - 1) / kBtBQ);
   const int n_key_tiles = (N + kBtBK - 1) / kBtBK;
-  // chunk length T: as long as the per-CTA diagonal tables (2 x heads x (64 T / heads + 130) floats) fit in shared
-  // memory, and long enough that the grid is at most ~4 CTAs per SM (each CTA pays a K/V load and a dK/dV flush)
+  // chunk length T: bt_pick_chunk, among the lengths whose per-CTA diagonal tables (2 x heads x (64 T / heads + 130)
+  // floats) fit in shared memory
   const int win_ld = bt_win_ld(heads);
   auto wacc_of = [&](int T) { return (T * kBtBQ + heads - 1) / heads + kBtBK + 2; };
   auto smem_of = [&](int T) { return kBoWin + 2 * heads * (win_ld + wacc_of(T)) * 4 + 1024; };
@@ -403,13 +483,7 @@ static int bt_config(int B, int N, int heads, BtConfig* cfg) {
     return units;
   };
   OMLM_CHECK_ARG(smem_of(1) <= kBtMaxSmem, "attn_bwd_tc: too many heads (%d) for the shared-memory bias tables", heads);
-  int tiles_per_chunk = 1;
-  for (int cand = 2; cand <= 2 * n_row_tiles; cand *= 2) {
-    const int T = cand < n_row_tiles ? cand : n_row_tiles;
-    if (smem_of(T) > kBtMaxSmem) break;
-    tiles_per_chunk = T;
-    if ((T >= 8 && units_of(T) * B <= 4L * num_sms()) || T == n_row_tiles) break;
-  }
+  int tiles_per_chunk = bt_pick_chunk(B, n_row_tiles, n_key_tiles, heads, [&](int T) { return smem_of(T) <= kBtMaxSmem; });
   if (const char* e = getenv("OMLM_ATTN_BWD_T")) {      // diagnostics: force the chunk length
     const int T = atoi(e);
     if (T >= 1 && T <= n_row_tiles && smem_of(T) <= kBtMaxSmem) tiles_per_chunk = T;
