@@ -147,6 +147,12 @@ int omlm_forgetful_mask(unsigned char* keep, int B, int N, int num_drop,
  * open_musiclm.py:134-136; negative rows add nothing) (fp32, 128-bit copies); replaces get_embeds + start-token concat
  * (open_musiclm.py:133-145).  scatter_add is its backward incl. the grad_shrink factor (utils.py:60-61). */
 int omlm_embed_gather(const float* table, const int* src_row, const int* src_row2, float* x, int M, int D, void* stream);
+/* The decode step's input rows with absolute position embeddings: x[m,:] = table[src_row[m],:] +
+ * table[pos_row_base + p,:], p = *pos_ptr + pos_offset (pos_ptr: device int, read by the kernel so that a captured
+ * CUDA graph uses the current position on every replay; one position row for all m).  A negative src_row, or p outside
+ * [0, pos_rows), adds nothing (the caller checks the bound before launching).  fp32, 128-bit copies. */
+int omlm_embed_gather_pos(const float* table, const int* src_row, const int* pos_ptr, int pos_offset, int pos_row_base,
+                          int pos_rows, float* x, int M, int D, void* stream);
 int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, int M, int D,
                            float scale, void* stream);
 

@@ -128,6 +128,31 @@ __global__ void embed_gather_kernel(const float* __restrict__ table, const int* 
   }
 }
 
+// Decode step with absolute position embeddings: x[m, :] = table[src_row[m], :] + table[pos_row_base + p, :] with
+// p = *pos_ptr + pos_offset, the same position row for every m.  The position is read on the device, so a captured CUDA
+// graph sees the current step on every replay.  A negative src_row, or p outside [0, pos_rows), contributes zero.
+__global__ void embed_gather_pos_kernel(const float* __restrict__ table, const int* __restrict__ src_row,
+                                        const int* __restrict__ pos_ptr, int pos_offset, int pos_row_base, int pos_rows,
+                                        float* __restrict__ x, int M, int D) {
+  const int vec_per_row = D >> 2;
+  const long long total = static_cast<long long>(M) * vec_per_row;
+  const int p = __ldg(pos_ptr) + pos_offset;
+  const bool has_pos = p >= 0 && p < pos_rows;
+  const float4* prow = reinterpret_cast<const float4*>(table + static_cast<long long>(pos_row_base + (has_pos ? p : 0)) * D);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int m = static_cast<int>(i / vec_per_row), v = static_cast<int>(i - static_cast<long long>(m) * vec_per_row);
+    const int r = src_row[m];
+    float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (r >= 0) val = reinterpret_cast<const float4*>(table + static_cast<long long>(r) * D)[v];
+    if (has_pos) {
+      const float4 q = prow[v];
+      val.x += q.x; val.y += q.y; val.z += q.z; val.w += q.w;
+    }
+    reinterpret_cast<float4*>(x + static_cast<long long>(m) * D)[v] = val;
+  }
+}
+
 // dtable[src_row[m], :] += scale * dx[m, :]   (scale = grad_shrink alpha, utils.py:60-61).
 __global__ void embed_scatter_kernel(float* __restrict__ dtable, const int* __restrict__ src_row,
                                      const float* __restrict__ dx, int M, int D, float scale) {
@@ -258,6 +283,22 @@ int omlm_embed_gather(const float* table, const int* src_row, const int* src_row
   const long long total = static_cast<long long>(M) * (D / 4);
   const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(num_sms()) * 16));
   OMLM_KLAUNCH((embed_gather_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, src_row, src_row2, x, M, D);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+
+int omlm_embed_gather_pos(const float* table, const int* src_row, const int* pos_ptr, int pos_offset, int pos_row_base,
+                          int pos_rows, float* x, int M, int D, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0, "embed_gather_pos: bad shape %d x %d", M, D);
+  OMLM_CHECK_ARG(table != nullptr && src_row != nullptr && pos_ptr != nullptr && x != nullptr,
+                 "embed_gather_pos: null pointer");
+  OMLM_CHECK_ARG(pos_row_base >= 0 && pos_rows > 0, "embed_gather_pos: bad position rows %d + [0, %d)", pos_row_base,
+                 pos_rows);
+  const long long total = static_cast<long long>(M) * (D / 4);
+  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(num_sms()) * 16));
+  OMLM_KLAUNCH((embed_gather_pos_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, src_row, pos_ptr,
+               pos_offset, pos_row_base, pos_rows, x, M, D);
   OMLM_LAUNCH_CHECK();
   return 0;
 }

@@ -64,11 +64,10 @@ def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
 class DecodeSession:
     """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens.
     seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
-    self.seeds)."""
+    self.seeds).  pred_start: position of the predicted sequence's start token in the prompt (_Plan.pos0[-1]); with
+    absolute position embeddings the token at position pos is token pos - pred_start - 1 of that sequence."""
 
-    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False):
-        if eng.abs_pos:
-            raise NotImplementedError("open_musiclm_b200 generate: absolute position embeddings are not supported by the decode path")
+    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0):
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
         if seeded and eng.h > 16:
@@ -89,6 +88,7 @@ class DecodeSession:
         self.next_row = torch.zeros(B, device=dev, dtype=torch.int32)
         self.counters = torch.zeros(2, device=dev, dtype=torch.int32)          # [sampled so far, block arrival counter]
         self.pos = torch.full((1,), n_prompt, device=dev, dtype=torch.int32)   # position the next decode step processes
+        self.pos_offset = -(pred_start + 1)
         # bias table for every distance the generation can reach (it depends on i - j only)
         N = self.n_max
         self.rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, Hr, dt=f32) for _ in range(3)], rp_a=[E(N, Hr, dt=f32) for _ in range(3)],
@@ -111,6 +111,15 @@ class DecodeSession:
             self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h, invariant=seeded)
 
     # ------------------------------------------------------------------------------------------ one incremental step
+    def embed(self, x):
+        """x = the input rows of the position self.pos: embedding row self.next_row, plus with absolute position
+        embeddings the predicted sequence's row for its token self.pos - pred_start - 1 (open_musiclm.py:134-136)."""
+        eng = self.eng
+        if eng.abs_pos:
+            lib.embed_gather_pos(eng.table, self.next_row, self.pos, self.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x)
+        else:
+            lib.embed_gather(eng.table, self.next_row, x)
+
     def step(self, qi_next: int):
         """Processes the position self.pos (embedding row self.next_row) through all layers and leaves the logits of
         head qi_next in self.logits (one launch per operation)."""
@@ -119,7 +128,7 @@ class DecodeSession:
         eng, B = self.eng, self.B
         pv, d, HD, F, Fp, h = eng.pview, eng.d, eng.HD, eng.F, eng.Fp, eng.h
         xa, xm = self.x
-        lib.embed_gather(eng.table, self.next_row, xa)
+        self.embed(xa)
         for l in range(eng.L):
             p, pk = f"transformer.layers.{l}.", eng.pk[l]
             lib.skinny_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"])
@@ -140,7 +149,7 @@ class DecodeSession:
         eng, ws, inv = self.eng, self.ws, self.seeded
         pv, F, h = eng.pview, eng.F, eng.h
         xa, xm = self.x
-        lib.embed_gather(eng.table, self.next_row, xa)
+        self.embed(xa)
         for l in range(eng.L):
             p, pk = f"transformer.layers.{l}.", eng.pk[l]
             lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws, invariant=inv)
@@ -222,31 +231,48 @@ class TokenConditionedTransformerWrapper(nn.Module):
         rows, CUDA-graph or eager execution, or earlier calls (on one GPU model and build; DESIGN section 4).  Engine.seed
         is left untouched.  seeds=torch.randint(2**62, (b,)) puts generation under torch.manual_seed.  Excludes
         uniform_noise.
+        Absolute position embeddings (use_absolute_position_embeddings=True): every token gets the row of its own
+        position within its own sequence, counted from 0, as in the reference's full forward; the row of a fed-back
+        token depends only on that sequence's prefix length and step, so seeded generation stays independent of the
+        batch.  As the reference's nn.Embedding lookup would, IndexError is raised (before anything runs, Engine.seed
+        untouched) when a conditioning sequence with its eos holds more than max_absolute_position_embeddings tokens,
+        or when prefix length + n_new - 1 exceeds it (the last sampled token is never fed back).
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
         if seeds is not None and uniform_noise is not None:
             raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
         m, eng = self.transformer, self.transformer.engine
-        was_training = m.training
-        m.eval()
-        dev = eng.dev
         S = len(self.token_sequences)
         assert len(conditioning_token_ids) == S - 1
         B = conditioning_token_ids[0].shape[0]
         info, eos = self.token_sequences[-1], self.eos_ids[-1]
         q = info.num_quantizers
+        init_step = pred_token_ids.shape[1] if pred_token_ids is not None else 0                    # :276
+        n_new = max(0, (max_time_steps - init_step) * q)
+        if eng.abs_pos and n_new > 0:
+            # the reference looks up arange(len) in each sequence's nn.Embedding(max_absolute_position_embeddings)
+            lim = eng.max_abs_pos
+            for s, t in enumerate(conditioning_token_ids):
+                n = t.numel() // B + (1 if append_eos_to_conditioning_tokens else 0)
+                if n > lim:
+                    raise IndexError(f"open_musiclm_b200 generate: conditioning sequence {s} has {n} tokens but "
+                                     f"max_absolute_position_embeddings is {lim}")
+            n_pre = pred_token_ids.numel() // B if pred_token_ids is not None else 0
+            if n_pre + n_new - 1 > lim:
+                raise IndexError(f"open_musiclm_b200 generate: the predicted sequence reaches {n_pre + n_new - 1} tokens "
+                                 f"({n_pre} given + {n_new} sampled - 1) but max_absolute_position_embeddings is {lim}")
+        was_training = m.training
+        m.eval()
+        dev = eng.dev
         cond = [t.to(dev, torch.int64).reshape(B, -1) for t in conditioning_token_ids]
         if append_eos_to_conditioning_tokens:                                                       # :288-290
             cond = [torch.cat([t, torch.full((B, 1), e, device=dev, dtype=torch.int64)], 1) for t, e in zip(cond, self.eos_ids)]
         if pred_token_ids is not None:
             assert pred_token_ids.shape[0] == B
-            init_step = pred_token_ids.shape[1]                                                     # :276
             prefix = pred_token_ids.to(dev, torch.int64).reshape(B, -1)
         else:
-            init_step = 0
             prefix = torch.empty(B, 0, device=dev, dtype=torch.int64)
-        n_new = max(0, (max_time_steps - init_step) * q)
         seed_vals = seeds_tensor(seeds, B, dev) if seeds is not None else None
         if n_new > 0:
             ids = cond + [prefix]
@@ -254,7 +280,7 @@ class TokenConditionedTransformerWrapper(nn.Module):
                 ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
                 append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
             pl = eng.plan(B, n_tok)
-            sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None)
+            sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1])
             if seed_vals is not None:
                 sess.seeds.copy_(seed_vals)
             ws = eng.workspace(pl, False)

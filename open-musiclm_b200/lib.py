@@ -161,6 +161,15 @@ def embed_gather(table, src_row, x, src_row2=None):
     call("omlm_embed_gather", _p(table), _p(src_row), _p(src_row2), _p(x), _I(M), _I(D), _stream())
 
 
+def embed_gather_pos(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x):
+    """x[m] = table[src_row[m]] + table[pos_row_base + pos[0] + pos_offset]; pos: int32 device tensor read by the
+    kernel (so a captured graph uses its current value).  A position outside [0, pos_rows) adds nothing."""
+    assert pos.dtype == torch.int32 and pos.is_cuda
+    M, D = x.shape
+    call("omlm_embed_gather_pos", _p(table), _p(src_row), _p(pos), _I(pos_offset), _I(pos_row_base), _I(pos_rows), _p(x),
+         _I(M), _I(D), _stream())
+
+
 def embed_scatter_add(dtable, src_row, dx, scale, first=None):
     """first: int32 row markers (INT_MAX, one per table row) -> the deterministic variant (omlm_embed_scatter_add_det)."""
     M, D = dx.shape
