@@ -249,7 +249,11 @@ int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float
  * loss_acc[0] += loss_scale * sum of row losses, loss_acc[1] += rows counted; dlogits bf16 [rows, ldd] =
  * (softmax - onehot) * grad_scale, zero in columns [C, Cp).  The label of row r is
  * labels[(r / rows_per_batch) * batch_stride + (r % rows_per_batch) * label_stride] (rows_per_batch <= 0: one flat
- * vector, labels[r * label_stride]) -- the strided label view of one quantizer's logit-head group, read in place. */
+ * vector, labels[r * label_stride]) -- the strided label view of one quantizer's logit-head group, read in place.
+ * Any class count C >= 1.  C <= 1280 with Cp <= 1280 keeps each row in registers; above that the row is streamed twice
+ * with 128-bit loads and 16-byte stores, which needs logits 16-byte aligned with ld % 4 == 0 and ld >= C, and (when
+ * dlogits is given) dlogits 16-byte aligned with ldd % 8 == 0, Cp % 8 == 0 and C <= Cp <= ldd (argument errors
+ * otherwise).  Both paths take 8 rows per CTA. */
 int omlm_cross_entropy(const float* logits, long ld, const int* labels, int label_stride, int rows_per_batch,
                        long batch_stride, int rows, int C, int ignore_index, float grad_scale, float loss_scale,
                        void* dlogits_bf16, long ldd, int Cp, float* loss_acc, void* stream);
