@@ -17,7 +17,7 @@
 extern "C" {
 #endif
 
-#define OMLM_B200_ABI_VERSION 3
+#define OMLM_B200_ABI_VERSION 4
 #define OMLM_MAX_SEQS 4
 
 const char* omlm_last_error(void);
@@ -182,9 +182,10 @@ int omlm_sgemm_small(const float* A, long sa_m, long sa_k, const float* B, long 
                      long sc_m, long sc_n, float* Z, const float* bias, int M, int N, int K, int act,
                      int accumulate, void* stream);
 int omlm_silu_bwd(const float* dA, const float* Z, float* dZ, void* dZ_bf16, long n, void* stream);
-/* bf16x3 operand split for near-fp32 products on the tensor cores: dst bf16 [R, 3C] = [hi|hi|lo] (activations)
- * or [hi|lo|hi] (weight_mode);  bias_silu: z += bias, a = silu(z). */
-int omlm_split3_bf16(const float* src, long src_ld, void* dst, int R, int C, int weight_mode, void* stream);
+/* bf16x3 operand split for near-fp32 products on the tensor cores: dst bf16 [R, 3 Cpad] = [hi|hi|lo] (activations)
+ * or [hi|lo|hi] (weight_mode), each third Cpad >= C columns wide with zeros in [C, Cpad) (Cpad % 8 == 0 puts every
+ * third on a 16-byte boundary);  bias_silu: z += bias, a = silu(z). */
+int omlm_split3_bf16(const float* src, long src_ld, void* dst, int R, int C, int Cpad, int weight_mode, void* stream);
 int omlm_bias_silu(float* z, const float* bias, float* a, int R, int C, void* stream);
 int omlm_colsum(const float* X, long s_m, long s_n, float* out, int M, int N, int accumulate, void* stream);
 int omlm_arange_f32(float* out, int n, void* stream);

@@ -106,18 +106,24 @@ __global__ void colsum_kernel(const float* __restrict__ X, long s_m, long s_n, f
 // bf16x3 split for near-fp32 tensor-core products:  x = hi + lo (both bf16).  With
 //   A3 = [a_hi | a_hi | a_lo]  and  W3 = [w_hi | w_lo | w_hi]   (K concatenated),
 // A3 . W3^T = a_hi w_hi + a_hi w_lo + a_lo w_hi  ~  a . w  to ~2^-16 relative, accumulated in fp32 by wgmma.
+// Each third is Cpad >= C columns wide, columns [C, Cpad) zero: with Cpad a multiple of 8 every third starts on a
+// 16-byte boundary, as a TMA view of one third needs, and the zero columns add nothing to the product.
 __global__ void split3_kernel(const float* __restrict__ src, long src_ld, __nv_bfloat16* __restrict__ dst, int R,
-                              int C, int weight_mode) {
-  const long total = static_cast<long>(R) * C;
+                              int C, int Cpad, int weight_mode) {
+  const long total = static_cast<long>(R) * Cpad;
   for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long>(gridDim.x) * blockDim.x) {
-    const int r = static_cast<int>(i / C), c = static_cast<int>(i - static_cast<long>(r) * C);
+    const int r = static_cast<int>(i / Cpad), c = static_cast<int>(i - static_cast<long>(r) * Cpad);
+    __nv_bfloat16* d = dst + static_cast<long>(r) * 3 * Cpad + c;
+    if (c >= C) {
+      d[0] = d[Cpad] = d[2 * Cpad] = __float2bfloat16_rn(0.f);
+      continue;
+    }
     const float v = src[r * src_ld + c];
     const __nv_bfloat16 hi = __float2bfloat16_rn(v);
     const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-    __nv_bfloat16* d = dst + static_cast<long>(r) * 3 * C + c;
     d[0] = hi;
-    d[C] = weight_mode ? lo : hi;
-    d[2 * C] = weight_mode ? hi : lo;
+    d[Cpad] = weight_mode ? lo : hi;
+    d[2 * Cpad] = weight_mode ? hi : lo;
   }
 }
 
@@ -187,12 +193,13 @@ int omlm_colsum(const float* X, long s_m, long s_n, float* out, int M, int N, in
   return 0;
 }
 
-int omlm_split3_bf16(const float* src, long src_ld, void* dst, int R, int C, int weight_mode, void* stream) {
+int omlm_split3_bf16(const float* src, long src_ld, void* dst, int R, int C, int Cpad, int weight_mode, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(R > 0 && C > 0, "split3: empty");
-  const long total = static_cast<long>(R) * C;
+  OMLM_CHECK_ARG(Cpad >= C && src_ld >= C, "split3: third width %d and source pitch %ld must be >= C = %d", Cpad, src_ld, C);
+  const long total = static_cast<long>(R) * Cpad;
   const int blocks = static_cast<int>(std::min<long>((total + 255) / 256, 2048));
-  OMLM_KLAUNCH((split3_kernel), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream), src, src_ld, reinterpret_cast<__nv_bfloat16*>(dst), R, C, weight_mode);
+  OMLM_KLAUNCH((split3_kernel), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream), src, src_ld, reinterpret_cast<__nv_bfloat16*>(dst), R, C, Cpad, weight_mode);
   OMLM_LAUNCH_CHECK();
   return 0;
 }

@@ -92,7 +92,7 @@ class DecodeSession:
         # bias table for every distance the generation can reach (it depends on i - j only)
         N = self.n_max
         self.rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, Hr, dt=f32) for _ in range(3)], rp_a=[E(N, Hr, dt=f32) for _ in range(3)],
-                       table=E(h, N, dt=f32), rp_a3=[E(N, 3 * Hr) for _ in range(2)])
+                       table=E(h, N, dt=f32), rp_a3=[E(N, 3 * eng.Hr8) for _ in range(2)])
         lib.arange_f32(self.rp["rp_in"])
         eng.refresh_packed()
         if eng.bias_type == "none":

@@ -114,6 +114,7 @@ class Engine:
         self.F = int(self.d * 2 * 4 / 3) if self.use_conv_ff else int(self.d * 4)
         self.Fp = _round_up(self.F, 128)           # interleaved GEGLU layout: groups of 128 channels
         self.Hr = self.d // 2                      # rel-pos MLP width
+        self.Hr8 = _round_up(self.Hr, 8)           # width of one third of its bf16x3 split operands (16-byte aligned thirds)
         self.C = [s.codebook_size + 1 for s in self.seqs]
         self.Cp = [_round_up(c, 64) for c in self.C]
         self.drop_p = float(module.ff_dropout)
@@ -147,18 +148,20 @@ class Engine:
         start = [(n, p) for n, p in named if n.startswith("start_tokens.")]
         decay = emb + [(n, p) for n, p in named if p.ndim >= 2 and not is_row_table(n)]
         nodecay = start + [(n, p) for n, p in named if p.ndim < 2 and not n.startswith("start_tokens.")]
+        # every slice starts on a 64-element boundary; the row tables (which come first) and the start tokens are also
+        # addressed as rows of one embedding "table", so they start on whole rows of d from it: lcm(64, d) apart
+        row_align = math.lcm(64, self.d)
         off, layout = 0, {}
         for n, p in decay:
             layout[n] = off
-            off = _round_up(off + p.numel(), 64)
+            off = _round_up(off + p.numel(), row_align if is_row_table(n) else 64)
         self.n_decay = off
         emb_off = layout[emb[0][0]]
-        # start tokens are addressed as rows of the embedding "table": keep them row-aligned to it
-        off = emb_off + _round_up(off - emb_off, self.d)
+        off = emb_off + _round_up(off - emb_off, row_align)
         self.n_decay = off
         for n, p in nodecay:
             layout[n] = off
-            off = _round_up(off + p.numel(), 64)
+            off = _round_up(off + p.numel(), row_align if n.startswith("start_tokens.") else 64)
         self.n_params_arena = off
         self.layout = layout
         arena_p = torch.zeros(off, device=self.dev, dtype=torch.float32)
@@ -179,6 +182,7 @@ class Engine:
         for n, p in emb:
             assert (layout[n] - emb_off) % self.d == 0
             (self.emb_row_base if n.startswith("embeddings.") else self.abs_row_base).append((layout[n] - emb_off) // self.d)
+        assert all((layout[n] - emb_off) % self.d == 0 for n, _ in start)
         self.start_row = [(layout[n] - emb_off) // self.d for n, _ in start]
         self.table = arena_p[emb_off:]
         self.dtable_emb = arena_g[emb_off:]
@@ -208,7 +212,7 @@ class Engine:
         self.pk_logit = [torch.empty(s.num_quantizers, cp, d, device=dev, dtype=a16) for s, cp in zip(self.seqs, self.Cp)]
         self.pk_logit_b = [torch.empty_like(t, dtype=bf) if dual else t for t in self.pk_logit]
         self._pack_table = None
-        self.pk_rp = [torch.empty(self.Hr, 3 * self.Hr, device=dev, dtype=torch.bfloat16) for _ in range(2)]   # rel-pos MLP layers 1, 2: [hi|lo|hi]
+        self.pk_rp = [torch.empty(self.Hr, 3 * self.Hr8, device=dev, dtype=torch.bfloat16) for _ in range(2)]  # rel-pos MLP layers 1, 2: [hi|lo|hi]
 
     def refresh_packed(self, force=False):
         ver = self.params_version()
@@ -312,7 +316,7 @@ class Engine:
             # rel-pos MLP
             rp_in=E(pl.N, 1, dt=f32), rp_z=[E(pl.N, self.Hr, dt=f32) for _ in range(3)],
             rp_a=[E(pl.N, self.Hr, dt=f32) for _ in range(3)], table=E(h, pl.N, dt=f32),
-            rp_a3=[E(pl.N, 3 * self.Hr) for _ in range(2)],
+            rp_a3=[E(pl.N, 3 * self.Hr8) for _ in range(2)],
         )
         if a16 != bf:   # fp16 forward operands (transient: one buffer each); xn / xn2 / hn / xf above are then the bf16
             ws.update(xn16=E(M, d, dt=a16), xn2_16=E(M, d, dt=a16), hn16=E(M, Fp, dt=a16),   # duplicates kept for backward
@@ -329,7 +333,7 @@ class Engine:
                 dhn=E(M, Fp), rowstat=E(M, Fp // 128, 2, dt=f32), du=E(M, 2 * Fp), dxn=E(M, d), dxraw=E(M, d),
                 d_o=E(M, HD), dqn=E(M, HD, dt=f32), dkvn=E(M, 128, dt=f32), dsum=E(M * h, dt=f32),
                 dq_raw=E(M, HD), dkv_raw=E(M, 128), dtable=E(h, pl.N, dt=f32),
-                rp_d0=E(pl.N, self.Hr, dt=f32), rp_d1=E(pl.N, self.Hr, dt=f32), rp_dz3=E(pl.N, 3 * self.Hr),
+                rp_d0=E(pl.N, self.Hr, dt=f32), rp_d1=E(pl.N, self.Hr, dt=f32), rp_dz3=E(pl.N, 3 * self.Hr8),
             )
         if det:
             self.add_det_scratch(pl, ws, train)
@@ -573,7 +577,7 @@ class Engine:
         ready("tail")
 
     def _relpos_backward(self, ws, N, det=False):
-        pv, gv, Hr, h = self.pview, self.gview, self.Hr, self.h
+        pv, gv, Hr, T, h = self.pview, self.gview, self.Hr, self.Hr8, self.h
         pre = "transformer.rel_pos_bias.net."
         dT = ws["dtable"]                                   # [h, N]: dY[n, hh] = dT[hh, n]
         a3 = ws["rp_a"][2]
@@ -588,9 +592,9 @@ class Engine:
                 # bf16x3 products, as in the forward pass (x y ~ x_hi y_hi + x_hi y_lo + x_lo y_hi: fp32-class): these
                 # gradients are sums of cancelling terms, so a plain bf16 operand rounding shows up amplified
                 lib.split3_bf16(d_cur, ws["rp_dz3"])                                                               # [hi | hi | lo]
-                dz_hi, dz_lo = ws["rp_dz3"][:, :Hr], ws["rp_dz3"][:, 2 * Hr:]
-                a_hi, a_lo = ws["rp_a3"][j - 1][:, :Hr], ws["rp_a3"][j - 1][:, 2 * Hr:]                            # forward split of a_{j-1}
-                w_hi, w_lo = self.pk_rp[j - 1][:, :Hr], self.pk_rp[j - 1][:, Hr:2 * Hr]                            # [hi | lo | hi]
+                dz_hi, dz_lo = ws["rp_dz3"][:, :Hr], ws["rp_dz3"][:, 2 * T:2 * T + Hr]                             # thirds start at 0, T, 2T
+                a_hi, a_lo = ws["rp_a3"][j - 1][:, :Hr], ws["rp_a3"][j - 1][:, 2 * T:2 * T + Hr]                   # forward split of a_{j-1}
+                w_hi, w_lo = self.pk_rp[j - 1][:, :Hr], self.pk_rp[j - 1][:, T:T + Hr]                             # [hi | lo | hi]
                 gw = gv[f"{pre}{j}.0.weight"]
                 for dz, a in ((dz_hi, a_hi), (dz_hi, a_lo), (dz_lo, a_hi)):                                         # dW_j += dz^T a
                     lib.gemm(dz, a, gw, a_mn=True, b_mn=True, M=Hr, N=Hr, K=N, addend=gw, block_n=128)

@@ -227,8 +227,11 @@ def silu_bwd(dA, Z, dZ, dZ_bf16=None):
 
 
 def split3_bf16(src, dst, weight_mode=False):
+    """dst bf16 [R, 3 Cpad] (contiguous) = the three split thirds of src [R, C], each Cpad = dst.shape[1] / 3 wide."""
     R, C = src.shape
-    call("omlm_split3_bf16", _p(src), _L(src.stride(0)), _p(dst), _I(R), _I(C), _I(int(weight_mode)), _stream())
+    assert dst.dtype == torch.bfloat16 and dst.is_contiguous() and dst.shape[0] == R and dst.shape[1] % 3 == 0
+    call("omlm_split3_bf16", _p(src), _L(src.stride(0)), _p(dst), _I(R), _I(C), _I(dst.shape[1] // 3), _I(int(weight_mode)),
+         _stream())
 
 
 def bias_silu(z, bias, a):

@@ -24,7 +24,7 @@ def test_abi_version_and_declared_symbols_are_exported():
     assert len(syms) >= 25
     for s in syms:
         assert hasattr(l, s), f"{s} declared in include/omlm_b200.h but not exported"
-    assert l.omlm_abi_version() == 3
+    assert l.omlm_abi_version() == 4
     l.omlm_last_error.restype = ctypes.c_char_p
     assert isinstance(l.omlm_last_error(), bytes)
 
