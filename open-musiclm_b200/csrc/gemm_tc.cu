@@ -6,6 +6,13 @@
 //                     previous slot, then runs the fused epilogue from its accumulator fragment (alpha, residual addend,
 //                     row remapping, split-K reductions, bf16 / fp32 stores, LayerNorm-backward row statistics).
 //
+// Staged epilogue (every launch whose output rows are the tile's rows, without atomics, with 16-byte-aligned rows):
+// each consumer warpgroup owns a ring of kEpiBoxes 64-row x 128-byte boxes in shared memory.  It writes its fragment
+// into a box, and one thread stores the box by TMA and goes on; the warpgroup only waits until a box has been read
+// out before it writes that box again, never for the global write, so the next tile's wgmma run under the stores.
+// The fp32 addend (and hn for the row statistics) comes into the same boxes by TMA: the first boxes of a tile are
+// requested before the tile's k-loop, the later ones as soon as an earlier box has been stored.
+//
 // Operand majors are template parameters so that one kernel serves the forward projections
 // (A K-major, B K-major: nn.Linear weights are [out,in]), the data-gradient GEMMs (B MN-major: the
 // same weight read "transposed" without a transposed copy) and the weight-gradient GEMMs
@@ -17,6 +24,7 @@
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
 #include <stdlib.h>
+#include <string.h>
 #include <algorithm>
 
 namespace omlm {
@@ -35,15 +43,15 @@ struct EpiParams {
   int atomic;     // 1: red.add into fp32 out (split-K)
   long split_stride;   // > 0 (deterministic split-K): split s stores its fp32 partial at out + s * split_stride, no atomics
   int vec_ok;     // out / addend rows 16-byte aligned: column pairs move as one vector
+  int staged;     // the tile goes out through the shared-memory boxes and TMA stores (see the top of this file)
   int row_split;  // >0: rows are two halves of row_split, each with row_valid live rows; <0: interleaved GEGLU groups of 128
   int row_valid;
   int n_valid;    // columns >= n_valid are dropped
   // row statistics (the d_hn data-gradient GEMM of the conv feed-forward): with d = this GEMM's fp32 output row and hn
   // the saved forward output, part[row, 2 n_blk + half] = (sum_c gamma[c] drop(d[c]), sum_c d[c] hn[c]) over each
-  // 128-column half tile -- the two row sums LayerNorm-backward needs (ffn_mid.cu), without a separate pass
-  const __nv_bfloat16* rs_hn;  // [M, rs_ldhn] bf16
-  long rs_ldhn;
-  const float* rs_gamma;       // [N] fp32 (zero in padded columns)
+  // 128-column half tile -- the two row sums LayerNorm-backward needs (ffn_mid.cu), without a separate pass.
+  // hn comes in by TMA through the epilogue's second tensor map.
+  const float* rs_gamma;      // [N] fp32 (zero in padded columns)
   const uint8_t* rs_keep;      // dropout keep bits [M, N/8] or nullptr
   float2* rs_part;             // [M, rs_parts]
   float rs_keep_scale;         // 1 / (1 - p)
@@ -61,16 +69,134 @@ struct GemmSmem {
   static constexpr int kMaxStages = 8;
 };
 
+// Staging boxes per consumer warpgroup.  Four leave room for 3 operand stages at 256-wide tiles (two boxes: 4 stages);
+// four measured faster in sum over the cfg2 GEMM shapes (DESIGN.md section 6).
+constexpr int kEpiBoxes = 4;
+constexpr int kBoxBytes = 64 * 128;         // 64 rows x 128 bytes: 32 fp32 or 64 bf16 columns (the 128B-swizzle limit)
+constexpr int kStagingBytes = 2 * kEpiBoxes * kBoxBytes;
+
+__device__ __forceinline__ void wg_bar_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory"); }
+
+// Byte offset of the column pair (8 g + 2 qc, +1) of row r in a 128B-swizzled box: 16-byte chunk c of row r sits at c ^ (r & 7).
+template <bool F32>
+__device__ __forceinline__ uint32_t box_offset(int r, int g, int qc) {
+  const int chunk = F32 ? 2 * g + (qc >> 1) : g;
+  return r * 128 + ((chunk ^ (r & 7)) << 4) + (F32 ? 8 * (qc & 1) : 4 * qc);
+}
+
+__device__ __forceinline__ void load_box(const CUtensorMap* tm, uint8_t* box, uint64_t* bar, int col, int row) {
+  mbar_expect_tx(bar, kBoxBytes);   // a box reaching past the tensor counts in full (zero-filled)
+  tma_load_2d(box, tm, bar, col, row);
+}
+
+// The staged epilogue of one tile for one consumer warpgroup (rows row0 .. row0 + 63, the first `live` boxes of
+// columns).  The arithmetic and, for the row statistics, the order of every sum are those of the direct epilogue.
+// seq counts the boxes this warpgroup has staged (slot = seq % kEpiBoxes); ephase holds one parity bit per slot.
+template <int BN, bool RS, bool F32>
+__device__ __forceinline__ void epilogue_staged(float (&acc)[BN / 2], const EpiParams& ep, const CUtensorMap* tmO,
+                                                const CUtensorMap* tmE, uint8_t* ring, uint64_t* ebar, uint32_t& seq,
+                                                uint32_t& ephase, int live, int n_blk, int row0, int M, int N, int cw,
+                                                bool leader) {
+  constexpr int kCols = F32 ? 32 : 64, kGroups = kCols / 8, kBoxesPerTile = BN / kCols;
+  constexpr int kBatch = RS ? 4 : kGroups;   // the row statistics load gamma and keep bits 4 column groups ahead
+  const bool with_e = RS || ep.addend != nullptr;
+  const int lane = threadIdx.x & 31, wq = (threadIdx.x >> 5) & 3, qr = lane >> 2, qc = lane & 3;
+  float rs1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][half]
+#pragma unroll
+  for (int b = 0; b < kBoxesPerTile; ++b) {
+    if (b >= live) break;
+    const uint32_t slot = seq % kEpiBoxes;
+    uint8_t* box = ring + slot * kBoxBytes;
+    if (with_e) {
+      mbar_wait(&ebar[slot], (ephase >> slot) & 1u);
+      ephase ^= 1u << slot;
+    } else {
+      if (leader) tma_store_wait_read<kEpiBoxes - 1>();   // the store that last used this slot has read it
+      wg_bar_sync(cw);
+    }
+#pragma unroll
+    for (int g0 = 0; g0 < kGroups; g0 += kBatch) {
+      float2 gam[kBatch];
+      uint32_t keep[2][kBatch];
+      if constexpr (RS) {
+#pragma unroll
+        for (int j = 0; j < kBatch; ++j) {
+          const int col = n_blk * BN + b * kCols + 8 * (g0 + j) + 2 * qc;
+          gam[j] = __ldg(reinterpret_cast<const float2*>(ep.rs_gamma + col));
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int row = row0 + wq * 16 + qr + hr * 8;
+            keep[hr][j] = (row < M && ep.rs_keep != nullptr) ? ep.rs_keep[static_cast<long>(row) * (N >> 3) + (col >> 3)] : 0xffu;
+          }
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < kBatch; ++j) {
+        const int i = b * kGroups + g0 + j;   // column group of the fragment
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = wq * 16 + qr + hr * 8;
+          uint8_t* p = box + box_offset<F32>(r, g0 + j, qc);
+          // rounded product, then the addend: the direct epilogue's order (a contracted fma would round once)
+          float v0 = __fmul_rn(acc[4 * i + 2 * hr], ep.alpha), v1 = __fmul_rn(acc[4 * i + 2 * hr + 1], ep.alpha);
+          if constexpr (RS) {
+            const uint32_t kb = keep[hr][j], hv = *reinterpret_cast<const uint32_t*>(p);
+            const int col = n_blk * BN + 8 * i + 2 * qc;
+            const int hf = (8 * i) / (BN / 2);
+            rs1[hr][hf] = fmaf(gam[j].x, ((kb >> (col & 7)) & 1u) ? v0 : 0.f, rs1[hr][hf]);
+            rs1[hr][hf] = fmaf(gam[j].y, ((kb >> ((col + 1) & 7)) & 1u) ? v1 : 0.f, rs1[hr][hf]);
+            rs2[hr][hf] = fmaf(v0, bf16lo(hv), rs2[hr][hf]);
+            rs2[hr][hf] = fmaf(v1, bf16hi(hv), rs2[hr][hf]);
+          }
+          if constexpr (F32) {
+            if (ep.addend != nullptr) { const float2 a = *reinterpret_cast<const float2*>(p); v0 += a.x; v1 += a.y; }
+            *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+          } else {
+            *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(v0, v1);
+          }
+        }
+      }
+    }
+    fence_proxy_async();   // the generic-proxy writes of every thread become visible to the TMA store
+    wg_bar_sync(cw);
+    if (leader) {
+      tma_store_2d(tmO, box, n_blk * BN + b * kCols, row0);
+      tma_store_commit();
+      if (with_e && b >= 1 && b - 1 + kEpiBoxes < live) {   // refill the previous box's slot once its store has read it
+        const uint32_t s = (seq - 1) % kEpiBoxes;
+        tma_store_wait_read<1>();
+        load_box(tmE, ring + s * kBoxBytes, &ebar[s], n_blk * BN + (b - 1 + kEpiBoxes) * kCols, row0);
+      }
+    }
+    ++seq;
+  }
+  if constexpr (RS) {       // quad reduction: the four lanes of a fragment row hold disjoint column pairs
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        float a1 = rs1[hr][hf], a2 = rs2[hr][hf];
+        a1 += __shfl_xor_sync(0xffffffffu, a1, 1); a1 += __shfl_xor_sync(0xffffffffu, a1, 2);
+        a2 += __shfl_xor_sync(0xffffffffu, a2, 1); a2 += __shfl_xor_sync(0xffffffffu, a2, 2);
+        const int row = row0 + wq * 16 + qr + hr * 8;
+        if (qc == 0 && row < M) ep.rs_part[static_cast<long>(row) * ep.rs_parts + 2 * n_blk + hf] = make_float2(a1 * ep.rs_keep_scale, a2);
+      }
+  }
+}
+
 template <int BN, int A_MN, int B_MN, bool F16, bool RS = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmE,
                  const EpiParams ep, const int M, const int N, const int K, const int splits, const int kStages) {
   using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atoms.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
+  uint8_t* staging = smem + kStages * S::kStageBytes;                 // [2 warpgroups][kEpiBoxes] boxes when ep.staged
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + (ep.staged ? kStagingBytes : 0));
   uint64_t* empty_bar = full_bar + S::kMaxStages;
+  uint64_t* epi_bar = empty_bar + S::kMaxStages;                      // [2 warpgroups][kEpiBoxes]: addend / hn box loaded
 
   const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
@@ -88,6 +214,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 2);        // one arrival per consumer warpgroup
+    }
+    if (ep.staged) {
+      tma_prefetch_desc(&tmO);
+      for (int i = 0; i < 2 * kEpiBoxes; ++i) mbar_init(&epi_bar[i], 1);
     }
     fence_barrier_init();
   }
@@ -137,6 +267,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int wq = (threadIdx.x >> 5) & 3;                   // warp within the warpgroup: 16 rows each
   const int qr = lane >> 2, qc = lane & 3;                 // fragment row / column pair within the warp's rows
   const bool leader = (threadIdx.x & 127) == 0;
+  uint8_t* ring = staging + cw * kEpiBoxes * kBoxBytes;
+  uint64_t* ebar = epi_bar + cw * kEpiBoxes;
+  const bool with_e = ep.staged && (RS || ep.addend != nullptr);
+  const int box_cols = (RS || !ep.out_f32) ? 64 : 32;
+  uint32_t seq = 0, ephase = 0;
   int stage = 0;
   uint32_t phase = 0;
   for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
@@ -145,6 +280,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int n_blk = tile % n_tiles, m_blk = tile / n_tiles;
     const int kb0 = split * kb_per_split;
     const int kb1 = min(kb_total, kb0 + kb_per_split);
+    const int row0 = m_blk * BM + cw * 64;
+    // boxes of this warpgroup's 64 rows that hold any output (none when the rows lie past M)
+    const int live = row0 < M ? max(0, min(BN / box_cols, (ep.n_valid - n_blk * BN + box_cols - 1) / box_cols)) : 0;
+    if (with_e && leader) {   // the tile's first addend / hn boxes load under its k-loop, once the last stores have read their slots
+      tma_store_wait_read<0>();
+      for (int j = 0; j < min(kEpiBoxes, live); ++j) {
+        const uint32_t s = (seq + j) % kEpiBoxes;
+        load_box(&tmE, ring + s * kBoxBytes, &ebar[s], n_blk * BN + j * box_cols, row0);
+      }
+    }
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -173,122 +318,99 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     wgmma_reg_fence(acc);
     if (prev >= 0 && leader) mbar_arrive(&empty_bar[prev]);
 
-    // ------------------------------------------------------------------ epilogue: rows r_lo, r_lo + 8 of the fragment
-    int row_in[2];
-    long orow[2], arow[2];
-    bool row_ok[2];
-#pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-      int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
-      row_in[hr] = row;
-      row_ok[hr] = row < M;
-      if (ep.row_split > 0) {
-        const int half = row / ep.row_split, r = row - half * ep.row_split;
-        row_ok[hr] = row_ok[hr] && r < ep.row_valid;
-        row = half * ep.row_valid + r;
-      } else if (ep.row_split < 0) {   // interleaved GEGLU rows: [128 value | 128 gate] per group of 128 channels
-        const int w256 = row & 255, ch = ((row >> 8) << 7) + (w256 & 127);
-        row_ok[hr] = row_ok[hr] && ch < ep.row_valid;
-        row = (w256 >> 7) * ep.row_valid + ch;
+    if constexpr (RS) {   // the row statistics are always staged (checked on the host)
+      epilogue_staged<BN, true, false>(acc, ep, &tmO, &tmE, ring, ebar, seq, ephase, live, n_blk, row0, M, N, cw, leader);
+    } else if (ep.staged) {
+      if (ep.out_f32) epilogue_staged<BN, false, true>(acc, ep, &tmO, &tmE, ring, ebar, seq, ephase, live, n_blk, row0, M, N, cw, leader);
+      else epilogue_staged<BN, false, false>(acc, ep, &tmO, &tmE, ring, ebar, seq, ephase, live, n_blk, row0, M, N, cw, leader);
+    } else {
+      // ------------------------------------------------------------------ direct epilogue: rows r_lo, r_lo + 8 of the fragment
+      // (atomic split-K, the row remaps, split-K partial slices, rows that are not 16-byte aligned)
+      long orow[2], arow[2];
+      bool row_ok[2];
+  #pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
+        row_ok[hr] = row < M;
+        if (ep.row_split > 0) {
+          const int half = row / ep.row_split, r = row - half * ep.row_split;
+          row_ok[hr] = row_ok[hr] && r < ep.row_valid;
+          row = half * ep.row_valid + r;
+        } else if (ep.row_split < 0) {   // interleaved GEGLU rows: [128 value | 128 gate] per group of 128 channels
+          const int w256 = row & 255, ch = ((row >> 8) << 7) + (w256 & 127);
+          row_ok[hr] = row_ok[hr] && ch < ep.row_valid;
+          row = (w256 >> 7) * ep.row_valid + ch;
+        }
+        orow[hr] = static_cast<long>(row) * ep.ldo;
+        arow[hr] = static_cast<long>(row) * ep.ldadd;
       }
-      orow[hr] = static_cast<long>(row) * ep.ldo;
-      arow[hr] = static_cast<long>(row) * ep.ldadd;
-    }
-    // The columns go in batches of kEpiBatch 8-column groups, and every global load of a batch (the addend; hn, keep
-    // bits and gamma for the row statistics) is issued before the batch's first store.  The stores may alias the loads
-    // (a weight gradient without split-K adds into its own output), so the compiler keeps each load behind every earlier
-    // store: loads interleaved with stores each waited a full memory latency, which on H100 cost more than the
-    // mainloop of the addend GEMMs (wo: 153 us with the addend against 58 us without, cfg2 shape, 400 W).
-    constexpr int kEpiBatch = RS ? 4 : 8;   // the row statistics hold three more operands per column pair
-    float rs1[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, rs2[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [row][half]
-#pragma unroll
-    for (int i0 = 0; i0 < BN / 8; i0 += kEpiBatch) {
-      float2 add[2][kEpiBatch], gam[kEpiBatch];
-      uint32_t hv[2][kEpiBatch], keep[2][kEpiBatch];
-#pragma unroll
-      for (int j = 0; j < kEpiBatch; ++j) {
-        const int col = n_blk * BN + 8 * (i0 + j) + 2 * qc;
-        const bool c0_ok = col < ep.n_valid, c1_ok = col + 1 < ep.n_valid;
-        if constexpr (RS) gam[j] = c0_ok ? __ldg(reinterpret_cast<const float2*>(ep.rs_gamma + col)) : make_float2(0.f, 0.f);
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          add[hr][j] = make_float2(0.f, 0.f);
-          hv[hr][j] = 0u;
-          keep[hr][j] = 0xffu;
-          if (!row_ok[hr] || !c0_ok) continue;
-          if (!RS && ep.addend != nullptr) {   // the row-statistics launch never has an addend (checked on the host)
-            const float* ap = ep.addend + arow[hr] + col;
-            if (c1_ok && ep.vec_ok) add[hr][j] = *reinterpret_cast<const float2*>(ap);
-            else { add[hr][j].x = ap[0]; if (c1_ok) add[hr][j].y = ap[1]; }
+      // The columns go in batches of kEpiBatch 8-column groups, and every addend load of a batch is issued before the
+      // batch's first store.  The stores may alias the loads (a weight gradient without split-K adds into its own
+      // output), so the compiler keeps each load behind every earlier store: loads interleaved with stores each waited a
+      // full memory latency.
+      constexpr int kEpiBatch = 8;
+  #pragma unroll
+      for (int i0 = 0; i0 < BN / 8; i0 += kEpiBatch) {
+        float2 add[2][kEpiBatch];
+  #pragma unroll
+        for (int j = 0; j < kEpiBatch; ++j) {
+          const int col = n_blk * BN + 8 * (i0 + j) + 2 * qc;
+          const bool c0_ok = col < ep.n_valid, c1_ok = col + 1 < ep.n_valid;
+  #pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            add[hr][j] = make_float2(0.f, 0.f);
+            if (!row_ok[hr] || !c0_ok) continue;
+            if (ep.addend != nullptr) {
+              const float* ap = ep.addend + arow[hr] + col;
+              if (c1_ok && ep.vec_ok) add[hr][j] = *reinterpret_cast<const float2*>(ap);
+              else { add[hr][j].x = ap[0]; if (c1_ok) add[hr][j].y = ap[1]; }
+            }
           }
-          if constexpr (RS) {
-            hv[hr][j] = *reinterpret_cast<const uint32_t*>(ep.rs_hn + static_cast<long>(row_in[hr]) * ep.rs_ldhn + col);
-            if (ep.rs_keep != nullptr) keep[hr][j] = ep.rs_keep[static_cast<long>(row_in[hr]) * (N >> 3) + (col >> 3)];
+        }
+  #pragma unroll
+        for (int j = 0; j < kEpiBatch; ++j) {
+          const int i = i0 + j;
+          const int col = n_blk * BN + 8 * i + 2 * qc;
+          if (col >= ep.n_valid) continue;
+          const bool pair = col + 1 < ep.n_valid && ep.vec_ok;
+  #pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            if (!row_ok[hr]) continue;
+            float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
+            if (ep.addend != nullptr) { v0 += add[hr][j].x; v1 += add[hr][j].y; }
+            if (ep.atomic) {
+              float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
+              if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
+              else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
+            } else if (ep.out_f32) {
+              float* op = reinterpret_cast<float*>(ep.out) + split * ep.split_stride + orow[hr] + col;
+              if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
+              else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
+            } else {
+              __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + orow[hr] + col;
+              if (pair) *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
+              else { op[0] = __float2bfloat16_rn(v0); if (col + 1 < ep.n_valid) op[1] = __float2bfloat16_rn(v1); }
+            }
           }
         }
       }
-#pragma unroll
-      for (int j = 0; j < kEpiBatch; ++j) {
-        const int i = i0 + j;
-        const int col = n_blk * BN + 8 * i + 2 * qc;
-        if (col >= ep.n_valid) continue;
-        const bool pair = col + 1 < ep.n_valid && ep.vec_ok;
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          if (!row_ok[hr]) continue;
-          float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
-          if constexpr (RS) {
-            const uint32_t kb = keep[hr][j];
-            const float2 g = gam[j];
-            const int hf = (8 * i) / (BN / 2);
-            rs1[hr][hf] = fmaf(g.x, ((kb >> (col & 7)) & 1u) ? v0 : 0.f, rs1[hr][hf]);
-            rs1[hr][hf] = fmaf(g.y, ((kb >> ((col + 1) & 7)) & 1u) ? v1 : 0.f, rs1[hr][hf]);
-            rs2[hr][hf] = fmaf(v0, bf16lo(hv[hr][j]), rs2[hr][hf]);
-            rs2[hr][hf] = fmaf(v1, bf16hi(hv[hr][j]), rs2[hr][hf]);
-          }
-          if (!RS && ep.addend != nullptr) { v0 += add[hr][j].x; v1 += add[hr][j].y; }
-          if (ep.atomic) {
-            float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
-            if (pair) asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(op), "f"(v0), "f"(v1) : "memory");
-            else { atomicAdd(op, v0); if (col + 1 < ep.n_valid) atomicAdd(op + 1, v1); }
-          } else if (ep.out_f32) {
-            float* op = reinterpret_cast<float*>(ep.out) + split * ep.split_stride + orow[hr] + col;
-            if (pair) *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
-            else { op[0] = v0; if (col + 1 < ep.n_valid) op[1] = v1; }
-          } else {
-            __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(ep.out) + orow[hr] + col;
-            if (pair) *reinterpret_cast<uint32_t*>(op) = pack_bf16x2(v0, v1);
-            else { op[0] = __float2bfloat16_rn(v0); if (col + 1 < ep.n_valid) op[1] = __float2bfloat16_rn(v1); }
-          }
-        }
-      }
-    }
-    if constexpr (RS) {       // quad reduction: the four lanes of a fragment row hold disjoint column pairs
-#pragma unroll
-      for (int hr = 0; hr < 2; ++hr)
-#pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          float a1 = rs1[hr][hf], a2 = rs2[hr][hf];
-          a1 += __shfl_xor_sync(0xffffffffu, a1, 1); a1 += __shfl_xor_sync(0xffffffffu, a1, 2);
-          a2 += __shfl_xor_sync(0xffffffffu, a2, 1); a2 += __shfl_xor_sync(0xffffffffu, a2, 2);
-          const int row = m_blk * BM + cw * 64 + wq * 16 + qr + hr * 8;
-          if (qc == 0 && row < M) ep.rs_part[static_cast<long>(row) * ep.rs_parts + 2 * n_blk + hf] = make_float2(a1 * ep.rs_keep_scale, a2);
-        }
     }
   }
+  if (ep.staged && leader) tma_store_wait_all();   // the boxes stay allocated until the last stores have completed
 }
 
 constexpr int kMaxDynSmem = 232448;      // 227 KB per CTA on sm_90
 constexpr int kBarrierBytes = 256;
 
 template <int BN, int A_MN, int B_MN, bool RS = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& ep, int M, int N, int K, int splits,
-                       int max_ctas, int f16, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const CUtensorMap& tmE,
+                       const EpiParams& ep, int M, int N, int K, int splits, int max_ctas, int f16, cudaStream_t stream) {
   using S = GemmSmem<BN>;
   auto kern = f16 ? gemm_bf16_kernel<BN, A_MN, B_MN, true, RS> : gemm_bf16_kernel<BN, A_MN, B_MN, false, RS>;
-  int stages = (kMaxDynSmem - 1024 - kBarrierBytes) / S::kStageBytes;
+  const int staging = ep.staged ? kStagingBytes : 0;
+  int stages = (kMaxDynSmem - 1024 - kBarrierBytes - staging) / S::kStageBytes;
   if (stages > 6) stages = 6;
-  const int smem_bytes = stages * S::kStageBytes + kBarrierBytes + 1024;
+  const int smem_bytes = stages * S::kStageBytes + staging + kBarrierBytes + 1024;
   static bool configured[2] = {false, false};
   if (!configured[f16]) {
     OMLM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
@@ -299,7 +421,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Epi
   int grid = num_sms();
   if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
   if (work < grid) grid = work;
-  OMLM_KLAUNCH((kern), grid, kGemmThreads, smem_bytes, stream, tmA, tmB, ep, M, N, K, splits, stages);
+  OMLM_KLAUNCH((kern), grid, kGemmThreads, smem_bytes, stream, tmA, tmB, tmO, tmE, ep, M, N, K, splits, stages);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
@@ -345,27 +467,42 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   ep.vec_ok = ((ldo * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
               (addend == nullptr || ((ldadd * 4) % 16 == 0 && (reinterpret_cast<uintptr_t>(addend) & 15) == 0));
   ep.row_split = row_split; ep.row_valid = row_valid; ep.n_valid = n_valid;
-  ep.rs_hn = nullptr; ep.rs_ldhn = 0; ep.rs_gamma = nullptr; ep.rs_keep = nullptr; ep.rs_part = nullptr; ep.rs_keep_scale = 1.f;
-  ep.rs_parts = 0;
+  ep.rs_gamma = nullptr; ep.rs_keep = nullptr; ep.rs_part = nullptr; ep.rs_keep_scale = 1.f; ep.rs_parts = 0;
+  // The staged epilogue stores whole boxes of tile rows by TMA: the output rows must be the tile's rows, without
+  // atomics, and TMA needs 16-byte-aligned bases and pitches.  The boxes hold one element type, so an addend goes
+  // with an fp32 output.  Stores are clipped to M x n_valid by the map, but only at 16-byte granularity in a row,
+  // so n_valid must end on a 16-byte boundary.
+  ep.staged = !ep.atomic && split_stride == 0 && row_split == 0 && ep.vec_ok && (addend == nullptr || out_f32) &&
+              (n_valid * esz) % 16 == 0;
+  CUtensorMap tmO, tmE;
+  memset(&tmO, 0, sizeof(tmO));
+  memset(&tmE, 0, sizeof(tmE));
+  if (ep.staged) {
+    rc = make_tmap_2d(&tmO, static_cast<int>(esz), out, (uint64_t)n_valid, (uint64_t)M, (uint64_t)(ldo * esz), out_f32 ? 32 : 64, 64);
+    if (rc == 0 && addend != nullptr) rc = make_tmap_2d(&tmE, 4, addend, (uint64_t)n_valid, (uint64_t)M, (uint64_t)(ldadd * 4), 32, 64);
+    if (rc) return rc;
+  }
   const int f16 = a_f16 ? 1 : 0;
   const int key = (block_n == 256 ? 4 : 0) | (a_mn_major ? 2 : 0) | (b_mn_major ? 1 : 0);
   if (rs != nullptr) {
     OMLM_CHECK_ARG(block_n == 256 && N % 256 == 0 && n_valid == N && !out_f32 && addend == nullptr && splits == 1 && row_split == 0 &&
-                   ep.vec_ok && rs->parts == 2 * (N / 256) && rs->ldhn % 8 == 0,
-                   "gemm row statistics: needs 256-wide tiles, N %% 256 == 0, a dense bf16 output and parts == N / 128");
+                   ep.vec_ok && rs->parts == 2 * (N / 256) && rs->ldhn % 8 == 0 && (reinterpret_cast<uintptr_t>(rs->hn) & 15) == 0,
+                   "gemm row statistics: needs 256-wide tiles, N %% 256 == 0, a dense bf16 output, 16-byte-aligned hn rows "
+                   "and parts == N / 128");
     OMLM_CHECK_ARG(key == 5, "gemm row statistics: only the A K-major / B MN-major 256-wide instantiation exists");
-    ep.rs_hn = reinterpret_cast<const __nv_bfloat16*>(rs->hn); ep.rs_ldhn = rs->ldhn;
+    rc = make_tmap_2d(&tmE, 2, rs->hn, (uint64_t)N, (uint64_t)M, (uint64_t)rs->ldhn * 2, 64, 64);
+    if (rc) return rc;
     ep.rs_gamma = rs->gamma; ep.rs_keep = reinterpret_cast<const uint8_t*>(rs->keep_bits);
     ep.rs_part = reinterpret_cast<float2*>(rs->part); ep.rs_keep_scale = rs->keep_scale; ep.rs_parts = rs->parts;
-    return launch_gemm<256, 0, 1, true>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    return launch_gemm<256, 0, 1, true>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
   }
   switch (key) {
-    case 0: return launch_gemm<128, 0, 0>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
-    case 1: return launch_gemm<128, 0, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
-    case 3: return launch_gemm<128, 1, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
-    case 4: return launch_gemm<256, 0, 0>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
-    case 5: return launch_gemm<256, 0, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
-    case 7: return launch_gemm<256, 1, 1>(tmA, tmB, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 0: return launch_gemm<128, 0, 0>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 1: return launch_gemm<128, 0, 1>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 3: return launch_gemm<128, 1, 1>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 4: return launch_gemm<256, 0, 0>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 5: return launch_gemm<256, 0, 1>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
+    case 7: return launch_gemm<256, 1, 1>(tmA, tmB, tmO, tmE, ep, M, N, K, splits, max_ctas, f16, stream);
     default:
       set_last_error("gemm: operand majors (a_mn=%d, b_mn=%d) not instantiated", a_mn_major, b_mn_major);
       return 1;
