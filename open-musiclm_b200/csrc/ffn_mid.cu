@@ -237,7 +237,7 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
 
   // ---- per-lane constants: 4 value + 4 gate channels, held as two fp32x2 pairs (channels 2q, 2q+1)
   const int c0 = g * 128 + lane * 4;                   // natural channel index of this lane's first channel
-  float2 wa[3][2], wg[3][2], gm[2], pm[2];             // taps [k][pair], gamma, 1/0 mask of real (un-padded) channels
+  float2 wa[3][2], wg[3][2], gm[2], pm[2];             // taps [k][pair], gamma, 1/0 mask of real (c < F) channels
   {
     const float4* wp = reinterpret_cast<const float4*>(a.conv_w + static_cast<long>(g * 256 + lane * 4) * 3);
     const float4* gp = reinterpret_cast<const float4*>(a.conv_w + static_cast<long>(g * 256 + 128 + lane * 4) * 3);
@@ -254,8 +254,10 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
       }
     const float4 gg = __ldg(reinterpret_cast<const float4*>(a.gamma + c0));   // zero in the padding
     gm[0] = make_float2(gg.x, gg.y); gm[1] = make_float2(gg.z, gg.w);
-    pm[0] = make_float2(gg.x != 0.f ? 1.f : 0.f, gg.y != 0.f ? 1.f : 0.f);
-    pm[1] = make_float2(gg.z != 0.f ? 1.f : 0.f, gg.w != 0.f ? 1.f : 0.f);
+    // padded channels are c >= F.  Not gamma == 0: a real channel whose gamma is exactly zero (zero-initialised, pruned)
+    // still has dh = rstd (-m1 - hhat m2) != 0, and with it a gradient in u and in its conv taps
+    pm[0] = make_float2(c0 < a.F ? 1.f : 0.f, c0 + 1 < a.F ? 1.f : 0.f);
+    pm[1] = make_float2(c0 + 2 < a.F ? 1.f : 0.f, c0 + 3 < a.F ? 1.f : 0.f);
   }
   const float keep_scale = a.drop_p > 0.f ? 1.f / (1.f - a.drop_p) : 1.f;
   asm volatile("cp.async.wait_all;" ::: "memory");
@@ -309,7 +311,7 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
         normal_cdf_pdf2(yg, phi, pdf);
         const float2 ge = mul2(yg, phi);
         const float2 hhat = mul2(fma2(ge, ya, nmean), rstd);
-        // dh = rstd * (gamma d - m1 - hhat m2), forced to 0 on padded channels (gamma == 0)
+        // dh = rstd * (gamma d - m1 - hhat m2), forced to 0 on padded channels (c >= F)
         const float2 dh = mul2(mul2(rstd, pm[q]), fma2(hhat, nm2, fma2(gm[q], d[q], nm1)));
         da0[q] = mul2(dh, ge);
         dg0[q] = mul2(mul2(dh, ya), fma2(yg, pdf, phi));
