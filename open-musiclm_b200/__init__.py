@@ -15,4 +15,4 @@ from .model import (TokenConditionedTransformer, TokenSequenceInfo, create_coars
                     create_fine_transformer, create_semantic_transformer)
 from .trainer import HotPathTrainer  # noqa: F401
 from .decode import TokenConditionedTransformerWrapper  # noqa: F401
-from .stages import CoarseStage, FineStage, MusicLM, NoiseStream, SemanticStage  # noqa: F401
+from .stages import CoarseStage, FineStage, MusicLM, NoiseStream, SemanticStage, prepare_audio  # noqa: F401

@@ -8,11 +8,15 @@ stream, every fine window on a slice of the coarse stream.  All arithmetic here 
 the compute is `TokenConditionedTransformerWrapper.generate` (KV-cache decode, decode.py).
 
 The tokenizers (CLAP-RVQ, MERT/HuBERT k-means, Encodec) are outside the hot path (SURVEY section 2): the stages accept
-them as opaque callables exactly like the reference and never need them when token ids are passed in.
+them as opaque callables exactly like the reference and never need them when token ids are passed in.  Audio
+continuation (MusicLM.forward(prime_wave=...)) and best-of-N sampling (MusicLM.generate_top_match) call the caller's
+wav2vec, codec and CLAP objects for the prime tokens and the similarity scores; the generation itself is the same
+prefill + KV-cache decode, driven with the prime's tokens as the predicted sequence's prefix.
 """
 from typing import List, Optional
 
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from .decode import TokenConditionedTransformerWrapper
@@ -177,8 +181,49 @@ def _windows(tokens: torch.Tensor, size: int, step: int):
     return [tokens[:, s:s + size] for s in range(0, T - size + 1, step)]
 
 
+# ---------------------------------------------------------------------------------------- audio helpers (utils.py:147-166)
+def _resample(wave: torch.Tensor, orig_hz, new_hz) -> torch.Tensor:
+    from torchaudio.functional import resample
+    return resample(wave, orig_hz, new_hz)
+
+
+def int16_to_float32(x: torch.Tensor) -> torch.Tensor:
+    return (x / 32767.0).type(torch.float32)
+
+
+def float32_to_int16(x: torch.Tensor) -> torch.Tensor:
+    return (torch.clamp(x, min=-1., max=1.) * 32767.).type(torch.int16)
+
+
+def zero_mean_unit_var_norm(x: torch.Tensor) -> torch.Tensor:
+    return (x - x.mean(dim=-1, keepdim=True)) / torch.sqrt(x.var(dim=-1, keepdim=True) + 1e-7)
+
+
+def prepare_audio(data: torch.Tensor, sample_hz, target_sample_hz, normalize=True, target_length_seconds=None) -> torch.Tensor:
+    """A [channels, n] wave -> the [1, m] mono wave a tokenizer at target_sample_hz takes: the channel mean (more than
+    one channel), optionally zero mean / unit variance, cropped to target_length_seconds, resampled, then rounded
+    through int16 as a file would store it."""
+    if data.shape[0] > 1:
+        data = data.mean(dim=0, keepdim=True)
+    if normalize:
+        data = zero_mean_unit_var_norm(data)
+    if target_length_seconds is not None and data.shape[1] > target_length_seconds * sample_hz:
+        data = data[:, :int(target_length_seconds * sample_hz)]
+    return int16_to_float32(float32_to_int16(_resample(data, sample_hz, target_sample_hz)))
+
+
+def _prime(t: torch.Tensor, b: int, q: int, device, what: str) -> torch.Tensor:
+    """Prime tokens [1 or b, T, q] ([1 or b, T] for the semantic stream) -> [b, T, q] int64 on `device`."""
+    if t.dim() == 2 and q == 1:
+        t = t.unsqueeze(-1)
+    if t.dim() != 3 or t.shape[-1] != q or t.shape[0] not in (1, b):
+        raise ValueError(f"open_musiclm_b200 MusicLM.generate_tokens: {what} must be [1 or {b}, T, {q}], got {tuple(t.shape)}")
+    return t.to(device, torch.int64).expand(b, -1, -1).contiguous()
+
+
 class MusicLM(nn.Module):
-    """open_musiclm.py:817-1035: text (clap tokens) -> semantic -> coarse -> fine token streams through sliding windows."""
+    """open_musiclm.py:817-1071: text (clap tokens), optionally continuing a prime wave -> semantic -> coarse -> fine token
+    streams through sliding windows; best-of-N sampling scored by CLAP (generate_top_match)."""
 
     def __init__(self, *, semantic_transformer=None, coarse_transformer=None, fine_transformer=None, wav2vec=None, clap=None,
                  neural_codec=None, stages=None):
@@ -198,12 +243,22 @@ class MusicLM(nn.Module):
     def generate_tokens(self, *, clap_token_ids, output_seconds=8, semantic_window_seconds=10, coarse_window_seconds=4,
                         fine_window_seconds=2, semantic_steps_per_second=50, acoustic_steps_per_second=75,
                         semantic_sliding_window_step_percent=0.5, coarse_sliding_window_step_percent=0.5,
-                        fine_sliding_window_step_percent=1, noise: Optional[NoiseStream] = None, return_all=False, seeds=None):
-        """The token-level body of MusicLM.forward (open_musiclm.py:925-1031, no audio prompt): returns the acoustic tokens
+                        fine_sliding_window_step_percent=1, noise: Optional[NoiseStream] = None, return_all=False, seeds=None,
+                        prime_semantic_token_ids=None, prime_coarse_token_ids=None, prime_fine_token_ids=None, coarse_only=False):
+        """The token-level body of MusicLM.forward (open_musiclm.py:913-1032): returns the acoustic tokens
         [b, T, coarse + fine quantizers] the reference would hand to the codec (return_all: also the three streams).
         seeds (optional): one unsigned 64-bit seed per prompt (list of ints or int64 tensor).  Every generate call then gets
         the per-sequence seeds window_seed(seeds[b], stage, window index), so the whole song of prompt b is a function
-        of (prompt b, seeds[b]), whatever else is in the batch.  Excludes noise."""
+        of (prompt b, prime, seeds[b]), whatever else is in the batch.  Excludes noise.
+        prime_{semantic,coarse,fine}_token_ids (audio continuation, all three or none): the tokens of a prime wave,
+        [1 or b, Ts, 1], [1 or b, Ta, coarse quantizers], [1 or b, Ta, fine quantizers].  The first window of every
+        stage is conditioned on the prime's tail, the streams are cropped so that the stages line up, and the full
+        prime acoustic streams come first in the output.  A prime with batch 1 is used for all b prompts, one with
+        batch b row by row (the reference tokenizes a single prime wave and so continues a single prompt).  With a fine
+        condition length > 0 (fine_sliding_window_step_percent < 1) the reference's streams cannot be joined; here the
+        coarse stream drops the prime tokens the first fine window was conditioned on, so both start after the prime.
+        coarse_only: stop after the coarse stage and return its stream [b, T, coarse quantizers] as it stands before
+        the crop that lines it up with the fine windows (forward's return_coarse_generated_wave)."""
         if seeds is not None and noise is not None:
             raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: seeds and noise exclude each other")
         if seeds is not None:
@@ -220,40 +275,122 @@ class MusicLM(nn.Module):
             return dict(seeds=[window_seed(s, stage, w) for s in seeds])
 
         sps, aps = semantic_steps_per_second, acoustic_steps_per_second
+        primes = (prime_semantic_token_ids, prime_coarse_token_ids, prime_fine_token_ids)
+        primed = prime_semantic_token_ids is not None
+        if any((p is not None) != primed for p in primes):
+            raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: pass all three prime token streams or none")
+        # ---- audio continuation: condition lengths, the prime's tails and the crops that line the stages up (:913-926)
+        sem_prime = coarse_prime = fine_prime = None
+        sem_adj = coarse_adj = fine_adj = 0
+        if primed:
+            B = clap_token_ids.shape[0]
+            qc = self.coarse.num_coarse_quantizers
+            qf = self.fine.transformer_wrapper.token_sequences[-1].num_quantizers
+            prime_sem = _prime(prime_semantic_token_ids, B, 1, self.semantic.device, "prime_semantic_token_ids")
+            prime_coarse = _prime(prime_coarse_token_ids, B, qc, self.coarse.device, "prime_coarse_token_ids")
+            prime_fine = _prime(prime_fine_token_ids, B, qf, self.fine.device, "prime_fine_token_ids")
+            cond_sem = int(sps * semantic_window_seconds * (1 - semantic_sliding_window_step_percent))
+            cond_coarse = int(aps * coarse_window_seconds * (1 - coarse_sliding_window_step_percent))
+            cond_fine = int(aps * fine_window_seconds * (1 - fine_sliding_window_step_percent))
+            sem_prime = prime_sem[:, -cond_sem:] if prime_sem.shape[1] >= cond_sem else prime_sem
+            coarse_prime = prime_coarse[:, -cond_coarse:]
+            fine_prime = prime_fine[:, -cond_fine:] if cond_fine > 0 else None
+            sem_adj = cond_sem - int(sps * coarse_window_seconds * (1 - coarse_sliding_window_step_percent))
+            coarse_adj = cond_coarse - int(aps * fine_window_seconds * (1 - fine_sliding_window_step_percent))
+            fine_adj = cond_fine
         common = dict(clap_token_ids=clap_token_ids, include_eos_in_output=False, append_eos_to_conditioning_tokens=True, noise=noise)
-        # ---- semantic stream: first window from scratch, then windows conditioned on the tail of the stream (:930-949)
-        sem = self.semantic.generate(semantic_token_ids=None, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps),
+        # ---- semantic stream: first window from the prime's tail (or scratch), then windows conditioned on the tail of
+        # the stream (:930-949); cropped to line up with the coarse windows (:952)
+        sem = self.semantic.generate(semantic_token_ids=sem_prime, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps),
                                      **common, **seeded(SEMANTIC))
         keep = int(semantic_window_seconds * sps * (1 - semantic_sliding_window_step_percent))
         while sem.shape[1] < int(output_seconds * sps):
             nxt = self.semantic.generate(semantic_token_ids=sem[:, -keep:], max_time_steps=int(semantic_window_seconds * sps), **common,
                                          **seeded(SEMANTIC))
             sem = torch.cat([sem, nxt[:, keep:]], 1)
-        # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail (:956-985)
+        sem = sem[:, sem_adj:]
+        # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail, the first one
+        # on the prime's (:956-985)
         win = int(coarse_window_seconds * sps - 1)
         coarse, keep = None, int(coarse_window_seconds * aps * (1 - coarse_sliding_window_step_percent))
         for sem_win in _windows(sem, win, int(win * coarse_sliding_window_step_percent)):
-            pred = self.coarse.generate(semantic_token_ids=sem_win, coarse_token_ids=None if coarse is None else coarse[:, -keep:],
+            pred = self.coarse.generate(semantic_token_ids=sem_win, coarse_token_ids=coarse_prime if coarse is None else coarse[:, -keep:],
                                         max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common, **seeded(COARSE))
             coarse = pred if coarse is None else torch.cat([coarse, pred[:, keep:]], 1)
-        # ---- fine stream: one window of coarse tokens per generate (:995-1024)
+        if coarse_only:                                                                                 # :986-989
+            return coarse
+        coarse = coarse[:, coarse_adj:]                                                                 # :992
+        # ---- fine stream: one window of coarse tokens per generate, the first one conditioned on the prime's tail (:995-1024)
         fwin = int(fine_window_seconds * aps)
         fine, keep = None, int(fwin * (1 - fine_sliding_window_step_percent))
         for coarse_win in _windows(coarse, fwin, int(fwin * fine_sliding_window_step_percent)):
-            cond = fine[:, -keep:] if (fine is not None and keep > 0) else None
+            cond = fine_prime if fine is None else (fine[:, -keep:] if keep > 0 else None)
             pred = self.fine.generate(coarse_token_ids=coarse_win, fine_token_ids=cond, max_time_steps=fwin, temperature=0.4, **common,
                                       **seeded(FINE))
             fine = pred if fine is None else torch.cat([fine, pred[:, keep:]], 1)
+        fine = fine[:, fine_adj:]                                                                       # :1026
+        # the coarse stream still starts with the fine_adj prime tokens the first fine window was conditioned on; the
+        # reference keeps them, so with a fine condition length > 0 its coarse and fine streams differ in length and
+        # cannot be joined.  Dropping them lines both up on the first token after the prime (no-op when fine_adj = 0).
+        coarse = coarse[:, fine_adj:]
+        if primed:                                                                                      # :1028-1030
+            fine, coarse = torch.cat([prime_fine, fine], 1), torch.cat([prime_coarse, coarse], 1)
         acoustic = torch.cat([coarse, fine], -1)                                                       # :1032
         return (acoustic, sem, coarse, fine) if return_all else acoustic
 
+    def prime_token_ids(self, prime_wave: torch.Tensor, prime_wave_sample_hz, semantic_window_seconds=10):
+        """A [channels, n] prime wave -> the prime_{semantic,coarse,fine}_token_ids of generate_tokens (batch 1), through
+        the caller's wav2vec (semantic ids at wav2vec.target_sample_hz, normalised wave) and codec (acoustic ids at
+        neural_codec.sample_rate, wave as it is), each fed the first semantic_window_seconds (open_musiclm.py:897-912)."""
+        if self.wav2vec is None or self.neural_codec is None:
+            raise ValueError("open_musiclm_b200 MusicLM: audio continuation (prime_wave) needs the wav2vec and neural_codec "
+                             "tokenizers; pass them to MusicLM(wav2vec=..., neural_codec=...)")
+        if prime_wave_sample_hz is None:
+            raise ValueError("open_musiclm_b200 MusicLM: prime_wave needs prime_wave_sample_hz")
+        wave_sem = prepare_audio(prime_wave, prime_wave_sample_hz, self.wav2vec.target_sample_hz, normalize=True,
+                                 target_length_seconds=semantic_window_seconds)
+        wave_codec = prepare_audio(prime_wave, prime_wave_sample_hz, self.neural_codec.sample_rate, normalize=False,
+                                   target_length_seconds=semantic_window_seconds)
+        sem = self.wav2vec(wave_sem, flatten=False)                                                     # :489-495
+        if isinstance(self.neural_codec, nn.Module):
+            self.neural_codec.eval()
+        indices = self.neural_codec(wave_codec, return_encoded=True)[1]                                 # :499-510
+        qc = self.coarse.num_coarse_quantizers
+        return dict(prime_semantic_token_ids=sem.reshape(sem.shape[0], -1, 1), prime_coarse_token_ids=indices[..., :qc],
+                    prime_fine_token_ids=indices[..., qc:])
+
     @torch.no_grad()
-    def forward(self, *, text: Optional[List[str]] = None, prime_wave=None, prime_wave_sample_hz=None, clap_token_ids=None, **kwargs):
-        """open_musiclm.py:860-1035 without the audio-prompt branch: text -> waveform (needs the CLAP quantizer and the codec)."""
-        if prime_wave is not None:
-            raise NotImplementedError("open_musiclm_b200 MusicLM.forward: audio continuation (prime_wave) needs the wav2vec / codec "
-                                      "tokenizers, which are outside the H100 hot path")
+    def forward(self, *, text: Optional[List[str]] = None, prime_wave=None, prime_wave_sample_hz=None, clap_token_ids=None,
+                semantic_window_seconds=10, return_coarse_generated_wave=False, **kwargs):
+        """open_musiclm.py:860-1035: text (or clap token ids) -> waveform [b, n] through the codec.  prime_wave ([channels, n]
+        at prime_wave_sample_hz): continue that audio (prime_token_ids, then generate_tokens); it needs the wav2vec and
+        the codec.  return_coarse_generated_wave: decode the coarse stream alone, before its crop (generate_tokens'
+        coarse_only).  Every other keyword goes to generate_tokens."""
         clap_token_ids = _clap_ids(clap_token_ids, self.clap, None, text)
-        acoustic = self.generate_tokens(clap_token_ids=clap_token_ids, **kwargs)
+        if prime_wave is not None:
+            kwargs.update(self.prime_token_ids(prime_wave, prime_wave_sample_hz, semantic_window_seconds))
+        tokens = self.generate_tokens(clap_token_ids=clap_token_ids, semantic_window_seconds=semantic_window_seconds,
+                                      coarse_only=return_coarse_generated_wave, **kwargs)
         assert self.neural_codec is not None, "a neural codec is needed to turn acoustic tokens into a waveform"
-        return self.neural_codec.decode_from_codebook_indices(acoustic)[:, 0]
+        return self.neural_codec.decode_from_codebook_indices(tokens)[:, 0]
+
+    @torch.no_grad()
+    def generate_top_match(self, *, text: List[str], num_samples=4, num_top_matches=1, **kwargs):
+        """open_musiclm.py:1039-1071: for every prompt, num_samples songs in one batch (forward(**kwargs)), scored by the
+        cosine similarity of the caller's CLAP embeddings of the prompt and of each song (resampled from
+        neural_codec.sample_rate to clap.sample_rate and rounded through int16).  Returns, per prompt, the
+        num_top_matches best waves [num_top_matches, n] and their similarities (on the CPU), best first.  seeds, if
+        given, holds one seed per sample and is used for every prompt."""
+        if self.clap is None or self.neural_codec is None:
+            raise ValueError("open_musiclm_b200 MusicLM.generate_top_match needs the clap and neural_codec models")
+        all_samples, all_similarities = [], []
+        for prompt in text:
+            samples = self.forward(text=[prompt] * num_samples, **kwargs)
+            text_latents = self.clap(text_input=[prompt], return_embedding=True).repeat(num_samples, 1)
+            clap_input = int16_to_float32(float32_to_int16(_resample(samples, self.neural_codec.sample_rate, self.clap.sample_rate)))
+            audio_latents = self.clap(audio_input=clap_input, return_embedding=True)
+            sim = F.cosine_similarity(text_latents.to(audio_latents.device), audio_latents, dim=-1)
+            top = sim.topk(num_top_matches, dim=0, sorted=True).indices
+            all_similarities.append(sim[top].detach().cpu())
+            all_samples.append(samples[top])
+        return all_samples, all_similarities
