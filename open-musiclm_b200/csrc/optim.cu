@@ -72,6 +72,9 @@ adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restri
   }
 }
 
+// one fp16 with the vector path's conversion (cvt.rn.satfinite): finite overflow saturates to +-65504, NaN stays NaN
+__device__ __forceinline__ __half f16_satfinite(float x) { return __ushort_as_half(static_cast<unsigned short>(pack_f16x2(x, 0.f) & 0xffffu)); }
+
 // dst[r, c] = src[map(r), c] for c < cols_valid and live r, else 0.
 // map: split_dst > 0: half = r / split_dst, rr = r % split_dst, live iff rr < split_src, src row = half*split_src + rr
 //      split_dst < 0: interleaved GEGLU order, groups of 128 channels stored as [128 value rows | 128 gate rows]:
@@ -93,7 +96,7 @@ __device__ __forceinline__ void store_quad(OutT* __restrict__ dst, long dst_ld, 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (c + j < cols_p) {
-        if constexpr (std::is_same<OutT, __half>::value) d[j] = __float2half_rn(fminf(fmaxf(v[j], -65504.f), 65504.f));
+        if constexpr (std::is_same<OutT, __half>::value) d[j] = f16_satfinite(v[j]);
         else if constexpr (sizeof(OutT) == 2) d[j] = __float2bfloat16_rn(v[j]);
         else d[j] = v[j];
       }
@@ -161,7 +164,7 @@ __device__ __forceinline__ void pack_quad(long i, const float* __restrict__ src,
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       if (c + j < cols_p) {
-        if constexpr (std::is_same<OutT, __half>::value) d[j] = __float2half_rn(fminf(fmaxf(v[j], -65504.f), 65504.f));
+        if constexpr (std::is_same<OutT, __half>::value) d[j] = f16_satfinite(v[j]);
         else if constexpr (sizeof(OutT) == 2) d[j] = __float2bfloat16_rn(v[j]);
         else d[j] = v[j];
       }

@@ -8,7 +8,8 @@ Semantics kept from the reference:
     key mask with zeroed conditioning ids, 15 % forgetful mask, FFN dropout (open_musiclm.py:328-410);
     loss = sum_{w_s>0} CE_s * n_s * w_s / sum_{w_s>0} n_s (open_musiclm.py:391-410).
   * loss / grad_accum_every per micro-batch (trainer.py:437-439); clip_grad_norm_(max_grad_norm);
-    AdamW(lr, betas (0.9, 0.99), eps 1e-8, wd on ndim>=2 params only) (optimizer.py:3-34);
+    AdamW(lr, betas (0.9, 0.99), eps 1e-8, wd on ndim>=2 params only; Adam when wd == 0) (optimizer.py:3-34), which
+    leaves the logit heads of sequences weighted 0 untouched (they have no gradient, open_musiclm.py:398);
     LinearLR(start_factor 1e-7, total_iters lr_warmup) when lr_warmup > 0 (optimizer.py:36-40).
   * DDP mean of gradients over ranks (trainer.py:154-155, 439) — here a single all-reduce(sum) of the
     arena after the last micro-batch, the 1/world factor folded into the clip/AdamW kernel
@@ -23,6 +24,25 @@ import torch.distributed as dist
 from . import lib
 from .dist_utils import BucketReducer, all_gather_, allreduce_sum_, grad_prescale, rank_seed, shard_of, world_info
 from .model import TokenConditionedTransformer
+
+
+def frozen_parameter_names(names, ce_weights):
+    """Parameters the reference never updates.  It adds a sequence's cross entropy only when its weight is > 0
+    (open_musiclm.py:398), so the logit head of a sequence weighted 0 keeps `grad is None`, and torch's optimizers skip
+    such a parameter: no weight decay, no moment update."""
+    return {n for n in names if n.startswith("logit_weights.") and not ce_weights[int(n.split(".")[1])] > 0}
+
+
+def live_ranges(n, frozen_spans):
+    """[0, n) without the arena spans [a, b) of the frozen parameters, as sorted disjoint (a, b) ranges."""
+    out, lo = [], 0
+    for a, b in sorted(frozen_spans):
+        if a > lo:
+            out.append((lo, a))
+        lo = max(lo, b)
+    if lo < n:
+        out.append((lo, n))
+    return out
 
 
 class LossHandle:
@@ -50,6 +70,10 @@ class HotPathTrainer:
         self.grad_accum_every = grad_accum_every
         self.mask_prob = mask_prob
         self.betas, self.eps, self.pad_id = betas, eps, pad_id
+        sizes = {n: p.numel() for n, p in transformer.named_parameters()}
+        self.frozen = frozen_parameter_names(sizes, self.ce_weights)
+        # the AdamW launches cover these arena ranges only: frozen parameters keep p, m and v bit for bit
+        self.live = live_ranges(eng.n_params_arena, [(eng.layout[n], eng.layout[n] + sizes[n]) for n in self.frozen])
         self.steps = 0
         self.pg = process_group
         self.world, self.rank = world_info(process_group)
@@ -184,7 +208,7 @@ class HotPathTrainer:
         else:
             if self.max_grad_norm is not None:
                 lib.grad_sumsq(eng.arena_g, eng.sumsq, prescale=grad_prescale(self.pg), part=eng.det_sumsq_part if det else None)
-            lib.adamw_step(eng.arena_p, eng.arena_g, eng.adam_m, eng.adam_v, eng.n_decay, self.hyper, eng.sumsq)
+            self._adamw(0, eng.n_params_arena)
         eng.arena_g.zero_()
         eng.refresh_packed(force=True)
         self.loss_out.copy_(self.loss_buf.sum() / self.grad_accum_every)
@@ -199,10 +223,18 @@ class HotPathTrainer:
                 lib.grad_sumsq(eng.arena_g[a:b], eng.sumsq, prescale=grad_prescale(self.pg), part=eng.det_sumsq_part if det else None)
             dist.all_reduce(eng.sumsq, op=dist.ReduceOp.SUM, group=self.pg)
         for a, b in parts:
-            lib.adamw_step(eng.arena_p[a:b], eng.arena_g[a:b], eng.adam_m[a:b], eng.adam_v[a:b], max(0, min(b - a, eng.n_decay - a)),
-                           self.hyper, eng.sumsq)
+            self._adamw(a, b)
         for lo, hi in self.reducer.slices():
             all_gather_(eng.arena_p[lo:hi], W, r, self.pg)
+
+    def _adamw(self, lo, hi):
+        """AdamW on the live parts of the arena range [lo, hi): one launch per part, decay below n_decay."""
+        eng = self.eng
+        for a, b in self.live:
+            a, b = max(a, lo), min(b, hi)
+            if a < b:
+                lib.adamw_step(eng.arena_p[a:b], eng.arena_g[a:b], eng.adam_m[a:b], eng.adam_v[a:b], max(0, min(b - a, eng.n_decay - a)),
+                               self.hyper, eng.sumsq)
 
     def _gather_optimizer_state(self):
         """Sharded update: every rank holds the Adam moments of its parts only -- make them complete everywhere (checkpoints)."""
@@ -333,10 +365,12 @@ class HotPathTrainer:
 
     # ------------------------------------------------------------------------------------------- checkpoint FILES
     def _torch_optimizer(self):
-        """A torch.optim.AdamW over the module's parameters, grouped like the reference's get_optimizer
-        (optimizer.py:3-34: ndim >= 2 with weight decay, the rest without) and carrying THIS trainer's moments, step
-        count and current learning rate — used only to read / write the reference's optimizer checkpoint format."""
+        """The torch optimizer the reference's get_optimizer builds over the module's parameters (optimizer.py:10-34):
+        with wd == 0 one Adam group in module order, else AdamW with ndim >= 2 decayed and the rest not — used only to
+        read / write the reference's optimizer checkpoint format."""
         params = list(self.transformer.parameters())
+        if self.wd == 0:
+            return torch.optim.Adam(params, lr=self.lr, betas=tuple(self.betas), eps=self.eps), params
         wd_params = [p for p in params if p.ndim >= 2]
         no_wd = [p for p in params if p.ndim < 2]
         opt = torch.optim.AdamW([{"params": wd_params}, {"params": no_wd, "weight_decay": 0}], lr=self.lr, weight_decay=self.wd,
@@ -356,6 +390,8 @@ class HotPathTrainer:
         name_of = {id(p): n for n, p in self.transformer.named_parameters()}
         if self.steps > 0:
             for p in ordered:
+                if name_of[id(p)] in self.frozen:
+                    continue                # no gradient, so torch keeps no state for it either
                 o = eng.layout[name_of[id(p)]]
                 opt.state[p] = {"step": torch.tensor(float(self.steps)), "exp_avg": eng.adam_m[o:o + p.numel()].view(p.shape).clone(),
                                 "exp_avg_sq": eng.adam_v[o:o + p.numel()].view(p.shape).clone()}
