@@ -603,6 +603,9 @@ int omlm_skinny_gemm(const void* A, long lda, int prologue, const void* W, long 
   OMLM_CHECK_ARG(prologue != 3 || (rowsum != nullptr && K % 128 == 0 && n_real > 0), "skinny_gemm: inner-norm prologue needs rowsum and K % 128 == 0");
   OMLM_CHECK_ARG(out_fmt == kFmtBF16 || out_fmt == kFmtF32 || out_fmt == kFmtF16, "skinny_gemm: out_fmt");
   OMLM_CHECK_ARG((reinterpret_cast<uintptr_t>(W) & 15) == 0, "skinny_gemm: W must be 16-byte aligned");
+  // prologues 0 and 3 read the 16-bit A two elements at a time (one 32-bit load)
+  OMLM_CHECK_ARG((prologue != 0 && prologue != 3) || ((reinterpret_cast<uintptr_t>(A) & 3) == 0 && lda % 2 == 0),
+                 "skinny_gemm: a 16-bit A needs a 4-byte aligned start and an even pitch (lda=%ld)", lda);
   SkinnyArgs a;
   a.A = A; a.W = reinterpret_cast<const uint16_t*>(W); a.gamma = gamma; a.rowsum = rowsum; a.addend = addend; a.out = out;
   a.lda = lda; a.ldw = ldw; a.ldadd = ldadd; a.ldo = ldo; a.B = B; a.N = N; a.K = K; a.prologue = prologue; a.f16 = w_f16;

@@ -276,6 +276,9 @@ static int dg_run(const void* A, long lda, int prologue, const void* W, long ldw
   OMLM_CHECK_ARG(prologue != 3 || (rowsum != nullptr && K % 128 == 0 && n_real > 0), "decode_gemm: inner-norm prologue needs rowsum and K % 128 == 0");
   OMLM_CHECK_ARG(out_fmt == kFmtBF16 || out_fmt == kFmtF32 || out_fmt == kFmtF16, "decode_gemm: out_fmt");
   OMLM_CHECK_ARG((reinterpret_cast<uintptr_t>(W) & 15) == 0, "decode_gemm: W must be 16-byte aligned");
+  // the prologue kernel reads a 16-bit A (prologues 0 and 3) two elements at a time (one 32-bit load)
+  OMLM_CHECK_ARG((prologue != 0 && prologue != 3) || ((reinterpret_cast<uintptr_t>(A) & 3) == 0 && lda % 2 == 0),
+                 "decode_gemm: a 16-bit A needs a 4-byte aligned start and an even pitch (lda=%ld)", lda);
   const DgPlan p = dg_plan(B, N, K, invariant);
   OMLM_CHECK_ARG(part_ws_bytes >= p.part_floats * 4 && (p.part_floats == 0 || part_ws != nullptr),
                  "decode_gemm: split-K workspace of %ld bytes, %ld needed", part_ws_bytes, p.part_floats * 4);

@@ -137,7 +137,7 @@ __device__ __forceinline__ void epilogue_staged(float (&acc)[BN / 2], const EpiP
         for (int hr = 0; hr < 2; ++hr) {
           const int r = wq * 16 + qr + hr * 8;
           uint8_t* p = box + box_offset<F32>(r, g0 + j, qc);
-          // rounded product, then the addend: the direct epilogue's order (a contracted fma would round once)
+          // rounded product, then the addend, as in the direct epilogue (a contracted fma would round once)
           float v0 = __fmul_rn(acc[4 * i + 2 * hr], ep.alpha), v1 = __fmul_rn(acc[4 * i + 2 * hr + 1], ep.alpha);
           if constexpr (RS) {
             const uint32_t kb = keep[hr][j], hv = *reinterpret_cast<const uint32_t*>(p);
@@ -376,7 +376,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   #pragma unroll
           for (int hr = 0; hr < 2; ++hr) {
             if (!row_ok[hr]) continue;
-            float v0 = acc[4 * i + 2 * hr] * ep.alpha, v1 = acc[4 * i + 2 * hr + 1] * ep.alpha;
+            // rounded product, then the addend (a contracted fma would round once and differ from the staged epilogue)
+            float v0 = __fmul_rn(acc[4 * i + 2 * hr], ep.alpha), v1 = __fmul_rn(acc[4 * i + 2 * hr + 1], ep.alpha);
             if (ep.addend != nullptr) { v0 += add[hr][j].x; v1 += add[hr][j].y; }
             if (ep.atomic) {
               float* op = reinterpret_cast<float*>(ep.out) + orow[hr] + col;
@@ -446,6 +447,8 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   OMLM_CHECK_ARG(splits == 1 || (out_f32 && addend == nullptr), "gemm: split-K needs fp32 atomic output and no addend");
   OMLM_CHECK_ARG(split_stride == 0 || (out_f32 && addend == nullptr && rs == nullptr), "gemm: partial slices need fp32 output");
   if (n_valid <= 0 || n_valid > N) n_valid = N;
+  // split-K adds onto the output's contents; that stays so when the clamp below leaves a single split
+  const bool accumulate = splits > 1 && split_stride == 0;
   {  // every split must own at least one k-block (an empty split would publish an unwritten accumulator)
     const int kb_total = (K + BK - 1) / BK;
     if (splits > kb_total) splits = kb_total;
@@ -462,7 +465,7 @@ static int gemm16_impl(const void* A, int a_f16, int a_mn_major, long lda, const
   if (rc) return rc;
   EpiParams ep;
   ep.out = out; ep.addend = addend; ep.ldo = ldo; ep.ldadd = ldadd; ep.alpha = alpha;
-  ep.out_f32 = out_f32; ep.atomic = (splits > 1 && split_stride == 0) ? 1 : 0; ep.split_stride = split_stride;
+  ep.out_f32 = out_f32; ep.atomic = accumulate ? 1 : 0; ep.split_stride = split_stride;
   const long esz = out_f32 ? 4 : 2;
   ep.vec_ok = ((ldo * esz) % 16 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0) &&
               (addend == nullptr || ((ldadd * 4) % 16 == 0 && (reinterpret_cast<uintptr_t>(addend) & 15) == 0));
