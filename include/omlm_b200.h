@@ -78,16 +78,17 @@ int omlm_gemm16_splitk_det(const void* A, int a_f16, int a_mn_major, long lda, c
                            int block_n, int max_ctas, float* part_ws, long part_ws_bytes, void* stream);
 int omlm_gemm16_splitk_det_workspace(int M, int N, int K, int splits, int row_split, int row_valid, int n_valid, long* part_bytes);
 /* omlm_layernorm_bwd: each CTA writes its dgamma sum as one row of part_ws (>= 4 * SMs * D floats), omlm_colsum adds
- * the rows to dgamma in CTA order. */
+ * the rows to dgamma in CTA order.  dgamma == NULL: no partial rows, no omlm_colsum. */
 int omlm_layernorm_bwd_det(const void* dy_bf16, const float* x, const float* stats, const float* gamma,
                            const float* dres, const void* draw_bf16, const int* src_row, float* dx,
                            void* dx_bf16, float* dgamma, int M, int D, float* part_ws, long part_ws_bytes, void* stream);
-/* omlm_qk_l2norm_bwd: per-CTA rows of (q scale | k scale) sums in part_ws (>= 8 * SMs * 128 floats), then omlm_colsum. */
+/* omlm_qk_l2norm_bwd: per-CTA rows of (q scale | k scale) sums in part_ws (>= 8 * SMs * 128 floats), then omlm_colsum
+ * for each scale gradient that is not NULL (both NULL: no partial rows). */
 int omlm_qk_l2norm_bwd_det(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
                            const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
                            float* dq_scale, float* dk_scale, int M, int heads, float* part_ws, long part_ws_bytes, void* stream);
 /* omlm_ffn_mid_bwd: per-CTA rows [B * ceil(N / 128), 7F] of (dgamma [F] | dconv_w [2F, 3]) sums in part_ws, then
- * omlm_colsum. */
+ * omlm_colsum; the part of a NULL output is neither written to part_ws nor summed. */
 int omlm_ffn_mid_bwd_det(const void* dhn, const void* hn, const void* u, const float* stats, const float* conv_w,
                          const float* gamma, const void* keep_bits, float* rowstat, int rowstat_parts, void* du, float* dgamma,
                          float* dconv_w, int B, int N, int F, int Fp, float drop_p, int act_f16, float* part_ws, long part_ws_bytes,
@@ -114,7 +115,8 @@ int omlm_grad_sumsq_det(const float* g, long n, float prescale, double* acc, dou
  * ints) are sized by omlm_attn_bwd_tc_det_workspace (iws_count may be larger).  iws[iws_count - 1] is an error word that
  * must be zero before the first call.  It is set to 1 if a turn was not granted within seconds: the kernel never hangs,
  * and that call's sums -- and those of every later call until the caller clears the word -- are added in arrival order,
- * correct up to rounding like omlm_attn_bwd_tc's but not reproducible. */
+ * correct up to rounding like omlm_attn_bwd_tc's but not reproducible.  dtable == NULL: as omlm_attn_bwd_tc; ws is not
+ * read (it may be NULL, ws_bytes 0), iws is still needed, and dqn / dkvn are bit-identical to the call with a table. */
 int omlm_attn_bwd_tc_det(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                          const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
                          float* dqn, float* dkvn, float* dtable, int B, int N, int heads, float scale,
@@ -163,8 +165,9 @@ int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, i
  * a bf16 copy of y for the weight-gradient GEMMs (one wgmma takes one operand format; gradients are bf16). */
 int omlm_layernorm_fwd(const float* x, const float* gamma, void* y16, int y_f16, void* ycopy_bf16, void* xraw_bf16,
                        float* stats, const int* dest_row, int M, int D, void* stream);
-/* dx = [dres] + [draw] + LN-backward(dy);  dgamma += sum_rows dy * xhat.  dy row for x row m is
- * src_row[m] when given (-1: no gradient).  dx_bf16 (optional): bf16 copy of dx for the next GEMMs. */
+/* dx = [dres] + [draw] + LN-backward(dy);  dgamma += sum_rows dy * xhat (dgamma may be NULL: gamma frozen, not
+ * summed).  dy row for x row m is src_row[m] when given (-1: no gradient).  dx_bf16 (optional): bf16 copy of dx for the
+ * next GEMMs. */
 int omlm_layernorm_bwd(const void* dy_bf16, const float* x, const float* stats, const float* gamma,
                        const float* dres, const void* draw_bf16, const int* src_row, float* dx,
                        void* dx_bf16, float* dgamma, int M, int D, void* stream);
@@ -172,6 +175,7 @@ int omlm_layernorm_bwd(const void* dy_bf16, const float* x, const float* stats, 
  * q_raw [M, heads*64], kv_raw [M,128] (k | v) -> qn, kvn (k normalised, v copied). */
 int omlm_qk_l2norm_fwd(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale,
                        void* qn, void* kvn, int M, int heads, void* stream);
+/* dq_scale / dk_scale (+= sum dy * xhat over rows) may each be NULL: that scale is frozen and its sum is skipped. */
 int omlm_qk_l2norm_bwd(const float* dqn, const float* dkvn, const void* q_raw, const void* kv_raw,
                        const float* q_scale, const float* k_scale, void* dq_raw, void* dkv_raw,
                        float* dq_scale, float* dk_scale, int M, int heads, void* stream);
@@ -213,7 +217,8 @@ int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* 
  * order, no shared-memory atomics), summed per CTA and added to dtable once; no scratch tensor.  The bias is read from a
  * per-tile window of the table in shared memory; the windows and diagonal tables limit heads to 58.
  * dqn, dkvn and dtable are reduced with floating-point atomics: reproducible up to accumulation order
- * (omlm_attn_bwd_tc_det fixes the order). */
+ * (omlm_attn_bwd_tc_det fixes the order).  dtable == NULL (nothing trains the bias table): a kernel variant without the
+ * fp32 dS staging and the diagonal sums runs; dqn and dkvn are computed in the same order as with a table. */
 int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                      const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
                      float* dqn, float* dkvn, float* dtable, int B, int N, int heads,
@@ -238,7 +243,8 @@ int omlm_ffn_norm_fwd(const void* h, const float* rowsum, const float* gamma, vo
                       int act_f16, void* stream);
 /* dhn, hn (saved forward output), keep_bits (from omlm_ffn_norm_fwd; may be NULL when drop_p == 0) -> du bf16 [B*N, 2Fp].
  * Parameter gradients are ACCUMULATED (+=) in the parameters' own layouts: dgamma [F] (inner LayerNorm gamma) and
- * dconv_w [2F, 3] (ds_conv.weight: value rows [0,F), gate rows [F,2F); may be NULL for the plain FeedForward).
+ * dconv_w [2F, 3] (ds_conv.weight: value rows [0,F), gate rows [F,2F)).  Either may be NULL (frozen; dconv_w also for the
+ * plain FeedForward): that sum is skipped.
  * rowstat: the LayerNorm-backward row sums (sum gamma*drop(dhn), sum dhn*hn) as fp32 [B*N, parts, 2]:
  *   rowstat_parts > 0: partial sums written by omlm_gemm16_rowstat (the d_hn GEMM's epilogue), parts = Fp / 128;
  *   rowstat_parts = 0: rowstat is a [B*N, 2] scratch and the sums are computed here by one extra pass over (dhn, hn). */

@@ -25,6 +25,11 @@
 // kernel adds the partial tables to dtable in unit order.  After a time-out the error word stays set and later calls
 // skip their waits, until the caller clears it: their sums are then added in arrival order (correct up to rounding, not
 // reproducible).
+//
+// Without the bias gradient (DTAB = false, dtable == NULL: nothing trains the bias table) the kernel skips the fp32 dS
+// staging, the diagonal sums, the two per-warpgroup tables and their flush, and in DET mode the partial tables and the
+// reduce kernel.  Everything else, and with it the order of every dQ, dK and dV sum, is unchanged: dQ and dK|dV are
+// bit-identical to the variant with the table.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/omlm_b200.h"
@@ -97,7 +102,7 @@ struct BtDet {
   float* dpart;     // [units, h, Wacc]
 };
 
-template <bool DET>
+template <bool DET, bool DTAB>
 __global__ void __launch_bounds__(kBtThreads, 1)
 attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmDO,
                    const __grid_constant__ CUtensorMap tmKV, const float* __restrict__ lse2, const float* __restrict__ dsum,
@@ -138,7 +143,8 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int i = 0; i < 2; ++i) { mbar_init(&qd_full[i], 1); mbar_init(&qd_empty[i], 2); }
     fence_barrier_init();
   }
-  for (int x = threadIdx.x; x < 2 * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
+  if constexpr (DTAB)
+    for (int x = threadIdx.x; x < 2 * h * Wacc; x += blockDim.x) dacc[x] = 0.f;
   __syncthreads();
 
   if (wg == 0) {
@@ -255,7 +261,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
             pp[e] = live ? bt_ex2(fmaf(x, sc2, wv[2 * c + e] * kBtL2e) - lse) : 0.f;
             dd[e] = pp[e] * (dp[4 * c + 2 * hr + e] - D);
           }
-          *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
+          if constexpr (DTAB) *reinterpret_cast<float2*>(sdsf + lr * kBtSdsLd + 8 * c + 2 * qc) = make_float2(dd[0], dd[1]);
           const uint32_t off = static_cast<uint32_t>(((c ^ (lr & 7)) << 4) + 4 * qc);
           *reinterpret_cast<uint32_t*>(prow + off) = pack_bf16x2(pp[0], pp[1]);
           *reinterpret_cast<uint32_t*>(drow + off) = pack_bf16x2(dd[0], dd[1]);
@@ -275,7 +281,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
         Wgmma<64, false>::ss<0, 1>(dq, make_smem_desc(sds + ks * 32, 16, 1024), make_smem_desc(sk + ks * 2048, 8192, 1024), ks > 0 ? 1u : 0u);
       }
       wgmma_commit();
-      {
+      if constexpr (DTAB) {
         // diagonal sums of the fp32 dS tile while the tensor cores run: thread-owned (head, diagonal) pairs, rows in order
         const int dlo = max(0, it_lo - kbase - 63), dhi = it_hi - kbase;
         const int W = dhi - dlo + 1;
@@ -353,6 +359,7 @@ attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       if (leader) bt_pass_turn(kv_turn);
     }
     // ---- flush the diagonal sums of this unit
+    if constexpr (!DTAB) return;
     asm volatile("bar.sync 3, 256;" ::: "memory");
     if constexpr (DET) {       // (warpgroup 1 + warpgroup 2) -> this unit's partial table; summed in unit order later
       float* up = det.dpart + static_cast<long>(blockIdx.x) * h * Wacc;
@@ -516,8 +523,10 @@ static int attn_bwd_tc_impl(const void* qn, const void* kvn, const void* d_o, co
   if (rc) return rc;
   const int units = B * cfg.units_per_batch;
   BtDet dp{nullptr, nullptr, nullptr, nullptr, nullptr};
+  const bool dtab = dtable != nullptr;
   if (det) {
-    OMLM_CHECK_ARG(ws != nullptr && iws != nullptr && ws_bytes >= static_cast<long>(units) * heads * cfg.wacc * 4 &&
+    // without the bias gradient the partial tables (ws) are not used
+    OMLM_CHECK_ARG((!dtab || (ws != nullptr && ws_bytes >= static_cast<long>(units) * heads * cfg.wacc * 4)) && iws != nullptr &&
                    iws_count >= bt_ints(B, cfg), "attn_bwd_tc_det: workspace too small (see omlm_attn_bwd_tc_det_workspace)");
     dp.turn_dq = iws;
     dp.turn_kv = iws + static_cast<long>(B) * cfg.n_row_tiles;
@@ -537,17 +546,21 @@ static int attn_bwd_tc_impl(const void* qn, const void* kvn, const void* d_o, co
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(B) * N, 256, 64, kBtBK);
   if (rc) return rc;
-  auto kern = det ? attn_bwd_tc_kernel<true> : attn_bwd_tc_kernel<false>;
-  static int configured[2] = {0, 0};
-  if (configured[det] < cfg.smem_bytes) {
+  // the variant without the table keeps the same chunk length and shared-memory layout (the chunk length decides the
+  // order of the dK|dV sums, so dQ, dK and dV stay bit-identical to the variant with the table)
+  auto kern = det ? (dtab ? attn_bwd_tc_kernel<true, true> : attn_bwd_tc_kernel<true, false>)
+                  : (dtab ? attn_bwd_tc_kernel<false, true> : attn_bwd_tc_kernel<false, false>);
+  const int variant = 2 * det + dtab;
+  static int configured[4] = {0, 0, 0, 0};
+  if (configured[variant] < cfg.smem_bytes) {
     OMLM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, cfg.smem_bytes));
-    configured[det] = cfg.smem_bytes;
+    configured[variant] = cfg.smem_bytes;
   }
   OMLM_KLAUNCH((kern), units, kBtThreads, cfg.smem_bytes, st,
       tmQ, tmDO, tmKV, lse2, dsum_scratch, table, table_ld, key_mask, dqn, dkvn, dtable, N, heads, scale,
       cfg.wacc, cfg.win_ld, cfg.tiles_per_chunk, B, dp);
   OMLM_LAUNCH_CHECK();
-  if (det) {
+  if (det && dtab) {
     OMLM_KLAUNCH((attn_bwd_dtable_reduce_kernel), (heads * N + 255) / 256, 256, 0, st,
         static_cast<const float*>(dp.dpart), static_cast<const int*>(dp.meta), units, heads, cfg.wacc, dtable, table_ld, N);
     OMLM_LAUNCH_CHECK();

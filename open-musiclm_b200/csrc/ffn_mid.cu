@@ -179,6 +179,7 @@ __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc, bool
 
 // DET: no atomics -- the warps' sums are combined in warp order and written to this CTA's row blockIdx.x of part
 // [gridDim.x, 7F] in the parameters' layouts (dgamma [F] | dconv_w [2F, 3]); omlm_colsum adds the rows in order.
+// dgamma / dconv_w may each be NULL (frozen, or no conv): that part is neither reduced nor written to part.
 template <bool F16, bool DET>
 __global__ void __launch_bounds__(kTileThreads, 2)
 ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, const float2* __restrict__ stats,
@@ -341,6 +342,7 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
       da2[q] = da1[q]; da1[q] = da0[q]; dg2[q] = dg1[q]; dg1[q] = dg0[q];
     }
   }
+  if (dgamma == nullptr && dconv_w == nullptr) return;
   if constexpr (DET) {
     __syncthreads();                                      // every warp is done with the u tile: reuse it
     float* wsum = reinterpret_cast<float*>(su);           // [warps][7][128]
@@ -361,7 +363,7 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
     float* prow = part + static_cast<long>(blockIdx.x) * 7 * a.F;
     for (int i = tid; i < 7 * 128; i += kTileThreads) {
       const int q = i >> 7, ch = g * 128 + (i & 127);
-      if (ch >= a.F) continue;
+      if (ch >= a.F || (q == 0 ? dgamma : dconv_w) == nullptr) continue;
       float v = 0.f;
 #pragma unroll
       for (int w = 0; w < kTileWarps; ++w) v += wsum[w * 7 * 128 + i];
@@ -390,7 +392,7 @@ ffn_mid_bwd_walk_kernel(const MidArgs a, const __nv_bfloat16* __restrict__ dhn, 
       const int q = i >> 7, ch = g * 128 + (i & 127);
       if (ch >= a.F) continue;
       const float v = sacc[i];
-      if (q == 0) atomicAdd(&dgamma[ch], v);
+      if (q == 0) { if (dgamma != nullptr) atomicAdd(&dgamma[ch], v); }
       else if (dconv_w != nullptr) {
         if (q < 4) atomicAdd(&dconv_w[static_cast<long>(ch) * 3 + (q - 1)], v);
         else atomicAdd(&dconv_w[(static_cast<long>(a.F) + ch) * 3 + (q - 4)], v);
@@ -460,9 +462,11 @@ static int ffn_mid_bwd_impl(const void* dhn, const void* hn, const void* u, cons
                                                                 reinterpret_cast<__nv_bfloat16*>(du), dgamma, dconv_w, part);
   OMLM_LAUNCH_CHECK();
   if (det) {
-    const int rc = omlm_colsum(part, 7L * F, 1, dgamma, row_blocks, F, 1, stream);
-    if (rc || dconv_w == nullptr) return rc;
-    return omlm_colsum(part + F, 7L * F, 1, dconv_w, row_blocks, 6 * F, 1, stream);
+    if (dgamma != nullptr) {
+      const int rc = omlm_colsum(part, 7L * F, 1, dgamma, row_blocks, F, 1, stream);
+      if (rc) return rc;
+    }
+    if (dconv_w != nullptr) return omlm_colsum(part + F, 7L * F, 1, dconv_w, row_blocks, 6 * F, 1, stream);
   }
   return 0;
 }

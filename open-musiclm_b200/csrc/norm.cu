@@ -76,6 +76,7 @@ layernorm_fwd_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 // ------------------------------------------------------------------------------------------------
 // LayerNorm backward.  dx = [dres] + [draw] + rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat))
 // dgamma[col] += sum_rows dy * xhat  (fp32; per-block partials in smem, one global atomic per column per block).
+// dgamma == NULL (gamma frozen): no dgamma reduction, no partial rows.
 // dy rows may be permuted (src_row: row of dy for this x row, -1 = no gradient).
 // One warp per row.  The row's operands (x, dy, dres, draw: up to 12 bytes per element) are brought to a per-warp,
 // double-buffered shared-memory stage with cp.async, so a warp always has the whole NEXT row in flight while it
@@ -200,6 +201,7 @@ layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const float* __restri
     }
     d_cur = d_nxt; d_nxt = d_nn;
   }
+  if (dgamma == nullptr) return;
   if constexpr (DET) {
     __syncthreads();                                  // every warp is done with its stage buffers: reuse them
     float* wdg = reinterpret_cast<float*>(lsm);       // [WARPS][kRow]
@@ -282,6 +284,7 @@ qk_l2norm_fwd_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat1
 // Outputs bf16 dq_raw [M, h*64], dkv_raw [M, 128] (value gradient passes through).
 // DET: the 32 vector slots of a block are combined in slot order and written as this block's row of part [gridDim.x,
 // 128] (q scale | k scale); omlm_colsum adds the rows in block order.
+// dq_scale / dk_scale may each be NULL (that scale frozen): its sum is not reduced; both NULL: no partial rows.
 template <bool DET>
 __global__ void __launch_bounds__(256)
 qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dkvn,
@@ -370,6 +373,7 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
       *reinterpret_cast<uint4*>(dst + sub * 8) = ov;
     }
   }
+  if (dq_scale == nullptr && dk_scale == nullptr) return;
   if constexpr (DET) {
     const int slot = threadIdx.x >> 3;
 #pragma unroll
@@ -388,8 +392,8 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
       atomicAdd(&sds[1][sub * 8 + i], dsk[i]);
     }
     __syncthreads();
-    if (threadIdx.x < 64) atomicAdd(&dq_scale[threadIdx.x], sds[0][threadIdx.x]);
-    else if (threadIdx.x < 128) atomicAdd(&dk_scale[threadIdx.x - 64], sds[1][threadIdx.x - 64]);
+    if (threadIdx.x < 64) { if (dq_scale != nullptr) atomicAdd(&dq_scale[threadIdx.x], sds[0][threadIdx.x]); }
+    else if (threadIdx.x < 128) { if (dk_scale != nullptr) atomicAdd(&dk_scale[threadIdx.x - 64], sds[1][threadIdx.x - 64]); }
   }
 }
 
@@ -426,7 +430,7 @@ static int launch_ln_bwd(const __nv_bfloat16* dy, const float* x, const float2* 
   OMLM_KLAUNCH((layernorm_bwd_kernel<NCHUNK, WARPS, DET>), blocks, WARPS * 32, smem, st, dy, x, stats, gamma, dres, draw, src_row, dx,
                                                                        dx_bf16, dgamma, M, D, rows_per_block, part);
   OMLM_LAUNCH_CHECK();
-  if (DET) return omlm_colsum(part, D, 1, dgamma, blocks, D, 1, st);
+  if (DET && dgamma != nullptr) return omlm_colsum(part, D, 1, dgamma, blocks, D, 1, st);
   return 0;
 }
 
@@ -518,9 +522,11 @@ static int qk_l2norm_bwd_impl(const float* dqn, const float* dkvn, const void* q
       dq_scale, dk_scale, M, heads, part);
   OMLM_LAUNCH_CHECK();
   if (det) {
-    const int rc = omlm_colsum(part, 128, 1, dq_scale, static_cast<int>(blocks), 64, 1, stream);
-    if (rc) return rc;
-    return omlm_colsum(part + 64, 128, 1, dk_scale, static_cast<int>(blocks), 64, 1, stream);
+    if (dq_scale != nullptr) {
+      const int rc = omlm_colsum(part, 128, 1, dq_scale, static_cast<int>(blocks), 64, 1, stream);
+      if (rc) return rc;
+    }
+    if (dk_scale != nullptr) return omlm_colsum(part + 64, 128, 1, dk_scale, static_cast<int>(blocks), 64, 1, stream);
   }
   return 0;
 }

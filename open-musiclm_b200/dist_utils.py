@@ -96,6 +96,13 @@ def plan_buckets(layout: Dict[str, int], sizes: Dict[str, int], total: int, dept
     return out
 
 
+def drop_frozen_buckets(plan: List[Tuple[str, List[Slice]]], trainable: Sequence[Slice]) -> List[Tuple[str, List[Slice]]]:
+    """The buckets of `plan` that overlap at least one arena span [a, b) of a trainable parameter.  The others hold only
+    frozen parameters and padding, whose gradient is zero on every rank: they are not communicated."""
+    live = lambda sl: any(lo < b and a < hi for lo, hi in sl for a, b in trainable)
+    return [(t, sl) for t, sl in plan if live(sl)]
+
+
 def shard_of(lo: int, hi: int, world: int, rank: int) -> Slice:
     """The part of the arena slice [lo, hi) that `rank` owns after a reduce-scatter (equal parts, rank order)."""
     n = hi - lo
@@ -170,6 +177,7 @@ class BucketReducer:
                 self._reduce(v)
 
     def join(self):
+        # (triggers of buckets left out of the plan, see drop_frozen_buckets, are ignored by fire)
         if self.world > 1:
             assert self.fired == self.order, f"buckets fired {self.fired}, expected {self.order}"
             if self.side is not None:

@@ -81,6 +81,46 @@ class _Plan:
             self.src_row2 = r2.reshape(-1).to(device)
 
 
+class _BackwardPlan:
+    """The backward work a set of frozen parameters (requires_grad=False, or logit heads without gradient) leaves.
+    A layer runs its backward pass when it holds a trainable parameter, when a gradient has to reach a layer or a row
+    table below it, or when the bias table is trained (its gradient sums every layer's dS).  Inside a layer each step
+    runs only when a trainable parameter or the gradient flowing further down consumes what it produces."""
+
+    def __init__(self, eng: "Engine", frozen):
+        self.frozen = frozenset(frozen)
+        tr = self.trains
+        names = list(eng.layout)
+        row_tables = [n for n in names if n.startswith(("embeddings.", "absolute_position_embeddings.", "start_tokens."))]
+        # 'none' has no bias parameters: its table gradient is never needed
+        self.dtable = any(tr(n) for n in names if n.startswith("transformer.rel_pos_bias."))
+        self.rows = any(tr(n) for n in row_tables)
+        self.rows_partial = self.rows and not all(tr(n) for n in row_tables)
+        layer_tr = [self.dtable or any(tr(n) for n in names if n.startswith(f"transformer.layers.{l}.")) for l in range(eng.L)]
+        below, acc = [], self.rows           # below[l]: a gradient must reach the input of layer l (l = L: the final norm)
+        for l in range(eng.L + 1):
+            below.append(acc)
+            acc = acc or (l < eng.L and layer_tr[l])
+        self.below = below
+        self.run = [layer_tr[l] or below[l] for l in range(eng.L)]
+        self.final_norm = below[eng.L] or tr("transformer.norm.gamma")
+        fk = eng.ffk
+        self.steps = []
+        for l in range(eng.L):
+            t = lambda k, l=l: k is not None and tr(f"transformer.layers.{l}.{k}")
+            g_in = below[l]
+            ln_a = g_in or t("0.norm.gamma")                                              # attention pre-norm backward
+            qk = ln_a or any(t(k) for k in ("0.to_q.weight", "0.to_kv.weight", "0.q_scale", "0.k_scale"))
+            attn = qk or self.dtable                                                      # attention backward
+            mid = attn or g_in or t("0.to_out.0.weight")                                  # gradient at the mid residual
+            ln_f = mid or t(fk["g1"])                                                     # feed-forward pre-norm backward
+            ffn = ln_f or t(fk["w1"]) or t(fk["gin"]) or t(fk["conv"])                    # d_hn GEMM + ffn_mid_bwd
+            self.steps.append(dict(g_in=g_in, ln_a=ln_a, qk=qk, attn=attn, mid=mid, ln_f=ln_f, ffn=ffn))
+
+    def trains(self, name):
+        return name not in self.frozen
+
+
 def itertools_accumulate(xs):
     t = 0
     out = []
@@ -139,6 +179,8 @@ class Engine:
         self.det_sumsq_part = None      # deterministic mode (see workspace()): per-CTA partials of grad_sumsq
         self.det_rows = None            #   and the row markers of the embedding scatter-add
         self._det_attn = weakref.WeakSet()   # every live attention-backward workspace (also those kept by captured graphs)
+        self._bwd_plans = {}
+        self._row_live = {}
 
     # ------------------------------------------------------------------------------------------ arena
     def _build_arena(self):
@@ -173,7 +215,8 @@ class Engine:
             v.copy_(p.data)
             p.data = v
             g = arena_g[o:o + p.numel()].view(p.shape)
-            p.grad = g
+            if p.requires_grad:          # a frozen parameter keeps grad None, as autograd leaves it
+                p.grad = g
             self.pview[n], self.gview[n] = v, g
         self.arena_p, self.arena_g = arena_p, arena_g
         # embedding table = [embeddings.0 | embeddings.1 | ... ] rows of d floats; start tokens further down
@@ -247,11 +290,33 @@ class Engine:
                 lib.split3_bf16(pv[f"transformer.rel_pos_bias.net.{j}.0.weight"], self.pk_rp[j - 1], weight_mode=True)
         self._packed_version = ver
 
-    def grad_bucket_plan(self, min_elems=4 << 20):
-        """All-reduce buckets of the gradient arena in backward-completion order (dist_utils.plan_buckets)."""
-        from .dist_utils import plan_buckets
+    def grad_bucket_plan(self, min_elems=4 << 20, frozen=()):
+        """All-reduce buckets of the gradient arena in backward-completion order (dist_utils.plan_buckets).  Buckets
+        that hold no trainable parameter (only names in `frozen`, and padding) are left out: their gradient is zero on
+        every rank and nothing reads it."""
+        from .dist_utils import drop_frozen_buckets, plan_buckets
         sizes = {n: p.numel() for n, p in self.m.named_parameters()}
-        return plan_buckets(self.layout, sizes, self.n_params_arena, self.L, min_elems)
+        plan = plan_buckets(self.layout, sizes, self.n_params_arena, self.L, min_elems)
+        return drop_frozen_buckets(plan, [(self.layout[n], self.layout[n] + sizes[n]) for n in sizes if n not in frozen])
+
+    def backward_plan(self, frozen=()) -> _BackwardPlan:
+        key = frozenset(frozen)
+        if key not in self._bwd_plans:
+            self._bwd_plans[key] = _BackwardPlan(self, key)
+        return self._bwd_plans[key]
+
+    def _trainable_rows(self, bp: _BackwardPlan, src_row):
+        """src_row with the rows of frozen row tables set to -1 (the scatter-add skips them), for a partly frozen set of
+        embedding / absolute-position tables and start tokens."""
+        live = self._row_live.get(bp.frozen)
+        if live is None:
+            live = torch.zeros(self.table.numel() // self.d, dtype=torch.bool)
+            for n, p in self.m.named_parameters():
+                if n.startswith(("embeddings.", "absolute_position_embeddings.", "start_tokens.")) and bp.trains(n):
+                    r0 = (self.layout[n] - self.emb_off) // self.d
+                    live[r0:r0 + p.numel() // self.d] = True
+            live = self._row_live[bp.frozen] = live.to(self.dev)
+        return torch.where(live[src_row.clamp(min=0).long()], src_row, torch.full_like(src_row, -1))
 
     def check_errors(self):
         """Raises if a token id outside an embedding table was seen since the last check (nn.Embedding's IndexError;
@@ -409,11 +474,13 @@ class Engine:
             lib.sgemm_small(w, (1, 1), ws["ones"], (1, 1), ws["table"], (ws["table"].stride(0), 1), self.h, N, 1)
         # 'none': the table stays zero
 
-    def bias_table_backward(self, ws, N, det=False):
+    def bias_table_backward(self, ws, N, det=False, bp: Optional[_BackwardPlan] = None):
+        """Gradients of the bias parameters from ws['dtable']; bp: the frozen ones are skipped."""
         if self.bias_type == "continuous":
-            self._relpos_backward(ws, N, det)
+            self._relpos_backward(ws, N, det, bp if bp is not None else self.backward_plan())
         elif self.bias_type == "t5":
             gw = self.gview["transformer.rel_pos_bias.relative_attention_bias.weight"]      # bucket 0 collects every delta
+            # (the table has a gradient only when this, the T5 path's one parameter, is trainable)
             lib.colsum(ws["dtable"], 1, ws["dtable"].stride(0), gw[0], N, self.h, accumulate=True)
 
     def _relpos_table(self, ws, N):
@@ -501,13 +568,22 @@ class Engine:
         else:
             lib.gemm(dy, x, gout, a_mn=True, b_mn=True, M=m, N=n, K=k, addend=gout, block_n=bn, max_ctas=self.bwd_max_ctas, **kw)
 
-    def backward_core(self, pl: _Plan, ws, src_row, key_mask, groups_with_grad, drop: bool = False, on_ready=None, det: bool = False):
+    def backward_core(self, pl: _Plan, ws, src_row, key_mask, groups_with_grad, drop: bool = False, on_ready=None, det: bool = False,
+                      frozen=()):
         """Consumes ws['dlogits'] (bf16, permuted rows) and accumulates every parameter gradient into arena_g.
         on_ready(trigger): called when a group of gradients is final -- 'heads', 'layer<l>' (matrices of layer l), 'tail'
         (everything else) -- so that a data-parallel caller can start reducing it underneath the rest of the pass.
         det: the fixed-order kernel variants (ws must hold their scratch, see add_det_scratch): bit-identical gradients
-        for identical inputs on the same GPU model."""
+        for identical inputs on the same GPU model.
+        frozen: names of parameters that get no gradient.  Their arena_g ranges are not written, and only the work a
+        trainable parameter needs runs (_BackwardPlan): no weight-gradient GEMM of a frozen matrix, no bias-table gradient
+        when nothing trains the table, and nothing below the lowest layer a gradient still has to reach.  The gradients of
+        the trainable parameters are those of the full pass (bit for bit in deterministic mode).  on_ready is still
+        called at every point (the data-parallel plan leaves the fully frozen buckets out, grad_bucket_plan)."""
         ready = on_ready if on_ready is not None else (lambda trigger: None)
+        bp = self.backward_plan(frozen)
+        tr = bp.trains
+        gw = lambda n: self.gview[n] if tr(n) else None        # parameter-gradient output, None when frozen
         part = ws["det_part"] if det else None
         wpart = ws["det_wgrad"] if det else None
         B, N, M, d, h, HD, F, Fp = pl.B, pl.N, pl.M, self.d, self.h, self.HD, self.F, self.Fp
@@ -516,7 +592,7 @@ class Engine:
         drop_p = self.drop_p if drop else 0.0
         # ---- logit heads
         gset = frozenset(groups_with_grad)
-        if ws.get("dxf_groups") != gset:      # rows of head groups without a gradient stay zero; the others are overwritten
+        if bp.final_norm and ws.get("dxf_groups") != gset:   # rows of head groups without a gradient stay zero; the others are overwritten
             ws["dxf"].zero_()
             ws["dxf_groups"] = gset
         for gi, (s, qi, cnt, base) in enumerate(pl.groups):
@@ -524,70 +600,108 @@ class Engine:
                 continue
             rows = B * cnt
             dl = ws["dlogits"][gi]
-            lib.gemm(dl, self.pk_logit_b[s][qi], ws["dxf"][base:base + rows], b_mn=True, M=rows, N=d, K=self.Cp[s], block_n=128, max_ctas=self.bwd_max_ctas)
-            self._wgrad(dl, ws["xf"][base:base + rows], gv[f"logit_weights.{s}"][qi], self.Cp[s], d, det_part=wpart, row_split=self.Cp[s],
-                        row_valid=self.C[s])
+            if bp.final_norm:
+                lib.gemm(dl, self.pk_logit_b[s][qi], ws["dxf"][base:base + rows], b_mn=True, M=rows, N=d, K=self.Cp[s], block_n=128, max_ctas=self.bwd_max_ctas)
+            if tr(f"logit_weights.{s}"):
+                self._wgrad(dl, ws["xf"][base:base + rows], gv[f"logit_weights.{s}"][qi], self.Cp[s], d, det_part=wpart, row_split=self.Cp[s],
+                            row_valid=self.C[s])
         ready("heads")
         dxa, dxb = ws["dx"]
-        lib.layernorm_bwd(ws["dxf"], x[2 * self.L], ws["st_o"], pv["transformer.norm.gamma"], dxa, gv["transformer.norm.gamma"],
-                          src_row=pl.dest_row, dx_bf16=ws["dx_bf"], part=part)
-        ws["dtable"].zero_()
+        if bp.final_norm:
+            lib.layernorm_bwd(ws["dxf"], x[2 * self.L], ws["st_o"], pv["transformer.norm.gamma"], dxa, gw("transformer.norm.gamma"),
+                              src_row=pl.dest_row, dx_bf16=ws["dx_bf"], part=part)
+        dtable = ws["dtable"] if bp.dtable else None
+        if dtable is not None:
+            dtable.zero_()
         for l in reversed(range(self.L)):
+            if not bp.run[l]:
+                ready(f"layer{l}")
+                continue
+            st = bp.steps[l]
             p, pk = f"transformer.layers.{l}.", self.pk[l]
             xa, xm = x[2 * l], x[2 * l + 1]
             # ---- conv feed-forward
             # d_hn = dx W2 with the LayerNorm-backward row sums (against the saved hn) taken in the GEMM's epilogue
             fk = self.ffk
             keep = ws["keep"][l] if drop_p > 0 else None
-            if Fp % 256 == 0:
-                lib.gemm_rowstat(ws["dx_bf"], pk["w2_b"], ws["dhn"], ws["hn"][l], pk["gin"], ws["rowstat"], b_mn=True, M=M, N=Fp, K=d,
-                                 keep_bits=keep, keep_scale=1.0 / (1.0 - drop_p) if drop_p > 0 else 1.0, max_ctas=self.bwd_max_ctas)
-                parts = Fp // 128
-            else:
-                lib.gemm(ws["dx_bf"], pk["w2_b"], ws["dhn"], b_mn=True, M=M, N=Fp, K=d, block_n=self._bn_for(M, Fp, d), max_ctas=self.bwd_max_ctas)
-                parts = 0
-            # (the tile kernel runs right behind the GEMM that wrote dhn, while dhn is still in L2; the weight gradient after it)
-            lib.ffn_mid_bwd(ws["dhn"], ws["hn"][l], ws["u"][l], ws["st_i"][l], pk["conv"], pk["gin"], ws["rowstat"], ws["du"],
-                            gv[p + fk["gin"]], gv[p + fk["conv"]] if fk["conv"] is not None else None, B, N, F, Fp, drop_p,
-                            keep_bits=keep, rowstat_parts=parts, part=part)
-            self._wgrad(ws["dx_bf"], ws["hn"][l], gv[p + fk["w2"]], d, Fp, det_part=wpart, n_valid=F)
-            lib.gemm(ws["du"], pk["w1_b"], ws["dxn"], b_mn=True, M=M, N=d, K=2 * Fp, block_n=self._bn_for(M, d, 2 * Fp), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["du"], ws["xn2"][l], gv[p + fk["w1"]], 2 * Fp, d, det_part=wpart, row_split=-1, row_valid=F)
-            lib.layernorm_bwd(ws["dxn"], xm, ws["st_f"][l], pv[p + fk["g1"]], dxb, gv[p + fk["g1"]], dres=dxa, dx_bf16=ws["dx_bf"], part=part)
+            if st["ffn"]:
+                if Fp % 256 == 0:
+                    lib.gemm_rowstat(ws["dx_bf"], pk["w2_b"], ws["dhn"], ws["hn"][l], pk["gin"], ws["rowstat"], b_mn=True, M=M, N=Fp, K=d,
+                                     keep_bits=keep, keep_scale=1.0 / (1.0 - drop_p) if drop_p > 0 else 1.0, max_ctas=self.bwd_max_ctas)
+                    parts = Fp // 128
+                else:
+                    lib.gemm(ws["dx_bf"], pk["w2_b"], ws["dhn"], b_mn=True, M=M, N=Fp, K=d, block_n=self._bn_for(M, Fp, d), max_ctas=self.bwd_max_ctas)
+                    parts = 0
+                # (the tile kernel runs right behind the GEMM that wrote dhn, while dhn is still in L2; the weight gradient after it)
+                lib.ffn_mid_bwd(ws["dhn"], ws["hn"][l], ws["u"][l], ws["st_i"][l], pk["conv"], pk["gin"], ws["rowstat"], ws["du"],
+                                gw(p + fk["gin"]), gw(p + fk["conv"]) if fk["conv"] is not None else None, B, N, F, Fp, drop_p,
+                                keep_bits=keep, rowstat_parts=parts, part=part)
+            if tr(p + fk["w2"]):
+                self._wgrad(ws["dx_bf"], ws["hn"][l], gv[p + fk["w2"]], d, Fp, det_part=wpart, n_valid=F)
+            if st["ln_f"]:
+                lib.gemm(ws["du"], pk["w1_b"], ws["dxn"], b_mn=True, M=M, N=d, K=2 * Fp, block_n=self._bn_for(M, d, 2 * Fp), max_ctas=self.bwd_max_ctas)
+            if tr(p + fk["w1"]):
+                self._wgrad(ws["du"], ws["xn2"][l], gv[p + fk["w1"]], 2 * Fp, d, det_part=wpart, row_split=-1, row_valid=F)
+            if st["ln_f"]:
+                lib.layernorm_bwd(ws["dxn"], xm, ws["st_f"][l], pv[p + fk["g1"]], dxb, gw(p + fk["g1"]), dres=dxa, dx_bf16=ws["dx_bf"], part=part)
             # ---- attention
-            lib.gemm(ws["dx_bf"], pk["wo_b"], ws["d_o"], b_mn=True, M=M, N=HD, K=d, block_n=self._bn_for(M, HD, d), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["dx_bf"], ws["o"][l], gv[p + "0.to_out.0.weight"], d, HD, det_part=wpart)
-            lib.attn_bwd_tc(ws["qn"][l], ws["kvn"][l], ws["d_o"], ws["o"][l], ws["lse"][l], ws["table"], key_mask, ws["dsum"],
-                            ws["dqn"], ws["dkvn"], ws["dtable"], B, N, h, det=ws["det_attn"] if det else None)
-            lib.qk_l2norm_bwd(ws["dqn"], ws["dkvn"], ws["q_raw"][l], ws["kv_raw"][l], pv[p + "0.q_scale"], pv[p + "0.k_scale"],
-                              ws["dq_raw"], ws["dkv_raw"], gv[p + "0.q_scale"], gv[p + "0.k_scale"], h, part=part)
-            lib.gemm(ws["dq_raw"], pk["wq_b"], ws["dxn"], b_mn=True, M=M, N=d, K=HD, block_n=self._bn_for(M, d, HD), max_ctas=self.bwd_max_ctas)
-            lib.gemm(ws["dkv_raw"], pk["wkv_b"], ws["dxraw"], b_mn=True, M=M, N=d, K=128, block_n=self._bn_for(M, d, 128), max_ctas=self.bwd_max_ctas)
-            self._wgrad(ws["dq_raw"], ws["xn"][l], gv[p + "0.to_q.weight"], HD, d, det_part=wpart)
-            self._wgrad(ws["dkv_raw"], ws["xraw"][l], gv[p + "0.to_kv.weight"], 128, d, det_part=wpart)
+            if st["attn"]:
+                lib.gemm(ws["dx_bf"], pk["wo_b"], ws["d_o"], b_mn=True, M=M, N=HD, K=d, block_n=self._bn_for(M, HD, d), max_ctas=self.bwd_max_ctas)
+            if tr(p + "0.to_out.0.weight"):
+                self._wgrad(ws["dx_bf"], ws["o"][l], gv[p + "0.to_out.0.weight"], d, HD, det_part=wpart)
+            if st["attn"]:
+                lib.attn_bwd_tc(ws["qn"][l], ws["kvn"][l], ws["d_o"], ws["o"][l], ws["lse"][l], ws["table"], key_mask, ws["dsum"],
+                                ws["dqn"], ws["dkvn"], dtable, B, N, h, det=ws["det_attn"] if det else None)
+            if st["qk"]:
+                lib.qk_l2norm_bwd(ws["dqn"], ws["dkvn"], ws["q_raw"][l], ws["kv_raw"][l], pv[p + "0.q_scale"], pv[p + "0.k_scale"],
+                                  ws["dq_raw"], ws["dkv_raw"], gw(p + "0.q_scale"), gw(p + "0.k_scale"), h, part=part)
+            if st["ln_a"]:
+                lib.gemm(ws["dq_raw"], pk["wq_b"], ws["dxn"], b_mn=True, M=M, N=d, K=HD, block_n=self._bn_for(M, d, HD), max_ctas=self.bwd_max_ctas)
+            if st["g_in"]:
+                lib.gemm(ws["dkv_raw"], pk["wkv_b"], ws["dxraw"], b_mn=True, M=M, N=d, K=128, block_n=self._bn_for(M, d, 128), max_ctas=self.bwd_max_ctas)
+            if tr(p + "0.to_q.weight"):
+                self._wgrad(ws["dq_raw"], ws["xn"][l], gv[p + "0.to_q.weight"], HD, d, det_part=wpart)
+            if tr(p + "0.to_kv.weight"):
+                self._wgrad(ws["dkv_raw"], ws["xraw"][l], gv[p + "0.to_kv.weight"], 128, d, det_part=wpart)
             ready(f"layer{l}")
-            lib.layernorm_bwd(ws["dxn"], xa, ws["st_a"][l], pv[p + "0.norm.gamma"], dxa, gv[p + "0.norm.gamma"], dres=dxb, draw=ws["dxraw"],
-                              dx_bf16=ws["dx_bf"], part=part)
+            if st["ln_a"]:
+                lib.layernorm_bwd(ws["dxn"], xa, ws["st_a"][l], pv[p + "0.norm.gamma"], dxa, gw(p + "0.norm.gamma"),
+                                  dres=dxb if st["g_in"] else None, draw=ws["dxraw"] if st["g_in"] else None, dx_bf16=ws["dx_bf"], part=part)
         # ---- embeddings + start tokens (grad_shrink: utils.py:60-61)
-        rows = self.det_rows if det else None
-        lib.embed_scatter_add(self.dtable_emb, src_row, dxa, self.alpha, first=rows)
-        if pl.src_row2 is not None:
-            lib.embed_scatter_add(self.dtable_emb, pl.src_row2, dxa, self.alpha, first=rows)
-        self.bias_table_backward(ws, N, det)
+        if bp.rows:
+            rows = self.det_rows if det else None
+            src1, src2 = src_row, pl.src_row2
+            if bp.rows_partial:
+                src1 = self._trainable_rows(bp, src1)
+                src2 = self._trainable_rows(bp, src2) if src2 is not None else None
+            lib.embed_scatter_add(self.dtable_emb, src1, dxa, self.alpha, first=rows)
+            if src2 is not None:
+                lib.embed_scatter_add(self.dtable_emb, src2, dxa, self.alpha, first=rows)
+        if dtable is not None:
+            self.bias_table_backward(ws, N, det, bp)
         ready("tail")
 
-    def _relpos_backward(self, ws, N, det=False):
+    def _relpos_backward(self, ws, N, det, bp: _BackwardPlan):
         pv, gv, Hr, T, h = self.pview, self.gview, self.Hr, self.Hr8, self.h
         pre = "transformer.rel_pos_bias.net."
+        tr = bp.trains
         dT = ws["dtable"]                                   # [h, N]: dY[n, hh] = dT[hh, n]
         a3 = ws["rp_a"][2]
-        lib.sgemm_small(dT, (N, 1), a3, (Hr, 1), gv[pre + "3.weight"], (Hr, 1), h, Hr, N, accumulate=True, det=det)   # dW4 = dY^T a3
-        lib.colsum(dT, 1, N, gv[pre + "3.bias"], N, h, accumulate=True)
+        if tr(pre + "3.weight"):
+            lib.sgemm_small(dT, (N, 1), a3, (Hr, 1), gv[pre + "3.weight"], (Hr, 1), h, Hr, N, accumulate=True, det=det)   # dW4 = dY^T a3
+        if tr(pre + "3.bias"):
+            lib.colsum(dT, 1, N, gv[pre + "3.bias"], N, h, accumulate=True)
+        # the MLP's gradient flows down only as far as its lowest trainable layer (j = 2, 1, 0)
+        lowest = min([j for j in (0, 1, 2) if tr(f"{pre}{j}.0.weight") or tr(f"{pre}{j}.0.bias")], default=3)
         d_cur, d_nxt = ws["rp_d0"], ws["rp_d1"]
-        lib.sgemm_small(dT, (1, N), pv[pre + "3.weight"], (Hr, 1), d_cur, (Hr, 1), N, Hr, h)                      # da3 = dY W4
+        if lowest < 3:
+            lib.sgemm_small(dT, (1, N), pv[pre + "3.weight"], (Hr, 1), d_cur, (Hr, 1), N, Hr, h)                  # da3 = dY W4
         for j in (2, 1, 0):
+            if j < lowest:
+                break
             lib.silu_bwd(d_cur, ws["rp_z"][j], d_cur)                                                              # dz_j (fp32, in place)
-            lib.colsum(d_cur, Hr, 1, gv[f"{pre}{j}.0.bias"], N, Hr, accumulate=True)
+            if tr(f"{pre}{j}.0.bias"):
+                lib.colsum(d_cur, Hr, 1, gv[f"{pre}{j}.0.bias"], N, Hr, accumulate=True)
             if j > 0:
                 # bf16x3 products, as in the forward pass (x y ~ x_hi y_hi + x_hi y_lo + x_lo y_hi: fp32-class): these
                 # gradients are sums of cancelling terms, so a plain bf16 operand rounding shows up amplified
@@ -596,13 +710,16 @@ class Engine:
                 a_hi, a_lo = ws["rp_a3"][j - 1][:, :Hr], ws["rp_a3"][j - 1][:, 2 * T:2 * T + Hr]                   # forward split of a_{j-1}
                 w_hi, w_lo = self.pk_rp[j - 1][:, :Hr], self.pk_rp[j - 1][:, T:T + Hr]                             # [hi | lo | hi]
                 gw = gv[f"{pre}{j}.0.weight"]
-                for dz, a in ((dz_hi, a_hi), (dz_hi, a_lo), (dz_lo, a_hi)):                                         # dW_j += dz^T a
-                    lib.gemm(dz, a, gw, a_mn=True, b_mn=True, M=Hr, N=Hr, K=N, addend=gw, block_n=128)
+                if tr(f"{pre}{j}.0.weight"):
+                    for dz, a in ((dz_hi, a_hi), (dz_hi, a_lo), (dz_lo, a_hi)):                                     # dW_j += dz^T a
+                        lib.gemm(dz, a, gw, a_mn=True, b_mn=True, M=Hr, N=Hr, K=N, addend=gw, block_n=128)
+                if j == lowest:
+                    break
                 lib.gemm(dz_hi, w_hi, d_nxt, b_mn=True, M=N, N=Hr, K=Hr, block_n=128)                               # da = dz W
                 lib.gemm(dz_hi, w_lo, d_nxt, b_mn=True, M=N, N=Hr, K=Hr, addend=d_nxt, block_n=128)
                 lib.gemm(dz_lo, w_hi, d_nxt, b_mn=True, M=N, N=Hr, K=Hr, addend=d_nxt, block_n=128)
                 d_cur, d_nxt = d_nxt, d_cur
-            else:
+            elif tr(f"{pre}0.0.weight"):
                 lib.sgemm_small(d_cur, (1, Hr), ws["rp_in"], (1, 1), gv[f"{pre}0.0.weight"], (1, 1), Hr, 1, N, accumulate=True, det=det)
 
     # ------------------------------------------------------------------------------------------ reference-API path
@@ -618,13 +735,19 @@ class Engine:
             self.start_row, append_eos=False, drop_last=False, mask_cond=False, mask_in=mask_in, want_labels=False,
             err_flag=self.err_flag)
         pl = self.plan(B, n_tok)
-        need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self._param_list)
+        # requires_grad is read at every call, as autograd reads it: frozen parameters get no gradient (grad stays None)
+        named = list(self.m.named_parameters())
+        frozen = frozenset(n for n, p in named if not p.requires_grad)
+        for n, p in named:
+            if n in frozen and p.grad is self.gview[n]:
+                p.grad = None           # the arena view handed out before the parameter was frozen, never written by autograd
+        need_grad = torch.is_grad_enabled() and len(frozen) < len(named)
         wanted = {len(self.seqs) - 1} if only_final else set(range(len(self.seqs)))
         drop = self.m.training and self.drop_p > 0
         if drop:
             self.seed += 1
         outs = _ApiFunction.apply(self, pl, src_row, key_mask, need_grad, wanted, drop, torch.are_deterministic_algorithms_enabled(),
-                                  *self._param_list)
+                                  frozen, *self._param_list)
         res, k = [], 0
         for s in range(len(self.seqs)):
             if s in wanted:
@@ -658,11 +781,11 @@ class _ApiFunction(torch.autograd.Function):
     forward(), libomlm_b200 backward in backward(); gradients are returned per parameter."""
 
     @staticmethod
-    def forward(ctx, eng: Engine, pl, src_row, key_mask, need_grad, wanted, drop, det, *params):
+    def forward(ctx, eng: Engine, pl, src_row, key_mask, need_grad, wanted, drop, det, frozen, *params):
         ws = eng.workspace(pl, need_grad, det)
         eng.forward_core(pl, ws, src_row, key_mask, need_grad, wanted, drop)
         ctx.eng, ctx.pl, ctx.src_row, ctx.key_mask, ctx.wanted, ctx.drop = eng, pl, src_row, key_mask, sorted(wanted), drop
-        ctx.need_grad = need_grad
+        ctx.need_grad, ctx.frozen = need_grad, frozen
         # the saved activations live in the shape's workspace, not in the graph: a second forward of the same shape before
         # this call's backward would overwrite them -- remember which forward owns the workspace and check in backward
         ws["generation"] = ws.get("generation", 0) + 1
@@ -692,11 +815,11 @@ class _ApiFunction(torch.autograd.Function):
         # gradients are produced in a scratch copy of the arena so that autograd can accumulate them itself
         saved = eng.arena_g.clone()
         eng.arena_g.zero_()
-        eng.backward_core(pl, ws, ctx.src_row, ctx.key_mask, with_grad, ctx.drop, det=det)
+        eng.backward_core(pl, ws, ctx.src_row, ctx.key_mask, with_grad, ctx.drop, det=det, frozen=ctx.frozen)
         fresh = eng.arena_g.clone()
         eng.arena_g.copy_(saved)
         outs = []
         for n, p in eng.m.named_parameters():
             o = eng.layout[n]
-            outs.append(fresh[o:o + p.numel()].view(p.shape))
-        return (None, None, None, None, None, None, None, None, *outs)
+            outs.append(None if n in ctx.frozen else fresh[o:o + p.numel()].view(p.shape))
+        return (None, None, None, None, None, None, None, None, None, *outs)

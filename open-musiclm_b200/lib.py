@@ -263,7 +263,8 @@ def attn_bwd(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dt
 
 
 def attn_bwd_tc(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads, scale=8.0, det=None):
-    """det: an AttnBwdDetWorkspace for this (B, N, heads) -> the fixed-order variant (omlm_attn_bwd_tc_det)."""
+    """det: an AttnBwdDetWorkspace for this (B, N, heads) -> the fixed-order variant (omlm_attn_bwd_tc_det).
+    dtable None: the variant without the bias gradient (dqn / dkvn as with a table)."""
     args = (_p(qn), _p(kvn), _p(d_o), _p(o), _p(lse2), _p(table), _I(table.stride(0)), _p(key_mask),
             _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale))
     if det is None:
@@ -306,10 +307,10 @@ def ffn_norm_fwd(h, rowsum, gamma, hn, stats, F, Fp, drop_p=0.0, seed=None, laye
 
 def ffn_mid_bwd(dhn, hn, u, stats, conv_w, gamma, rowstat, du, dgamma, dconv_w, B, N, F, Fp, drop_p=0.0, keep_bits=None, rowstat_parts=0,
                 part=None):
-    """dgamma [F] / dconv_w [2F, 3] (or None) are accumulated in the parameters' own layouts; rowstat_parts > 0: rowstat
-    holds the partial row sums written by gemm_rowstat, else it is a [M, 2] scratch."""
+    """dgamma [F] / dconv_w [2F, 3] (each may be None: not summed) are accumulated in the parameters' own layouts;
+    rowstat_parts > 0: rowstat holds the partial row sums written by gemm_rowstat, else it is a [M, 2] scratch."""
     assert u.dtype in _T16 and hn.dtype == dhn.dtype == du.dtype == torch.bfloat16
-    assert dgamma.numel() == F and (dconv_w is None or dconv_w.numel() == 6 * F)
+    assert (dgamma is None or dgamma.numel() == F) and (dconv_w is None or dconv_w.numel() == 6 * F)
     args = (_p(dhn), _p(hn), _p(u), _p(stats), _p(conv_w), _p(gamma), _p(keep_bits), _p(rowstat), _I(rowstat_parts), _p(du),
             _p(dgamma), _p(dconv_w), _I(B), _I(N), _I(F), _I(Fp), _F(drop_p), _I(int(u.dtype == torch.float16)))
     if part is None:

@@ -26,11 +26,15 @@ from .dist_utils import BucketReducer, all_gather_, allreduce_sum_, grad_prescal
 from .model import TokenConditionedTransformer
 
 
-def frozen_parameter_names(names, ce_weights):
-    """Parameters the reference never updates.  It adds a sequence's cross entropy only when its weight is > 0
-    (open_musiclm.py:398), so the logit head of a sequence weighted 0 keeps `grad is None`, and torch's optimizers skip
-    such a parameter: no weight decay, no moment update."""
-    return {n for n in names if n.startswith("logit_weights.") and not ce_weights[int(n.split(".")[1])] > 0}
+def frozen_parameter_names(names, ce_weights, requires_grad=None):
+    """Parameters the reference never updates, because their `grad` stays None and torch's optimizers and
+    clip_grad_norm_ skip such a parameter (no weight decay, no moment update, no part in the norm):
+      * the logit head of a sequence weighted 0: the reference adds a sequence's cross entropy only when its weight
+        is > 0 (open_musiclm.py:398);
+      * every parameter the user froze: requires_grad (name -> bool, optional) is False."""
+    rg = requires_grad if requires_grad is not None else {}
+    return {n for n in names if (n.startswith("logit_weights.") and not ce_weights[int(n.split(".")[1])] > 0)
+            or not rg.get(n, True)}
 
 
 def live_ranges(n, frozen_spans):
@@ -71,7 +75,10 @@ class HotPathTrainer:
         self.mask_prob = mask_prob
         self.betas, self.eps, self.pad_id = betas, eps, pad_id
         sizes = {n: p.numel() for n, p in transformer.named_parameters()}
-        self.frozen = frozen_parameter_names(sizes, self.ce_weights)
+        # read once, like the loss weights: the backward pass, the AdamW ranges, the gradient buckets and the captured
+        # graphs are planned for this set (train_step raises if requires_grad changes afterwards)
+        self._requires_grad = {n: p.requires_grad for n, p in transformer.named_parameters()}
+        self.frozen = frozen_parameter_names(sizes, self.ce_weights, self._requires_grad)
         # the AdamW launches cover these arena ranges only: frozen parameters keep p, m and v bit for bit
         self.live = live_ranges(eng.n_params_arena, [(eng.layout[n], eng.layout[n] + sizes[n]) for n in self.frozen])
         self.steps = 0
@@ -109,7 +116,7 @@ class HotPathTrainer:
             # pass), every rank runs clip + AdamW on its 1/world of the arena only, then the parameters are all-gathered --
             # the same bytes on the wire as one all-reduce, but the optimiser pass shrinks by 1/world.  The all-gather of
             # the fp32 parameters is exposed at the end of the step; off by default (not measured on H100).
-            plan = eng.grad_bucket_plan()
+            plan = eng.grad_bucket_plan(frozen=self.frozen)
             self.shard_opt = os.environ.get("OMLM_SHARD_OPT", "0") == "1" and all((hi - lo) % self.world == 0 for _, sl in plan for lo, hi in sl)
             self.reducer = BucketReducer(eng.arena_g, plan, process_group, side_stream=torch.cuda.Stream(priority=prio), scatter=self.shard_opt)
             nccl_ctas = int(os.environ.get("NCCL_MAX_CTAS", "0") or 0)
@@ -168,7 +175,8 @@ class HotPathTrainer:
                                   part=ws["det_part"] if det else None)
         loss = acc[0]
         if backward:
-            eng.backward_core(pl, ws, src_row, key_mask, weighted, drop, on_ready=reducer.fire if reducer is not None else None, det=det)
+            eng.backward_core(pl, ws, src_row, key_mask, weighted, drop, on_ready=reducer.fire if reducer is not None else None, det=det,
+                              frozen=self.frozen)
         return loss
 
     def _set_hyper(self):
@@ -298,10 +306,18 @@ class HotPathTrainer:
         With torch.use_deterministic_algorithms(True) the step runs the fixed-order kernel variants: the same inputs,
         build, world size and GPU model (SM count) give bit-identical losses, gradient norms, parameters and Adam
         moments, eagerly and under graph replay.  The mode is part of the graph key: toggling it re-captures.
+        Parameters with requires_grad=False at construction are frozen as in the reference: no gradient (their arena_g
+        range stays zero), no part in the clip norm, no AdamW update, no optimizer state in save(); the backward pass
+        runs only the work the trainable parameters need.
         transformer.engine.check_errors() raises if a deterministic step could not keep its order (never expected; the
         attention backward gives up waiting for an accumulation turn after seconds instead of hanging)."""
         assert len(micro_batches) == self.grad_accum_every
         eng = self.eng
+        changed = sorted(n for n, p in self.transformer.named_parameters() if p.requires_grad != self._requires_grad[n])
+        if changed:
+            raise RuntimeError(f"requires_grad changed after this HotPathTrainer was built (for {changed[:4]}"
+                               f"{' ...' if len(changed) > 4 else ''}): the frozen set is read at construction; "
+                               "construct a new HotPathTrainer")
         det = torch.are_deterministic_algorithms_enabled()
         self.transformer.train()
         eng.refresh_packed()        # no-op unless the parameters were written from outside (load_state_dict, manual edits):
@@ -310,7 +326,7 @@ class HotPathTrainer:
             self._step_body(micro_batches, det)
             self.steps += 1
             return self.loss_out
-        key = (det,) + tuple(tuple(t.shape) for mb in micro_batches for t in mb)
+        key = (det, frozenset(self.frozen)) + tuple(tuple(t.shape) for mb in micro_batches for t in mb)
         st = self._graphs.pop(key, None)
         if st is not None:
             self._graphs[key] = st                   # most recently used
