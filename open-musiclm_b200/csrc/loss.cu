@@ -189,6 +189,9 @@ static int cross_entropy_impl(const float* logits, long ld, const int* labels, i
   if (rows_per_batch <= 0) { rows_per_batch = rows; batch_stride = 0; }      // one flat label vector
   const int blocks = (rows + 7) / 8;
   if (part != nullptr) OMLM_CHECK_ARG(part_bytes >= blocks * 8L, "cross_entropy_det: partials need %ld bytes", blocks * 8L);
+  // both kernels write every column below Cp of a gradient row: a row narrower than C would lose part of its gradient
+  if (dlogits_bf16 != nullptr)
+    OMLM_CHECK_ARG(Cp >= C && ldd >= Cp, "cross_entropy: dlogits needs C <= Cp <= ldd (C=%d, Cp=%d, ldd=%ld)", C, Cp, ldd);
   if (C > 32 * kCeMaxPerLane || Cp > 32 * kCeMaxPerLane) {
     // rows too long for registers: the streaming kernel (128-bit loads and 16-byte stores)
     OMLM_CHECK_ARG(reinterpret_cast<uintptr_t>(logits) % 16 == 0 && ld % 4 == 0 && ld >= C,

@@ -280,6 +280,7 @@ qk_l2norm_fwd_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat1
 }
 
 // l2norm * scale backward.  y = s * x/|x|.  dx = (s*dy - xh * (xh . s*dy)) / |x| ;  ds += dy * xh.
+// |x| < 1e-12 (F.normalize's clamp, e.g. the zero q / k of a pad row): y = s * x / 1e-12, dx = s*dy / 1e-12.
 // dqn: fp32 [M, h*64] (atomically accumulated by the attention backward); dkvn: fp32 [M, 128].
 // Outputs bf16 dq_raw [M, h*64], dkv_raw [M, 128] (value gradient passes through).
 // DET: the 32 vector slots of a block are combined in slot order and written as this block's row of part [gridDim.x,
@@ -342,7 +343,8 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
       ss += __shfl_xor_sync(0xffffffffu, ss, 1);
       ss += __shfl_xor_sync(0xffffffffu, ss, 2);
       ss += __shfl_xor_sync(0xffffffffu, ss, 4);
-      const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
+      const float nrm = sqrtf(ss);
+      const float inv = 1.f / fmaxf(nrm, 1e-12f);
       float s[8];
       if (norm) {
         const float4 s0 = *reinterpret_cast<const float4*>(sc + sub * 8);
@@ -363,6 +365,8 @@ qk_l2norm_bwd_kernel(const float* __restrict__ dqn, const float* __restrict__ dk
       dot += __shfl_xor_sync(0xffffffffu, dot, 1);
       dot += __shfl_xor_sync(0xffffffffu, dot, 2);
       dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+      // below the clamp F.normalize divides by the constant eps, whose gradient has no projection term: dx = s dy / eps
+      if (nrm < 1e-12f) dot = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) o[i] = norm ? (sg[i] - xh[i] * dot) * inv : g[i];
     }

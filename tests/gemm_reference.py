@@ -37,7 +37,7 @@ Prologue bound.  The prologue operand is y = (x - mean) rstd gamma (prologue 2: 
 prologue 3: mean = s1 / n_real, var = max(s2 / n_real - mean^2, 0) from the row sums), rounded to the 16-bit format.
 The fp32 statistics err by: the lane sums gamma(ceil(n / 32) + 6) of their absolute sums, the divisions u', the
 variance additionally 2 |mean| dmean (+ dmean^2) and the cancellation u' (s2 / n + mean^2) of prologue 3; rstd then
-errs relatively by dvar / (2 (var + eps)) plus rsqrtf's 2 ulp.  The three fp32 products of y each round (3 u'), so
+errs relatively by dvar / (2 (var + eps)), half a unit for the eps addition and rsqrtf's 2 ulp (2^-22 relative).  The three fp32 products of y each round (3 u'), so
 
     |y32 - y| <= (|gamma| rstd (dmean + u' |x - mean|) + |y| (drstd + 3 u')) (1 + 2^-10)
 
@@ -166,11 +166,7 @@ def decode_operand(A, prologue, wdt, gamma_=None, rowsum=None, n_real=0, K=None)
         return x, torch.zeros_like(x)
     g = gamma_[:K].double()
     if prologue == 2:
-        n, mean = K, x.mean(-1, keepdim=True)
-        var = ((x - mean) ** 2).mean(-1, keepdim=True)
-        ga = gamma(math.ceil(K / 32) + 6)
-        dmean = ga * x.abs().mean(-1, keepdim=True) + U * mean.abs()
-        dvar = (ga * var + 2 * dmean * (x - mean).abs().mean(-1, keepdim=True) + dmean ** 2) * (1 + 2 * U) + U * var
+        mean, var, dmean, dvar = ln_stats(x, math.ceil(K / 32) + 6)
     else:
         rs = rowsum.double()[:, :K // 128]
         s1, s2 = rs[..., 0].sum(-1, keepdim=True), rs[..., 1].sum(-1, keepdim=True)
@@ -181,9 +177,30 @@ def decode_operand(A, prologue, wdt, gamma_=None, rowsum=None, n_real=0, K=None)
         dmean = ga * rs[..., 0].abs().sum(-1, keepdim=True) / n + U * mean.abs()
         ds2 = ga * rs[..., 1].abs().sum(-1, keepdim=True) / n + U * s2.abs() / n
         dvar = ds2 + 2 * mean.abs() * dmean + dmean ** 2 + 2 * U * (s2.abs() / n + mean ** 2)
-    rstd = 1.0 / torch.sqrt(var + EPS)
+    return ln_y(x, g, mean, var, dmean, dvar)
+
+
+def ln_stats(x, chain):
+    """Float64 (mean, var) of the rows of x, and the bounds (dmean, dvar) of fp32 statistics whose sums put each term
+    through at most `chain` roundings (the square's product included) before the divisions by the row length."""
+    mean = x.mean(-1, keepdim=True)
+    var = ((x - mean) ** 2).mean(-1, keepdim=True)
+    ga = gamma(chain)
+    dmean = ga * x.abs().mean(-1, keepdim=True) + U * mean.abs()
+    dvar = (ga * var + 2 * dmean * (x - mean).abs().mean(-1, keepdim=True) + dmean ** 2) * (1 + 2 * U) + U * var
+    return mean, var, dmean, dvar
+
+
+def ln_rstd(var, dvar):
+    """Float64 rstd = 1 / sqrt(var + eps) and the relative bound of rsqrtf(var32 + eps) against it: the variance error,
+    the rounding of the eps addition and rsqrtf's 2 ulp (at most 2^-22 relative)."""
+    return 1.0 / torch.sqrt(var + EPS), dvar / (2 * (var + EPS)) + U / 2 + 2.0 ** -22
+
+
+def ln_y(x, g, mean, var, dmean, dvar):
+    """(y64 = (x - mean) rstd gamma, bound of the fp32 y = ((x - mean32) * rstd32) * gamma against it)."""
+    rstd, drstd = ln_rstd(var, dvar)
     y = (x - mean) * rstd * g
-    drstd = dvar / (2 * (var + EPS)) + 2 * 2.0 ** -24
     e = (g.abs() * rstd * (dmean + U * (x - mean).abs()) + y.abs() * (drstd + 3 * U)) * SECOND_ORDER
     return y, e
 
