@@ -366,6 +366,19 @@ int omlm_sample(const float* logits, long ld, int C, int top_k, float temperatur
 int omlm_sample_seeded(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                        const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
                        int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
+/* Nucleus (top-p, Holtzman et al. 2019) sampling on top of omlm_sample / omlm_sample_seeded, 0 < top_p < 1 (anything
+ * else is rejected).  For one row: eos and the top-k set K as in omlm_sample; p_c = softmax(l / temperature) over K, the
+ * distribution the Gumbel-argmax samples from; the nucleus is
+ *     N = { c in K : sum of p_j over j in K with l_j > l_c  <  top_p }
+ * -- the smallest prefix of K by value whose mass reaches top_p, with equal values all in N or all out; the most likely
+ * value is always in N.  The token is the argmax over N of l_c / temperature + g_c, with g_c drawn from the same uniform
+ * the other samplers would use for class c (supplied, Philox keyed by *seed, or by seeds[b] when seeds is not NULL;
+ * seeds and uniform exclude each other).  A NaN logit is never in N and has no mass; a row whose maximum over K is not
+ * finite samples as omlm_sample does.  The sums behind N run in a fixed order, so a row's token does not depend on the
+ * batch or the row.  Counters and outputs as omlm_sample. */
+int omlm_sample_nucleus(const float* logits, long ld, int C, int top_k, float temperature, float top_p, int allow_eos,
+                        const float* uniform, const unsigned long long* seed, const unsigned long long* seeds, long long* tokens,
+                        long tokens_ld, int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
 
 #ifdef __cplusplus
 }

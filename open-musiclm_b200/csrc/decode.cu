@@ -13,7 +13,7 @@
 //                   LayerNorm of fp32 rows (transformer.py:24-31), or the inner FFN LayerNorm from the fused row sums
 //   attn_decode     l2norm * scale of the new q / k, cache append, scores against the whole cache + bias, softmax, P V
 //   conv_geglu      causal depthwise conv over (state, new row), GEGLU with exact-erf GELU, LayerNorm row sums
-//   sample          eos rule, top-k, Gumbel-argmax (utils.py:71-84), next embedding row
+//   sample          eos rule, top-k, optionally the top-p nucleus, Gumbel-argmax (utils.py:71-84), next embedding row
 // Rounding points mirror the training-path forward (16-bit GEMM operands, bf16 P, fp32 accumulation) so that an
 // incremental step reproduces the full forward's logits to accumulation-order noise.
 #include "common.cuh"
@@ -480,13 +480,24 @@ decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restric
 // seeds[b] on the counter (c, step, 0, 0x5eed) -- a stream that depends neither on the row b nor on the batch.
 // Writes tokens[b, t] (t = *step_ptr), the embedding-table row of the sampled token for the next step, and advances
 // the device-side counters (*step_ptr, *pos_ptr) once per launch.  grid B, 256 threads.
+//
+// kNucleus (top_p in (0, 1)): the Gumbel-argmax runs over the nucleus N of the top-k set K instead of K.  With
+// p_c = exp((l_c - max_K l) / T) and Z = sum of p over K, N = { c in K : sum of p_j over j in K with l_j > l_c < top_p Z }:
+// the smallest prefix of K by value whose mass reaches top_p, with equal values all in or all out.  Z and every masked
+// mass are summed in one fixed order (thread-strided, then the same shuffle tree, then warps 0..7), so a row's N
+// depends only on the row.  The threshold key is found by bitwise bisection over the sort keys: the largest key v whose
+// mass at or above v is still >= top_p Z; N is then K's entries with key >= v.  NaN logits get no mass and are never in
+// N; a row whose maximum over K is not finite samples over K as the kNucleus = false kernel does.  The uniforms are
+// the ones the false kernel draws for the same class; classes outside N draw none.  Another [C] array in shared memory
+// holds p: 192 KB at C = 16384.
+template <bool kNucleus>
 __global__ void __launch_bounds__(256)
 sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float temperature, int allow_eos,
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
               const unsigned long long* __restrict__ seeds,
               long long* __restrict__ tokens, long tokens_ld, int* __restrict__ next_row, int row_offset,
-              int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B) {
-  extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys
+              int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B, float top_p) {
+  extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys (kNucleus: then [C] weights p)
   float* lg = sm_l;
   uint32_t* key = reinterpret_cast<uint32_t*>(sm_l + C);
   __shared__ float rv[8];
@@ -530,15 +541,69 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     s_tie_budget = k - above;
   }
   __syncthreads();
+  if constexpr (kNucleus) {
+    __shared__ float s_mx[8];
+    __shared__ double s_mass[8];
+    float* p = sm_l + 2 * C;
+    const int lane = tid & 31, warp = tid >> 5;
+    // K, kept in lg from here on: an entry outside K becomes NaN, which the arg-max below skips
+    float mx = -INFINITY;
+    for (int c = tid; c < C; c += 256) {
+      bool keep = key[c] > thr;
+      if (!keep && key[c] == thr) {
+        int rank = 0;
+        for (int j = 0; j < c; ++j) rank += key[j] == thr;
+        keep = rank < s_tie_budget;
+      }
+      if (!keep) lg[c] = __int_as_float(0x7fffffff);
+      else mx = fmaxf(mx, lg[c]);                                 // fmaxf ignores a NaN logit
+    }
+    mx = warp_max(mx);
+    if (lane == 0) s_mx[warp] = mx;
+    __syncthreads();
+    mx = s_mx[0];
+    for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_mx[w]);
+    if (isfinite(mx)) {                                           // the same on every thread of the block
+      for (int c = tid; c < C; c += 256) p[c] = isnan(lg[c]) ? 0.f : expf((lg[c] - mx) / temperature);
+      __syncthreads();
+      // mass of the keys >= cand, in the fixed order; every thread gets the same value (a + b == b + a in the tree)
+      auto mass_from = [&](uint32_t cand) -> double {
+        double s = 0.0;
+        for (int c = tid; c < C; c += 256) s += key[c] >= cand ? static_cast<double>(p[c]) : 0.0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) s_mass[warp] = s;
+        __syncthreads();
+        double t = 0.0;
+        for (int w = 0; w < 8; ++w) t += s_mass[w];
+        __syncthreads();
+        return t;
+      };
+      const double target = static_cast<double>(top_p) * mass_from(0u);   // every key is >= 0: the mass is Z
+      uint32_t nthr = 0;
+      for (int bit = 31; bit >= 0; --bit) {
+        const uint32_t cand = nthr | (1u << bit);
+        if (mass_from(cand) >= target) nthr = cand;
+      }
+      for (int c = tid; c < C; c += 256)
+        if (key[c] < nthr) lg[c] = __int_as_float(0x7fffffff);
+    }
+    __syncthreads();
+  }
   float best = -INFINITY;
   int best_i = 0x7fffffff;
   const unsigned long long seed = seeds != nullptr ? seeds[b] : (seed_ptr != nullptr ? *seed_ptr : 0ull);
   for (int c = tid; c < C; c += 256) {
-    bool keep = key[c] > thr;
-    if (!keep && key[c] == thr) {
-      int rank = 0;
-      for (int j = 0; j < c; ++j) rank += key[j] == thr;
-      keep = rank < s_tie_budget;
+    bool keep;
+    if constexpr (kNucleus) {
+      keep = !isnan(lg[c]);                                      // N (or K, when the row's maximum is not finite)
+    } else {
+      keep = key[c] > thr;
+      if (!keep && key[c] == thr) {
+        int rank = 0;
+        for (int j = 0; j < c; ++j) rank += key[j] == thr;
+        keep = rank < s_tie_budget;
+      }
     }
     if (!keep) continue;
     float u;
@@ -586,6 +651,25 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     if (pos_ptr != nullptr) pos_ptr[0] = pos_ptr[0] + 1;
     __threadfence();
   }
+}
+
+template <bool kNucleus>
+static int launch_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
+                         const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                         int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float top_p, void* stream) {
+  OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384 && temperature > 0.f && top_k >= 1 && top_k <= C, "sample: bad arguments");
+  OMLM_CHECK_ARG(seeds == nullptr || uniform == nullptr, "sample: per-sequence seeds and supplied uniforms exclude each other");
+  // 128 KB (nucleus: 192 KB) at C = 16384: above the 48 KB a launch gets without the opt-in
+  const int smem = (kNucleus ? 3 : 2) * C * 4;
+  static int configured = 0;
+  if (smem > configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel<kNucleus>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = smem;
+  }
+  OMLM_KLAUNCH((sample_kernel<kNucleus>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature,
+               allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p);
+  OMLM_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace omlm
@@ -674,19 +758,16 @@ int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, 
 int omlm_sample_seeded(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                        const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
                        int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream) {
-  using namespace omlm;
-  OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384 && temperature > 0.f && top_k >= 1 && top_k <= C, "sample: bad arguments");
-  OMLM_CHECK_ARG(seeds == nullptr || uniform == nullptr, "sample: per-sequence seeds and supplied uniforms exclude each other");
-  const int smem = 2 * C * 4;                     // 128 KB at C = 16384: above the 48 KB a launch gets without the opt-in
-  static int configured = 0;
-  if (smem > configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = smem;
-  }
-  OMLM_KLAUNCH((sample_kernel), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature, allow_eos, uniform, seed,
-               seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B);
-  OMLM_LAUNCH_CHECK();
-  return 0;
+  return omlm::launch_sample<false>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
+                                    row_offset, step_ptr, pos_ptr, B, 1.f, stream);
+}
+
+int omlm_sample_nucleus(const float* logits, long ld, int C, int top_k, float temperature, float top_p, int allow_eos,
+                        const float* uniform, const unsigned long long* seed, const unsigned long long* seeds, long long* tokens,
+                        long tokens_ld, int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream) {
+  OMLM_CHECK_ARG(top_p > 0.f && top_p < 1.f, "sample_nucleus: top_p %g outside (0, 1)", static_cast<double>(top_p));
+  return omlm::launch_sample<true>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
+                                   row_offset, step_ptr, pos_ptr, B, top_p, stream);
 }
 
 int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,

@@ -15,7 +15,11 @@ per sequence instead of once per head.  The choice follows from the batch size; 
 Seeded generation (`generate(seeds=...)`) takes the tensor-core path at every batch size, with the GEMM's K split fixed
 independently of B (omlm_decode_gemm_invariant), and draws each sequence's noise from its own seed: the tokens of a
 sequence are then a function of its own inputs and seed, not of the batch it runs in (DESIGN section 4).
+
+Nucleus sampling (`generate(top_p=...)`) runs in the same captured step, through omlm_sample_nucleus; its semantics are
+stated in `generate`'s docstring.
 """
+import numbers
 from typing import List, Optional, Sequence
 
 import torch
@@ -59,6 +63,21 @@ def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
         raise ValueError(f"open_musiclm_b200 generate: {len(vals)} seeds for {B} sequences")
     vals = [v & 0xFFFFFFFFFFFFFFFF for v in vals]
     return torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in vals], dtype=torch.int64, device=device)
+
+
+def check_top_p(top_p, where: str = "generate"):
+    """The nucleus mass of a generate call: None or 1 (no nucleus filtering) -> None, a number in (0, 1) -> that float;
+    anything else (NaN, a bool, a non-number, a value outside (0, 1]) raises ValueError."""
+    if top_p is None:
+        return None
+    if isinstance(top_p, bool) or not isinstance(top_p, numbers.Real):
+        raise ValueError(f"open_musiclm_b200 {where}: top_p must be None or a number in (0, 1], not {top_p!r}")
+    p = float(top_p)
+    if p == 1.0:
+        return None
+    if not 0.0 < p < 1.0:           # also rejects NaN
+        raise ValueError(f"open_musiclm_b200 {where}: top_p must lie in (0, 1], got {top_p!r}")
+    return p
 
 
 class DecodeSession:
@@ -164,20 +183,20 @@ class DecodeSession:
         lib.decode_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"], ws=ws,
                         invariant=inv)
 
-    def sample(self, qi: int, top_k: int, temperature: float, allow_eos: bool, uniform, seed, bump_pos: bool):
+    def sample(self, qi: int, top_k: int, temperature: float, allow_eos: bool, uniform, seed, bump_pos: bool, top_p=None):
         eng = self.eng
         S = len(eng.seqs) - 1
         q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
         row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
         lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                   self.counters, self.pos if bump_pos else None, self.B, seeds=self.seeds)
+                   self.counters, self.pos if bump_pos else None, self.B, seeds=self.seeds, top_p=top_p)
 
-    def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True):
+    def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True, top_p=None):
         """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
-        key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded)
+        key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p)
         g = self._graphs.get(key)
         if g is None or not use_graph:
-            body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True))
+            body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True, top_p))
             if not use_graph:
                 body()
                 return
@@ -220,7 +239,7 @@ class TokenConditionedTransformerWrapper(nn.Module):
     def generate(self, *, conditioning_token_ids: List[torch.Tensor], pred_token_ids: Optional[torch.Tensor] = None,
                  max_time_steps=512, filter_thres=0.9, temperature=1., include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, allow_eos_in_output=False, uniform_noise: Optional[torch.Tensor] = None,
-                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, **kwargs):
+                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, top_p=None, **kwargs):
         """Same contract as open_musiclm.py:253-326.  uniform_noise (optional, [n_sampled, b, codebook+1] in (0, 1)):
         the uniform draws behind the Gumbel noise, one slice per sampled token in order — parity runs pass the stream
         torch's default CPU generator would have produced; by default the noise comes from a device Philox stream keyed
@@ -237,11 +256,23 @@ class TokenConditionedTransformerWrapper(nn.Module):
         batch.  As the reference's nn.Embedding lookup would, IndexError is raised (before anything runs, Engine.seed
         untouched) when a conditioning sequence with its eos holds more than max_absolute_position_embeddings tokens,
         or when prefix length + n_new - 1 exceeds it (the last sampled token is never fed back).
+        top_p (optional, nucleus sampling, Holtzman et al. 2019): for one row, with eos forbidden as above and the top-k
+        set K chosen as above (exactly k entries; among values equal to the k-th largest the lower index wins; -0.0
+        equals +0.0), let p_c = softmax(l / temperature) over K, the distribution the Gumbel-argmax samples from.  The
+        nucleus is N = {c in K : sum of p_j over j in K with l_j > l_c < top_p}: the smallest prefix of K, by value,
+        whose mass reaches top_p, extended to include ties (equal values are all in N or all out; the most likely token
+        is always in).  The token is the argmax over N of l_c / temperature + g_c, where g_c comes from exactly the
+        uniform the sampler uses without top_p (uniform_noise, the Engine.seed stream, or the sequence's seed); classes
+        outside N are skipped.  A NaN logit is never in N and adds no mass; a row with no finite logit in K samples as
+        without top_p.  N depends only on the row, so seeded generation stays independent of the batch.  None or 1.0:
+        no nucleus filtering, bit-identical to a call without top_p.  Any other value must lie in (0, 1); NaN, a bool or
+        an out-of-range value raises ValueError before anything runs (Engine.seed untouched).
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
         if seeds is not None and uniform_noise is not None:
             raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
+        top_p = check_top_p(top_p)
         m, eng = self.transformer, self.transformer.engine
         S = len(self.token_sequences)
         assert len(conditioning_token_ids) == S - 1
@@ -301,15 +332,16 @@ class TokenConditionedTransformerWrapper(nn.Module):
             C = info.codebook_size + 1
             if trace_logits is not None:
                 trace_logits.append(sess.logits[:, :C].clone())
-            sess.sample(p0 % q, top_k, temperature, allow(p0), uni, eng.seed, bump_pos=False)
+            sess.sample(p0 % q, top_k, temperature, allow(p0), uni, eng.seed, bump_pos=False, top_p=top_p)
             for s in range(1, n_new):
                 p = p0 + s
                 if trace_logits is not None:      # eager, in two halves, so that the logits can be copied in between
                     sess.step(p % q)
                     trace_logits.append(sess.logits[:, :C].clone())
-                    sess.sample(p % q, top_k, temperature, allow(p), uni, eng.seed, True)
+                    sess.sample(p % q, top_k, temperature, allow(p), uni, eng.seed, True, top_p=top_p)
                 else:
-                    sess.step_and_sample((p - 1) % q, p % q, top_k, temperature, allow(p), uni, eng.seed, use_graph=use_cuda_graph)
+                    sess.step_and_sample((p - 1) % q, p % q, top_k, temperature, allow(p), uni, eng.seed, use_graph=use_cuda_graph,
+                                         top_p=top_p)
             if seed_vals is None:
                 eng.seed += 1
             sampled = torch.cat([prefix, sess.tokens[:, :n_new]], 1)

@@ -488,8 +488,17 @@ def decode_conv_geglu(u_new, state, conv_w, h_out, rowsum):
          _I(int(u_new.dtype == torch.float16)), _stream())
 
 
-def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B, seeds=None):
-    """seeds: int64 [B] device tensor of per-sequence seeds (raw 64-bit patterns) -> omlm_sample_seeded."""
+def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B, seeds=None,
+           top_p=None):
+    """seeds: int64 [B] device tensor of per-sequence seeds (raw 64-bit patterns) -> omlm_sample_seeded.
+    top_p: nucleus sampling (omlm_sample_nucleus, which rejects values outside (0, 1)); None or 1.0 samples over the
+    whole top-k set through omlm_sample / omlm_sample_seeded."""
+    if top_p is not None and top_p != 1.0:
+        assert seeds is None or (seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B)
+        call("omlm_sample_nucleus", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _F(top_p),
+             _I(int(allow_eos)), _p(uniform), _p(seed), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset),
+             _p(counters), _p(pos), _I(B), _stream())
+        return
     if seeds is None:
         call("omlm_sample", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _I(int(allow_eos)), _p(uniform),
              _p(seed), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())

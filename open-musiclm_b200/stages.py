@@ -19,7 +19,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .decode import TokenConditionedTransformerWrapper
+from .decode import TokenConditionedTransformerWrapper, check_top_p
 from .model import TokenConditionedTransformer
 
 
@@ -212,6 +212,16 @@ def prepare_audio(data: torch.Tensor, sample_hz, target_sample_hz, normalize=Tru
     return int16_to_float32(float32_to_int16(_resample(data, sample_hz, target_sample_hz)))
 
 
+def _stage_top_p(top_p):
+    """MusicLM.generate_tokens' top_p -> one checked value (None or a float in (0, 1)) per stage, semantic, coarse, fine."""
+    where = "MusicLM.generate_tokens"
+    if isinstance(top_p, (list, tuple)):
+        if len(top_p) != 3:
+            raise ValueError(f"open_musiclm_b200 {where}: top_p as a sequence needs 3 values (semantic, coarse, fine), got {len(top_p)}")
+        return [check_top_p(p, where) for p in top_p]
+    return [check_top_p(top_p, where)] * 3
+
+
 def _prime(t: torch.Tensor, b: int, q: int, device, what: str) -> torch.Tensor:
     """Prime tokens [1 or b, T, q] ([1 or b, T] for the semantic stream) -> [b, T, q] int64 on `device`."""
     if t.dim() == 2 and q == 1:
@@ -244,7 +254,8 @@ class MusicLM(nn.Module):
                         fine_window_seconds=2, semantic_steps_per_second=50, acoustic_steps_per_second=75,
                         semantic_sliding_window_step_percent=0.5, coarse_sliding_window_step_percent=0.5,
                         fine_sliding_window_step_percent=1, noise: Optional[NoiseStream] = None, return_all=False, seeds=None,
-                        prime_semantic_token_ids=None, prime_coarse_token_ids=None, prime_fine_token_ids=None, coarse_only=False):
+                        prime_semantic_token_ids=None, prime_coarse_token_ids=None, prime_fine_token_ids=None, coarse_only=False,
+                        top_p=None):
         """The token-level body of MusicLM.forward (open_musiclm.py:913-1032): returns the acoustic tokens
         [b, T, coarse + fine quantizers] the reference would hand to the codec (return_all: also the three streams).
         seeds (optional): one unsigned 64-bit seed per prompt (list of ints or int64 tensor).  Every generate call then gets
@@ -258,7 +269,11 @@ class MusicLM(nn.Module):
         condition length > 0 (fine_sliding_window_step_percent < 1) the reference's streams cannot be joined; here the
         coarse stream drops the prime tokens the first fine window was conditioned on, so both start after the prime.
         coarse_only: stop after the coarse stage and return its stream [b, T, coarse quantizers] as it stands before
-        the crop that lines it up with the fine windows (forward's return_coarse_generated_wave)."""
+        the crop that lines it up with the fine windows (forward's return_coarse_generated_wave).
+        top_p (nucleus sampling, TokenConditionedTransformerWrapper.generate): None, one value for every stage, or a
+        sequence of three values (semantic, coarse, fine), each None or a number in (0, 1]; every window's generate call
+        gets its stage's value.  A sequence of another length or a bad value raises ValueError before the first window."""
+        stage_top_p = _stage_top_p(top_p)
         if seeds is not None and noise is not None:
             raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: seeds and noise exclude each other")
         if seeds is not None:
@@ -273,6 +288,12 @@ class MusicLM(nn.Module):
             w = counter.get(stage, 0)
             counter[stage] = w + 1
             return dict(seeds=[window_seed(s, stage, w) for s in seeds])
+
+        def sampling(stage):           # this stage's seeds and nucleus mass (passed only when set)
+            kw = seeded(stage)
+            if stage_top_p[stage] is not None:
+                kw["top_p"] = stage_top_p[stage]
+            return kw
 
         sps, aps = semantic_steps_per_second, acoustic_steps_per_second
         primes = (prime_semantic_token_ids, prime_coarse_token_ids, prime_fine_token_ids)
@@ -302,11 +323,11 @@ class MusicLM(nn.Module):
         # ---- semantic stream: first window from the prime's tail (or scratch), then windows conditioned on the tail of
         # the stream (:930-949); cropped to line up with the coarse windows (:952)
         sem = self.semantic.generate(semantic_token_ids=sem_prime, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps),
-                                     **common, **seeded(SEMANTIC))
+                                     **common, **sampling(SEMANTIC))
         keep = int(semantic_window_seconds * sps * (1 - semantic_sliding_window_step_percent))
         while sem.shape[1] < int(output_seconds * sps):
             nxt = self.semantic.generate(semantic_token_ids=sem[:, -keep:], max_time_steps=int(semantic_window_seconds * sps), **common,
-                                         **seeded(SEMANTIC))
+                                         **sampling(SEMANTIC))
             sem = torch.cat([sem, nxt[:, keep:]], 1)
         sem = sem[:, sem_adj:]
         # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail, the first one
@@ -315,7 +336,7 @@ class MusicLM(nn.Module):
         coarse, keep = None, int(coarse_window_seconds * aps * (1 - coarse_sliding_window_step_percent))
         for sem_win in _windows(sem, win, int(win * coarse_sliding_window_step_percent)):
             pred = self.coarse.generate(semantic_token_ids=sem_win, coarse_token_ids=coarse_prime if coarse is None else coarse[:, -keep:],
-                                        max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common, **seeded(COARSE))
+                                        max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common, **sampling(COARSE))
             coarse = pred if coarse is None else torch.cat([coarse, pred[:, keep:]], 1)
         if coarse_only:                                                                                 # :986-989
             return coarse
@@ -326,7 +347,7 @@ class MusicLM(nn.Module):
         for coarse_win in _windows(coarse, fwin, int(fwin * fine_sliding_window_step_percent)):
             cond = fine_prime if fine is None else (fine[:, -keep:] if keep > 0 else None)
             pred = self.fine.generate(coarse_token_ids=coarse_win, fine_token_ids=cond, max_time_steps=fwin, temperature=0.4, **common,
-                                      **seeded(FINE))
+                                      **sampling(FINE))
             fine = pred if fine is None else torch.cat([fine, pred[:, keep:]], 1)
         fine = fine[:, fine_adj:]                                                                       # :1026
         # the coarse stream still starts with the fine_adj prime tokens the first fine window was conditioned on; the
