@@ -155,6 +155,10 @@ int omlm_embed_gather(const float* table, const int* src_row, const int* src_row
  * [0, pos_rows), adds nothing (the caller checks the bound before launching).  fp32, 128-bit copies. */
 int omlm_embed_gather_pos(const float* table, const int* src_row, const int* pos_ptr, int pos_offset, int pos_row_base,
                           int pos_rows, float* x, int M, int D, void* stream);
+/* omlm_embed_gather_pos with one position per row, for prompts of different lengths in one batch: p = pos[m] +
+ * pos_offset, pos a device int array [M].  The shared-position entry point above keeps its single read. */
+int omlm_embed_gather_pos_ragged(const float* table, const int* src_row, const int* pos, int pos_offset, int pos_row_base,
+                                 int pos_rows, float* x, int M, int D, void* stream);
 int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, int M, int D,
                            float scale, void* stream);
 
@@ -298,6 +302,9 @@ int omlm_gather_windows(const void* src_i16, const long long* start, long long* 
  * (open_musiclm.py:303-307).  Batches of B <= 16 rows run the SIMT weight-streaming kernels of csrc/decode.cu
  * (omlm_skinny_gemm, omlm_attn_decode); 16 < B <= 256 run the tensor-core GEMM of csrc/decode_gemm.cu (omlm_decode_gemm)
  * and the cache-sharing attention omlm_attn_decode_mqa.
+ * Every sequence is at the position the device int *pos_ptr holds; when the prompts of one batch differ in length, the
+ * _ragged forms of the attention entry points (and omlm_embed_gather_pos_ragged) read one position per sequence from a
+ * device int array pos [B] instead, and omlm_decode_advance_pos takes over the position bump from the sampler.
  * out[b, n] = A[b, :] . W[n, :] (+ addend[b, n]);  W 16-bit [N, ldw] (w_f16: fp16, else bf16).  prologue builds the
  * activation rows in W's format: 0 = A already 16-bit [B, lda];  1 = A fp32, rounded;  2 = LayerNorm(A fp32) * gamma
  * (transformer.py:24-31);  3 = A = h 16-bit [B, K] with the fused per-128-channel sums rowsum [B, K/128, 2]:
@@ -346,6 +353,20 @@ int omlm_attn_decode(const void* q_raw, const void* kv_raw, const float* q_scale
 int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
                          long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
                          int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream);
+/* omlm_attn_decode and omlm_attn_decode_mqa with one position per sequence: sequence b appends its [k | v] at n = pos[b]
+ * and attends over its keys 0..pos[b] with bias deltas pos[b] - j (pos: device int array [B], each entry < max_pos).  In
+ * the _mqa form a sequence uses the slices its own n covers, counts its arrivals and combines them in slice order exactly
+ * as it would alone, so its output is bit-identical to the same sequence in a call with B = 1. */
+int omlm_attn_decode_ragged(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                            long cache_ld_b, const float* table, int table_ld, const int* pos, int max_pos, void* out, int B,
+                            int heads, float scale, void* stream);
+int omlm_attn_decode_mqa_ragged(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                                long cache_ld_b, const float* table, int table_ld, const int* pos, int max_pos, void* out, int B,
+                                int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream);
+/* Per-sequence position bump of a decode step whose prompts differ in length (the sampler is then called with
+ * pos_ptr = NULL): pos[b] += 1 while pos[b] < pos_last[b], the last position sequence b processes.  A sequence that
+ * has all its tokens keeps its position, so one captured step serves every step of the call.  Device int arrays [B]. */
+int omlm_decode_advance_pos(int* pos, const int* pos_last, int B, void* stream);
 /* CausalDSConv + GEGLU for one new row (transformer.py:122-137): u_new [B, 2Fp] against state [B, 2, 2Fp] (rows t-2, t-1,
  * shifted in place) -> h [B, Fp], rowsum [B, Fp/128, 2]. */
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,

@@ -144,9 +144,11 @@ skinny_gemm_kernel(const SkinnyArgs a) {
 
 // ------------------------------------------------------------------------------------------------ attention, one new position
 // grid (B, h), 128 threads.  q_raw [B, h*64] bf16, kv_raw [B, 128] bf16 (this step's projections, un-normalised),
-// cache [B, Nmax, 128] bf16, table [h, table_ld] fp32, *pos_ptr = n = index of the new position (keys 0..n).
+// cache [B, Nmax, 128] bf16, table [h, table_ld] fp32, n = index of the new position (keys 0..n): *pos_ptr for every
+// sequence, or pos_ptr[b] with kRowPos (prompts of different lengths in one batch).
 constexpr int kAdThreads = 128;
 
+template <bool kRowPos>
 __global__ void __launch_bounds__(kAdThreads)
 attn_decode_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16* __restrict__ kv_raw,
                    const float* __restrict__ q_scale, const float* __restrict__ k_scale,
@@ -158,7 +160,7 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16*
   __shared__ float red[kAdThreads / 32];
   __shared__ float so[16][64];
   const int b = blockIdx.x, head = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = *pos_ptr;
+  const int n = pos_ptr[kRowPos ? b : 0];
   // ---- l2norm * scale of the new query / key (utils.py:68-69, transformer.py:269-271), rounded to bf16 like the
   //      training path's qn / kvn tensors; head 0 appends [k | v] to the cache for the steps to come
   if (warp < 2) {
@@ -258,13 +260,15 @@ attn_decode_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16*
 // takes row n from this step's projections (and appends it to the cache: exactly one CTA covers n), and leaves per head
 // the split's (max, sum) and unnormalised P V in a workspace.  The last split of a sequence to finish (per-sequence
 // counter) combines the splits in order 0, 1, ... -- fixed order, deterministic -- and writes out.
+// kRowPos: n = pos_ptr[b] per sequence.  The splits a sequence takes part in (n / 128 + 1 of them), its arrival count
+// and its combine order are then those of the same sequence run alone, so its output is bit-identical to that run.
 // Rounding points of attn_decode: bf16 q / k after l2norm * scale, scores in the exp2 domain, P rounded to bf16 (here
 // relative to the split's own maximum), fp32 normaliser.
 constexpr int kMqThreads = 256, kMqKeys = 128;
 constexpr int kMqRow = 272;                          // bytes per staged K | V row: 256 + 16 of padding (bank spread)
 constexpr int kMqScLd = kMqKeys + 1;                 // score row pitch (floats)
 
-template <int HM>                                    // HM >= heads: 4, 8 or 16
+template <int HM, bool kRowPos>                      // HM >= heads: 4, 8 or 16
 __global__ void __launch_bounds__(kMqThreads)
 attn_decode_mqa_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloat16* __restrict__ kv_raw,
                        const float* __restrict__ q_scale, const float* __restrict__ k_scale,
@@ -280,7 +284,7 @@ attn_decode_mqa_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloa
   __shared__ float s_m[HM], s_l[HM];
   __shared__ int s_last;
   const int split = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = *pos_ptr;
+  const int n = pos_ptr[kRowPos ? b : 0];
   const int j0 = split * kMqKeys;
   if (j0 > n) return;                                // beyond this step's keys (the grid covers max_pos)
   const int nk = min(kMqKeys, n + 1 - j0), active = n / kMqKeys + 1;
@@ -416,7 +420,7 @@ attn_decode_mqa_kernel(const __nv_bfloat16* __restrict__ q_raw, const __nv_bfloa
   if (tid == 0) counters[b] = 0;                     // ready for the next step (or graph replay)
 }
 
-template <int HM>
+template <int HM, bool kRowPos>
 static int launch_attn_decode_mqa(dim3 grid, cudaStream_t st, const void* q_raw, const void* kv_raw, const float* q_scale,
                                   const float* k_scale, void* cache, long cache_ld_b, const float* table, int table_ld,
                                   const int* pos_ptr, void* out, int heads, float scale, float* part_o, float2* part_ml,
@@ -424,10 +428,10 @@ static int launch_attn_decode_mqa(dim3 grid, cudaStream_t st, const void* q_raw,
   constexpr int smem = kMqKeys * kMqRow + HM * kMqScLd * 4;
   static bool configured = false;
   if (!configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_decode_mqa_kernel<HM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    OMLM_CUDA(cudaFuncSetAttribute(attn_decode_mqa_kernel<HM, kRowPos>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = true;
   }
-  OMLM_KLAUNCH((attn_decode_mqa_kernel<HM>), grid, kMqThreads, smem, st,
+  OMLM_KLAUNCH((attn_decode_mqa_kernel<HM, kRowPos>), grid, kMqThreads, smem, st,
       reinterpret_cast<const __nv_bfloat16*>(q_raw), reinterpret_cast<const __nv_bfloat16*>(kv_raw), q_scale, k_scale,
       reinterpret_cast<__nv_bfloat16*>(cache), cache_ld_b, table, table_ld, pos_ptr, reinterpret_cast<__nv_bfloat16*>(out), heads,
       scale, part_o, part_ml, counters, max_splits);
@@ -672,6 +676,54 @@ static int launch_sample(const float* logits, long ld, int C, int top_k, float t
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ per-row positions
+// Prompts of different lengths: after each step's sample, pos[b] advances by one while it is below pos_last[b], the
+// last position sequence b processes.  A sequence that has all its tokens keeps its position, so its cache and position
+// lookups stay inside the range that sequence alone would use.  One thread per sequence.
+__global__ void decode_advance_pos_kernel(int* __restrict__ pos, const int* __restrict__ pos_last, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < B && pos[b] < pos_last[b]) pos[b] = pos[b] + 1;
+}
+
+template <bool kRowPos>
+static int launch_attn_decode(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                              long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
+                              int heads, float scale, void* stream) {
+  OMLM_CHECK_ARG(B >= 1 && heads >= 1 && max_pos >= 1 && table_ld >= max_pos, "attn_decode: bad shape");
+  const int smem = max_pos * 4;
+  OMLM_CHECK_ARG(smem <= 200 * 1024, "attn_decode: context %d too long", max_pos);
+  static int configured = 0;
+  if (smem > configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(attn_decode_kernel<kRowPos>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = smem;
+  }
+  OMLM_KLAUNCH((attn_decode_kernel<kRowPos>), dim3(B, heads), kAdThreads, smem, reinterpret_cast<cudaStream_t>(stream),
+      reinterpret_cast<const __nv_bfloat16*>(q_raw), reinterpret_cast<const __nv_bfloat16*>(kv_raw), q_scale, k_scale,
+      reinterpret_cast<__nv_bfloat16*>(cache), cache_ld_b, table, table_ld, pos_ptr, reinterpret_cast<__nv_bfloat16*>(out), heads, scale);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+
+template <bool kRowPos>
+static int attn_decode_mqa_dispatch(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                                    long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out,
+                                    int B, int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream) {
+  OMLM_CHECK_ARG(B >= 1 && heads >= 1 && heads <= 16 && max_pos >= 1 && table_ld >= max_pos, "attn_decode_mqa: bad shape");
+  const int max_splits = (max_pos + kMqKeys - 1) / kMqKeys;
+  const long need = static_cast<long>(B) * max_splits * heads * (64 + 2) * 4;
+  OMLM_CHECK_ARG(ws != nullptr && counters != nullptr && ws_bytes >= need, "attn_decode_mqa: workspace of %ld bytes, %ld needed", ws_bytes, need);
+  float* part_o = ws;
+  float2* part_ml = reinterpret_cast<float2*>(ws + static_cast<long>(B) * max_splits * heads * 64);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(max_splits, B);
+  if (heads <= 4) return launch_attn_decode_mqa<4, kRowPos>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table,
+                                                            table_ld, pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+  if (heads <= 8) return launch_attn_decode_mqa<8, kRowPos>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table,
+                                                            table_ld, pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+  return launch_attn_decode_mqa<16, kRowPos>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
+                                             pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+}
+
 }  // namespace omlm
 
 extern "C" {
@@ -709,40 +761,37 @@ int omlm_skinny_gemm(const void* A, long lda, int prologue, const void* W, long 
 int omlm_attn_decode(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
                      long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
                      int heads, float scale, void* stream) {
-  using namespace omlm;
-  OMLM_CHECK_ARG(B >= 1 && heads >= 1 && max_pos >= 1 && table_ld >= max_pos, "attn_decode: bad shape");
-  const int smem = max_pos * 4;
-  OMLM_CHECK_ARG(smem <= 200 * 1024, "attn_decode: context %d too long", max_pos);
-  static int configured = 0;
-  if (smem > configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    configured = smem;
-  }
-  OMLM_KLAUNCH((attn_decode_kernel), dim3(B, heads), kAdThreads, smem, reinterpret_cast<cudaStream_t>(stream), 
-      reinterpret_cast<const __nv_bfloat16*>(q_raw), reinterpret_cast<const __nv_bfloat16*>(kv_raw), q_scale, k_scale,
-      reinterpret_cast<__nv_bfloat16*>(cache), cache_ld_b, table, table_ld, pos_ptr, reinterpret_cast<__nv_bfloat16*>(out), heads, scale);
-  OMLM_LAUNCH_CHECK();
-  return 0;
+  return omlm::launch_attn_decode<false>(q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld, pos_ptr, max_pos, out,
+                                         B, heads, scale, stream);
+}
+
+int omlm_attn_decode_ragged(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                            long cache_ld_b, const float* table, int table_ld, const int* pos, int max_pos, void* out, int B,
+                            int heads, float scale, void* stream) {
+  return omlm::launch_attn_decode<true>(q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld, pos, max_pos, out,
+                                        B, heads, scale, stream);
 }
 
 int omlm_attn_decode_mqa(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
                          long cache_ld_b, const float* table, int table_ld, const int* pos_ptr, int max_pos, void* out, int B,
                          int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream) {
+  return omlm::attn_decode_mqa_dispatch<false>(q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld, pos_ptr, max_pos,
+                                               out, B, heads, scale, ws, ws_bytes, counters, stream);
+}
+
+int omlm_attn_decode_mqa_ragged(const void* q_raw, const void* kv_raw, const float* q_scale, const float* k_scale, void* cache,
+                                long cache_ld_b, const float* table, int table_ld, const int* pos, int max_pos, void* out, int B,
+                                int heads, float scale, float* ws, long ws_bytes, int* counters, void* stream) {
+  return omlm::attn_decode_mqa_dispatch<true>(q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld, pos, max_pos,
+                                              out, B, heads, scale, ws, ws_bytes, counters, stream);
+}
+
+int omlm_decode_advance_pos(int* pos, const int* pos_last, int B, void* stream) {
   using namespace omlm;
-  OMLM_CHECK_ARG(B >= 1 && heads >= 1 && heads <= 16 && max_pos >= 1 && table_ld >= max_pos, "attn_decode_mqa: bad shape");
-  const int max_splits = (max_pos + kMqKeys - 1) / kMqKeys;
-  const long need = static_cast<long>(B) * max_splits * heads * (64 + 2) * 4;
-  OMLM_CHECK_ARG(ws != nullptr && counters != nullptr && ws_bytes >= need, "attn_decode_mqa: workspace of %ld bytes, %ld needed", ws_bytes, need);
-  float* part_o = ws;
-  float2* part_ml = reinterpret_cast<float2*>(ws + static_cast<long>(B) * max_splits * heads * 64);
-  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const dim3 grid(max_splits, B);
-  if (heads <= 4) return launch_attn_decode_mqa<4>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
-                                                   pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
-  if (heads <= 8) return launch_attn_decode_mqa<8>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
-                                                   pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
-  return launch_attn_decode_mqa<16>(grid, st, q_raw, kv_raw, q_scale, k_scale, cache, cache_ld_b, table, table_ld,
-                                    pos_ptr, out, heads, scale, part_o, part_ml, counters, max_splits);
+  OMLM_CHECK_ARG(B >= 1 && pos != nullptr && pos_last != nullptr, "decode_advance_pos: bad arguments");
+  OMLM_KLAUNCH((decode_advance_pos_kernel), (B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream), pos, pos_last, B);
+  OMLM_LAUNCH_CHECK();
+  return 0;
 }
 
 int omlm_decode_conv_geglu(const void* u_new, void* state, const float* conv_w, void* h_out, float* rowsum, int B, int Fp,

@@ -18,6 +18,10 @@ sequence are then a function of its own inputs and seed, not of the batch it run
 
 Nucleus sampling (`generate(top_p=...)`) runs in the same captured step, through omlm_sample_nucleus; its semantics are
 stated in `generate`'s docstring.
+
+Prefixes of different lengths (`generate(pred_lengths=...)`) run the same step with one position per sequence
+(DecodeSession.pos [B], the _ragged attention and gather entry points, omlm_decode_advance_pos in place of the
+sampler's position bump); every row gets what it would get alone (DESIGN section 4).
 """
 import numbers
 from typing import List, Optional, Sequence
@@ -45,6 +49,11 @@ class _Capture:
     def after_u(self, l, u):
         s = self.s
         rows = u.view(s.B, s.n_prompt, -1)
+        if s.ragged:                  # rows n_b - 2, n_b - 1 of each sequence's own prompt (zero before its first row)
+            idx = s.prompt_len[:, None] + torch.arange(-2, 0, device=rows.device)
+            hist = rows[torch.arange(s.B, device=rows.device)[:, None], idx.clamp_min(0)]
+            s.conv[l].copy_(hist.masked_fill((idx < 0)[..., None], 0))
+            return
         k = min(2, s.n_prompt)
         s.conv[l].zero_()
         s.conv[l][:, 2 - k:].copy_(rows[:, s.n_prompt - k:])
@@ -80,13 +89,46 @@ def check_top_p(top_p, where: str = "generate"):
     return p
 
 
+def check_pred_lengths(pred_lengths, pred_token_ids, B: int):
+    """generate's pred_lengths -> a list of B ints in [0, pred_token_ids.shape[1]], or None when it is None or every
+    value equals pred_token_ids.shape[1] (nothing ragged: the shared-position path).  A wrong count, a value out of
+    range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError."""
+    if pred_lengths is None:
+        return None
+    where = "open_musiclm_b200 generate: pred_lengths"
+    if pred_token_ids is None:
+        raise ValueError(f"{where} needs pred_token_ids")
+    if isinstance(pred_lengths, torch.Tensor):
+        if pred_lengths.dtype != torch.int64 or pred_lengths.dim() != 1:
+            raise ValueError(f"{where} must be a list of ints or an int64 tensor of shape [{B}], not a {pred_lengths.dtype} "
+                             f"tensor of shape {list(pred_lengths.shape)}")
+        vals = [int(v) for v in pred_lengths.tolist()]
+    else:
+        vals = list(pred_lengths)
+        for v in vals:
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral):
+                raise ValueError(f"{where} must hold ints, not {v!r}")
+        vals = [int(v) for v in vals]
+    if len(vals) != B:
+        raise ValueError(f"{where} has {len(vals)} values for {B} sequences")
+    n = pred_token_ids.shape[1]
+    for b, v in enumerate(vals):
+        if not 0 <= v <= n:
+            raise ValueError(f"{where}[{b}] = {v} lies outside [0, {n}] (pred_token_ids has {n} time steps)")
+    return None if all(v == n for v in vals) else vals
+
+
 class DecodeSession:
     """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens.
     seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
     self.seeds).  pred_start: position of the predicted sequence's start token in the prompt (_Plan.pos0[-1]); with
-    absolute position embeddings the token at position pos is token pos - pred_start - 1 of that sequence."""
+    absolute position embeddings the token at position pos is token pos - pred_start - 1 of that sequence.
+    ragged (prompts of different lengths): (prompt_len, pos_init, pos_last), B ints each: sequence b's real prompt
+    length, its first decode position and the last position it processes; self.pos is then one position per sequence
+    and n_max the cache capacity.  Otherwise self.pos is one counter for the whole batch, starting at n_prompt."""
 
-    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0):
+    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0, ragged=None,
+                 n_max: Optional[int] = None):
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
         if seeded and eng.h > 16:
@@ -94,7 +136,7 @@ class DecodeSession:
         self.eng, self.B, self.n_prompt, self.n_new, self.seeded = eng, B, n_prompt, n_new, seeded
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
         d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
-        self.n_max = n_prompt + n_new
+        self.n_max = n_prompt + n_new if n_max is None else n_max
         E = lambda *shape, dt=bf: torch.empty(*shape, device=dev, dtype=dt)
         self.cache = [E(B, self.n_max, 128) for _ in range(eng.L)]
         self.conv = [E(B, 2, 2 * Fp, dt=a16) for _ in range(eng.L)]
@@ -106,7 +148,13 @@ class DecodeSession:
         self.tokens = torch.zeros(B, max(n_new, 1), device=dev, dtype=torch.int64)
         self.next_row = torch.zeros(B, device=dev, dtype=torch.int32)
         self.counters = torch.zeros(2, device=dev, dtype=torch.int32)          # [sampled so far, block arrival counter]
-        self.pos = torch.full((1,), n_prompt, device=dev, dtype=torch.int32)   # position the next decode step processes
+        self.ragged = ragged is not None
+        if self.ragged:          # per sequence: the position the next decode step processes, and the last one it will
+            i32 = lambda v: torch.tensor(v, device=dev, dtype=torch.int32)
+            self.prompt_len = torch.tensor(ragged[0], device=dev, dtype=torch.int64)
+            self.pos, self.pos_last = i32(ragged[1]), i32(ragged[2])
+        else:
+            self.pos = torch.full((1,), n_prompt, device=dev, dtype=torch.int32)   # position the next decode step processes
         self.pos_offset = -(pred_start + 1)
         # bias table for every distance the generation can reach (it depends on i - j only)
         N = self.n_max
@@ -135,7 +183,8 @@ class DecodeSession:
         embeddings the predicted sequence's row for its token self.pos - pred_start - 1 (open_musiclm.py:134-136)."""
         eng = self.eng
         if eng.abs_pos:
-            lib.embed_gather_pos(eng.table, self.next_row, self.pos, self.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x)
+            lib.embed_gather_pos(eng.table, self.next_row, self.pos, self.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x,
+                                 ragged=self.ragged)
         else:
             lib.embed_gather(eng.table, self.next_row, x)
 
@@ -153,7 +202,7 @@ class DecodeSession:
             lib.skinny_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"])
             lib.skinny_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1)
             lib.attn_decode(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
-                            self.n_max, self.o, h)
+                            self.n_max, self.o, h, ragged=self.ragged)
             lib.skinny_gemm(self.o, pk["wo_b"], xm, addend=xa)
             lib.skinny_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]])
             lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
@@ -174,7 +223,7 @@ class DecodeSession:
             lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws, invariant=inv)
             lib.decode_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1, ws=ws, invariant=inv)
             lib.attn_decode_mqa(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
-                                self.n_max, self.o, h, ws=ws)
+                                self.n_max, self.o, h, ws=ws, ragged=self.ragged)
             lib.decode_gemm(self.o, pk["wo_b"], xm, addend=xa, ws=ws, invariant=inv)
             lib.decode_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]], ws=ws, invariant=inv)
             lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
@@ -189,7 +238,9 @@ class DecodeSession:
         q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
         row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
         lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                   self.counters, self.pos if bump_pos else None, self.B, seeds=self.seeds, top_p=top_p)
+                   self.counters, self.pos if bump_pos and not self.ragged else None, self.B, seeds=self.seeds, top_p=top_p)
+        if bump_pos and self.ragged:
+            lib.decode_advance_pos(self.pos, self.pos_last)
 
     def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True, top_p=None):
         """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
@@ -239,7 +290,7 @@ class TokenConditionedTransformerWrapper(nn.Module):
     def generate(self, *, conditioning_token_ids: List[torch.Tensor], pred_token_ids: Optional[torch.Tensor] = None,
                  max_time_steps=512, filter_thres=0.9, temperature=1., include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, allow_eos_in_output=False, uniform_noise: Optional[torch.Tensor] = None,
-                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, top_p=None, **kwargs):
+                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, top_p=None, pred_lengths=None, **kwargs):
         """Same contract as open_musiclm.py:253-326.  uniform_noise (optional, [n_sampled, b, codebook+1] in (0, 1)):
         the uniform draws behind the Gumbel noise, one slice per sampled token in order — parity runs pass the stream
         torch's default CPU generator would have produced; by default the noise comes from a device Philox stream keyed
@@ -267,12 +318,28 @@ class TokenConditionedTransformerWrapper(nn.Module):
         without top_p.  N depends only on the row, so seeded generation stays independent of the batch.  None or 1.0:
         no nucleus filtering, bit-identical to a call without top_p.  Any other value must lie in (0, 1); NaN, a bool or
         an out-of-range value raises ValueError before anything runs (Engine.seed untouched).
+        pred_lengths (optional, prefixes of different lengths in one batch): one int per row (a list, or an int64 tensor
+        of shape [b]); pred_lengths[r] is the number of leading time steps of pred_token_ids[r] that are real, a whole
+        number in [0, pred_token_ids.shape[1]].  The steps after it are padding and are never read, whatever they hold
+        (-1 included).  Row r is then generated exactly as a call with that row alone and its first pred_lengths[r]
+        steps as pred_token_ids would generate it: (max_time_steps - pred_lengths[r]) * q sampled tokens after its own
+        prefix, eos masking per row, the output [b, max(max_time_steps, max(pred_lengths)), q] (rows shorter than that,
+        which only happens when a prefix is longer than max_time_steps, end in -1).  The decode loop runs as many steps
+        as the row with the most tokens to sample; a row that has all its tokens keeps its position and its further
+        samples are discarded.  Sample index t of a row is its own t-th sampled token: with seeds, row r's tokens
+        depend only on its conditioning, its real prefix, seeds[r] and the sampling arguments, on both decode paths;
+        uniform_noise is [max over rows of n_new, b, codebook+1], row r using its first n_new slices.  With absolute
+        position embeddings the IndexError check above applies per row, to the rows that sample.  A wrong count, a value
+        out of range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError before anything
+        runs (Engine.seed untouched).  None, or every value equal to pred_token_ids.shape[1]: exactly the call without
+        it.  trace_logits then holds every row's logits at every step; a row past its last token holds discarded values.
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
         if seeds is not None and uniform_noise is not None:
             raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
         top_p = check_top_p(top_p)
+        lengths = check_pred_lengths(pred_lengths, pred_token_ids, conditioning_token_ids[0].shape[0])  # None: one length
         m, eng = self.transformer, self.transformer.engine
         S = len(self.token_sequences)
         assert len(conditioning_token_ids) == S - 1
@@ -281,6 +348,9 @@ class TokenConditionedTransformerWrapper(nn.Module):
         q = info.num_quantizers
         init_step = pred_token_ids.shape[1] if pred_token_ids is not None else 0                    # :276
         n_new = max(0, (max_time_steps - init_step) * q)
+        if lengths is not None:
+            n_new_b = [max(0, (max_time_steps - n) * q) for n in lengths]                           # per row, :276
+            n_new = max(n_new_b)
         if eng.abs_pos and n_new > 0:
             # the reference looks up arange(len) in each sequence's nn.Embedding(max_absolute_position_embeddings)
             lim = eng.max_abs_pos
@@ -289,10 +359,16 @@ class TokenConditionedTransformerWrapper(nn.Module):
                 if n > lim:
                     raise IndexError(f"open_musiclm_b200 generate: conditioning sequence {s} has {n} tokens but "
                                      f"max_absolute_position_embeddings is {lim}")
-            n_pre = pred_token_ids.numel() // B if pred_token_ids is not None else 0
-            if n_pre + n_new - 1 > lim:
-                raise IndexError(f"open_musiclm_b200 generate: the predicted sequence reaches {n_pre + n_new - 1} tokens "
-                                 f"({n_pre} given + {n_new} sampled - 1) but max_absolute_position_embeddings is {lim}")
+            if lengths is None:
+                n_pre = pred_token_ids.numel() // B if pred_token_ids is not None else 0
+                if n_pre + n_new - 1 > lim:
+                    raise IndexError(f"open_musiclm_b200 generate: the predicted sequence reaches {n_pre + n_new - 1} tokens "
+                                     f"({n_pre} given + {n_new} sampled - 1) but max_absolute_position_embeddings is {lim}")
+            else:
+                for b, (n, k) in enumerate(zip(lengths, n_new_b)):          # only rows that sample feed tokens back
+                    if k > 0 and n * q + k - 1 > lim:
+                        raise IndexError(f"open_musiclm_b200 generate: the predicted sequence of row {b} reaches {n * q + k - 1} "
+                                         f"tokens ({n * q} given + {k} sampled - 1) but max_absolute_position_embeddings is {lim}")
         was_training = m.training
         m.eval()
         dev = eng.dev
@@ -305,29 +381,50 @@ class TokenConditionedTransformerWrapper(nn.Module):
         else:
             prefix = torch.empty(B, 0, device=dev, dtype=torch.int64)
         seed_vals = seeds_tensor(seeds, B, dev) if seeds is not None else None
+        if lengths is not None:
+            # the prompt: the prefixes cut to the longest real prefix of a row that samples (a row that samples nothing
+            # takes part cut to it), right-padded with token 0.  The predicted sequence comes last, so causal attention
+            # keeps every real position away from the padding and the prefill runs unchanged.
+            n_real = torch.tensor(lengths, device=dev, dtype=torch.int64)[:, None] * q
+            Lp = max([n for n, k in zip(lengths, n_new_b) if k > 0], default=0)
+            L_eff = [min(n, Lp) for n in lengths]
+            prompt = prefix[:, :Lp * q].masked_fill(torch.arange(Lp * q, device=dev)[None] >= n_real.clamp(max=Lp * q), 0)
+        else:
+            prompt = prefix
         if n_new > 0:
-            ids = cond + [prefix]
+            ids = cond + [prompt]
             _, src_row, key_mask, _, n_tok = lib.token_plan(
                 ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
                 append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
             pl = eng.plan(B, n_tok)
-            sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1])
+            if lengths is None:
+                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1])
+            else:
+                # per row: real prompt length, last position the row processes (a row with all its tokens stays there),
+                # first decode position; the cache holds the longest prompt and every row's new positions
+                P = [pl.pos0[-1] + 1 + n * q for n in L_eff]
+                pos_last = [p + max(k, 1) - 2 for p, k in zip(P, n_new_b)]
+                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1],
+                                     ragged=(P, [min(p, e) for p, e in zip(P, pos_last)], pos_last),
+                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]))
             if seed_vals is not None:
                 sess.seeds.copy_(seed_vals)
             ws = eng.workspace(pl, False)
             eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_Capture(sess))
             # logits of the prompt's last position: final sequence, position p_last = its token count, head p_last mod q
+            # (per row: its own last real position; every prefix is whole time steps, so the head is the same)
             p_last = n_tok[-1]
             gi = next(i for i, (s, qi, cnt, base) in enumerate(pl.groups) if s == S - 1 and qi == p_last % q)
             cnt = pl.groups[gi][2]
-            rows = torch.arange(B, device=dev) * cnt + p_last // q
+            last = p_last // q if lengths is None else torch.tensor(L_eff, device=dev)
+            rows = torch.arange(B, device=dev) * cnt + last
             sess.logits[:, :eng.Cp[S - 1]].copy_(ws["logits"][gi][rows])
             top_k = max(int((1 - filter_thres) * (info.codebook_size + 1)), 1)                      # utils.py:80
             uni = None
             if uniform_noise is not None:
                 uni = uniform_noise.to(dev, torch.float32).contiguous()
                 assert uni.shape == (n_new, B, info.codebook_size + 1), uni.shape
-            p0 = prefix.shape[1]                                     # flat index of the first sampled token
+            p0 = prompt.shape[1]                                     # flat index of the first sampled token
             allow = lambda p: bool(allow_eos_in_output and (p % q) == q - 1)                        # :311-313
             C = info.codebook_size + 1
             if trace_logits is not None:
@@ -344,9 +441,20 @@ class TokenConditionedTransformerWrapper(nn.Module):
                                          top_p=top_p)
             if seed_vals is None:
                 eng.seed += 1
-            sampled = torch.cat([prefix, sess.tokens[:, :n_new]], 1)
+            new = sess.tokens[:, :n_new]
+        if lengths is None:
+            sampled = torch.cat([prefix, new], 1) if n_new > 0 else prefix
         else:
-            sampled = prefix
+            # row b: its n_real[b] prefix tokens, then its n_new_b[b] samples, then -1 up to the widest row
+            width = max(max_time_steps, max(lengths)) * q
+            col = torch.arange(width, device=dev)[None]
+            n_end = n_real + torch.tensor(n_new_b, device=dev, dtype=torch.int64)[:, None]
+            sampled = torch.full((B, width), -1, device=dev, dtype=torch.int64)
+            sampled[:, :min(width, prefix.shape[1])] = prefix[:, :width]
+            sampled.masked_fill_(col >= n_real, -1)
+            if n_new > 0:
+                sampled = torch.where((col >= n_real) & (col < n_end), new.gather(1, (col - n_real).clamp(0, n_new - 1).expand(B, -1)),
+                                      sampled)
         eos_mask = (sampled == eos).float()                                                         # utils.py:86-93
         if include_eos_in_output:
             eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))

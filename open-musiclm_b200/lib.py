@@ -161,13 +161,16 @@ def embed_gather(table, src_row, x, src_row2=None):
     call("omlm_embed_gather", _p(table), _p(src_row), _p(src_row2), _p(x), _I(M), _I(D), _stream())
 
 
-def embed_gather_pos(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x):
+def embed_gather_pos(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x, ragged=False):
     """x[m] = table[src_row[m]] + table[pos_row_base + pos[0] + pos_offset]; pos: int32 device tensor read by the
-    kernel (so a captured graph uses its current value).  A position outside [0, pos_rows) adds nothing."""
+    kernel (so a captured graph uses its current value).  A position outside [0, pos_rows) adds nothing.
+    ragged: pos holds one position per row, pos[m] (omlm_embed_gather_pos_ragged)."""
     assert pos.dtype == torch.int32 and pos.is_cuda
     M, D = x.shape
-    call("omlm_embed_gather_pos", _p(table), _p(src_row), _p(pos), _I(pos_offset), _I(pos_row_base), _I(pos_rows), _p(x),
-         _I(M), _I(D), _stream())
+    if ragged:
+        _check_row_pos(pos, M)
+    call("omlm_embed_gather_pos_ragged" if ragged else "omlm_embed_gather_pos", _p(table), _p(src_row), _p(pos), _I(pos_offset),
+         _I(pos_row_base), _I(pos_rows), _p(x), _I(M), _I(D), _stream())
 
 
 def embed_scatter_add(dtable, src_row, dx, scale, first=None):
@@ -466,19 +469,38 @@ def decode_gemm(A, W, out, *, prologue=0, gamma=None, rowsum=None, n_real=0, add
          _stream())
 
 
-def attn_decode_mqa(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, ws=None, scale=8.0):
+def _check_row_pos(pos, B):
+    assert pos.dtype == torch.int32 and pos.is_cuda and pos.is_contiguous() and pos.numel() >= B, "ragged: pos needs one int32 per row"
+
+
+def attn_decode_mqa(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, ws=None, scale=8.0, ragged=False):
     """attn_decode's contract with every cached row read once per sequence (omlm_attn_decode_mqa), 1 <= heads <= 16."""
     B = q_raw.shape[0]
+    if ragged:
+        _check_row_pos(pos, B)
     if ws is None:
         ws = DecodeWorkspace(q_raw.device, B, [(1, 8)], max_pos=max_pos, heads=heads)
-    call("omlm_attn_decode_mqa", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(cache), _L(cache.stride(0)), _p(table),
+    call("omlm_attn_decode_mqa_ragged" if ragged else "omlm_attn_decode_mqa", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale),
+         _p(cache), _L(cache.stride(0)), _p(table),
          _I(table.stride(0)), _p(pos), _I(max_pos), _p(out), _I(B), _I(heads), _F(scale), _p(ws.attn), _L(ws.attn.numel() * 4),
          _p(ws.counters), _stream())
 
 
-def attn_decode(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, scale=8.0):
-    call("omlm_attn_decode", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(cache), _L(cache.stride(0)), _p(table),
+def attn_decode(q_raw, kv_raw, q_scale, k_scale, cache, table, pos, max_pos, out, heads, scale=8.0, ragged=False):
+    """One decode step's attention at position pos[0] for every sequence (omlm_attn_decode); ragged: sequence b at its
+    own position pos[b] (omlm_attn_decode_ragged, and likewise for attn_decode_mqa)."""
+    if ragged:
+        _check_row_pos(pos, q_raw.shape[0])
+    call("omlm_attn_decode_ragged" if ragged else "omlm_attn_decode", _p(q_raw), _p(kv_raw), _p(q_scale), _p(k_scale), _p(cache),
+         _L(cache.stride(0)), _p(table),
          _I(table.stride(0)), _p(pos), _I(max_pos), _p(out), _I(q_raw.shape[0]), _I(heads), _F(scale), _stream())
+
+
+def decode_advance_pos(pos, pos_last):
+    """pos[b] += 1 where pos[b] < pos_last[b] (int32 device tensors [B]; omlm_decode_advance_pos)."""
+    assert pos.dtype == pos_last.dtype == torch.int32 and pos.is_contiguous() and pos_last.is_contiguous()
+    assert pos.numel() == pos_last.numel()
+    call("omlm_decode_advance_pos", _p(pos), _p(pos_last), _I(pos.numel()), _stream())
 
 
 def decode_conv_geglu(u_new, state, conv_w, h_out, rowsum):

@@ -19,7 +19,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .decode import TokenConditionedTransformerWrapper, check_top_p
+from .decode import TokenConditionedTransformerWrapper, check_pred_lengths, check_top_p
 from .model import TokenConditionedTransformer
 
 
@@ -57,8 +57,11 @@ def window_seed(seed: int, stage: int, window: int) -> int:
     return splitmix64((int(seed) & _MASK64) ^ splitmix64((stage << 32) | window))
 
 
-def _n_new(pred_token_ids, max_time_steps: int, q: int) -> int:
+def _n_new(pred_token_ids, max_time_steps: int, q: int, lengths=None) -> int:
+    """Sampled tokens of a generate call: with per-row prefix lengths (checked), those of the row that samples most."""
     init = 0 if pred_token_ids is None else pred_token_ids.shape[1]
+    if lengths is not None:
+        init = min(lengths)
     return max(0, (max_time_steps - init) * q)
 
 
@@ -79,7 +82,8 @@ class _Stage(nn.Module):
     def _generate(self, conditioning: List[torch.Tensor], pred, noise: Optional[NoiseStream], **kw):
         q = self.transformer_wrapper.token_sequences[-1].num_quantizers
         if noise is not None:
-            kw["uniform_noise"] = noise.take(_n_new(pred, kw["max_time_steps"], q))
+            lengths = check_pred_lengths(kw.get("pred_lengths"), pred, conditioning[0].shape[0])   # raises before the take
+            kw["uniform_noise"] = noise.take(_n_new(pred, kw["max_time_steps"], q, lengths))
         return self.transformer_wrapper.generate(conditioning_token_ids=conditioning, pred_token_ids=pred, **kw)
 
 
