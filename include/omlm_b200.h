@@ -400,6 +400,19 @@ int omlm_sample_seeded(const float* logits, long ld, int C, int top_k, float tem
 int omlm_sample_nucleus(const float* logits, long ld, int C, int top_k, float temperature, float top_p, int allow_eos,
                         const float* uniform, const unsigned long long* seed, const unsigned long long* seeds, long long* tokens,
                         long tokens_ld, int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
+/* The samplers above with sampling arguments per sequence (a batch whose rows are independent requests, or one prompt
+ * at several settings).  top_k_rows (int [B]), temperature_rows and top_p_rows (float [B]) are optional device arrays;
+ * where one is given, sequence b uses element b, otherwise the scalar top_k / temperature (checked as in omlm_sample).
+ * A row's k is clamped to [1, C]; a row whose top_p lies outside (0, 1), NaN included, is not narrowed to a nucleus.
+ * With top_p_rows the nucleus kernel runs (3 C floats of shared memory instead of 2), without it the plain one; a row
+ * that is not narrowed samples bit-identically to omlm_sample_seeded with its own k and temperature, and a row with
+ * top_p in (0, 1) to omlm_sample_nucleus.  The values reach the arithmetic as the scalar entry points take them, so a
+ * row's token equals the token a call with that row's scalars gives.  Any value in the arrays keeps every access in
+ * bounds.  uniform, seed, seeds, counters and outputs as omlm_sample_seeded. */
+int omlm_sample_rows(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                     const float* temperature_rows, const float* top_p_rows, int allow_eos, const float* uniform,
+                     const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                     int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
 
 #ifdef __cplusplus
 }

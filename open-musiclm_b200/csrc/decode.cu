@@ -494,13 +494,21 @@ decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restric
 // N; a row whose maximum over K is not finite samples over K as the kNucleus = false kernel does.  The uniforms are
 // the ones the false kernel draws for the same class; classes outside N draw none.  Another [C] array in shared memory
 // holds p: 192 KB at C = 16384.
+//
+// Per-row arguments (omlm_sample_rows): when top_k_rows / temperature_rows / top_p_rows is non-null, block b takes its
+// k, T or top_p from element b instead of the scalar.  A row's k is clamped to [1, C], and a row whose top_p lies
+// outside (0, 1) (NaN included) skips the nucleus narrowing, so that row samples exactly as the kNucleus = false kernel
+// (the narrowing at top_p = 1 would still drop classes whose p underflows to 0).  Every shared and global access stays
+// inside its array for any value read, and every loop has a fixed trip count.
 template <bool kNucleus>
 __global__ void __launch_bounds__(256)
 sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float temperature, int allow_eos,
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
               const unsigned long long* __restrict__ seeds,
               long long* __restrict__ tokens, long tokens_ld, int* __restrict__ next_row, int row_offset,
-              int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B, float top_p) {
+              int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B, float top_p,
+              const int* __restrict__ top_k_rows, const float* __restrict__ temperature_rows,
+              const float* __restrict__ top_p_rows) {
   extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys (kNucleus: then [C] weights p)
   float* lg = sm_l;
   uint32_t* key = reinterpret_cast<uint32_t*>(sm_l + C);
@@ -508,6 +516,11 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   __shared__ int ri[8];
   __shared__ uint32_t s_thr;
   const int b = blockIdx.x, tid = threadIdx.x;
+  if (top_k_rows != nullptr) k = min(max(top_k_rows[b], 1), C);
+  if (temperature_rows != nullptr) temperature = temperature_rows[b];
+  if constexpr (kNucleus) {
+    if (top_p_rows != nullptr) top_p = top_p_rows[b];
+  }
   const int step = *step_ptr;
   // Sort keys: an order-preserving map float -> uint, with -0.0 mapped like +0.0 so that the two zeros are equal values
   // and the tie rule below (lower index wins) applies between them, as it does in torch.topk's comparison.
@@ -567,7 +580,7 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     __syncthreads();
     mx = s_mx[0];
     for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_mx[w]);
-    if (isfinite(mx)) {                                           // the same on every thread of the block
+    if (isfinite(mx) && top_p > 0.f && top_p < 1.f) {             // the same on every thread of the block
       for (int c = tid; c < C; c += 256) p[c] = isnan(lg[c]) ? 0.f : expf((lg[c] - mx) / temperature);
       __syncthreads();
       // mass of the keys >= cand, in the fixed order; every thread gets the same value (a + b == b + a in the tree)
@@ -660,8 +673,12 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
 template <bool kNucleus>
 static int launch_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                          const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
-                         int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float top_p, void* stream) {
-  OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384 && temperature > 0.f && top_k >= 1 && top_k <= C, "sample: bad arguments");
+                         int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float top_p, void* stream,
+                         const int* top_k_rows = nullptr, const float* temperature_rows = nullptr,
+                         const float* top_p_rows = nullptr) {
+  OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384, "sample: bad arguments");
+  OMLM_CHECK_ARG(temperature_rows != nullptr || temperature > 0.f, "sample: temperature %g", static_cast<double>(temperature));
+  OMLM_CHECK_ARG(top_k_rows != nullptr || (top_k >= 1 && top_k <= C), "sample: top_k %d outside [1, %d]", top_k, C);
   OMLM_CHECK_ARG(seeds == nullptr || uniform == nullptr, "sample: per-sequence seeds and supplied uniforms exclude each other");
   // 128 KB (nucleus: 192 KB) at C = 16384: above the 48 KB a launch gets without the opt-in
   const int smem = (kNucleus ? 3 : 2) * C * 4;
@@ -671,7 +688,8 @@ static int launch_sample(const float* logits, long ld, int C, int top_k, float t
     configured = smem;
   }
   OMLM_KLAUNCH((sample_kernel<kNucleus>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature,
-               allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p);
+               allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p, top_k_rows,
+               temperature_rows, top_p_rows);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
@@ -817,6 +835,17 @@ int omlm_sample_nucleus(const float* logits, long ld, int C, int top_k, float te
   OMLM_CHECK_ARG(top_p > 0.f && top_p < 1.f, "sample_nucleus: top_p %g outside (0, 1)", static_cast<double>(top_p));
   return omlm::launch_sample<true>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
                                    row_offset, step_ptr, pos_ptr, B, top_p, stream);
+}
+
+int omlm_sample_rows(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                     const float* temperature_rows, const float* top_p_rows, int allow_eos, const float* uniform,
+                     const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                     int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream) {
+  if (top_p_rows != nullptr)
+    return omlm::launch_sample<true>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
+                                     row_offset, step_ptr, pos_ptr, B, 1.f, stream, top_k_rows, temperature_rows, top_p_rows);
+  return omlm::launch_sample<false>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
+                                    row_offset, step_ptr, pos_ptr, B, 1.f, stream, top_k_rows, temperature_rows, nullptr);
 }
 
 int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,

@@ -22,7 +22,12 @@ stated in `generate`'s docstring.
 Prefixes of different lengths (`generate(pred_lengths=...)`) run the same step with one position per sequence
 (DecodeSession.pos [B], the _ragged attention and gather entry points, omlm_decode_advance_pos in place of the
 sampler's position bump); every row gets what it would get alone (DESIGN section 4).
+
+Sampling arguments per row (temperature, filter_thres, top_p, max_time_steps given as one value per row) reach the
+sampler as device arrays (DecodeSession.rows, omlm_sample_rows); rows that sample different numbers of tokens take the
+per-row-position path above.  Every row again gets what it would get alone (DESIGN section 4).
 """
+import math
 import numbers
 from typing import List, Optional, Sequence
 
@@ -118,6 +123,71 @@ def check_pred_lengths(pred_lengths, pred_token_ids, B: int):
     return None if all(v == n for v in vals) else vals
 
 
+def _row_values(value, B: int, name: str, integer: bool):
+    """value's per-row form (a list or tuple of B values, or a 1-D tensor of B values: int64 when integer, floating
+    point otherwise) -> a list of B Python values; None for a single value (a 0-d tensor included)."""
+    where = f"open_musiclm_b200 generate: {name}"
+    if isinstance(value, torch.Tensor):
+        if value.dim() == 0:
+            return None
+        if value.dim() != 1 or (value.dtype != torch.int64 if integer else not value.is_floating_point()):
+            raise ValueError(f"{where} per row must be a 1-D {'int64' if integer else 'floating-point'} tensor of shape [{B}], not a "
+                             f"{value.dtype} tensor of shape {list(value.shape)}")
+        vals = value.tolist()
+    elif isinstance(value, (list, tuple)):
+        vals = list(value)
+    else:
+        return None
+    if len(vals) != B:
+        raise ValueError(f"{where} has {len(vals)} values for {B} sequences")
+    return vals
+
+
+def _collapse(vals):
+    return vals[0] if all(v == vals[0] for v in vals) else vals
+
+
+def check_sampling_rows(B: int, C: int, temperature, filter_thres, top_p, max_time_steps):
+    """generate's temperature, filter_thres, top_p and max_time_steps, each one value or one value per row ->
+    (temperature, top_k, top_p, max_time_steps): a single value each (top_k None: filter_thres is a single value, unchecked;
+    top_p through check_top_p; temperature and max_time_steps as given), or a list of B checked values (floats, the
+    top-k sizes max(int((1 - filter_thres) C), 1), floats or None, ints).  A list whose values are all equal collapses to that value.  A wrong count, a bool or a non-number,
+    a temperature that is not finite and > 0, a filter_thres that is not finite or gives k > C, a bad top_p element or
+    a max_time_steps element that is not a non-negative int raises ValueError naming the keyword."""
+    def number(name, v, integer=False):
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral if integer else numbers.Real):
+            raise ValueError(f"open_musiclm_b200 generate: {name} must hold {'ints' if integer else 'numbers'}, not {v!r}")
+        return int(v) if integer else float(v)
+
+    temps = _row_values(temperature, B, "temperature", False)
+    if temps is not None:
+        temps = [number("temperature", v) for v in temps]
+        for b, t in enumerate(temps):
+            if not (math.isfinite(t) and t > 0):
+                raise ValueError(f"open_musiclm_b200 generate: temperature[{b}] = {t!r} is not a finite number > 0")
+        temperature = _collapse(temps)
+    thres = _row_values(filter_thres, B, "filter_thres", False)
+    top_k = None
+    if thres is not None:
+        top_k = []
+        for b, t in enumerate(number("filter_thres", v) for v in thres):
+            k = max(int((1 - t) * C), 1) if math.isfinite(t) else None                           # utils.py:80
+            if k is None or k > C:
+                raise ValueError(f"open_musiclm_b200 generate: filter_thres[{b}] = {t!r} does not give a top-k size in [1, {C}]")
+            top_k.append(k)
+        top_k = _collapse(top_k)
+    ps = _row_values(top_p, B, "top_p", False)
+    top_p = check_top_p(top_p) if ps is None else _collapse([check_top_p(p) for p in ps])
+    steps = _row_values(max_time_steps, B, "max_time_steps", True)
+    if steps is not None:
+        steps = [number("max_time_steps", v, integer=True) for v in steps]
+        for b, n in enumerate(steps):
+            if n < 0:
+                raise ValueError(f"open_musiclm_b200 generate: max_time_steps[{b}] = {n} is negative")
+        max_time_steps = _collapse(steps)
+    return temperature, top_k, top_p, max_time_steps
+
+
 class DecodeSession:
     """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens.
     seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
@@ -125,10 +195,12 @@ class DecodeSession:
     absolute position embeddings the token at position pos is token pos - pred_start - 1 of that sequence.
     ragged (prompts of different lengths): (prompt_len, pos_init, pos_last), B ints each: sequence b's real prompt
     length, its first decode position and the last position it processes; self.pos is then one position per sequence
-    and n_max the cache capacity.  Otherwise self.pos is one counter for the whole batch, starting at n_prompt."""
+    and n_max the cache capacity.  Otherwise self.pos is one counter for the whole batch, starting at n_prompt.
+    rows (sampling arguments per sequence): (top_k, temperature, top_p), B values each (top_p None: no nucleus);
+    self.rows then holds them as device arrays, which every sample() reads instead of its scalar arguments."""
 
     def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0, ragged=None,
-                 n_max: Optional[int] = None):
+                 n_max: Optional[int] = None, rows=None):
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
         if seeded and eng.h > 16:
@@ -156,6 +228,13 @@ class DecodeSession:
         else:
             self.pos = torch.full((1,), n_prompt, device=dev, dtype=torch.int32)   # position the next decode step processes
         self.pos_offset = -(pred_start + 1)
+        self.rows = None
+        if rows is not None:     # filled here, before any graph capture; top_p_rows only when some row has a nucleus
+            k, t, p = rows
+            self.rows = dict(top_k_rows=torch.tensor(k, device=dev, dtype=torch.int32),
+                             temperature_rows=torch.tensor(t, device=dev, dtype=f32),
+                             top_p_rows=None if all(v is None for v in p) else
+                             torch.tensor([1.0 if v is None else v for v in p], device=dev, dtype=f32))
         # bias table for every distance the generation can reach (it depends on i - j only)
         N = self.n_max
         self.rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, Hr, dt=f32) for _ in range(3)], rp_a=[E(N, Hr, dt=f32) for _ in range(3)],
@@ -237,14 +316,22 @@ class DecodeSession:
         S = len(eng.seqs) - 1
         q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
         row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
-        lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                   self.counters, self.pos if bump_pos and not self.ragged else None, self.B, seeds=self.seeds, top_p=top_p)
+        pos = self.pos if bump_pos and not self.ragged else None
+        if self.rows is not None:        # per-row arguments: top_k, temperature and top_p are not used
+            lib.sample(self.logits, eng.C[S], 1, 1.0, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
+                       self.counters, pos, self.B, seeds=self.seeds, **self.rows)
+        else:
+            lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
+                       self.counters, pos, self.B, seeds=self.seeds, top_p=top_p)
         if bump_pos and self.ragged:
             lib.decode_advance_pos(self.pos, self.pos_last)
 
     def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True, top_p=None):
         """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
-        key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p)
+        if self.rows is not None:        # the arrays' contents are read at replay; only the kernel choice is captured
+            key = (qi, qi_next, "rows", bool(allow_eos_next), uniform is not None, self.seeded, self.rows["top_p_rows"] is not None)
+        else:
+            key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p)
         g = self._graphs.get(key)
         if g is None or not use_graph:
             body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True, top_p))
@@ -333,24 +420,43 @@ class TokenConditionedTransformerWrapper(nn.Module):
         out of range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError before anything
         runs (Engine.seed untouched).  None, or every value equal to pred_token_ids.shape[1]: exactly the call without
         it.  trace_logits then holds every row's logits at every step; a row past its last token holds discarded values.
+        Sampling arguments per row: temperature, filter_thres and top_p each take one value for every row (as above) or
+        one per row, a list or tuple of b values or a 1-D floating-point tensor of shape [b] (top_p: None or 1 in a list,
+        1.0 in a tensor, means no nucleus for that row); max_time_steps likewise, as ints or an int64 tensor.  Row r is
+        then generated exactly as a call with that row alone would generate it with the scalars temperature=float(v[r]),
+        filter_thres=float(v[r]), top_p=v[r], max_time_steps=int(v[r]), its own conditioning, real prefix and seed, and
+        every other argument shared: n_new_r = max(0, (max_time_steps_r - len_r) q) sampled tokens, the t-th with
+        sample index t, eos masking per row; the output is [b, W, q] with W = max over rows of max(max_time_steps_r,
+        len_r), rows ending in -1 as with pred_lengths, and uniform_noise is [max_r n_new_r, b, codebook+1].  Rows that
+        sample different numbers of tokens run the pred_lengths path (a row with all its tokens stops).  A wrong count,
+        a bool or a non-number, a temperature that is not finite and > 0, a filter_thres that is not finite or whose top-k
+        size exceeds codebook+1, a top_p element outside (0, 1] or a negative max_time_steps raises ValueError before
+        anything runs (Engine.seed untouched).  A list of equal values is that single value, so with all four equal and
+        no ragged pred_lengths the call is exactly the single-value call.
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
         if seeds is not None and uniform_noise is not None:
             raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
-        top_p = check_top_p(top_p)
-        lengths = check_pred_lengths(pred_lengths, pred_token_ids, conditioning_token_ids[0].shape[0])  # None: one length
+        B = conditioning_token_ids[0].shape[0]
+        info, eos = self.token_sequences[-1], self.eos_ids[-1]
+        C = info.codebook_size + 1
+        temperature, top_k, top_p, max_time_steps = check_sampling_rows(B, C, temperature, filter_thres, top_p, max_time_steps)
+        lengths = check_pred_lengths(pred_lengths, pred_token_ids, B)                               # None: one length
+        per_row = any(isinstance(v, list) for v in (temperature, top_k, top_p))     # sampled from per-row arrays
         m, eng = self.transformer, self.transformer.engine
         S = len(self.token_sequences)
         assert len(conditioning_token_ids) == S - 1
-        B = conditioning_token_ids[0].shape[0]
-        info, eos = self.token_sequences[-1], self.eos_ids[-1]
         q = info.num_quantizers
         init_step = pred_token_ids.shape[1] if pred_token_ids is not None else 0                    # :276
-        n_new = max(0, (max_time_steps - init_step) * q)
-        if lengths is not None:
-            n_new_b = [max(0, (max_time_steps - n) * q) for n in lengths]                           # per row, :276
+        steps_b = max_time_steps if isinstance(max_time_steps, list) else [max_time_steps] * B
+        if isinstance(max_time_steps, list) or lengths is not None:
+            n_new_b = [max(0, (t - n) * q) for t, n in zip(steps_b, lengths or [init_step] * B)]   # per row, :276
+            if lengths is None and len(set(n_new_b)) > 1:
+                lengths = [init_step] * B        # rows that sample different numbers of tokens: the per-row-position path
             n_new = max(n_new_b)
+        else:
+            n_new = max(0, (max_time_steps - init_step) * q)
         if eng.abs_pos and n_new > 0:
             # the reference looks up arange(len) in each sequence's nn.Embedding(max_absolute_position_embeddings)
             lim = eng.max_abs_pos
@@ -397,8 +503,13 @@ class TokenConditionedTransformerWrapper(nn.Module):
                 ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
                 append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
             pl = eng.plan(B, n_tok)
+            if top_k is None:
+                top_k = max(int((1 - filter_thres) * C), 1)                                          # utils.py:80
+            rows = None
+            if per_row:                          # every argument as B values (a single value repeated)
+                rows = tuple(v if isinstance(v, list) else [v] * B for v in (top_k, temperature, top_p))
             if lengths is None:
-                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1])
+                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1], rows=rows)
             else:
                 # per row: real prompt length, last position the row processes (a row with all its tokens stays there),
                 # first decode position; the cache holds the longest prompt and every row's new positions
@@ -406,7 +517,7 @@ class TokenConditionedTransformerWrapper(nn.Module):
                 pos_last = [p + max(k, 1) - 2 for p, k in zip(P, n_new_b)]
                 sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1],
                                      ragged=(P, [min(p, e) for p, e in zip(P, pos_last)], pos_last),
-                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]))
+                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]), rows=rows)
             if seed_vals is not None:
                 sess.seeds.copy_(seed_vals)
             ws = eng.workspace(pl, False)
@@ -419,14 +530,12 @@ class TokenConditionedTransformerWrapper(nn.Module):
             last = p_last // q if lengths is None else torch.tensor(L_eff, device=dev)
             rows = torch.arange(B, device=dev) * cnt + last
             sess.logits[:, :eng.Cp[S - 1]].copy_(ws["logits"][gi][rows])
-            top_k = max(int((1 - filter_thres) * (info.codebook_size + 1)), 1)                      # utils.py:80
             uni = None
             if uniform_noise is not None:
                 uni = uniform_noise.to(dev, torch.float32).contiguous()
                 assert uni.shape == (n_new, B, info.codebook_size + 1), uni.shape
             p0 = prompt.shape[1]                                     # flat index of the first sampled token
             allow = lambda p: bool(allow_eos_in_output and (p % q) == q - 1)                        # :311-313
-            C = info.codebook_size + 1
             if trace_logits is not None:
                 trace_logits.append(sess.logits[:, :C].clone())
             sess.sample(p0 % q, top_k, temperature, allow(p0), uni, eng.seed, bump_pos=False, top_p=top_p)
@@ -446,7 +555,7 @@ class TokenConditionedTransformerWrapper(nn.Module):
             sampled = torch.cat([prefix, new], 1) if n_new > 0 else prefix
         else:
             # row b: its n_real[b] prefix tokens, then its n_new_b[b] samples, then -1 up to the widest row
-            width = max(max_time_steps, max(lengths)) * q
+            width = max(max(t, n) for t, n in zip(steps_b, lengths)) * q
             col = torch.arange(width, device=dev)[None]
             n_end = n_real + torch.tensor(n_new_b, device=dev, dtype=torch.int64)[:, None]
             sampled = torch.full((B, width), -1, device=dev, dtype=torch.int64)

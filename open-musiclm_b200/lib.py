@@ -511,10 +511,21 @@ def decode_conv_geglu(u_new, state, conv_w, h_out, rowsum):
 
 
 def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B, seeds=None,
-           top_p=None):
+           top_p=None, top_k_rows=None, temperature_rows=None, top_p_rows=None):
     """seeds: int64 [B] device tensor of per-sequence seeds (raw 64-bit patterns) -> omlm_sample_seeded.
     top_p: nucleus sampling (omlm_sample_nucleus, which rejects values outside (0, 1)); None or 1.0 samples over the
-    whole top-k set through omlm_sample / omlm_sample_seeded."""
+    whole top-k set through omlm_sample / omlm_sample_seeded.
+    top_k_rows (int32 [B]), temperature_rows, top_p_rows (float32 [B]): per-sequence arguments (omlm_sample_rows); each
+    one given replaces its scalar; top_p_rows selects the nucleus kernel and is the only way to pass top_p with them."""
+    if top_k_rows is not None or temperature_rows is not None or top_p_rows is not None:
+        assert top_p is None or top_p == 1.0, "per-row sampling takes its nucleus masses through top_p_rows"
+        for t, dt in ((top_k_rows, torch.int32), (temperature_rows, torch.float32), (top_p_rows, torch.float32)):
+            assert t is None or (t.dtype == dt and t.is_cuda and t.is_contiguous() and t.numel() >= B)
+        assert seeds is None or (seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B)
+        call("omlm_sample_rows", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _p(top_k_rows), _F(temperature),
+             _p(temperature_rows), _p(top_p_rows), _I(int(allow_eos)), _p(uniform), _p(seed), _p(seeds), _p(tokens),
+             _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
+        return
     if top_p is not None and top_p != 1.0:
         assert seeds is None or (seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B)
         call("omlm_sample_nucleus", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _F(top_p),
