@@ -159,6 +159,10 @@ int omlm_embed_gather_pos(const float* table, const int* src_row, const int* pos
  * pos_offset, pos a device int array [M].  The shared-position entry point above keeps its single read. */
 int omlm_embed_gather_pos_ragged(const float* table, const int* src_row, const int* pos, int pos_offset, int pos_row_base,
                                  int pos_rows, float* x, int M, int D, void* stream);
+/* omlm_embed_gather_pos_ragged with one predicted-sequence offset per row as well: p = pos[m] + pos_offset[m] (pos and
+ * pos_offset device int arrays [M]), for the rows of a generation session, whose conditioning lengths differ. */
+int omlm_embed_gather_pos_rows(const float* table, const int* src_row, const int* pos, const int* pos_offset, int pos_row_base,
+                               int pos_rows, float* x, int M, int D, void* stream);
 int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, int M, int D,
                            float scale, void* stream);
 
@@ -413,6 +417,17 @@ int omlm_sample_rows(const float* logits, long ld, int C, int top_k, const int* 
                      const float* temperature_rows, const float* top_p_rows, int allow_eos, const float* uniform,
                      const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
                      int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, void* stream);
+/* omlm_sample_rows with one sample index per sequence, for a generation session whose rows joined at different steps:
+ * sequence b reads t = step_rows[b] (device int [B]) in place of the shared counter, draws from Philox on the counter
+ * (c, t, 0, 0x5eed) under seeds[b] (required; no supplied uniforms), writes tokens[b, t] and next_row[b], and sets
+ * step_rows[b] = t + 1.  A sequence with t outside [0, min(n_rows[b], tokens_ld)) (n_rows: device int [B], the number
+ * of tokens sequence b samples) writes nothing and keeps t.  Positions are not advanced (omlm_decode_advance_pos).
+ * Per-row arrays, kernel choice and arithmetic as omlm_sample_rows: with every t equal, its tokens are bit-identical
+ * to omlm_sample_rows with seeds at that sample index. */
+int omlm_sample_rows_indexed(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                             const float* temperature_rows, const float* top_p_rows, int allow_eos, const unsigned long long* seeds,
+                             long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_rows, const int* n_rows,
+                             int B, void* stream);
 
 #ifdef __cplusplus
 }

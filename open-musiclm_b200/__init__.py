@@ -7,6 +7,7 @@ Only what the TokenConditionedTransformer training path needs lives here:
   model.py    drop-in `TokenConditionedTransformer`, `create_{semantic,coarse,fine}_transformer`
   trainer.py  H100-native SingleStageTrainer step loop (`HotPathTrainer`)
   decode.py   `TokenConditionedTransformerWrapper.generate`: KV-cache autoregressive decoding
+  session.py  `GenerationSession`: continuous batching, rows joining and leaving a running decode
   stages.py   `SemanticStage` / `CoarseStage` / `FineStage` and the windowed three-stage `MusicLM` generation
 """
 __version__ = "0.1.0"
@@ -15,4 +16,5 @@ from .model import (TokenConditionedTransformer, TokenSequenceInfo, create_coars
                     create_fine_transformer, create_semantic_transformer)
 from .trainer import HotPathTrainer  # noqa: F401
 from .decode import TokenConditionedTransformerWrapper  # noqa: F401
+from .session import GenerationSession  # noqa: F401
 from .stages import CoarseStage, FineStage, MusicLM, NoiseStream, SemanticStage, prepare_audio  # noqa: F401

@@ -500,7 +500,13 @@ decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restric
 // outside (0, 1) (NaN included) skips the nucleus narrowing, so that row samples exactly as the kNucleus = false kernel
 // (the narrowing at top_p = 1 would still drop classes whose p underflows to 0).  Every shared and global access stays
 // inside its array for any value read, and every loop has a fixed trip count.
-template <bool kNucleus>
+//
+// Per-row sample index (kRowStep, omlm_sample_rows_indexed: the rows of a generation session, which joined at different
+// steps): block b reads its own sample index t = step_ptr[b] instead of the shared counter and uses it for the Philox
+// counter and the output column.  A row with t outside [0, min(n_rows[b], tokens_ld)) -- it has all its samples, or its
+// slot is free -- writes nothing.  Otherwise block b writes its token and sets step_ptr[b] = t + 1 itself: no block
+// reads another's index, so there is no arrival counter, and pos_ptr is unused (omlm_decode_advance_pos moves positions).
+template <bool kNucleus, bool kRowStep>
 __global__ void __launch_bounds__(256)
 sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float temperature, int allow_eos,
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
@@ -508,7 +514,7 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
               long long* __restrict__ tokens, long tokens_ld, int* __restrict__ next_row, int row_offset,
               int* __restrict__ step_ptr, int* __restrict__ pos_ptr, int B, float top_p,
               const int* __restrict__ top_k_rows, const float* __restrict__ temperature_rows,
-              const float* __restrict__ top_p_rows) {
+              const float* __restrict__ top_p_rows, const int* __restrict__ n_rows) {
   extern __shared__ float sm_l[];          // [C] logits, then [C] sort keys (kNucleus: then [C] weights p)
   float* lg = sm_l;
   uint32_t* key = reinterpret_cast<uint32_t*>(sm_l + C);
@@ -521,7 +527,10 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   if constexpr (kNucleus) {
     if (top_p_rows != nullptr) top_p = top_p_rows[b];
   }
-  const int step = *step_ptr;
+  const int step = kRowStep ? step_ptr[b] : *step_ptr;
+  if constexpr (kRowStep) {
+    if (step < 0 || step >= n_rows[b] || step >= tokens_ld) return;     // the same on every thread of the block
+  }
   // Sort keys: an order-preserving map float -> uint, with -0.0 mapped like +0.0 so that the two zeros are equal values
   // and the tie rule below (lower index wins) applies between them, as it does in torch.topk's comparison.
   // A NaN logit maps above +inf (or below -inf for a negative NaN), so it can take a top-k slot, but its noisy score
@@ -654,6 +663,10 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     tokens[b * tokens_ld + step] = best_i;
     next_row[b] = row_offset + best_i;
   }
+  if constexpr (kRowStep) {
+    if (tid == 0) step_ptr[b] = step + 1;                       // every thread read it before the first barrier
+    return;
+  }
   // the counters advance once per launch, after every block has read them: last block to finish does it
   __shared__ bool last;
   __threadfence();
@@ -670,26 +683,28 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   }
 }
 
-template <bool kNucleus>
+template <bool kNucleus, bool kRowStep = false>
 static int launch_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                          const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
                          int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float top_p, void* stream,
                          const int* top_k_rows = nullptr, const float* temperature_rows = nullptr,
-                         const float* top_p_rows = nullptr) {
+                         const float* top_p_rows = nullptr, const int* n_rows = nullptr) {
   OMLM_CHECK_ARG(B >= 1 && C >= 2 && C <= 16384, "sample: bad arguments");
   OMLM_CHECK_ARG(temperature_rows != nullptr || temperature > 0.f, "sample: temperature %g", static_cast<double>(temperature));
   OMLM_CHECK_ARG(top_k_rows != nullptr || (top_k >= 1 && top_k <= C), "sample: top_k %d outside [1, %d]", top_k, C);
   OMLM_CHECK_ARG(seeds == nullptr || uniform == nullptr, "sample: per-sequence seeds and supplied uniforms exclude each other");
+  OMLM_CHECK_ARG(!kRowStep || (seeds != nullptr && step_ptr != nullptr && n_rows != nullptr),
+                 "sample_rows_indexed: seeds, step_rows and n_rows are required");
   // 128 KB (nucleus: 192 KB) at C = 16384: above the 48 KB a launch gets without the opt-in
   const int smem = (kNucleus ? 3 : 2) * C * 4;
   static int configured = 0;
   if (smem > configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel<kNucleus>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel<kNucleus, kRowStep>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
-  OMLM_KLAUNCH((sample_kernel<kNucleus>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k, temperature,
-               allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p, top_k_rows,
-               temperature_rows, top_p_rows);
+  OMLM_KLAUNCH((sample_kernel<kNucleus, kRowStep>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k,
+               temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p,
+               top_k_rows, temperature_rows, top_p_rows, n_rows);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
@@ -846,6 +861,19 @@ int omlm_sample_rows(const float* logits, long ld, int C, int top_k, const int* 
                                      row_offset, step_ptr, pos_ptr, B, 1.f, stream, top_k_rows, temperature_rows, top_p_rows);
   return omlm::launch_sample<false>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row,
                                     row_offset, step_ptr, pos_ptr, B, 1.f, stream, top_k_rows, temperature_rows, nullptr);
+}
+
+int omlm_sample_rows_indexed(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                             const float* temperature_rows, const float* top_p_rows, int allow_eos, const unsigned long long* seeds,
+                             long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_rows, const int* n_rows,
+                             int B, void* stream) {
+  if (top_p_rows != nullptr)
+    return omlm::launch_sample<true, true>(logits, ld, C, top_k, temperature, allow_eos, nullptr, nullptr, seeds, tokens, tokens_ld,
+                                           next_row, row_offset, step_rows, nullptr, B, 1.f, stream, top_k_rows, temperature_rows,
+                                           top_p_rows, n_rows);
+  return omlm::launch_sample<false, true>(logits, ld, C, top_k, temperature, allow_eos, nullptr, nullptr, seeds, tokens, tokens_ld,
+                                          next_row, row_offset, step_rows, nullptr, B, 1.f, stream, top_k_rows, temperature_rows,
+                                          nullptr, n_rows);
 }
 
 int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,

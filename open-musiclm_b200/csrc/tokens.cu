@@ -130,12 +130,15 @@ __global__ void embed_gather_kernel(const float* __restrict__ table, const int* 
 
 // Decode step with absolute position embeddings: x[m, :] = table[src_row[m], :] + table[pos_row_base + p, :] with
 // p = *pos_ptr + pos_offset, the same position row for every m (kRowPos: p = pos_ptr[m] + pos_offset, each sequence at
-// its own position).  The position is read on the device, so a captured CUDA graph sees the current step on every
-// replay.  A negative src_row, or p outside [0, pos_rows), contributes zero.
-template <bool kRowPos>
-__global__ void embed_gather_pos_kernel(const float* __restrict__ table, const int* __restrict__ src_row,
-                                        const int* __restrict__ pos_ptr, int pos_offset, int pos_row_base, int pos_rows,
-                                        float* __restrict__ x, int M, int D) {
+// its own position; kRowOffset: p = pos_ptr[m] + pos_offset_rows[m], each sequence also with its own predicted-sequence
+// start, as in a generation session whose rows have conditioning of different lengths).  The position is read on the
+// device, so a captured CUDA graph sees the current step on every replay.  A negative src_row, or p outside
+// [0, pos_rows), contributes zero.
+template <bool kRowPos, bool kRowOffset>
+__device__ __forceinline__ void embed_gather_pos_body(const float* __restrict__ table, const int* __restrict__ src_row,
+                                                      const int* __restrict__ pos_ptr, int pos_offset,
+                                                      const int* __restrict__ pos_offset_rows, int pos_row_base, int pos_rows,
+                                                      float* __restrict__ x, int M, int D) {
   const int vec_per_row = D >> 2;
   const long long total = static_cast<long long>(M) * vec_per_row;
   int p = 0;
@@ -150,7 +153,7 @@ __global__ void embed_gather_pos_kernel(const float* __restrict__ table, const i
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int m = static_cast<int>(i / vec_per_row), v = static_cast<int>(i - static_cast<long long>(m) * vec_per_row);
     if constexpr (kRowPos) {
-      p = __ldg(pos_ptr + m) + pos_offset;
+      p = __ldg(pos_ptr + m) + (kRowOffset ? __ldg(pos_offset_rows + m) : pos_offset);
       has_pos = p >= 0 && p < pos_rows;
       prow = reinterpret_cast<const float4*>(table + static_cast<long long>(pos_row_base + (has_pos ? p : 0)) * D);
     }
@@ -163,6 +166,19 @@ __global__ void embed_gather_pos_kernel(const float* __restrict__ table, const i
     }
     reinterpret_cast<float4*>(x + static_cast<long long>(m) * D)[v] = val;
   }
+}
+
+template <bool kRowPos>
+__global__ void embed_gather_pos_kernel(const float* __restrict__ table, const int* __restrict__ src_row,
+                                        const int* __restrict__ pos_ptr, int pos_offset, int pos_row_base, int pos_rows,
+                                        float* __restrict__ x, int M, int D) {
+  embed_gather_pos_body<kRowPos, false>(table, src_row, pos_ptr, pos_offset, nullptr, pos_row_base, pos_rows, x, M, D);
+}
+
+__global__ void embed_gather_pos_rows_kernel(const float* __restrict__ table, const int* __restrict__ src_row,
+                                             const int* __restrict__ pos, const int* __restrict__ pos_offset_rows,
+                                             int pos_row_base, int pos_rows, float* __restrict__ x, int M, int D) {
+  embed_gather_pos_body<true, true>(table, src_row, pos, 0, pos_offset_rows, pos_row_base, pos_rows, x, M, D);
 }
 
 // dtable[src_row[m], :] += scale * dx[m, :]   (scale = grad_shrink alpha, utils.py:60-61).
@@ -247,18 +263,23 @@ static int launch_scatter_det(float* dtable, const int* src_row, const float* dx
   return 0;
 }
 
-template <bool kRowPos>
+template <bool kRowPos, bool kRowOffset = false>
 static int launch_embed_gather_pos(const float* table, const int* src_row, const int* pos_ptr, int pos_offset, int pos_row_base,
-                                   int pos_rows, float* x, int M, int D, void* stream) {
+                                   int pos_rows, float* x, int M, int D, void* stream, const int* pos_offset_rows = nullptr) {
   OMLM_CHECK_ARG(M > 0 && D > 0 && D % 4 == 0, "embed_gather_pos: bad shape %d x %d", M, D);
-  OMLM_CHECK_ARG(table != nullptr && src_row != nullptr && pos_ptr != nullptr && x != nullptr,
-                 "embed_gather_pos: null pointer");
+  OMLM_CHECK_ARG(table != nullptr && src_row != nullptr && pos_ptr != nullptr && x != nullptr &&
+                 (!kRowOffset || pos_offset_rows != nullptr), "embed_gather_pos: null pointer");
   OMLM_CHECK_ARG(pos_row_base >= 0 && pos_rows > 0, "embed_gather_pos: bad position rows %d + [0, %d)", pos_row_base,
                  pos_rows);
   const long long total = static_cast<long long>(M) * (D / 4);
   const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(num_sms()) * 16));
-  OMLM_KLAUNCH((embed_gather_pos_kernel<kRowPos>), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, src_row, pos_ptr,
-               pos_offset, pos_row_base, pos_rows, x, M, D);
+  if constexpr (kRowOffset) {
+    OMLM_KLAUNCH((embed_gather_pos_rows_kernel), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, src_row, pos_ptr,
+                 pos_offset_rows, pos_row_base, pos_rows, x, M, D);
+  } else {
+    OMLM_KLAUNCH((embed_gather_pos_kernel<kRowPos>), grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), table, src_row, pos_ptr,
+                 pos_offset, pos_row_base, pos_rows, x, M, D);
+  }
   OMLM_LAUNCH_CHECK();
   return 0;
 }
@@ -323,6 +344,11 @@ int omlm_embed_gather_pos(const float* table, const int* src_row, const int* pos
 int omlm_embed_gather_pos_ragged(const float* table, const int* src_row, const int* pos, int pos_offset, int pos_row_base,
                                  int pos_rows, float* x, int M, int D, void* stream) {
   return omlm::launch_embed_gather_pos<true>(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x, M, D, stream);
+}
+
+int omlm_embed_gather_pos_rows(const float* table, const int* src_row, const int* pos, const int* pos_offset, int pos_row_base,
+                               int pos_rows, float* x, int M, int D, void* stream) {
+  return omlm::launch_embed_gather_pos<true, true>(table, src_row, pos, 0, pos_row_base, pos_rows, x, M, D, stream, pos_offset);
 }
 
 int omlm_embed_scatter_add(float* dtable, const int* src_row, const float* dx, int M, int D,

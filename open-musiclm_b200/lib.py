@@ -173,6 +173,16 @@ def embed_gather_pos(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x,
          _I(pos_row_base), _I(pos_rows), _p(x), _I(M), _I(D), _stream())
 
 
+def embed_gather_pos_rows(table, src_row, pos, pos_offset, pos_row_base, pos_rows, x):
+    """embed_gather_pos with a position and a predicted-sequence offset per row: x[m] = table[src_row[m]] +
+    table[pos_row_base + pos[m] + pos_offset[m]] (int32 device tensors [M]; omlm_embed_gather_pos_rows)."""
+    M, D = x.shape
+    _check_row_pos(pos, M)
+    _check_row_pos(pos_offset, M)
+    call("omlm_embed_gather_pos_rows", _p(table), _p(src_row), _p(pos), _p(pos_offset), _I(pos_row_base), _I(pos_rows), _p(x),
+         _I(M), _I(D), _stream())
+
+
 def embed_scatter_add(dtable, src_row, dx, scale, first=None):
     """first: int32 row markers (INT_MAX, one per table row) -> the deterministic variant (omlm_embed_scatter_add_det)."""
     M, D = dx.shape
@@ -539,6 +549,20 @@ def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next
     assert seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B
     call("omlm_sample_seeded", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _F(temperature), _I(int(allow_eos)), _p(uniform),
          _p(seed), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
+
+
+def sample_rows_indexed(logits, C, allow_eos, seeds, tokens, next_row, row_offset, step_rows, n_rows, top_k_rows, temperature_rows,
+                        top_p_rows=None):
+    """omlm_sample_rows_indexed: sequence b samples its token at its own index t = step_rows[b] (int32 [B]) under
+    seeds[b] (int64 [B]) while t < n_rows[b] (int32 [B]) and then sets step_rows[b] = t + 1; per-row top_k_rows (int32),
+    temperature_rows and top_p_rows (float32, None: no row narrows to a nucleus) as in omlm_sample_rows."""
+    B = logits.shape[0]
+    for t, dt in ((seeds, torch.int64), (step_rows, torch.int32), (n_rows, torch.int32), (top_k_rows, torch.int32),
+                  (temperature_rows, torch.float32), (top_p_rows, torch.float32)):
+        assert t is None or (t.dtype == dt and t.is_cuda and t.is_contiguous() and t.numel() >= B)
+    call("omlm_sample_rows_indexed", _p(logits), _L(logits.stride(0)), _I(C), _I(1), _p(top_k_rows), _F(1.0), _p(temperature_rows),
+         _p(top_p_rows), _I(int(allow_eos)), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(step_rows),
+         _p(n_rows), _I(B), _stream())
 
 
 def gather_windows(src_i16, start, out):
