@@ -272,6 +272,11 @@ int omlm_ffn_mid_bwd(const void* dhn, const void* hn, const void* u, const float
 int omlm_cross_entropy(const float* logits, long ld, const int* labels, int label_stride, int rows_per_batch,
                        long batch_stride, int rows, int C, int ignore_index, float grad_scale, float loss_scale,
                        void* dlogits_bf16, long ldd, int Cp, float* loss_acc, void* stream);
+/* Per-row log-probability of the label, out[r] = l[label_r] - logsumexp(row r) (fp32 [rows]): omlm_cross_entropy's row
+ * loss, negated, from the same kernel bodies (labels, strided view and layout conditions as there; no gradient, no sum).
+ * A label outside [0, C) gives 0.  Any C. */
+int omlm_token_logprob(const float* logits, long ld, const int* labels, int label_stride, int rows_per_batch, long batch_stride,
+                       int rows, int C, float* out, void* stream);
 
 /* ---- optimiser (trainer.py:443-449, optimizer.py:3-34) ------------------------------------------
  * hyper (device, 9 floats): lr, beta1, beta2, eps, wd, 1-beta1^t, 1-beta2^t, max_grad_norm, grad prescale.
@@ -428,6 +433,31 @@ int omlm_sample_rows_indexed(const float* logits, long ld, int C, int top_k, con
                              const float* temperature_rows, const float* top_p_rows, int allow_eos, const unsigned long long* seeds,
                              long long* tokens, long tokens_ld, int* next_row, int row_offset, int* step_rows, const int* n_rows,
                              int B, void* stream);
+/* Token log-probabilities beside the token (float [B, tokens_ld] device arrays, written at the token's [b, t]).  They
+ * share the tokens' allocation: logprobs must start right after tokens' B rows (at tokens + B * tokens_ld, read as
+ * float) and sample_logprobs right after logprobs (logprobs + B * tokens_ld); anything else is an argument error.  The
+ * pointers are checked, not passed to the kernel, so the samplers without log-probabilities keep their code.
+ *   logprobs[b, t]        = l_c - (m + log sum_j exp(l_j - m)), over the raw row (all C classes, eos included, before
+ *                           eos masking, temperature, top-k and top-p; m = its maximum): the model's log p of the token;
+ *   sample_logprobs[b, t] = (l_c - m_S) / T - log sum_{j in S} exp((l_j - m_S) / T): its log p under the distribution
+ *                           it was drawn from, S the candidate set (eos rule, top-k set K, then the nucleus N when the
+ *                           row is narrowed); NaN entries are never in S, -inf entries add no mass.
+ * The sums run in a fixed order (double accumulators of expf terms), so both values depend only on the row.  Tokens,
+ * counters and every other argument as omlm_sample_rows (top_k_rows, temperature_rows, top_p_rows may be NULL; the
+ * nucleus kernel runs when top_p_rows is given or the scalar top_p, in (0, 1], is below 1): the tokens are bit-identical
+ * to the entry points without log-probabilities. */
+int omlm_sample_logprob(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                        const float* temperature_rows, float top_p, const float* top_p_rows, int allow_eos, const float* uniform,
+                        const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                        int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float* logprobs,
+                        float* sample_logprobs, void* stream);
+/* omlm_sample_rows_indexed with the two log-probabilities of omlm_sample_logprob, written at [b, step_rows[b]] by the
+ * rows that sample. */
+int omlm_sample_rows_indexed_logprob(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                                     const float* temperature_rows, const float* top_p_rows, int allow_eos,
+                                     const unsigned long long* seeds, long long* tokens, long tokens_ld, int* next_row,
+                                     int row_offset, int* step_rows, const int* n_rows, int B, float* logprobs,
+                                     float* sample_logprobs, void* stream);
 
 #ifdef __cplusplus
 }

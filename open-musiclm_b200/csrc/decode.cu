@@ -506,7 +506,17 @@ decode_conv_geglu_kernel(const uint16_t* __restrict__ u_new, uint16_t* __restric
 // counter and the output column.  A row with t outside [0, min(n_rows[b], tokens_ld)) -- it has all its samples, or its
 // slot is free -- writes nothing.  Otherwise block b writes its token and sets step_ptr[b] = t + 1 itself: no block
 // reads another's index, so there is no arrival counter, and pos_ptr is unused (omlm_decode_advance_pos moves positions).
-template <bool kNucleus, bool kRowStep>
+//
+// Token log-probabilities (kLogprob, omlm_sample_logprob / omlm_sample_rows_indexed_logprob): beside tokens[b, t] the
+// block writes lp_out[b, t] = l_c - (m + log sum_j exp(l_j - m)) over the raw row (all C classes, eos included, before
+// any masking; m its maximum) and slp_out[b, t] = (l_c - m_S) / T - log sum_{j in S} exp((l_j - m_S) / T), where S is the
+// candidate set the token was drawn from (eos rule, K, then N when the row is narrowed; NaN entries never in S).  The
+// non-nucleus kernel marks the entries outside K as NaN in lg while it samples, so S = the non-NaN entries of lg in both
+// kernels.  The expf terms are summed in double in the fixed order of the nucleus mass (thread-strided, shuffle tree,
+// warps 0..7): both values depend only on the row.  lp_out and slp_out are not parameters: they follow the tokens in
+// the same allocation (float [B, tokens_ld] each, right after tokens' B rows), so the kernel's signature, and with it
+// the code of the instantiations without kLogprob, stays what it was before the flag existed.
+template <bool kNucleus, bool kRowStep, bool kLogprob = false>
 __global__ void __launch_bounds__(256)
 sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float temperature, int allow_eos,
               const float* __restrict__ uniform, const unsigned long long* __restrict__ seed_ptr,
@@ -630,6 +640,9 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
         for (int j = 0; j < c; ++j) rank += key[j] == thr;
         keep = rank < s_tie_budget;
       }
+      if constexpr (kLogprob) {
+        if (!keep) lg[c] = __int_as_float(0x7fffffff);           // S = the non-NaN entries of lg (read after a barrier)
+      }
     }
     if (!keep) continue;
     float u;
@@ -663,6 +676,52 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
     tokens[b * tokens_ld + step] = best_i;
     next_row[b] = row_offset + best_i;
   }
+  if constexpr (kLogprob) {                                    // tid 0 holds the token
+    __shared__ float s_red_mx[8];
+    __shared__ double s_red_sum[8];
+    const int lane = tid & 31, warp = tid >> 5;
+    auto block_max = [&](float v) -> float {
+      v = warp_max(v);
+      if (lane == 0) s_red_mx[warp] = v;
+      __syncthreads();
+      float t = s_red_mx[0];
+      for (int w = 1; w < 8; ++w) t = fmaxf(t, s_red_mx[w]);
+      __syncthreads();
+      return t;
+    };
+    auto block_sum = [&](double s) -> double {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) s_red_sum[warp] = s;
+      __syncthreads();
+      double t = 0.0;
+      for (int w = 0; w < 8; ++w) t += s_red_sum[w];
+      __syncthreads();
+      return t;
+    };
+    const float* raw = logits + b * ld;
+    float m = -INFINITY;
+    for (int c = tid; c < C; c += 256) m = fmaxf(m, raw[c]);
+    const float raw_max = block_max(m);
+    double s = 0.0;
+    for (int c = tid; c < C; c += 256) s += static_cast<double>(expf(raw[c] - raw_max));
+    const double raw_sum = block_sum(s);
+    m = -INFINITY;
+    for (int c = tid; c < C; c += 256) m = fmaxf(m, lg[c]);     // fmaxf skips the NaN entries (outside S)
+    const float set_max = block_max(m);
+    s = 0.0;
+    for (int c = tid; c < C; c += 256)
+      s += isnan(lg[c]) ? 0.0 : static_cast<double>(expf((lg[c] - set_max) / temperature));
+    const double set_mass = block_sum(s);
+    if (tid == 0) {
+      // the outputs follow the tokens in one allocation: float [B, tokens_ld] log p, then float [B, tokens_ld] sample log p
+      float* lp_out = reinterpret_cast<float*>(tokens + static_cast<long>(B) * tokens_ld);
+      float* slp_out = lp_out + static_cast<long>(B) * tokens_ld;
+      const int c = min(max(best_i, 0), C - 1);                 // a row with no finite score keeps best_i = INT_MAX
+      lp_out[b * tokens_ld + step] = static_cast<float>(static_cast<double>(logits[b * ld + c]) - raw_max - log(raw_sum));
+      slp_out[b * tokens_ld + step] = static_cast<float>(static_cast<double>((lg[c] - set_max) / temperature) - log(set_mass));
+    }
+  }
   if constexpr (kRowStep) {
     if (tid == 0) step_ptr[b] = step + 1;                       // every thread read it before the first barrier
     return;
@@ -683,7 +742,7 @@ sample_kernel(const float* __restrict__ logits, long ld, int C, int k, float tem
   }
 }
 
-template <bool kNucleus, bool kRowStep = false>
+template <bool kNucleus, bool kRowStep = false, bool kLogprob = false>
 static int launch_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,
                          const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
                          int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float top_p, void* stream,
@@ -699,14 +758,20 @@ static int launch_sample(const float* logits, long ld, int C, int top_k, float t
   const int smem = (kNucleus ? 3 : 2) * C * 4;
   static int configured = 0;
   if (smem > configured) {
-    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel<kNucleus, kRowStep>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    OMLM_CUDA(cudaFuncSetAttribute(sample_kernel<kNucleus, kRowStep, kLogprob>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
-  OMLM_KLAUNCH((sample_kernel<kNucleus, kRowStep>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C, top_k,
-               temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p,
-               top_k_rows, temperature_rows, top_p_rows, n_rows);
+  OMLM_KLAUNCH((sample_kernel<kNucleus, kRowStep, kLogprob>), B, 256, smem, reinterpret_cast<cudaStream_t>(stream), logits, ld, C,
+               top_k, temperature, allow_eos, uniform, seed, seeds, tokens, tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B,
+               top_p, top_k_rows, temperature_rows, top_p_rows, n_rows);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+// The kLogprob samplers' output layout: logprobs at the end of tokens' B rows, sample_logprobs right after logprobs.
+static bool logprob_layout(const long long* tokens, long tokens_ld, int B, const float* logprobs, const float* sample_logprobs) {
+  const float* lp = reinterpret_cast<const float*>(tokens + static_cast<long>(B) * tokens_ld);
+  return logprobs == lp && sample_logprobs == lp + static_cast<long>(B) * tokens_ld;
 }
 
 // ------------------------------------------------------------------------------------------------ per-row positions
@@ -874,6 +939,39 @@ int omlm_sample_rows_indexed(const float* logits, long ld, int C, int top_k, con
   return omlm::launch_sample<false, true>(logits, ld, C, top_k, temperature, allow_eos, nullptr, nullptr, seeds, tokens, tokens_ld,
                                           next_row, row_offset, step_rows, nullptr, B, 1.f, stream, top_k_rows, temperature_rows,
                                           nullptr, n_rows);
+}
+
+int omlm_sample_logprob(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                        const float* temperature_rows, float top_p, const float* top_p_rows, int allow_eos, const float* uniform,
+                        const unsigned long long* seed, const unsigned long long* seeds, long long* tokens, long tokens_ld,
+                        int* next_row, int row_offset, int* step_ptr, int* pos_ptr, int B, float* logprobs,
+                        float* sample_logprobs, void* stream) {
+  OMLM_CHECK_ARG(top_p > 0.f && top_p <= 1.f, "sample_logprob: top_p %g outside (0, 1]", static_cast<double>(top_p));
+  OMLM_CHECK_ARG(omlm::logprob_layout(tokens, tokens_ld, B, logprobs, sample_logprobs),
+                 "sample_logprob: logprobs and sample_logprobs must follow tokens' B rows in its allocation");
+  if (top_p_rows != nullptr || top_p < 1.f)
+    return omlm::launch_sample<true, false, true>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens,
+                                                  tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, top_p, stream, top_k_rows,
+                                                  temperature_rows, top_p_rows, nullptr);
+  return omlm::launch_sample<false, false, true>(logits, ld, C, top_k, temperature, allow_eos, uniform, seed, seeds, tokens,
+                                                 tokens_ld, next_row, row_offset, step_ptr, pos_ptr, B, 1.f, stream, top_k_rows,
+                                                 temperature_rows, nullptr, nullptr);
+}
+
+int omlm_sample_rows_indexed_logprob(const float* logits, long ld, int C, int top_k, const int* top_k_rows, float temperature,
+                                     const float* temperature_rows, const float* top_p_rows, int allow_eos,
+                                     const unsigned long long* seeds, long long* tokens, long tokens_ld, int* next_row,
+                                     int row_offset, int* step_rows, const int* n_rows, int B, float* logprobs,
+                                     float* sample_logprobs, void* stream) {
+  OMLM_CHECK_ARG(omlm::logprob_layout(tokens, tokens_ld, B, logprobs, sample_logprobs),
+                 "sample_rows_indexed_logprob: logprobs and sample_logprobs must follow tokens' B rows in its allocation");
+  if (top_p_rows != nullptr)
+    return omlm::launch_sample<true, true, true>(logits, ld, C, top_k, temperature, allow_eos, nullptr, nullptr, seeds, tokens,
+                                                 tokens_ld, next_row, row_offset, step_rows, nullptr, B, 1.f, stream, top_k_rows,
+                                                 temperature_rows, top_p_rows, n_rows);
+  return omlm::launch_sample<false, true, true>(logits, ld, C, top_k, temperature, allow_eos, nullptr, nullptr, seeds, tokens,
+                                                tokens_ld, next_row, row_offset, step_rows, nullptr, B, 1.f, stream, top_k_rows,
+                                                temperature_rows, nullptr, n_rows);
 }
 
 int omlm_sample(const float* logits, long ld, int C, int top_k, float temperature, int allow_eos, const float* uniform,

@@ -17,11 +17,13 @@ constexpr int kCeMaxPerLane = 40;
 // row -- a strided view, read in place.
 // DET (part != nullptr): instead of the two atomics, the block writes (loss_scale * its loss sum, its row count) to
 // part[blockIdx.x]; omlm_colsum adds the blocks' pairs to loss_acc in block order.
+template <bool kRowOut>
 __global__ void __launch_bounds__(256)
 ce_fwd_bwd_kernel(const float* __restrict__ logits, long ld, const int* __restrict__ labels, int label_stride,
                   int rows_per_batch, long batch_stride,
                   int rows, int C, int ignore_index, float grad_scale, float loss_scale, __nv_bfloat16* __restrict__ dlogits,
-                  long ldd, int Cp, float* __restrict__ loss_acc, float2* __restrict__ part) {
+                  long ldd, int Cp, float* __restrict__ loss_acc, float2* __restrict__ part,
+                  float* __restrict__ row_out) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * 8 + warp;
   float my_loss = 0.f, my_cnt = 0.f;
@@ -45,10 +47,13 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long ld, const int* __restri
       se += v[i];
     }
     se = warp_sum(se);
-    const bool ignored = (label == ignore_index);
+    const bool ignored = (label == ignore_index) || (kRowOut && (label < 0 || label >= C));
     if (!ignored && lane == 0) {
       my_loss = (mx + logf(se)) - lr[label];
       my_cnt = 1.f;
+    }
+    if constexpr (kRowOut) {
+      if (lane == 0) row_out[row] = ignored ? 0.f : -my_loss;
     }
     if (dlogits != nullptr) {
       const float inv = ignored ? 0.f : grad_scale / se;
@@ -64,6 +69,7 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long ld, const int* __restri
       }
     }
   }
+  if constexpr (kRowOut) return;                       // the same on every thread: no loss sum, no barrier
   __shared__ float sl[8], sc[8];
   if (lane == 0) { sl[warp] = my_loss; sc[warp] = my_cnt; }
   __syncthreads();
@@ -102,11 +108,13 @@ __device__ __forceinline__ uint4 ce_grad8(float4 a, float4 b, int c0, int C, flo
 // same on every run.  Pass 2 reads the row again (mostly from L2: the warp has just read it) and writes eight bf16
 // gradients per 16-byte store.  Columns beyond C are never read.  Ignored rows are written as zeros
 // without reading the row again.
+template <bool kRowOut>
 __global__ void __launch_bounds__(256)
 ce_stream_kernel(const float* __restrict__ logits, long ld, const int* __restrict__ labels, int label_stride,
                  int rows_per_batch, long batch_stride,
                  int rows, int C, int ignore_index, float grad_scale, float loss_scale, __nv_bfloat16* __restrict__ dlogits,
-                 long ldd, int Cp, float* __restrict__ loss_acc, float2* __restrict__ part) {
+                 long ldd, int Cp, float* __restrict__ loss_acc, float2* __restrict__ part,
+                  float* __restrict__ row_out) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * 8 + warp;
   float my_loss = 0.f, my_cnt = 0.f;
@@ -115,7 +123,7 @@ ce_stream_kernel(const float* __restrict__ logits, long ld, const int* __restric
     const float4* l4 = reinterpret_cast<const float4*>(lr);
     const int rb = row / rows_per_batch;
     const int label = labels[rb * batch_stride + static_cast<long>(row - rb * rows_per_batch) * label_stride];
-    const bool ignored = (label == ignore_index);
+    const bool ignored = (label == ignore_index) || (kRowOut && (label < 0 || label >= C));
     // ---- pass 1: online max / sum of exp
     const int n4 = C >> 2;
     float m = -INFINITY, s = 0.f;
@@ -139,6 +147,9 @@ ce_stream_kernel(const float* __restrict__ logits, long ld, const int* __restric
     if (!ignored && lane == 0) {
       my_loss = (mx + logf(se)) - lr[label];
       my_cnt = 1.f;
+    }
+    if constexpr (kRowOut) {
+      if (lane == 0) row_out[row] = ignored ? 0.f : -my_loss;
     }
     // ---- pass 2: dlogits, eight columns per 16-byte store
     if (dlogits != nullptr) {
@@ -167,6 +178,7 @@ ce_stream_kernel(const float* __restrict__ logits, long ld, const int* __restric
       }
     }
   }
+  if constexpr (kRowOut) return;                       // the same on every thread: no loss sum, no barrier
   __shared__ float sl[8], sc[8];
   if (lane == 0) { sl[warp] = my_loss; sc[warp] = my_cnt; }
   __syncthreads();
@@ -200,16 +212,16 @@ static int cross_entropy_impl(const float* logits, long ld, const int* labels, i
       OMLM_CHECK_ARG(reinterpret_cast<uintptr_t>(dlogits_bf16) % 16 == 0 && ldd % 8 == 0 && Cp % 8 == 0 && Cp >= C && ldd >= Cp,
                      "cross_entropy: C=%d needs 16-byte aligned dlogits with ldd %% 8 == 0, Cp %% 8 == 0 and C <= Cp <= ldd "
                      "(Cp=%d, ldd=%ld)", C, Cp, ldd);
-    OMLM_KLAUNCH((ce_stream_kernel), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream),
+    OMLM_KLAUNCH((ce_stream_kernel<false>), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream),
         logits, ld, labels, label_stride, rows_per_batch, batch_stride, rows, C, ignore_index, grad_scale, loss_scale,
-        reinterpret_cast<__nv_bfloat16*>(dlogits_bf16), ldd, Cp, loss_acc, reinterpret_cast<float2*>(part));
+        reinterpret_cast<__nv_bfloat16*>(dlogits_bf16), ldd, Cp, loss_acc, reinterpret_cast<float2*>(part), nullptr);
     OMLM_LAUNCH_CHECK();
     if (part != nullptr) return omlm_colsum(part, 2, 1, loss_acc, blocks, 2, 1, stream);
     return 0;
   }
-  OMLM_KLAUNCH((ce_fwd_bwd_kernel), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream),
+  OMLM_KLAUNCH((ce_fwd_bwd_kernel<false>), blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream),
       logits, ld, labels, label_stride, rows_per_batch, batch_stride, rows, C, ignore_index, grad_scale, loss_scale,
-      reinterpret_cast<__nv_bfloat16*>(dlogits_bf16), ldd, Cp, loss_acc, reinterpret_cast<float2*>(part));
+      reinterpret_cast<__nv_bfloat16*>(dlogits_bf16), ldd, Cp, loss_acc, reinterpret_cast<float2*>(part), nullptr);
   OMLM_LAUNCH_CHECK();
   if (part != nullptr) return omlm_colsum(part, 2, 1, loss_acc, blocks, 2, 1, stream);
   return 0;
@@ -230,4 +242,27 @@ extern "C" int omlm_cross_entropy_det(const float* logits, long ld, const int* l
   OMLM_CHECK_ARG(part_ws != nullptr, "cross_entropy_det: no partials buffer");
   return cross_entropy_impl(logits, ld, labels, label_stride, rows_per_batch, batch_stride, rows, C, ignore_index, grad_scale,
                             loss_scale, dlogits_bf16, ldd, Cp, loss_acc, part_ws, part_ws_bytes, stream);
+}
+
+// The per-row value of the kernels above, written out instead of summed: out[r] = log softmax(row r)[label_r] =
+// l[label] - (mx + log se), bit for bit the negated row loss of omlm_cross_entropy.  The same kernel bodies (kRowOut);
+// no gradient, no loss sum.  A label outside [0, C) (ignore_index included) gives 0.
+extern "C" int omlm_token_logprob(const float* logits, long ld, const int* labels, int label_stride, int rows_per_batch,
+                                  long batch_stride, int rows, int C, float* out, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(rows > 0 && C > 0 && out != nullptr, "token_logprob: bad arguments (rows=%d, C=%d)", rows, C);
+  if (rows_per_batch <= 0) { rows_per_batch = rows; batch_stride = 0; }
+  const int blocks = (rows + 7) / 8;
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (C > 32 * kCeMaxPerLane) {
+    OMLM_CHECK_ARG(reinterpret_cast<uintptr_t>(logits) % 16 == 0 && ld % 4 == 0 && ld >= C,
+                   "token_logprob: C=%d needs 16-byte aligned logits with ld %% 4 == 0 and ld >= C (ld=%ld)", C, ld);
+    OMLM_KLAUNCH((ce_stream_kernel<true>), blocks, 256, 0, st, logits, ld, labels, label_stride, rows_per_batch, batch_stride,
+                 rows, C, -100, 0.f, 0.f, nullptr, 0L, 0, nullptr, nullptr, out);
+  } else {
+    OMLM_KLAUNCH((ce_fwd_bwd_kernel<true>), blocks, 256, 0, st, logits, ld, labels, label_stride, rows_per_batch, batch_stride,
+                 rows, C, -100, 0.f, 0.f, nullptr, 0L, 0, nullptr, nullptr, out);
+  }
+  OMLM_LAUNCH_CHECK();
+  return 0;
 }

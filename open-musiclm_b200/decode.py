@@ -197,10 +197,12 @@ class DecodeSession:
     length, its first decode position and the last position it processes; self.pos is then one position per sequence
     and n_max the cache capacity.  Otherwise self.pos is one counter for the whole batch, starting at n_prompt.
     rows (sampling arguments per sequence): (top_k, temperature, top_p), B values each (top_p None: no nucleus);
-    self.rows then holds them as device arrays, which every sample() reads instead of its scalar arguments."""
+    self.rows then holds them as device arrays, which every sample() reads instead of its scalar arguments.
+    logprob: the sampler also writes each token's two log-probabilities into self.lp and self.slp (fp32 [B, n_new], in
+    the allocation of self.tokens, right after it, as omlm_sample_logprob requires)."""
 
     def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0, ragged=None,
-                 n_max: Optional[int] = None, rows=None):
+                 n_max: Optional[int] = None, rows=None, logprob: bool = False):
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
         if seeded and eng.h > 16:
@@ -217,7 +219,13 @@ class DecodeSession:
         self.u_new, self.h = E(B, 2 * Fp, dt=a16), E(B, Fp, dt=a16)
         self.rowsum = E(B, Fp // 128, 2, dt=f32)
         self.logits = E(B, max(eng.Cp), dt=f32)
-        self.tokens = torch.zeros(B, max(n_new, 1), device=dev, dtype=torch.int64)
+        W = max(n_new, 1)
+        self.logprob = logprob
+        self.lp = self.slp = None
+        if logprob:              # the samplers' layout: tokens [B, W] int64, then lp and slp [B, W] fp32 each
+            self.tokens, self.lp, self.slp = lib.logprob_buffers(B, W, dev)
+        else:
+            self.tokens = torch.zeros(B, W, device=dev, dtype=torch.int64)
         self.next_row = torch.zeros(B, device=dev, dtype=torch.int32)
         self.counters = torch.zeros(2, device=dev, dtype=torch.int32)          # [sampled so far, block arrival counter]
         self.ragged = ragged is not None
@@ -319,19 +327,20 @@ class DecodeSession:
         pos = self.pos if bump_pos and not self.ragged else None
         if self.rows is not None:        # per-row arguments: top_k, temperature and top_p are not used
             lib.sample(self.logits, eng.C[S], 1, 1.0, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                       self.counters, pos, self.B, seeds=self.seeds, **self.rows)
+                       self.counters, pos, self.B, seeds=self.seeds, logprobs=self.lp, sample_logprobs=self.slp, **self.rows)
         else:
             lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                       self.counters, pos, self.B, seeds=self.seeds, top_p=top_p)
+                       self.counters, pos, self.B, seeds=self.seeds, top_p=top_p, logprobs=self.lp, sample_logprobs=self.slp)
         if bump_pos and self.ragged:
             lib.decode_advance_pos(self.pos, self.pos_last)
 
     def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True, top_p=None):
         """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
         if self.rows is not None:        # the arrays' contents are read at replay; only the kernel choice is captured
-            key = (qi, qi_next, "rows", bool(allow_eos_next), uniform is not None, self.seeded, self.rows["top_p_rows"] is not None)
+            key = (qi, qi_next, "rows", bool(allow_eos_next), uniform is not None, self.seeded, self.rows["top_p_rows"] is not None,
+                   self.logprob)
         else:
-            key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p)
+            key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p, self.logprob)
         g = self._graphs.get(key)
         if g is None or not use_graph:
             body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True, top_p))
@@ -349,6 +358,55 @@ class DecodeSession:
                 body()
             self._graphs[key] = g
         g.replay()
+
+
+def prefix_labels(prompt, q: int, C: int):
+    """int32 [B, n + q] labels of the predicted sequence's prompt tokens [B, n] for omlm_token_logprob, padded with -100
+    (a label outside [0, C) is not scored): group qi's row t predicts flat token t q + qi, read through the strided view
+    (offset qi, stride q, one row of n + q per sequence), so its last row (the next token) reads the padding."""
+    B, n = prompt.shape
+    lab = torch.full((B, n + q), -100, device=prompt.device, dtype=torch.int32)
+    lab[:, :n] = torch.where((prompt >= 0) & (prompt < C), prompt, -100).to(torch.int32)
+    return lab
+
+
+def prefix_logprobs(eng, pl, ws, prompt, q: int, C: int):
+    """[B, n] float32: the log-probability of every prompt token of the predicted sequence under the prefill's logits row
+    for its position (the head groups ws["logits"][gi] of the last sequence; the row that predicts the next token is
+    not scored)."""
+    B, n = prompt.shape
+    S = len(eng.seqs) - 1
+    lab = prefix_labels(prompt, q, C)
+    out = torch.zeros(B, n, device=prompt.device, dtype=torch.float32)
+    for gi, (s, qi, cnt, base) in enumerate(pl.groups):
+        m = len(range(qi, n, q))
+        if s != S or m == 0:
+            continue
+        row = torch.empty(B * cnt, device=prompt.device, dtype=torch.float32)
+        lib.token_logprob(ws["logits"][gi], lab.view(-1)[qi:], C, row, label_stride=q, rows_per_batch=cnt, batch_stride=n + q)
+        out[:, qi::q] = row.view(B, cnt)[:, :m]
+    return out
+
+
+def assemble_logprobs(sampled, pre_lp, lp_new, slp_new, n_real, n_end):
+    """The [B, W] logprobs and sample_logprobs of generate's flat output `sampled` (after the eos masking): row b's
+    columns below n_real[b] are prefix tokens (pre_lp [B, >= their count], sample log p 0), columns n_real[b] ...
+    n_end[b] - 1 its samples in order (lp_new, slp_new [B, n_new]; None when nothing was sampled), and every column
+    that holds -1 is 0 in both.  n_real, n_end: int64 [B, 1]."""
+    B, W = sampled.shape
+    col = torch.arange(W, device=sampled.device)[None]
+    lp = torch.zeros(B, W, device=sampled.device, dtype=torch.float32)
+    w = min(W, pre_lp.shape[1])
+    lp[:, :w] = pre_lp[:, :w]
+    lp.masked_fill_(col >= n_real, 0.0)
+    slp = torch.zeros_like(lp)
+    if lp_new is not None:
+        in_new = (col >= n_real) & (col < n_end)
+        src = (col - n_real).clamp(0, lp_new.shape[1] - 1).expand(B, -1)
+        lp = torch.where(in_new, lp_new.gather(1, src), lp)
+        slp = torch.where(in_new, slp_new.gather(1, src), slp)
+    gone = sampled == -1
+    return lp.masked_fill(gone, 0.0), slp.masked_fill(gone, 0.0)
 
 
 class TokenConditionedTransformerWrapper(nn.Module):
@@ -377,7 +435,8 @@ class TokenConditionedTransformerWrapper(nn.Module):
     def generate(self, *, conditioning_token_ids: List[torch.Tensor], pred_token_ids: Optional[torch.Tensor] = None,
                  max_time_steps=512, filter_thres=0.9, temperature=1., include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, allow_eos_in_output=False, uniform_noise: Optional[torch.Tensor] = None,
-                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, top_p=None, pred_lengths=None, **kwargs):
+                 use_cuda_graph=True, trace_logits: Optional[list] = None, seeds=None, top_p=None, pred_lengths=None,
+                 return_logprobs=False, **kwargs):
         """Same contract as open_musiclm.py:253-326.  uniform_noise (optional, [n_sampled, b, codebook+1] in (0, 1)):
         the uniform draws behind the Gumbel noise, one slice per sampled token in order — parity runs pass the stream
         torch's default CPU generator would have produced; by default the noise comes from a device Philox stream keyed
@@ -433,9 +492,24 @@ class TokenConditionedTransformerWrapper(nn.Module):
         size exceeds codebook+1, a top_p element outside (0, 1] or a negative max_time_steps raises ValueError before
         anything runs (Engine.seed untouched).  A list of equal values is that single value, so with all four equal and
         no ragged pred_lengths the call is exactly the single-value call.
+        return_logprobs (a bool): True returns (tokens, logprobs, sample_logprobs), three [b, n, q] tensors, the two new
+        ones float32 on the device.  logprobs[b, i, j] is the model's log-probability of the token at [b, i, j] given
+        everything before it: l_c - (m + log sum_j exp(l_j - m)) over the fp32 logits row the engine computed for that
+        position (all codebook+1 classes, eos included, before eos masking, temperature, top-k and top-p): for a sampled
+        token the row it was sampled from (the row trace_logits copies), for a prefix token the prefill's row at its
+        position.  sample_logprobs[b, i, j] is the log-probability of a sampled token under the distribution it was drawn
+        from, (l_c - m_S) / T - log sum_{j in S} exp((l_j - m_S) / T) with S the candidate set the sampler builds (eos rule,
+        top-k set K, then the nucleus N with top_p; NaN entries never in S, -inf entries add no mass), the row's own k, T
+        and top_p; the 24-bit uniforms' discretisation is not modelled.  Prefix tokens have sample_logprobs 0, and every
+        position whose token is -1 has 0 in both.  The tokens are bit-identical to the call without return_logprobs.  With
+        nothing to sample the prefill still runs, so generate(pred_token_ids=x, max_time_steps=x.shape[1],
+        return_logprobs=True) scores the given sequence x teacher-forced (any codebook size).  Seeded rows' values depend
+        only on that row, as its tokens do.
         trace_logits (tests): receives a copy of the [b, codebook+1] logits every token was sampled from."""
         if kwargs:
             raise NotImplementedError(f"open_musiclm_b200 generate: unsupported arguments {sorted(kwargs)}")
+        if not isinstance(return_logprobs, bool):
+            raise ValueError(f"open_musiclm_b200 generate: return_logprobs must be a bool, not {return_logprobs!r}")
         if seeds is not None and uniform_noise is not None:
             raise ValueError("open_musiclm_b200 generate: seeds and uniform_noise exclude each other")
         B = conditioning_token_ids[0].shape[0]
@@ -493,23 +567,29 @@ class TokenConditionedTransformerWrapper(nn.Module):
             # keeps every real position away from the padding and the prefill runs unchanged.
             n_real = torch.tensor(lengths, device=dev, dtype=torch.int64)[:, None] * q
             Lp = max([n for n, k in zip(lengths, n_new_b) if k > 0], default=0)
+            if return_logprobs:              # every real prefix token needs its prefill row
+                Lp = max(Lp, max(lengths))
             L_eff = [min(n, Lp) for n in lengths]
             prompt = prefix[:, :Lp * q].masked_fill(torch.arange(Lp * q, device=dev)[None] >= n_real.clamp(max=Lp * q), 0)
         else:
             prompt = prefix
-        if n_new > 0:
+        pre_lp = None
+        if n_new > 0 or (return_logprobs and prompt.shape[1] > 0):
             ids = cond + [prompt]
             _, src_row, key_mask, _, n_tok = lib.token_plan(
                 ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
                 append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
             pl = eng.plan(B, n_tok)
+            sess = None
+        if n_new > 0:
             if top_k is None:
                 top_k = max(int((1 - filter_thres) * C), 1)                                          # utils.py:80
             rows = None
             if per_row:                          # every argument as B values (a single value repeated)
                 rows = tuple(v if isinstance(v, list) else [v] * B for v in (top_k, temperature, top_p))
             if lengths is None:
-                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1], rows=rows)
+                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1], rows=rows,
+                                     logprob=return_logprobs)
             else:
                 # per row: real prompt length, last position the row processes (a row with all its tokens stays there),
                 # first decode position; the cache holds the longest prompt and every row's new positions
@@ -517,11 +597,15 @@ class TokenConditionedTransformerWrapper(nn.Module):
                 pos_last = [p + max(k, 1) - 2 for p, k in zip(P, n_new_b)]
                 sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1],
                                      ragged=(P, [min(p, e) for p, e in zip(P, pos_last)], pos_last),
-                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]), rows=rows)
+                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]), rows=rows, logprob=return_logprobs)
             if seed_vals is not None:
                 sess.seeds.copy_(seed_vals)
+        if n_new > 0 or (return_logprobs and prompt.shape[1] > 0):
             ws = eng.workspace(pl, False)
-            eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_Capture(sess))
+            eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_Capture(sess) if sess is not None else None)
+            if return_logprobs and prompt.shape[1] > 0:
+                pre_lp = prefix_logprobs(eng, pl, ws, prompt, q, C)
+        if n_new > 0:
             # logits of the prompt's last position: final sequence, position p_last = its token count, head p_last mod q
             # (per row: its own last real position; every prefix is whole time steps, so the head is the same)
             p_last = n_tok[-1]
@@ -553,6 +637,8 @@ class TokenConditionedTransformerWrapper(nn.Module):
             new = sess.tokens[:, :n_new]
         if lengths is None:
             sampled = torch.cat([prefix, new], 1) if n_new > 0 else prefix
+            n_real = torch.full((B, 1), prefix.shape[1], device=dev, dtype=torch.int64)
+            n_end = n_real + n_new
         else:
             # row b: its n_real[b] prefix tokens, then its n_new_b[b] samples, then -1 up to the widest row
             width = max(max(t, n) for t, n in zip(steps_b, lengths)) * q
@@ -570,6 +656,12 @@ class TokenConditionedTransformerWrapper(nn.Module):
         sampled = sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1)
         if was_training:
             m.train()
+        if return_logprobs:
+            if pre_lp is None:
+                pre_lp = torch.zeros(B, prompt.shape[1], device=dev, dtype=torch.float32)
+            lp, slp = assemble_logprobs(sampled, pre_lp, sess.lp[:, :n_new] if n_new > 0 else None,
+                                        sess.slp[:, :n_new] if n_new > 0 else None, n_real, n_end)
+            return sampled.view(B, -1, q), lp.view(B, -1, q), slp.view(B, -1, q)
         return sampled.view(B, -1, q)                                                               # :323-324
 
     def forward(self, *, all_token_ids: List[torch.Tensor], return_loss: bool = False, **kwargs):

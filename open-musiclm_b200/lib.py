@@ -359,6 +359,15 @@ def cross_entropy(logits, labels, C, loss_acc, *, grad_scale=0.0, dlogits=None, 
         call("omlm_cross_entropy_det", *args, _p(part), _L(part.numel() * 4), _stream())
 
 
+def token_logprob(logits, labels, C, out, *, label_stride=1, rows=None, rows_per_batch=0, batch_stride=0):
+    """out[r] (float32) = log softmax(logits[r, :C])[label_r] through omlm_token_logprob; labels int32 as in cross_entropy
+    (a label outside [0, C) gives 0)."""
+    rows = logits.shape[0] if rows is None else rows
+    assert labels.dtype == torch.int32 and out.dtype == torch.float32 and out.numel() >= rows
+    call("omlm_token_logprob", _p(logits), _L(logits.stride(0)), _p(labels), _I(label_stride), _I(rows_per_batch), _L(batch_stride),
+         _I(rows), _I(C), _p(out), _stream())
+
+
 def grad_sumsq(g, acc, prescale=1.0, part=None):
     """part: float64 scratch (>= 4 * SMs) -> the deterministic variant (omlm_grad_sumsq_det)."""
     if part is None:
@@ -521,12 +530,25 @@ def decode_conv_geglu(u_new, state, conv_w, h_out, rowsum):
 
 
 def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next_row, row_offset, counters, pos, B, seeds=None,
-           top_p=None, top_k_rows=None, temperature_rows=None, top_p_rows=None):
+           top_p=None, top_k_rows=None, temperature_rows=None, top_p_rows=None, logprobs=None, sample_logprobs=None):
     """seeds: int64 [B] device tensor of per-sequence seeds (raw 64-bit patterns) -> omlm_sample_seeded.
     top_p: nucleus sampling (omlm_sample_nucleus, which rejects values outside (0, 1)); None or 1.0 samples over the
     whole top-k set through omlm_sample / omlm_sample_seeded.
     top_k_rows (int32 [B]), temperature_rows, top_p_rows (float32 [B]): per-sequence arguments (omlm_sample_rows); each
-    one given replaces its scalar; top_p_rows selects the nucleus kernel and is the only way to pass top_p with them."""
+    one given replaces its scalar; top_p_rows selects the nucleus kernel and is the only way to pass top_p with them.
+    logprobs, sample_logprobs (float32 [B, tokens' width]): also write each token's two log-probabilities
+    (omlm_sample_logprob, the same tokens).  They must follow tokens in its allocation (tokens' B rows, then logprobs,
+    then sample_logprobs; see logprob_buffers)."""
+    if logprobs is not None:
+        for t in (logprobs, sample_logprobs, top_k_rows, temperature_rows, top_p_rows):
+            assert t is None or (t.dtype == (torch.int32 if t is top_k_rows else torch.float32) and t.is_cuda and t.is_contiguous())
+        assert sample_logprobs is not None and logprobs.stride(0) == sample_logprobs.stride(0) == tokens.stride(0)
+        assert seeds is None or (seeds.dtype == torch.int64 and seeds.is_contiguous() and seeds.numel() >= B)
+        call("omlm_sample_logprob", _p(logits), _L(logits.stride(0)), _I(C), _I(top_k), _p(top_k_rows), _F(temperature),
+             _p(temperature_rows), _F(1.0 if top_p is None else top_p), _p(top_p_rows), _I(int(allow_eos)), _p(uniform), _p(seed),
+             _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _p(logprobs),
+             _p(sample_logprobs), _stream())
+        return
     if top_k_rows is not None or temperature_rows is not None or top_p_rows is not None:
         assert top_p is None or top_p == 1.0, "per-row sampling takes its nucleus masses through top_p_rows"
         for t, dt in ((top_k_rows, torch.int32), (temperature_rows, torch.float32), (top_p_rows, torch.float32)):
@@ -551,15 +573,31 @@ def sample(logits, C, top_k, temperature, allow_eos, uniform, seed, tokens, next
          _p(seed), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(counters), _p(pos), _I(B), _stream())
 
 
+def logprob_buffers(B, W, device):
+    """(tokens int64 [B, W], logprobs, sample_logprobs float32 [B, W]) in the one allocation the log-probability
+    samplers require."""
+    store = torch.zeros(2 * B * W, device=device, dtype=torch.int64)
+    lp, slp = store[B * W:].view(torch.float32).view(2, B, W).unbind(0)
+    return store[:B * W].view(B, W), lp, slp
+
+
 def sample_rows_indexed(logits, C, allow_eos, seeds, tokens, next_row, row_offset, step_rows, n_rows, top_k_rows, temperature_rows,
-                        top_p_rows=None):
+                        top_p_rows=None, logprobs=None, sample_logprobs=None):
     """omlm_sample_rows_indexed: sequence b samples its token at its own index t = step_rows[b] (int32 [B]) under
     seeds[b] (int64 [B]) while t < n_rows[b] (int32 [B]) and then sets step_rows[b] = t + 1; per-row top_k_rows (int32),
-    temperature_rows and top_p_rows (float32, None: no row narrows to a nucleus) as in omlm_sample_rows."""
+    temperature_rows and top_p_rows (float32, None: no row narrows to a nucleus) as in omlm_sample_rows.
+    logprobs, sample_logprobs: as in sample (omlm_sample_rows_indexed_logprob)."""
     B = logits.shape[0]
     for t, dt in ((seeds, torch.int64), (step_rows, torch.int32), (n_rows, torch.int32), (top_k_rows, torch.int32),
                   (temperature_rows, torch.float32), (top_p_rows, torch.float32)):
         assert t is None or (t.dtype == dt and t.is_cuda and t.is_contiguous() and t.numel() >= B)
+    if logprobs is not None:
+        assert sample_logprobs is not None and logprobs.stride(0) == sample_logprobs.stride(0) == tokens.stride(0)
+        assert logprobs.dtype == sample_logprobs.dtype == torch.float32
+        call("omlm_sample_rows_indexed_logprob", _p(logits), _L(logits.stride(0)), _I(C), _I(1), _p(top_k_rows), _F(1.0),
+             _p(temperature_rows), _p(top_p_rows), _I(int(allow_eos)), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row),
+             _I(row_offset), _p(step_rows), _p(n_rows), _I(B), _p(logprobs), _p(sample_logprobs), _stream())
+        return
     call("omlm_sample_rows_indexed", _p(logits), _L(logits.stride(0)), _I(C), _I(1), _p(top_k_rows), _F(1.0), _p(temperature_rows),
          _p(top_p_rows), _I(int(allow_eos)), _p(seeds), _p(tokens), _L(tokens.stride(0)), _p(next_row), _I(row_offset), _p(step_rows),
          _p(n_rows), _I(B), _stream())

@@ -19,7 +19,7 @@ from collections import deque
 import torch
 
 from . import lib
-from .decode import MAX_BATCH, DecodeSession, check_sampling_rows, seeds_tensor
+from .decode import MAX_BATCH, DecodeSession, check_sampling_rows, prefix_logprobs, seeds_tensor
 
 
 class _Row:
@@ -108,10 +108,10 @@ class _SlotDecode(DecodeSession):
     """DecodeSession over `slots` rows with one position, last position, sample index, token count, seed, predicted-
     sequence offset and set of sampling arguments per row, every one a device array that installs rewrite."""
 
-    def __init__(self, eng, slots: int, max_positions: int):
+    def __init__(self, eng, slots: int, max_positions: int, logprob: bool = False):
         zeros = [0] * slots
         super().__init__(eng, slots, 0, max_positions, seeded=True, ragged=(zeros, zeros, zeros), n_max=max_positions,
-                         rows=(zeros, [1.0] * slots, [None] * slots))
+                         rows=(zeros, [1.0] * slots, [None] * slots), logprob=logprob)
         dev = eng.dev
         self.rows["top_p_rows"] = torch.ones(slots, device=dev, dtype=torch.float32)
         self.t = torch.zeros(slots, device=dev, dtype=torch.int32)
@@ -134,7 +134,7 @@ class _SlotDecode(DecodeSession):
         row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
         lib.sample_rows_indexed(self.logits, eng.C[S], allow_eos, self.seeds, self.tokens, self.next_row, row_offset, self.t,
                                 self.n_rows, self.rows["top_k_rows"], self.rows["temperature_rows"],
-                                self.rows["top_p_rows"] if nucleus else None)
+                                self.rows["top_p_rows"] if nucleus else None, logprobs=self.lp, sample_logprobs=self.slp)
         lib.decode_advance_pos(self.pos, self.pos_last)
 
 
@@ -156,13 +156,18 @@ class GenerationSession:
     use_cuda_graph: replay each step from one CUDA graph per (quantizer slot, kind, nucleus or not), captured on first
     use and never again.  trace_logits (tests): run eagerly and keep the [n, codebook+1] logits each row's tokens were
     sampled from, returned by `traced_logits(handle)` once the row has finished.
+    return_logprobs: `finished()` maps each handle to (tokens, logprobs, sample_logprobs), each [n, q], with the
+    definitions of `generate(..., return_logprobs=True)`; the prefix values come from the row's own prefill.
 
     The transformer's weights are packed when the session is created; train it between sessions, not during one.
     Every row gets exactly what `generate` gives that row alone with seeds=[seed] and the same arguments; free and
     finished slots keep computing values nobody reads."""
 
     def __init__(self, wrapper, slots: int, max_positions: int, allow_eos_in_output=False, include_eos_in_output=False,
-                 append_eos_to_conditioning_tokens=True, max_queue: int = 0, use_cuda_graph=True, trace_logits=False):
+                 append_eos_to_conditioning_tokens=True, max_queue: int = 0, use_cuda_graph=True, trace_logits=False,
+                 return_logprobs=False):
+        if not isinstance(return_logprobs, bool):
+            raise ValueError(f"open_musiclm_b200 GenerationSession: return_logprobs must be a bool, not {return_logprobs!r}")
         for name, v in (("slots", slots), ("max_positions", max_positions), ("max_queue", max_queue)):
             if isinstance(v, bool) or not isinstance(v, numbers.Integral):
                 raise ValueError(f"open_musiclm_b200 GenerationSession: {name} must be an int, not {v!r}")
@@ -181,6 +186,7 @@ class GenerationSession:
         self.allow_eos, self.include_eos, self.append_eos = bool(allow_eos_in_output), bool(include_eos_in_output), \
             bool(append_eos_to_conditioning_tokens)
         self.use_graph, self.trace = bool(use_cuda_graph) and not trace_logits, bool(trace_logits)
+        self.logprob = return_logprobs
         self.sched = SlotSchedule(self.slots, self.q, int(max_queue))
         self._next_handle = 0
         self._done = {}
@@ -193,7 +199,7 @@ class GenerationSession:
     def _device_state(self):
         if self.dec is None:
             self.eng = self.m.engine
-            self.dec = _SlotDecode(self.eng, self.slots, self.max_positions)
+            self.dec = _SlotDecode(self.eng, self.slots, self.max_positions, logprob=self.logprob)
         return self.dec
 
     # ------------------------------------------------------------------------------------------------ requests
@@ -255,7 +261,12 @@ class GenerationSession:
         prefix = pred_token_ids.to(dev, torch.int64).reshape(1, -1) if pred_token_ids is not None else \
             torch.empty(1, 0, device=dev, dtype=torch.int64)
         if n == 0:
-            self._done[handle] = self._output(prefix[0], prefix.new_empty(0))
+            if self.logprob:             # nothing to sample: generate's teacher-forced scoring of the prefix
+                self._done[handle] = tuple(t[0] for t in self.w.generate(
+                    conditioning_token_ids=cond, pred_token_ids=pred_token_ids, max_time_steps=len_pre, return_logprobs=True,
+                    include_eos_in_output=self.include_eos, append_eos_to_conditioning_tokens=self.append_eos))
+            else:
+                self._done[handle] = self._output(prefix[0], prefix.new_empty(0))
             if self.trace:
                 self._traced[handle] = torch.empty(0, self.C, device=dev)
             return handle
@@ -274,7 +285,7 @@ class GenerationSession:
 
     def finished(self):
         """{handle: [n, q] int64 tokens} of the rows that finished since the last call (device tensors): exactly
-        generate(...)[0] for that row alone."""
+        generate(...)[0] for that row alone.  With return_logprobs: {handle: (tokens, logprobs, sample_logprobs)}."""
         done, self._done = self._done, {}
         return done
 
@@ -283,13 +294,20 @@ class GenerationSession:
         return self._traced.pop(handle)
 
     # ------------------------------------------------------------------------------------------------ decoding
-    def _output(self, prefix, new):
-        """generate's output for one row: prefix then samples, everything after an eos masked with -1, [n, q]."""
+    def _output(self, prefix, new, lp=None):
+        """generate's output for one row: prefix then samples, everything after an eos masked with -1, [n, q].  lp:
+        (prefix logprobs, new logprobs, new sample logprobs) -> (tokens, logprobs, sample_logprobs), 0 where -1."""
         sampled = torch.cat([prefix, new])[None]
         eos_mask = (sampled == self.eos).float()                                                  # utils.py:86-93
         if self.include_eos:
             eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))
-        return sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1).view(-1, self.q)
+        sampled = sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1)
+        if lp is None:
+            return sampled.view(-1, self.q)
+        pre, lp_new, slp_new = lp
+        gone = sampled[0] == -1
+        return (sampled.view(-1, self.q), torch.cat([pre, lp_new]).masked_fill(gone, 0.0).view(-1, self.q),
+                torch.cat([torch.zeros_like(pre), slp_new]).masked_fill(gone, 0.0).view(-1, self.q))
 
     def _run(self, key, body):
         """body() eagerly, or from its CUDA graph: one eager run first (lazy cudaFuncSetAttribute calls are not
@@ -328,6 +346,9 @@ class GenerationSession:
             assert pl.N == row.P and pl.pos0[-1] == row.pred_start, (pl.N, row.P)
             ws = eng.workspace(pl, False)
             eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_SlotCapture(dec, row.slot, pl.N))
+            if self.logprob:
+                a["prefix_lp"] = prefix_logprobs(eng, pl, ws, a["prefix"], self.q, self.C)[0] if a["prefix"].shape[1] else \
+                    torch.zeros(0, device=eng.dev)
             p_last = n_tok[-1]
             gi = next(i for i, (s, qi, cnt, base) in enumerate(pl.groups) if s == S - 1 and qi == p_last % self.q)
             dec.logits[row.slot, :eng.Cp[S - 1]].copy_(ws["logits"][gi][p_last // self.q])
@@ -386,7 +407,8 @@ class GenerationSession:
                     self._run(("full", qi, nucleus), lambda qi=qi: (dec.step(qi), dec.sample_rows(qi, allow(qi), nucleus)))
             for row in sched.advance():
                 a = row.payload
-                self._done[row.handle] = self._output(a["prefix"][0], dec.tokens[row.slot, :row.n].clone())
+                lp = (a["prefix_lp"], dec.lp[row.slot, :row.n].clone(), dec.slp[row.slot, :row.n].clone()) if self.logprob else None
+                self._done[row.handle] = self._output(a["prefix"][0], dec.tokens[row.slot, :row.n].clone(), lp)
                 if self.trace:
                     lo = row.trace_start - self._trace_base
                     self._traced[row.handle] = torch.stack([lg[row.slot] for lg in self._trace[lo:lo + row.n]])

@@ -142,6 +142,8 @@ class CoarseStage(_Stage):
     def generate(self, *, semantic_token_ids, coarse_token_ids=None, conditioning_text=None, conditioning_audio=None,
                  clap_token_ids=None, filter_thres=0.9, temperature=1., max_time_steps=10 * 600, include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, reconstruct_wave=False, noise: Optional[NoiseStream] = None, **kwargs):
+        if reconstruct_wave and kwargs.get("return_logprobs", False):
+            raise ValueError("open_musiclm_b200 generate: reconstruct_wave returns a wave, it cannot return log-probabilities")
         clap_token_ids = _clap_ids(clap_token_ids, self.clap, conditioning_audio, conditioning_text)
         out = self._generate([clap_token_ids, semantic_token_ids], coarse_token_ids, noise, max_time_steps=max_time_steps,
                              filter_thres=filter_thres, temperature=temperature, include_eos_in_output=include_eos_in_output,
@@ -169,6 +171,8 @@ class FineStage(_Stage):
     def generate(self, *, coarse_token_ids, fine_token_ids=None, conditioning_text=None, conditioning_audio=None,
                  clap_token_ids=None, filter_thres=0.9, temperature=1., max_time_steps=3 * 600, include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, reconstruct_wave=False, noise: Optional[NoiseStream] = None, **kwargs):
+        if reconstruct_wave and kwargs.get("return_logprobs", False):
+            raise ValueError("open_musiclm_b200 generate: reconstruct_wave returns a wave, it cannot return log-probabilities")
         clap_token_ids = _clap_ids(clap_token_ids, self.clap, conditioning_audio, conditioning_text)
         out = self._generate([clap_token_ids, coarse_token_ids], fine_token_ids, noise, max_time_steps=max_time_steps,
                              filter_thres=filter_thres, temperature=temperature, include_eos_in_output=include_eos_in_output,
