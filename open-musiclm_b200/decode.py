@@ -19,13 +19,14 @@ sequence are then a function of its own inputs and seed, not of the batch it run
 Nucleus sampling (`generate(top_p=...)`) runs in the same captured step, through omlm_sample_nucleus; its semantics are
 stated in `generate`'s docstring.
 
-Prefixes of different lengths (`generate(pred_lengths=...)`) run the same step with one position per sequence
-(DecodeSession.pos [B], the _ragged attention and gather entry points, omlm_decode_advance_pos in place of the
-sampler's position bump); every row gets what it would get alone (DESIGN section 4).
-
-Sampling arguments per row (temperature, filter_thres, top_p, max_time_steps given as one value per row) reach the
-sampler as device arrays (DecodeSession.rows, omlm_sample_rows); rows that sample different numbers of tokens take the
-per-row-position path above.  Every row again gets what it would get alone (DESIGN section 4).
+Every call decodes per row: each sequence has its own position, last position and predicted-sequence offset
+(DecodeSession.pos, pos_last, pos_offset, read by the _ragged attention and omlm_embed_gather_pos_rows, advanced by
+omlm_decode_advance_pos) and its own sampling arguments (DecodeSession.top_k, temperature, top_p, read by
+omlm_sample_rows).  So prefixes of different lengths (`generate(pred_lengths=...)`), sampling arguments given one per
+row, and rows that sample different numbers of tokens need no path of their own, and every row gets what it would get
+alone (DESIGN section 4).  A call is one flow: check (check_sampling_rows, check_pred_lengths), plan (plan_rows,
+check_abs_positions), prompt, prefill, decode loop, assemble (assemble_output); GenerationSession runs the same pieces
+for one row at a time.
 """
 import math
 import numbers
@@ -41,27 +42,48 @@ SKINNY_MAX_BATCH = 16      # up to here the SIMT kernels (skinny_gemm, attn_deco
 MAX_BATCH = 256            # sequences per generate() call
 
 
-class _Capture:
-    """Receives the per-layer K/V rows and pre-conv FFN rows of the prompt from Engine.forward_core."""
+class GraphCache:
+    """Runs a body by key: eagerly the first time (lazy cudaFuncSetAttribute calls are not capturable), captured into a
+    CUDA graph the second time and replayed from then on.  Disabled, every call runs the body eagerly."""
 
-    def __init__(self, sess):
-        self.s = sess
+    def __init__(self, enabled: bool = True):
+        self.enabled, self.graphs, self._warm = enabled, {}, set()
+
+    def run(self, key, body):
+        if not self.enabled:
+            body()
+            return
+        g = self.graphs.get(key)
+        if g is None:
+            if key not in self._warm:
+                body()
+                self._warm.add(key)
+                return
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                body()
+            self.graphs[key] = g
+        g.replay()
+
+
+class _PromptCapture:
+    """Receives the prompt's per-layer K/V rows and pre-conv FFN rows from Engine.forward_core into rows `rows` (a
+    slice) of a DecodeSession: the K/V rows of all n prompt positions, and as conv history rows p - 2, p - 1 of each
+    sequence's own prompt length p (prompt_len, a device array; zero before its first row)."""
+
+    def __init__(self, dec, rows, n, prompt_len):
+        self.dec, self.rows, self.n = dec, rows, n
+        idx = prompt_len[:, None].long() + torch.arange(-2, 0, device=prompt_len.device)
+        self.before = (idx < 0)[..., None]
+        self.idx = (torch.arange(len(prompt_len), device=prompt_len.device)[:, None] * n + idx.clamp_min(0)).view(-1)
 
     def after_kv(self, l, kvn):
-        s = self.s
-        s.cache[l][:, :s.n_prompt].copy_(kvn.view(s.B, s.n_prompt, 128))
+        self.dec.cache[l][self.rows, :self.n].copy_(kvn.view(-1, self.n, 128))
 
     def after_u(self, l, u):
-        s = self.s
-        rows = u.view(s.B, s.n_prompt, -1)
-        if s.ragged:                  # rows n_b - 2, n_b - 1 of each sequence's own prompt (zero before its first row)
-            idx = s.prompt_len[:, None] + torch.arange(-2, 0, device=rows.device)
-            hist = rows[torch.arange(s.B, device=rows.device)[:, None], idx.clamp_min(0)]
-            s.conv[l].copy_(hist.masked_fill((idx < 0)[..., None], 0))
-            return
-        k = min(2, s.n_prompt)
-        s.conv[l].zero_()
-        s.conv[l][:, 2 - k:].copy_(rows[:, s.n_prompt - k:])
+        hist = u.view(-1, u.shape[-1])[self.idx].view(-1, 2, u.shape[-1])
+        self.dec.conv[l][self.rows].copy_(hist.masked_fill(self.before, 0))
 
 
 def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
@@ -96,7 +118,7 @@ def check_top_p(top_p, where: str = "generate"):
 
 def check_pred_lengths(pred_lengths, pred_token_ids, B: int):
     """generate's pred_lengths -> a list of B ints in [0, pred_token_ids.shape[1]], or None when it is None or every
-    value equals pred_token_ids.shape[1] (nothing ragged: the shared-position path).  A wrong count, a value out of
+    value equals pred_token_ids.shape[1] (every prefix whole).  A wrong count, a value out of
     range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError."""
     if pred_lengths is None:
         return None
@@ -188,31 +210,51 @@ def check_sampling_rows(B: int, C: int, temperature, filter_thres, top_p, max_ti
     return temperature, top_k, top_p, max_time_steps
 
 
-class DecodeSession:
-    """Caches and scratch of one generate() call: B sequences, a prompt of n_prompt positions, up to n_new new tokens.
-    seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
-    self.seeds).  pred_start: position of the predicted sequence's start token in the prompt (_Plan.pos0[-1]); with
-    absolute position embeddings the token at position pos is token pos - pred_start - 1 of that sequence.
-    ragged (prompts of different lengths): (prompt_len, pos_init, pos_last), B ints each: sequence b's real prompt
-    length, its first decode position and the last position it processes; self.pos is then one position per sequence
-    and n_max the cache capacity.  Otherwise self.pos is one counter for the whole batch, starting at n_prompt.
-    rows (sampling arguments per sequence): (top_k, temperature, top_p), B values each (top_p None: no nucleus);
-    self.rows then holds them as device arrays, which every sample() reads instead of its scalar arguments.
-    logprob: the sampler also writes each token's two log-probabilities into self.lp and self.slp (fp32 [B, n_new], in
-    the allocation of self.tokens, right after it, as omlm_sample_logprob requires)."""
+_FLOAT_ROWS = ("temperature", "top_p")
 
-    def __init__(self, eng, B: int, n_prompt: int, n_new: int, seeded: bool = False, pred_start: int = 0, ragged=None,
-                 n_max: Optional[int] = None, rows=None, logprob: bool = False):
+
+def row_arrays(dev, B: int, **values):
+    """Per-row device state: each keyword one value or a list of B values -> a [B] device array, float32 for
+    temperature and top_p and int32 otherwise (top_p: None or a list of Nones -> None; a None element -> 1.0).  All of
+    them go up in one non-blocking copy, which CUDA stages from pageable memory before it returns, so that building the
+    state never waits for the device.  (Pinned memory would not help: every graph capture empties PyTorch's pinned
+    cache, and pinning anew costs more than the copy.)"""
+    names, host = [], []
+    for name, v in values.items():
+        if name == "top_p" and (v is None or (isinstance(v, list) and all(p is None for p in v))):
+            continue
+        v = v if isinstance(v, list) else [v] * B
+        dt = torch.float32 if name in _FLOAT_ROWS else torch.int32
+        names.append((name, dt))
+        host.append(torch.tensor([1.0 if x is None else x for x in v], dtype=dt).view(torch.int32))
+    up = torch.stack(host).to(dev, non_blocking=True)
+    out = {name: row.view(dt) for (name, dt), row in zip(names, up)}
+    out.setdefault("top_p", None)
+    return out
+
+
+class DecodeSession:
+    """Caches and scratch of one decode: B sequences, caches of n_max positions, up to n_new new tokens per sequence.
+    rows (row_arrays): the per-sequence state every step and sample reads, as device arrays [B]: pos (the position the
+    next decode step processes), pos_last (the last position the sequence processes; the advance after each sample
+    stops there), pos_offset (with absolute position embeddings the token at position p is token p + pos_offset of the
+    predicted sequence), and the sampling arguments top_k, temperature and top_p (None: no row narrows to a nucleus).
+    seeded: batch-invariant mode (tensor-core path with the B-independent GEMM split at every B, per-sequence seeds in
+    self.seeds).  logprob: the sampler also writes each token's two log-probabilities into self.lp and self.slp (fp32
+    [B, n_new], in the allocation of self.tokens, right after it, as omlm_sample_logprob requires).  use_graph: replay
+    step_and_sample from one CUDA graph per key."""
+
+    def __init__(self, eng, B: int, n_max: int, n_new: int, rows, seeded: bool = False, logprob: bool = False,
+                 use_graph: bool = True):
         if B > MAX_BATCH:
             raise lib.OmlmError(f"open_musiclm_b200 generate: batch sizes above {MAX_BATCH} are not supported by the decode kernels")
         if seeded and eng.h > 16:
             raise lib.OmlmError(f"open_musiclm_b200 generate: seeded generation supports at most 16 heads ({eng.h} given)")
-        self.eng, self.B, self.n_prompt, self.n_new, self.seeded = eng, B, n_prompt, n_new, seeded
+        self.eng, self.B, self.n_max, self.n_new, self.seeded = eng, B, n_max, n_new, seeded
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
         d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
-        self.n_max = n_prompt + n_new if n_max is None else n_max
         E = lambda *shape, dt=bf: torch.empty(*shape, device=dev, dtype=dt)
-        self.cache = [E(B, self.n_max, 128) for _ in range(eng.L)]
+        self.cache = [E(B, n_max, 128) for _ in range(eng.L)]
         self.conv = [E(B, 2, 2 * Fp, dt=a16) for _ in range(eng.L)]
         self.x = [E(B, d, dt=f32) for _ in range(2)]
         self.q_raw, self.kv_raw, self.o = E(B, HD), E(B, 128), E(B, HD)
@@ -228,23 +270,10 @@ class DecodeSession:
             self.tokens = torch.zeros(B, W, device=dev, dtype=torch.int64)
         self.next_row = torch.zeros(B, device=dev, dtype=torch.int32)
         self.counters = torch.zeros(2, device=dev, dtype=torch.int32)          # [sampled so far, block arrival counter]
-        self.ragged = ragged is not None
-        if self.ragged:          # per sequence: the position the next decode step processes, and the last one it will
-            i32 = lambda v: torch.tensor(v, device=dev, dtype=torch.int32)
-            self.prompt_len = torch.tensor(ragged[0], device=dev, dtype=torch.int64)
-            self.pos, self.pos_last = i32(ragged[1]), i32(ragged[2])
-        else:
-            self.pos = torch.full((1,), n_prompt, device=dev, dtype=torch.int32)   # position the next decode step processes
-        self.pos_offset = -(pred_start + 1)
-        self.rows = None
-        if rows is not None:     # filled here, before any graph capture; top_p_rows only when some row has a nucleus
-            k, t, p = rows
-            self.rows = dict(top_k_rows=torch.tensor(k, device=dev, dtype=torch.int32),
-                             temperature_rows=torch.tensor(t, device=dev, dtype=f32),
-                             top_p_rows=None if all(v is None for v in p) else
-                             torch.tensor([1.0 if v is None else v for v in p], device=dev, dtype=f32))
+        self.pos, self.pos_last, self.pos_offset = rows["pos"], rows["pos_last"], rows["pos_offset"]
+        self.top_k, self.temperature, self.top_p = rows["top_k"], rows["temperature"], rows["top_p"]
         # bias table for every distance the generation can reach (it depends on i - j only)
-        N = self.n_max
+        N = n_max
         self.rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, Hr, dt=f32) for _ in range(3)], rp_a=[E(N, Hr, dt=f32) for _ in range(3)],
                        table=E(h, N, dt=f32), rp_a3=[E(N, 3 * eng.Hr8) for _ in range(2)])
         lib.arange_f32(self.rp["rp_in"])
@@ -255,109 +284,73 @@ class DecodeSession:
             self.rp["ones"] = torch.ones(N, device=dev, dtype=f32)
         eng.build_bias_table(self.rp, N)
         self.table = self.rp["table"]
-        self._graphs = {}
+        self.graphs = GraphCache(use_graph)
         # more than 16 sequences, or seeded mode: tensor-core GEMMs and the cache-sharing attention, with their scratch
-        # allocated here so that graph capture allocates nothing
+        # allocated here so that graph capture allocates nothing.  Both paths have the same rounding points (fp32 sums
+        # in another order); seeded mode fixes the GEMMs' K split independently of B, and attn_decode_mqa's
+        # per-sequence CTAs already are.
         self.batched = B > SKINNY_MAX_BATCH or seeded
         self.seeds = torch.zeros(B, device=dev, dtype=torch.int64) if seeded else None
         if self.batched:
             shapes = [(HD, d), (128, d), (d, HD), (2 * Fp, d), (d, Fp)] + [(cp, d) for cp in eng.Cp]
-            self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=self.n_max, heads=h, invariant=seeded)
+            ws = self.ws = lib.DecodeWorkspace(dev, B, shapes, max_pos=n_max, heads=h, invariant=seeded)
+            self._gemm = lambda *a, **k: lib.decode_gemm(*a, ws=ws, invariant=seeded, **k)
+            self._attn = lambda *a: lib.attn_decode_mqa(*a, ws=ws, ragged=True)
+        else:
+            self._gemm = lib.skinny_gemm
+            self._attn = lambda *a: lib.attn_decode(*a, ragged=True)
 
     # ------------------------------------------------------------------------------------------ one incremental step
     def embed(self, x):
-        """x = the input rows of the position self.pos: embedding row self.next_row, plus with absolute position
-        embeddings the predicted sequence's row for its token self.pos - pred_start - 1 (open_musiclm.py:134-136)."""
+        """x = the input rows of the positions self.pos: embedding row self.next_row, plus with absolute position
+        embeddings the predicted sequence's row for its token pos + pos_offset (open_musiclm.py:134-136)."""
         eng = self.eng
         if eng.abs_pos:
-            lib.embed_gather_pos(eng.table, self.next_row, self.pos, self.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x,
-                                 ragged=self.ragged)
+            lib.embed_gather_pos_rows(eng.table, self.next_row, self.pos, self.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x)
         else:
             lib.embed_gather(eng.table, self.next_row, x)
 
     def step(self, qi_next: int):
-        """Processes the position self.pos (embedding row self.next_row) through all layers and leaves the logits of
+        """Processes the positions self.pos (embedding rows self.next_row) through all layers and leaves the logits of
         head qi_next in self.logits (one launch per operation)."""
-        if self.batched:
-            return self.step_batched(qi_next)
-        eng, B = self.eng, self.B
-        pv, d, HD, F, Fp, h = eng.pview, eng.d, eng.HD, eng.F, eng.Fp, eng.h
-        xa, xm = self.x
-        self.embed(xa)
-        for l in range(eng.L):
-            p, pk = f"transformer.layers.{l}.", eng.pk[l]
-            lib.skinny_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"])
-            lib.skinny_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1)
-            lib.attn_decode(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
-                            self.n_max, self.o, h, ragged=self.ragged)
-            lib.skinny_gemm(self.o, pk["wo_b"], xm, addend=xa)
-            lib.skinny_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]])
-            lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
-            lib.skinny_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm)
-        S = len(eng.seqs) - 1
-        lib.skinny_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"])
-
-    def step_batched(self, qi_next: int):
-        """step for more than 16 sequences (or seeded mode): the same operations on the tensor-core GEMM and the
-        cache-sharing attention (same rounding points; fp32 sums in another order).  Seeded mode fixes the GEMMs' K split
-        independently of B; attn_decode_mqa's per-sequence CTAs already are."""
-        eng, ws, inv = self.eng, self.ws, self.seeded
+        eng, gemm = self.eng, self._gemm
         pv, F, h = eng.pview, eng.F, eng.h
         xa, xm = self.x
         self.embed(xa)
         for l in range(eng.L):
             p, pk = f"transformer.layers.{l}.", eng.pk[l]
-            lib.decode_gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"], ws=ws, invariant=inv)
-            lib.decode_gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1, ws=ws, invariant=inv)
-            lib.attn_decode_mqa(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
-                                self.n_max, self.o, h, ws=ws, ragged=self.ragged)
-            lib.decode_gemm(self.o, pk["wo_b"], xm, addend=xa, ws=ws, invariant=inv)
-            lib.decode_gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]], ws=ws, invariant=inv)
+            gemm(xa, pk["wq"], self.q_raw, prologue=2, gamma=pv[p + "0.norm.gamma"])
+            gemm(xa, pk["wkv_b"], self.kv_raw, prologue=1)
+            self._attn(self.q_raw, self.kv_raw, pv[p + "0.q_scale"], pv[p + "0.k_scale"], self.cache[l], self.table, self.pos,
+                       self.n_max, self.o, h)
+            gemm(self.o, pk["wo_b"], xm, addend=xa)
+            gemm(xm, pk["w1"], self.u_new, prologue=2, gamma=pv[p + eng.ffk["g1"]])
             lib.decode_conv_geglu(self.u_new, self.conv[l], pk["conv"], self.h, self.rowsum)
-            lib.decode_gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm, ws=ws, invariant=inv)
+            gemm(self.h, pk["w2"], xa, prologue=3, gamma=pk["gin"], rowsum=self.rowsum, n_real=F, addend=xm)
         S = len(eng.seqs) - 1
-        lib.decode_gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"], ws=ws,
-                        invariant=inv)
+        gemm(xa, eng.pk_logit[S][qi_next], self.logits[:, :eng.Cp[S]], prologue=2, gamma=pv["transformer.norm.gamma"])
 
-    def sample(self, qi: int, top_k: int, temperature: float, allow_eos: bool, uniform, seed, bump_pos: bool, top_p=None):
+    def row_offset(self, qi: int) -> int:
+        """Embedding row of token 0 of quantizer slot qi in the predicted sequence."""
         eng = self.eng
         S = len(eng.seqs) - 1
-        q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
-        row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
-        pos = self.pos if bump_pos and not self.ragged else None
-        if self.rows is not None:        # per-row arguments: top_k, temperature and top_p are not used
-            lib.sample(self.logits, eng.C[S], 1, 1.0, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                       self.counters, pos, self.B, seeds=self.seeds, logprobs=self.lp, sample_logprobs=self.slp, **self.rows)
-        else:
-            lib.sample(self.logits, eng.C[S], top_k, temperature, allow_eos, uniform, seed, self.tokens, self.next_row, row_offset,
-                       self.counters, pos, self.B, seeds=self.seeds, top_p=top_p, logprobs=self.lp, sample_logprobs=self.slp)
-        if bump_pos and self.ragged:
+        return eng.emb_row_base[S] + (eng.seqs[S].codebook_size * qi if eng.seqs[S].num_quantizers > 1 else 0)
+
+    def sample(self, qi: int, allow_eos: bool, uniform, seed, advance: bool = True):
+        """Every sequence samples the token of quantizer slot qi with its own arguments; then (advance) every position
+        moves on, up to its sequence's last."""
+        eng = self.eng
+        lib.sample(self.logits, eng.C[-1], 1, 1.0, allow_eos, uniform, seed, self.tokens, self.next_row, self.row_offset(qi),
+                   self.counters, None, self.B, seeds=self.seeds, top_k_rows=self.top_k, temperature_rows=self.temperature,
+                   top_p_rows=self.top_p, logprobs=self.lp, sample_logprobs=self.slp)
+        if advance:
             lib.decode_advance_pos(self.pos, self.pos_last)
 
-    def step_and_sample(self, qi: int, qi_next: int, top_k, temperature, allow_eos_next, uniform, seed, use_graph=True, top_p=None):
-        """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next."""
-        if self.rows is not None:        # the arrays' contents are read at replay; only the kernel choice is captured
-            key = (qi, qi_next, "rows", bool(allow_eos_next), uniform is not None, self.seeded, self.rows["top_p_rows"] is not None,
-                   self.logprob)
-        else:
-            key = (qi, qi_next, top_k, float(temperature), bool(allow_eos_next), uniform is not None, self.seeded, top_p, self.logprob)
-        g = self._graphs.get(key)
-        if g is None or not use_graph:
-            body = lambda: (self.step(qi_next), self.sample(qi_next, top_k, temperature, allow_eos_next, uniform, seed, True, top_p))
-            if not use_graph:
-                body()
-                return
-            count = self._graphs.get(("warm",) + key, 0)
-            if count < 1:                 # one eager run first (lazy cudaFuncSetAttribute calls are not capturable)
-                body()
-                self._graphs[("warm",) + key] = count + 1
-                return
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
-            self._graphs[key] = g
-        g.replay()
+    def step_and_sample(self, qi: int, qi_next: int, allow_eos_next, uniform, seed):
+        """decode step on the token sampled for quantizer slot qi, then sample the token of slot qi_next.  The arrays'
+        contents are read at replay; only the kernel choice is captured."""
+        self.graphs.run((qi, qi_next, bool(allow_eos_next), uniform is not None),
+                        lambda: (self.step(qi_next), self.sample(qi_next, allow_eos_next, uniform, seed)))
 
 
 def prefix_labels(prompt, q: int, C: int):
@@ -388,25 +381,96 @@ def prefix_logprobs(eng, pl, ws, prompt, q: int, C: int):
     return out
 
 
-def assemble_logprobs(sampled, pre_lp, lp_new, slp_new, n_real, n_end):
-    """The [B, W] logprobs and sample_logprobs of generate's flat output `sampled` (after the eos masking): row b's
-    columns below n_real[b] are prefix tokens (pre_lp [B, >= their count], sample log p 0), columns n_real[b] ...
-    n_end[b] - 1 its samples in order (lp_new, slp_new [B, n_new]; None when nothing was sampled), and every column
-    that holds -1 is 0 in both.  n_real, n_end: int64 [B, 1]."""
-    B, W = sampled.shape
-    col = torch.arange(W, device=sampled.device)[None]
-    lp = torch.zeros(B, W, device=sampled.device, dtype=torch.float32)
-    w = min(W, pre_lp.shape[1])
-    lp[:, :w] = pre_lp[:, :w]
-    lp.masked_fill_(col >= n_real, 0.0)
+def plan_rows(pred_token_ids, B: int, q: int, lengths, max_time_steps):
+    """Per row of a generate call: (n_real, n_new), the number of real prefix tokens and the number of tokens to sample
+    (open_musiclm.py:276).  lengths: check_pred_lengths' result (None: every prefix is whole); max_time_steps: one int
+    or B ints, as check_sampling_rows returns it.  A prefix given flat as [b, n] on a stage with q > 1 is n tokens,
+    and sampling continues at quantizer n mod q."""
+    T = 0 if pred_token_ids is None else pred_token_ids.shape[1]
+    per_step = math.prod(pred_token_ids.shape[2:]) if T else q          # prefix tokens per step of pred_token_ids.shape[1]
+    if lengths is not None and per_step != q:
+        raise ValueError(f"open_musiclm_b200 generate: pred_lengths needs pred_token_ids of whole time steps, [b, t, {q}]")
+    lengths = lengths if lengths is not None else [T] * B
+    steps = max_time_steps if isinstance(max_time_steps, list) else [max_time_steps] * B
+    return [n * per_step for n in lengths], [max(0, (t - n) * q) for t, n in zip(steps, lengths)]
+
+
+def check_abs_positions(where: str, lim: int, cond_lens, n_real, n_new):
+    """The reference looks up arange(len) in each sequence's nn.Embedding(max_absolute_position_embeddings): IndexError
+    when something is sampled and a conditioning sequence (with its eos) has more than lim tokens, or a row that
+    samples feeds back a token past lim (its last sampled token is never fed back).  The message names the row when the
+    rows differ."""
+    if not any(n_new):
+        return
+    for s, n in enumerate(cond_lens):
+        if n > lim:
+            raise IndexError(f"{where}: conditioning sequence {s} has {n} tokens but max_absolute_position_embeddings is {lim}")
+    row = len(set(zip(n_real, n_new))) > 1
+    for b, (n, k) in enumerate(zip(n_real, n_new)):
+        if k > 0 and n + k - 1 > lim:
+            raise IndexError(f"{where}: the predicted sequence{f' of row {b}' if row else ''} reaches {n + k - 1} tokens "
+                             f"({n} given + {k} sampled - 1) but max_absolute_position_embeddings is {lim}")
+
+
+def prefill(wrapper, cond, prompt, append_eos: bool, dec=None, rows=slice(None), prompt_len=None):
+    """Runs the prompt (conditioning sequences, eos appended when append_eos, then the predicted sequence's prompt
+    tokens) through the regular forward once.  With a DecodeSession dec it also writes the prompt's caches into dec's
+    rows `rows` (_PromptCapture) and the logits of each sequence's last real prompt position into dec.logits; that
+    position is prompt_len - 1 (int device array [b]), and the last real prompt tokens of all sequences share a
+    quantizer slot.  Returns (plan, workspace) for prefix_logprobs."""
+    eng = wrapper.transformer.engine
+    B, S, q = prompt.shape[0], len(eng.seqs), eng.seqs[-1].num_quantizers
+    if append_eos:                                                                                   # open_musiclm.py:288-290
+        cond = [torch.cat([t, torch.full((B, 1), e, device=eng.dev, dtype=torch.int64)], 1) for t, e in zip(cond, wrapper.eos_ids)]
+    _, src_row, key_mask, _, n_tok = lib.token_plan(
+        cond + [prompt], [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
+        append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
+    pl = eng.plan(B, n_tok)
+    ws = eng.workspace(pl, False)
+    capture = None if dec is None else _PromptCapture(dec, rows, pl.N, prompt_len)
+    eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=capture)
+    if dec is not None:
+        # final sequence, head group of the next token's quantizer slot; in it, each sequence's row of its last token
+        gi = next(i for i, (s, qi, cnt, base) in enumerate(pl.groups) if s == S - 1 and qi == n_tok[-1] % q)
+        cnt = pl.groups[gi][2]
+        last = torch.arange(B, device=eng.dev) * cnt + (prompt_len - pl.pos0[-1] - 1) // q
+        dec.logits[rows, :eng.Cp[S - 1]].copy_(ws["logits"][gi][last])
+    return pl, ws
+
+
+def assemble_output(prefix, new, n_real, n_end, width: int, eos: int, include_eos: bool, q: int, logprobs=None):
+    """generate's output [b, width / q, q]: row r holds its n_real[r] prefix tokens (prefix [b, >= that]), then its
+    samples new[r, :n_end[r] - n_real[r]], then -1; everything after an eos is -1 (the eos too unless include_eos;
+    utils.py:86-93).  n_real, n_end: ints or int tensors [b, 1].  logprobs: (pre_lp [b, >= the prefix tokens' count]
+    or None for zeros, lp_new, slp_new [b, >= the samples' count]) -> (tokens, logprobs, sample_logprobs): prefix
+    columns take pre_lp (sample log p 0), sampled columns lp_new and slp_new in order, and every -1 is 0 in both."""
+    B, n_new = new.shape
+    col = torch.arange(width, device=prefix.device)[None]
+    in_new = (col >= n_real) & (col < n_end)
+    src = (col - n_real).clamp(0, max(n_new - 1, 0)).expand(B, -1)
+    sampled = torch.full((B, width), -1, device=prefix.device, dtype=torch.int64)
+    sampled[:, :min(width, prefix.shape[1])] = prefix[:, :width]
+    sampled.masked_fill_(col >= n_real, -1)
+    if n_new > 0:
+        sampled = torch.where(in_new, new.gather(1, src), sampled)
+    eos_mask = (sampled == eos).float()
+    if include_eos:
+        eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))
+    sampled = sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1)
+    if logprobs is None:
+        return sampled.view(B, -1, q)
+    pre_lp, lp_new, slp_new = logprobs
+    lp = torch.zeros(B, width, device=prefix.device, dtype=torch.float32)
+    if pre_lp is not None:
+        w = min(width, pre_lp.shape[1])
+        lp[:, :w] = pre_lp[:, :w]
+        lp.masked_fill_(col >= n_real, 0.0)
     slp = torch.zeros_like(lp)
-    if lp_new is not None:
-        in_new = (col >= n_real) & (col < n_end)
-        src = (col - n_real).clamp(0, lp_new.shape[1] - 1).expand(B, -1)
+    if n_new > 0:
         lp = torch.where(in_new, lp_new.gather(1, src), lp)
         slp = torch.where(in_new, slp_new.gather(1, src), slp)
     gone = sampled == -1
-    return lp.masked_fill(gone, 0.0), slp.masked_fill(gone, 0.0)
+    return sampled.view(B, -1, q), lp.masked_fill(gone, 0.0).view(B, -1, q), slp.masked_fill(gone, 0.0).view(B, -1, q)
 
 
 class TokenConditionedTransformerWrapper(nn.Module):
@@ -516,153 +580,77 @@ class TokenConditionedTransformerWrapper(nn.Module):
         info, eos = self.token_sequences[-1], self.eos_ids[-1]
         C = info.codebook_size + 1
         temperature, top_k, top_p, max_time_steps = check_sampling_rows(B, C, temperature, filter_thres, top_p, max_time_steps)
-        lengths = check_pred_lengths(pred_lengths, pred_token_ids, B)                               # None: one length
-        per_row = any(isinstance(v, list) for v in (temperature, top_k, top_p))     # sampled from per-row arrays
+        lengths = check_pred_lengths(pred_lengths, pred_token_ids, B)
         m, eng = self.transformer, self.transformer.engine
-        S = len(self.token_sequences)
-        assert len(conditioning_token_ids) == S - 1
+        assert len(conditioning_token_ids) == len(self.token_sequences) - 1
         q = info.num_quantizers
-        init_step = pred_token_ids.shape[1] if pred_token_ids is not None else 0                    # :276
-        steps_b = max_time_steps if isinstance(max_time_steps, list) else [max_time_steps] * B
-        if isinstance(max_time_steps, list) or lengths is not None:
-            n_new_b = [max(0, (t - n) * q) for t, n in zip(steps_b, lengths or [init_step] * B)]   # per row, :276
-            if lengths is None and len(set(n_new_b)) > 1:
-                lengths = [init_step] * B        # rows that sample different numbers of tokens: the per-row-position path
-            n_new = max(n_new_b)
-        else:
-            n_new = max(0, (max_time_steps - init_step) * q)
-        if eng.abs_pos and n_new > 0:
-            # the reference looks up arange(len) in each sequence's nn.Embedding(max_absolute_position_embeddings)
-            lim = eng.max_abs_pos
-            for s, t in enumerate(conditioning_token_ids):
-                n = t.numel() // B + (1 if append_eos_to_conditioning_tokens else 0)
-                if n > lim:
-                    raise IndexError(f"open_musiclm_b200 generate: conditioning sequence {s} has {n} tokens but "
-                                     f"max_absolute_position_embeddings is {lim}")
-            if lengths is None:
-                n_pre = pred_token_ids.numel() // B if pred_token_ids is not None else 0
-                if n_pre + n_new - 1 > lim:
-                    raise IndexError(f"open_musiclm_b200 generate: the predicted sequence reaches {n_pre + n_new - 1} tokens "
-                                     f"({n_pre} given + {n_new} sampled - 1) but max_absolute_position_embeddings is {lim}")
-            else:
-                for b, (n, k) in enumerate(zip(lengths, n_new_b)):          # only rows that sample feed tokens back
-                    if k > 0 and n * q + k - 1 > lim:
-                        raise IndexError(f"open_musiclm_b200 generate: the predicted sequence of row {b} reaches {n * q + k - 1} "
-                                         f"tokens ({n * q} given + {k} sampled - 1) but max_absolute_position_embeddings is {lim}")
+        n_real, n_new = plan_rows(pred_token_ids, B, q, lengths, max_time_steps)
+        N = max(n_new)                                               # decode steps: those of the row that samples most
+        eos_len = 1 if append_eos_to_conditioning_tokens else 0
+        if eng.abs_pos:
+            check_abs_positions("open_musiclm_b200 generate", eng.max_abs_pos, [t.numel() // B + eos_len for t in conditioning_token_ids],
+                                n_real, n_new)
         was_training = m.training
         m.eval()
         dev = eng.dev
         cond = [t.to(dev, torch.int64).reshape(B, -1) for t in conditioning_token_ids]
-        if append_eos_to_conditioning_tokens:                                                       # :288-290
-            cond = [torch.cat([t, torch.full((B, 1), e, device=dev, dtype=torch.int64)], 1) for t, e in zip(cond, self.eos_ids)]
         if pred_token_ids is not None:
             assert pred_token_ids.shape[0] == B
             prefix = pred_token_ids.to(dev, torch.int64).reshape(B, -1)
         else:
             prefix = torch.empty(B, 0, device=dev, dtype=torch.int64)
         seed_vals = seeds_tensor(seeds, B, dev) if seeds is not None else None
-        if lengths is not None:
-            # the prompt: the prefixes cut to the longest real prefix of a row that samples (a row that samples nothing
-            # takes part cut to it), right-padded with token 0.  The predicted sequence comes last, so causal attention
-            # keeps every real position away from the padding and the prefill runs unchanged.
-            n_real = torch.tensor(lengths, device=dev, dtype=torch.int64)[:, None] * q
-            Lp = max([n for n, k in zip(lengths, n_new_b) if k > 0], default=0)
-            if return_logprobs:              # every real prefix token needs its prefill row
-                Lp = max(Lp, max(lengths))
-            L_eff = [min(n, Lp) for n in lengths]
-            prompt = prefix[:, :Lp * q].masked_fill(torch.arange(Lp * q, device=dev)[None] >= n_real.clamp(max=Lp * q), 0)
-        else:
-            prompt = prefix
-        pre_lp = None
-        if n_new > 0 or (return_logprobs and prompt.shape[1] > 0):
-            ids = cond + [prompt]
-            _, src_row, key_mask, _, n_tok = lib.token_plan(
-                ids, [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
-                append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
-            pl = eng.plan(B, n_tok)
-            sess = None
-        if n_new > 0:
-            if top_k is None:
-                top_k = max(int((1 - filter_thres) * C), 1)                                          # utils.py:80
-            rows = None
-            if per_row:                          # every argument as B values (a single value repeated)
-                rows = tuple(v if isinstance(v, list) else [v] * B for v in (top_k, temperature, top_p))
-            if lengths is None:
-                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1], rows=rows,
-                                     logprob=return_logprobs)
-            else:
-                # per row: real prompt length, last position the row processes (a row with all its tokens stays there),
-                # first decode position; the cache holds the longest prompt and every row's new positions
-                P = [pl.pos0[-1] + 1 + n * q for n in L_eff]
-                pos_last = [p + max(k, 1) - 2 for p, k in zip(P, n_new_b)]
-                sess = DecodeSession(eng, B, pl.N, n_new, seeded=seed_vals is not None, pred_start=pl.pos0[-1],
-                                     ragged=(P, [min(p, e) for p, e in zip(P, pos_last)], pos_last),
-                                     n_max=max([pl.N] + [p + k for p, k in zip(P, n_new_b)]), rows=rows, logprob=return_logprobs)
+        # the prompt: the prefixes cut to the longest real prefix of a row that samples (of every row, for the prefix
+        # log-probabilities; a longer prefix takes part cut to it), right-padded with token 0.  The predicted sequence
+        # comes last, so causal attention keeps every real position away from the padding.  Row r's prompt is P[r]
+        # positions long: it processes P[r], P[r] + 1, ... up to its last position, where it stays.
+        Lp = max([n for n, k in zip(n_real, n_new) if k > 0 or return_logprobs], default=0)
+        pred_start = sum(t.shape[1] + eos_len + 1 for t in cond)
+        P = [pred_start + 1 + min(n, Lp) for n in n_real]
+        state = dict(prompt_len=P, n_real=n_real, n_end=[n + k for n, k in zip(n_real, n_new)])
+        if N > 0:
+            pos_last = [p + max(k, 1) - 2 for p, k in zip(P, n_new)]
+            state.update(pos=[min(p, e) for p, e in zip(P, pos_last)], pos_last=pos_last, pos_offset=-(pred_start + 1),
+                         top_k=max(int((1 - filter_thres) * C), 1) if top_k is None else top_k,                  # utils.py:80
+                         temperature=temperature, top_p=top_p)
+        rows = row_arrays(dev, B, **state)
+        prompt = prefix[:, :Lp].masked_fill(torch.arange(Lp, device=dev)[None] >= rows["n_real"][:, None], 0)
+        sess = None
+        if N > 0:
+            sess = DecodeSession(eng, B, max(P[b] + n_new[b] for b in range(B)), N, rows, seeded=seed_vals is not None,
+                                 logprob=return_logprobs, use_graph=use_cuda_graph)
             if seed_vals is not None:
                 sess.seeds.copy_(seed_vals)
-        if n_new > 0 or (return_logprobs and prompt.shape[1] > 0):
-            ws = eng.workspace(pl, False)
-            eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_Capture(sess) if sess is not None else None)
-            if return_logprobs and prompt.shape[1] > 0:
+        pre_lp = lp_new = slp_new = None
+        if N > 0 or (return_logprobs and Lp > 0):
+            pl, ws = prefill(self, cond, prompt, append_eos_to_conditioning_tokens, sess, prompt_len=rows["prompt_len"])
+            assert pl.pos0[-1] == pred_start, (pl.pos0, pred_start)
+            if return_logprobs and Lp > 0:
                 pre_lp = prefix_logprobs(eng, pl, ws, prompt, q, C)
-        if n_new > 0:
-            # logits of the prompt's last position: final sequence, position p_last = its token count, head p_last mod q
-            # (per row: its own last real position; every prefix is whole time steps, so the head is the same)
-            p_last = n_tok[-1]
-            gi = next(i for i, (s, qi, cnt, base) in enumerate(pl.groups) if s == S - 1 and qi == p_last % q)
-            cnt = pl.groups[gi][2]
-            last = p_last // q if lengths is None else torch.tensor(L_eff, device=dev)
-            rows = torch.arange(B, device=dev) * cnt + last
-            sess.logits[:, :eng.Cp[S - 1]].copy_(ws["logits"][gi][rows])
+        new = prefix.new_empty(B, 0)
+        if N > 0:
             uni = None
             if uniform_noise is not None:
                 uni = uniform_noise.to(dev, torch.float32).contiguous()
-                assert uni.shape == (n_new, B, info.codebook_size + 1), uni.shape
-            p0 = prompt.shape[1]                                     # flat index of the first sampled token
+                assert uni.shape == (N, B, info.codebook_size + 1), uni.shape
             allow = lambda p: bool(allow_eos_in_output and (p % q) == q - 1)                        # :311-313
             if trace_logits is not None:
                 trace_logits.append(sess.logits[:, :C].clone())
-            sess.sample(p0 % q, top_k, temperature, allow(p0), uni, eng.seed, bump_pos=False, top_p=top_p)
-            for s in range(1, n_new):
-                p = p0 + s
+            sess.sample(Lp % q, allow(Lp), uni, eng.seed, advance=False)
+            for p in range(Lp + 1, Lp + N):                          # p: flat index of the sampled token
                 if trace_logits is not None:      # eager, in two halves, so that the logits can be copied in between
                     sess.step(p % q)
                     trace_logits.append(sess.logits[:, :C].clone())
-                    sess.sample(p % q, top_k, temperature, allow(p), uni, eng.seed, True, top_p=top_p)
+                    sess.sample(p % q, allow(p), uni, eng.seed)
                 else:
-                    sess.step_and_sample((p - 1) % q, p % q, top_k, temperature, allow(p), uni, eng.seed, use_graph=use_cuda_graph,
-                                         top_p=top_p)
+                    sess.step_and_sample((p - 1) % q, p % q, allow(p), uni, eng.seed)
             if seed_vals is None:
                 eng.seed += 1
-            new = sess.tokens[:, :n_new]
-        if lengths is None:
-            sampled = torch.cat([prefix, new], 1) if n_new > 0 else prefix
-            n_real = torch.full((B, 1), prefix.shape[1], device=dev, dtype=torch.int64)
-            n_end = n_real + n_new
-        else:
-            # row b: its n_real[b] prefix tokens, then its n_new_b[b] samples, then -1 up to the widest row
-            width = max(max(t, n) for t, n in zip(steps_b, lengths)) * q
-            col = torch.arange(width, device=dev)[None]
-            n_end = n_real + torch.tensor(n_new_b, device=dev, dtype=torch.int64)[:, None]
-            sampled = torch.full((B, width), -1, device=dev, dtype=torch.int64)
-            sampled[:, :min(width, prefix.shape[1])] = prefix[:, :width]
-            sampled.masked_fill_(col >= n_real, -1)
-            if n_new > 0:
-                sampled = torch.where((col >= n_real) & (col < n_end), new.gather(1, (col - n_real).clamp(0, n_new - 1).expand(B, -1)),
-                                      sampled)
-        eos_mask = (sampled == eos).float()                                                         # utils.py:86-93
-        if include_eos_in_output:
-            eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))
-        sampled = sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1)
+            new, lp_new, slp_new = sess.tokens[:, :N], sess.lp, sess.slp
         if was_training:
             m.train()
-        if return_logprobs:
-            if pre_lp is None:
-                pre_lp = torch.zeros(B, prompt.shape[1], device=dev, dtype=torch.float32)
-            lp, slp = assemble_logprobs(sampled, pre_lp, sess.lp[:, :n_new] if n_new > 0 else None,
-                                        sess.slp[:, :n_new] if n_new > 0 else None, n_real, n_end)
-            return sampled.view(B, -1, q), lp.view(B, -1, q), slp.view(B, -1, q)
-        return sampled.view(B, -1, q)                                                               # :323-324
+        return assemble_output(prefix, new, rows["n_real"][:, None], rows["n_end"][:, None], max(state["n_end"]), eos,
+                               include_eos_in_output, q, (pre_lp, lp_new, slp_new) if return_logprobs else None)
 
     def forward(self, *, all_token_ids: List[torch.Tensor], return_loss: bool = False, **kwargs):
         """open_musiclm.py:328-411.  return_loss=True: (loss, None, None) with the loss computed by the fused path

@@ -19,7 +19,8 @@ from collections import deque
 import torch
 
 from . import lib
-from .decode import MAX_BATCH, DecodeSession, check_sampling_rows, prefix_logprobs, seeds_tensor
+from .decode import (MAX_BATCH, DecodeSession, GraphCache, assemble_output, check_abs_positions, check_sampling_rows, plan_rows,
+                     prefill, prefix_logprobs, row_arrays, seeds_tensor)
 
 
 class _Row:
@@ -88,53 +89,22 @@ class SlotSchedule:
         return done
 
 
-class _SlotCapture:
-    """Receives the prompt's K/V rows and pre-conv FFN rows from Engine.forward_core (one row) into one slot."""
-
-    def __init__(self, dec, slot, n):
-        self.dec, self.slot, self.n = dec, slot, n
-
-    def after_kv(self, l, kvn):
-        self.dec.cache[l][self.slot, :self.n].copy_(kvn.view(self.n, 128))
-
-    def after_u(self, l, u):
-        rows, conv = u.view(self.n, -1), self.dec.conv[l][self.slot]
-        k = min(2, self.n)
-        conv.zero_()
-        conv[2 - k:].copy_(rows[self.n - k:])
-
-
 class _SlotDecode(DecodeSession):
-    """DecodeSession over `slots` rows with one position, last position, sample index, token count, seed, predicted-
-    sequence offset and set of sampling arguments per row, every one a device array that installs rewrite."""
+    """DecodeSession over `slots` rows with, on top of its per-row state, one sample index and token count per row,
+    device arrays that installs rewrite."""
 
-    def __init__(self, eng, slots: int, max_positions: int, logprob: bool = False):
-        zeros = [0] * slots
-        super().__init__(eng, slots, 0, max_positions, seeded=True, ragged=(zeros, zeros, zeros), n_max=max_positions,
-                         rows=(zeros, [1.0] * slots, [None] * slots), logprob=logprob)
-        dev = eng.dev
-        self.rows["top_p_rows"] = torch.ones(slots, device=dev, dtype=torch.float32)
-        self.t = torch.zeros(slots, device=dev, dtype=torch.int32)
-        self.n_rows = torch.zeros(slots, device=dev, dtype=torch.int32)
-        self.pos_offset_rows = torch.zeros(slots, device=dev, dtype=torch.int32)
-
-    def embed(self, x):
-        eng = self.eng
-        if eng.abs_pos:
-            lib.embed_gather_pos_rows(eng.table, self.next_row, self.pos, self.pos_offset_rows, eng.abs_row_base[-1], eng.max_abs_pos, x)
-        else:
-            lib.embed_gather(eng.table, self.next_row, x)
+    def __init__(self, eng, slots: int, max_positions: int, logprob: bool):
+        rows = row_arrays(eng.dev, slots, pos=0, pos_last=0, pos_offset=0, top_k=0, temperature=1.0, top_p=1.0)
+        super().__init__(eng, slots, max_positions, max_positions, rows, seeded=True, logprob=logprob)
+        self.t = torch.zeros(slots, device=eng.dev, dtype=torch.int32)
+        self.n_rows = torch.zeros(slots, device=eng.dev, dtype=torch.int32)
 
     def sample_rows(self, qi: int, allow_eos: bool, nucleus: bool):
         """Every row with tokens left samples the token of quantizer slot qi at its own sample index; then every
         position advances (up to its row's last)."""
-        eng = self.eng
-        S = len(eng.seqs) - 1
-        q, cb = eng.seqs[S].num_quantizers, eng.seqs[S].codebook_size
-        row_offset = eng.emb_row_base[S] + (cb * qi if q > 1 else 0)
-        lib.sample_rows_indexed(self.logits, eng.C[S], allow_eos, self.seeds, self.tokens, self.next_row, row_offset, self.t,
-                                self.n_rows, self.rows["top_k_rows"], self.rows["temperature_rows"],
-                                self.rows["top_p_rows"] if nucleus else None, logprobs=self.lp, sample_logprobs=self.slp)
+        lib.sample_rows_indexed(self.logits, self.eng.C[-1], allow_eos, self.seeds, self.tokens, self.next_row, self.row_offset(qi),
+                                self.t, self.n_rows, self.top_k, self.temperature, self.top_p if nucleus else None,
+                                logprobs=self.lp, sample_logprobs=self.slp)
         lib.decode_advance_pos(self.pos, self.pos_last)
 
 
@@ -193,13 +163,13 @@ class GenerationSession:
         self._traced = {}
         self._trace = []               # trace mode: the [slots, C] logits of every sample point since _trace_base
         self._trace_base = 0
-        self._graphs, self._warm = {}, set()
+        self._graphs = GraphCache(self.use_graph)
         self.eng = self.dec = None     # the engine and the slots' device state, made by the first step that runs a row
 
     def _device_state(self):
         if self.dec is None:
             self.eng = self.m.engine
-            self.dec = _SlotDecode(self.eng, self.slots, self.max_positions, logprob=self.logprob)
+            self.dec = _SlotDecode(self.eng, self.slots, self.max_positions, self.logprob)
         return self.dec
 
     # ------------------------------------------------------------------------------------------------ requests
@@ -238,18 +208,11 @@ class GenerationSession:
             [v.item() if isinstance(v, torch.Tensor) else v]
         temperature, top_k, top_p, max_time_steps = check_sampling_rows(1, self.C, one(temperature), one(filter_thres), one(top_p),
                                                                         one(max_time_steps))
-        len_pre = pred_token_ids.shape[1] if pred_token_ids is not None else 0
-        n = max(0, (max_time_steps - len_pre) * q)
+        (n_pre,), (n,) = plan_rows(pred_token_ids, 1, q, None, max_time_steps)
         cond_lens = [t.numel() + (1 if self.append_eos else 0) for t in conditioning_token_ids]
-        P, pred_start = self._prompt_lengths(cond_lens, len_pre * q)
-        if self.m.use_absolute_position_embeddings and n > 0:      # generate's checks for one row
-            lim = int(self.m.max_absolute_position_embeddings)
-            for s, c in enumerate(cond_lens):
-                if c > lim:
-                    raise IndexError(f"{where}: conditioning sequence {s} has {c} tokens but max_absolute_position_embeddings is {lim}")
-            if len_pre * q + n - 1 > lim:
-                raise IndexError(f"{where}: the predicted sequence reaches {len_pre * q + n - 1} tokens ({len_pre * q} given + {n} "
-                                 f"sampled - 1) but max_absolute_position_embeddings is {lim}")
+        P, pred_start = self._prompt_lengths(cond_lens, n_pre)
+        if self.m.use_absolute_position_embeddings:
+            check_abs_positions(where, int(self.m.max_absolute_position_embeddings), cond_lens, [n_pre], [n])
         if P + n > self.max_positions:
             raise ValueError(f"{where}: the prompt's {P} positions plus {n} sampled tokens exceed max_positions = {self.max_positions}")
         if n > 0:
@@ -263,7 +226,7 @@ class GenerationSession:
         if n == 0:
             if self.logprob:             # nothing to sample: generate's teacher-forced scoring of the prefix
                 self._done[handle] = tuple(t[0] for t in self.w.generate(
-                    conditioning_token_ids=cond, pred_token_ids=pred_token_ids, max_time_steps=len_pre, return_logprobs=True,
+                    conditioning_token_ids=cond, pred_token_ids=pred_token_ids, max_time_steps=max_time_steps, return_logprobs=True,
                     include_eos_in_output=self.include_eos, append_eos_to_conditioning_tokens=self.append_eos))
             else:
                 self._done[handle] = self._output(prefix[0], prefix.new_empty(0))
@@ -281,7 +244,7 @@ class GenerationSession:
 
     @property
     def graph_count(self) -> int:
-        return len(self._graphs)
+        return len(self._graphs.graphs)
 
     def finished(self):
         """{handle: [n, q] int64 tokens} of the rows that finished since the last call (device tensors): exactly
@@ -295,77 +258,35 @@ class GenerationSession:
 
     # ------------------------------------------------------------------------------------------------ decoding
     def _output(self, prefix, new, lp=None):
-        """generate's output for one row: prefix then samples, everything after an eos masked with -1, [n, q].  lp:
-        (prefix logprobs, new logprobs, new sample logprobs) -> (tokens, logprobs, sample_logprobs), 0 where -1."""
-        sampled = torch.cat([prefix, new])[None]
-        eos_mask = (sampled == self.eos).float()                                                  # utils.py:86-93
-        if self.include_eos:
-            eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))
-        sampled = sampled.masked_fill(eos_mask.cumsum(-1) > 0, -1)
-        if lp is None:
-            return sampled.view(-1, self.q)
-        pre, lp_new, slp_new = lp
-        gone = sampled[0] == -1
-        return (sampled.view(-1, self.q), torch.cat([pre, lp_new]).masked_fill(gone, 0.0).view(-1, self.q),
-                torch.cat([torch.zeros_like(pre), slp_new]).masked_fill(gone, 0.0).view(-1, self.q))
-
-    def _run(self, key, body):
-        """body() eagerly, or from its CUDA graph: one eager run first (lazy cudaFuncSetAttribute calls are not
-        capturable), captured on the second use, replayed from then on."""
-        if not self.use_graph:
-            body()
-            return
-        g = self._graphs.get(key)
-        if g is None:
-            if key not in self._warm:
-                body()
-                self._warm.add(key)
-                return
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                body()
-            self._graphs[key] = g
-        g.replay()
+        """generate's output for one row from its prefix [n_pre] and samples [n]: [n_pre + n, q] tokens; with lp =
+        (prefix logprobs or None, new logprobs, new sample logprobs): (tokens, logprobs, sample_logprobs)."""
+        out = assemble_output(prefix[None], new[None], prefix.shape[0], prefix.shape[0] + new.shape[0], prefix.shape[0] + new.shape[0],
+                              self.eos, self.include_eos, self.q, None if lp is None else tuple(None if t is None else t[None] for t in lp))
+        return out[0] if lp is None else tuple(t[0] for t in out)
 
     def _install(self, rows):
         """Prefills each joining row alone and writes its prompt's K/V rows, conv history and last logits into its
         slot, then sets the slot's arrays.  Runs after the boundary step (which writes every slot's cache and conv
         history at the slot's old position) and before the boundary sample."""
-        eng, dec, w = self.eng, self.dec, self.w
-        S = len(w.token_sequences)
+        eng, dec, dev = self.eng, self.dec, self.eng.dev
         for row in rows:
             a = row.payload
-            cond = a["cond"]
-            if self.append_eos:                                                                   # open_musiclm.py:288-290
-                cond = [torch.cat([t, torch.full((1, 1), e, device=eng.dev, dtype=torch.int64)], 1) for t, e in zip(cond, w.eos_ids)]
-            _, src_row, key_mask, _, n_tok = lib.token_plan(
-                cond + [a["prefix"]], [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs], eng.emb_row_base,
-                eng.start_row, append_eos=False, drop_last=False, mask_cond=False, want_labels=False, err_flag=eng.err_flag)
-            pl = eng.plan(1, n_tok)
+            pl, ws = prefill(self.w, a["cond"], a["prefix"], self.append_eos, dec, slice(row.slot, row.slot + 1),
+                             torch.full((1,), row.P, device=dev))
             assert pl.N == row.P and pl.pos0[-1] == row.pred_start, (pl.N, row.P)
-            ws = eng.workspace(pl, False)
-            eng.forward_core(pl, ws, src_row, key_mask, False, {S - 1}, False, capture=_SlotCapture(dec, row.slot, pl.N))
             if self.logprob:
-                a["prefix_lp"] = prefix_logprobs(eng, pl, ws, a["prefix"], self.q, self.C)[0] if a["prefix"].shape[1] else \
-                    torch.zeros(0, device=eng.dev)
-            p_last = n_tok[-1]
-            gi = next(i for i, (s, qi, cnt, base) in enumerate(pl.groups) if s == S - 1 and qi == p_last % self.q)
-            dec.logits[row.slot, :eng.Cp[S - 1]].copy_(ws["logits"][gi][p_last // self.q])
-        dev = eng.dev
+                a["prefix_lp"] = prefix_logprobs(eng, pl, ws, a["prefix"], self.q, self.C)[0] if a["prefix"].shape[1] else None
         idx = torch.tensor([r.slot for r in rows], device=dev)
-        i32 = lambda v: torch.tensor(v, device=dev, dtype=torch.int32)
         states = [r.device_state() for r in rows]
-        dec.pos[idx] = i32([s["pos"] for s in states])
-        dec.pos_last[idx] = i32([s["pos_last"] for s in states])
-        dec.pos_offset_rows[idx] = i32([s["pos_offset"] for s in states])
-        dec.t[idx] = i32([0] * len(rows))
-        dec.n_rows[idx] = i32([r.n for r in rows])
+        vals = row_arrays(dev, len(rows), pos=[s["pos"] for s in states], pos_last=[s["pos_last"] for s in states],
+                          pos_offset=[s["pos_offset"] for s in states], t=0, n=[r.n for r in rows],
+                          top_k=[r.payload["top_k"] for r in rows], temperature=[r.payload["temperature"] for r in rows],
+                          top_p=[r.payload["top_p"] for r in rows])
+        for name, dst in (("pos", dec.pos), ("pos_last", dec.pos_last), ("pos_offset", dec.pos_offset), ("t", dec.t), ("n", dec.n_rows),
+                          ("top_k", dec.top_k), ("temperature", dec.temperature)):
+            dst[idx] = vals[name]
+        dec.top_p[idx] = vals["top_p"] if vals["top_p"] is not None else 1.0
         dec.seeds[idx] = seeds_tensor([r.payload["seed"] for r in rows], len(rows), dev)
-        dec.rows["top_k_rows"][idx] = i32([r.payload["top_k"] for r in rows])
-        dec.rows["temperature_rows"][idx] = torch.tensor([r.payload["temperature"] for r in rows], device=dev, dtype=torch.float32)
-        dec.rows["top_p_rows"][idx] = torch.tensor([1.0 if r.payload["top_p"] is None else r.payload["top_p"] for r in rows],
-                                                   device=dev, dtype=torch.float32)
 
     def _sample_point(self):
         if self.trace:
@@ -395,16 +316,16 @@ class GenerationSession:
             for qi in range(q):
                 if qi == 0 and joined:
                     if running:
-                        self._run(("step", 0), lambda: dec.step(0))
+                        self._graphs.run(("step", 0), lambda: dec.step(0))
                     self._install(joined)
                     self._sample_point()
-                    self._run(("sample", 0, nucleus), lambda: dec.sample_rows(0, allow(0), nucleus))
+                    self._graphs.run(("sample", 0, nucleus), lambda: dec.sample_rows(0, allow(0), nucleus))
                 elif self.trace:
                     dec.step(qi)
                     self._sample_point()
                     dec.sample_rows(qi, allow(qi), nucleus)
                 else:
-                    self._run(("full", qi, nucleus), lambda qi=qi: (dec.step(qi), dec.sample_rows(qi, allow(qi), nucleus)))
+                    self._graphs.run(("full", qi, nucleus), lambda qi=qi: (dec.step(qi), dec.sample_rows(qi, allow(qi), nucleus)))
             for row in sched.advance():
                 a = row.payload
                 lp = (a["prefix_lp"], dec.lp[row.slot, :row.n].clone(), dec.slp[row.slot, :row.n].clone()) if self.logprob else None

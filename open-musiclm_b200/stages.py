@@ -19,7 +19,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .decode import TokenConditionedTransformerWrapper, check_pred_lengths, check_sampling_rows, check_top_p
+from .decode import TokenConditionedTransformerWrapper, check_pred_lengths, check_sampling_rows, check_top_p, plan_rows
 from .model import TokenConditionedTransformer
 
 
@@ -57,15 +57,6 @@ def window_seed(seed: int, stage: int, window: int) -> int:
     return splitmix64((int(seed) & _MASK64) ^ splitmix64((stage << 32) | window))
 
 
-def _n_new(pred_token_ids, max_time_steps, q: int, B: int, lengths=None) -> int:
-    """Sampled tokens of a generate call: with per-row prefix lengths or max_time_steps (checked), those of the row that
-    samples most."""
-    init = 0 if pred_token_ids is None else pred_token_ids.shape[1]
-    lengths = lengths if lengths is not None else [init] * B
-    steps = max_time_steps if isinstance(max_time_steps, list) else [max_time_steps] * B
-    return max(max(0, (t - n) * q) for t, n in zip(steps, lengths))
-
-
 class _Stage(nn.Module):
     """Common part of the three stages: the wrapper, the device, the conditioning order."""
 
@@ -87,7 +78,7 @@ class _Stage(nn.Module):
             steps = check_sampling_rows(B, info.codebook_size + 1, kw["temperature"], kw["filter_thres"], kw.get("top_p"),
                                         kw["max_time_steps"])[3]
             lengths = check_pred_lengths(kw.get("pred_lengths"), pred, B)
-            kw["uniform_noise"] = noise.take(_n_new(pred, steps, info.num_quantizers, B, lengths))
+            kw["uniform_noise"] = noise.take(max(plan_rows(pred, B, info.num_quantizers, lengths, steps)[1]))
         return self.transformer_wrapper.generate(conditioning_token_ids=conditioning, pred_token_ids=pred, **kw)
 
 

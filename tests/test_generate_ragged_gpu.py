@@ -287,7 +287,7 @@ def test_seeded_ragged_rows_equal_each_row_alone(B, top_p):
 
 
 # ------------------------------------------------------------------------------------------------ 5. limits
-def test_absolute_position_limit_is_checked_per_row(monkeypatch):
+def test_absolute_position_limit_is_checked_per_row_offsets(monkeypatch):
     """max_absolute_position_embeddings = T q - 1: every row that samples reaches exactly that many tokens and
     generates; a row whose prefix (garbage ids in its padding, and longer than max_time_steps) samples nothing is
     exempt.  One more step raises IndexError naming the first row that samples, before anything runs (Engine.seed
@@ -317,8 +317,8 @@ def test_absolute_position_limit_is_checked_per_row(monkeypatch):
     assert int(eng.err_flag.item()) == 0
     assert out.shape == (B, steps, q) and torch.equal(out[0], pred[0])
     s = sessions[-1]
-    pos, pos_last = s.pos.cpu(), s.pos_last.cpu()
-    assert bool((pos <= pos_last).all()) and int(pos_last.max()) + s.pos_offset < lim
+    pos, pos_last, pos_offset = s.pos.cpu(), s.pos_last.cpu(), s.pos_offset.cpu()
+    assert bool((pos <= pos_last).all()) and int((pos_last + pos_offset).max()) < lim
     for b in range(1, B):
         alone = _alone(w, cond, pred, b, lengths[b], max_time_steps=T, seeds=[seeds[b]])
         assert torch.equal(out[b, :T], alone[0]) and bool((out[b, T:] == -1).all()), b

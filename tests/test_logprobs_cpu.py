@@ -122,15 +122,16 @@ def test_reconstruct_wave_with_logprobs_raises():
 
 
 @pytest.mark.parametrize("include_eos", [False, True])
-def test_assembly_of_prefix_sampled_and_masked_positions(include_eos):
+def test_assemble_output_prefix_sampled_and_masked_positions(include_eos):
     """Two rows of different prefix lengths (ragged) and sample counts, an eos in row 0's samples: prefix columns take
     the prefix values (sample log p 0), sampled columns the decode's in order, columns past a row's end and every -1
     (after the eos, or the eos itself without include_eos) are 0; a non-ragged row is the plain concatenation."""
-    from open_musiclm_b200.decode import assemble_logprobs
+    from open_musiclm_b200.decode import assemble_output
     eos = 9
     n_real = torch.tensor([[2], [4]])
     n_end = n_real + torch.tensor([[4], [2]])
     tokens = torch.tensor([[1, 2, 5, eos, 6, 7], [3, 4, 5, 6, 8, 1]])
+    prefix, new = tokens[:, :4], torch.tensor([[5, eos, 6, 7], [8, 1, 0, 0]])  # row 0: 2 prefix tokens; row 1: 4
     eos_mask = (tokens == eos).float()
     if include_eos:
         eos_mask = torch.nn.functional.pad(eos_mask, (1, -1))
@@ -138,16 +139,16 @@ def test_assembly_of_prefix_sampled_and_masked_positions(include_eos):
     pre = -torch.arange(1, 5, dtype=torch.float32).repeat(2, 1)                  # [2, 4]: -1 -2 -3 -4
     lp_new = -torch.arange(10, 14, dtype=torch.float32).repeat(2, 1)             # -10 -11 -12 -13
     slp_new = lp_new / 10
-    lp, slp = assemble_logprobs(sampled, pre, lp_new, slp_new, n_real, n_end)
+    out, lp, slp = (t[..., 0] for t in assemble_output(prefix, new, n_real, n_end, 6, eos, include_eos, 1, (pre, lp_new, slp_new)))
+    assert torch.equal(out, sampled)
     want0 = [-1, -2, -10, -11 if include_eos else 0, 0, 0]
     assert lp[0].tolist() == want0
     assert torch.allclose(slp[0], torch.tensor([0, 0, -1.0, -1.1 if include_eos else 0, 0, 0]))
     assert lp[1].tolist() == [-1, -2, -3, -4, -10, -11] and torch.allclose(slp[1], torch.tensor([0, 0, 0, 0, -1.0, -1.1]))
-    short = sampled.clone()
-    short[1, 5] = -1                                                             # padding of a shorter row
-    lp, slp = assemble_logprobs(short, pre, lp_new, slp_new, n_real, n_real + torch.tensor([[4], [1]]))
-    assert lp[1, 5] == 0 and slp[1, 5] == 0 and lp[1, 4] == -10
-    lp, slp = assemble_logprobs(sampled[:, :4], pre, None, None, torch.full((2, 1), 4), torch.full((2, 1), 4))
+    out, lp, slp = (t[..., 0] for t in assemble_output(prefix, new, n_real, n_real + torch.tensor([[4], [1]]), 6, eos, include_eos, 1,
+                                                       (pre, lp_new, slp_new)))
+    assert out[1, 5] == -1 and lp[1, 5] == 0 and slp[1, 5] == 0 and lp[1, 4] == -10    # padding of a shorter row
+    out, lp, slp = (t[..., 0] for t in assemble_output(prefix, new[:, :0], 4, 4, 4, eos, include_eos, 1, (pre, None, None)))
     assert lp[1].tolist() == [-1, -2, -3, -4] and bool((slp == 0).all())
 
 

@@ -32,7 +32,7 @@ def main():
         raise SystemExit("time_decode_abspos: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
     from open_musiclm_b200 import lib
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     n = args.context
@@ -48,7 +48,7 @@ def main():
     for B in [int(b) for b in args.batches.split(",")]:
         sess = {}
         for abs_pos, (_, eng) in engines.items():
-            s = DecodeSession(eng, B, n, 8, pred_start=n - j - 1)
+            s = DecodeSession(eng, B, n + 8, 8, row_arrays("cuda", B, pos=n, pos_last=n, pos_offset=j - n, top_k=1, temperature=1.0))
             g = torch.Generator(device="cuda").manual_seed(B)
             for c in s.cache:
                 c.copy_(torch.randn(c.shape, device="cuda", generator=g) * 0.3)
@@ -70,7 +70,7 @@ def main():
         eng = engines[True][1]
         x = s.x[0]
         plain = lambda: [lib.embed_gather(eng.table, s.next_row, x) for _ in range(20)]
-        with_pos = lambda: [lib.embed_gather_pos(eng.table, s.next_row, s.pos, s.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x)
+        with_pos = lambda: [lib.embed_gather_pos_rows(eng.table, s.next_row, s.pos, s.pos_offset, eng.abs_row_base[-1], eng.max_abs_pos, x)
                             for _ in range(20)]
         for key, f in (("embed_gather_us", plain), ("embed_gather_pos_us", with_pos)):
             med, spread = stat([t / 20 * 1e3 for t in time_graph(f, max(args.reps // 4, 10))])

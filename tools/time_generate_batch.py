@@ -69,7 +69,7 @@ def main():
         raise SystemExit("time_generate_batch: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
     from open_musiclm_b200 import lib
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     torch.manual_seed(0)
@@ -81,7 +81,7 @@ def main():
     n = args.context
     rows = []
     for B in [int(b) for b in args.batches.split(",")]:
-        sess = DecodeSession(eng, B, n, 8)
+        sess = DecodeSession(eng, B, n + 8, 8, row_arrays("cuda", B, pos=n, pos_last=n, pos_offset=0, top_k=1, temperature=1.0))
         g = torch.Generator(device="cuda").manual_seed(B)
         for c in sess.cache:
             c.copy_(torch.randn(c.shape, device="cuda", generator=g) * 0.3)
@@ -129,7 +129,7 @@ def main():
         print(f"B={gm['B']:>2} {gm['matrix']} [{gm['N']}x{gm['K']}]: skinny_gemm {gm['skinny_gemm']['us']:.1f} us "
               f"({gm['skinny_gemm']['spread_us']:.1f}), decode_gemm {gm['decode_gemm']['us']:.1f} us ({gm['decode_gemm']['spread_us']:.1f})")
     for B in [int(b) for b in args.profile.split(",") if b]:
-        sess = DecodeSession(eng, B, n, 8)
+        sess = DecodeSession(eng, B, n + 8, 8, row_arrays("cuda", B, pos=n, pos_last=n, pos_offset=0, top_k=1, temperature=1.0))
         for c in sess.cache + sess.conv:
             c.zero_()
         sess.pos.fill_(n)

@@ -6,8 +6,9 @@ what the per-row sampler costs, and what one per-row call saves against one call
    {40, 256} x C in {1025, 16384}: a CUDA graph of --inner launches replayed --reps times, CUDA events, variants
    alternated run by run.
 2. One decode step + sample of the musiclm_small coarse stage (d = 1024, L = 6, h = 8) at B = 40 and a context of
-   --context positions, replayed from a CUDA graph as tools/time_sample_nucleus.py does: single-value arguments against
-   per-row arrays (the same 40 temperatures 0.5 ... 1.5, k = 0.1 C, top_p 0.9 in every other row), alternated.
+   --context positions, replayed from a CUDA graph as tools/time_sample_nucleus.py does, with per-row arguments (40
+   temperatures 0.5 ... 1.5, k = 0.1 C, top_p 0.9 in every other row).  DESIGN section 6 keeps the comparison with the
+   single-value session this package no longer has.
 3. A settings sweep: 5 prompts (12 clap + 40 semantic tokens, no prefix, max_time_steps 30) at 8 settings (temperature
    x top_p in {0.7, 1.0} x {None, 0.8, 0.9, 0.95}) as one per-row call of 40 rows against 8 single-value calls of 5
    rows; host clock around each, ending in a device synchronise, alternated, median of --runs after one warm-up.
@@ -61,7 +62,7 @@ def main():
         raise SystemExit("time_generate_per_row: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
     from open_musiclm_b200 import lib
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     dev = "cuda"
@@ -103,25 +104,22 @@ def main():
     k = max(int(0.1 * C), 1)
     temps = [0.5 + b / (B - 1) for b in range(B)]
     tops = [0.9 if b % 2 else None for b in range(B)]
-    sessions = {"single": DecodeSession(eng, B, n, 8), "rows": DecodeSession(eng, B, n, 8, rows=([k] * B, temps, tops))}
-    graphs = {}
-    for v, s in sessions.items():
-        g = torch.Generator(device=dev).manual_seed(B)
-        for c in s.cache:
-            c.copy_(torch.randn(c.shape, device=dev, generator=g) * 0.3)
-        for c in s.conv:
-            c.zero_()
-        s.pos.fill_(n)
+    s = DecodeSession(eng, B, n + 8, 8, row_arrays(dev, B, pos=n, pos_last=n, pos_offset=0, top_k=k, temperature=temps, top_p=tops))
+    g = torch.Generator(device=dev).manual_seed(B)
+    for c in s.cache:
+        c.copy_(torch.randn(c.shape, device=dev, generator=g) * 0.3)
+    for c in s.conv:
+        c.zero_()
 
-        def step(s=s):
-            s.step(0)
-            s.counters.zero_()
-            s.sample(0, k, 0.95, False, None, eng.seed, bump_pos=False, top_p=0.9)
-        graphs[v] = graph_of(step)
+    def step():
+        s.step(0)
+        s.counters.zero_()
+        s.sample(0, False, None, eng.seed, advance=False)
+    graphs = {"rows": graph_of(step)}
     res = alternate(graphs, 100, args.runs)
     decode = dict(B=B, context=n, **{v: dict(ms_per_step=res[v][0], spread_ms=res[v][1], runs_ms=res[v][2]) for v in graphs})
     print(json.dumps(decode), flush=True)
-    del graphs, sessions
+    del graphs, s
     torch.cuda.empty_cache()
 
     # ---- 3. a sweep of 8 settings x 5 prompts
@@ -158,9 +156,9 @@ def main():
         a, b = r["single"], r["rows"]
         print(f"{r['C']:>6} {r['B']:>4} {str(r['top_p']):>6} {a['us_per_launch']:>8.2f} ({a['spread_us']:.2f}) "
               f"{b['us_per_launch']:>8.2f} ({b['spread_us']:.2f})")
-    a, b = decode["single"], decode["rows"]
-    print(f"\nmusiclm_small coarse, B = {B}, context {n}: decode step + sample from a CUDA graph, ms: single value "
-          f"{a['ms_per_step']:.4f} ({a['spread_ms']:.4f}), per row {b['ms_per_step']:.4f} ({b['spread_ms']:.4f})")
+    b = decode["rows"]
+    print(f"\nmusiclm_small coarse, B = {B}, context {n}: decode step + sample from a CUDA graph, per-row arguments, ms "
+          f"{b['ms_per_step']:.4f} ({b['spread_ms']:.4f})")
     print(f"\nsweep of {len(settings)} settings x {P} prompts, max_time_steps {T}, median of {args.runs} (spread)")
     for c, r in sweep.items():
         print(f"  {c:<12} {r['median_ms']:9.1f} ms ({r['spread_ms']:.1f})")

@@ -7,9 +7,10 @@ end to end (host clock around generate, ending in a device synchronise; prefill,
 included), alternating, median of --runs after one warm-up of each:
   ragged     one call with pred_lengths: 90 decode steps for all 40 rows
   per_length one call per distinct length (21 calls of 1 or 2 rows: the SIMT path)
-  uniform    one call of the same 40 rows with no prefix (90 steps, the shared-position kernels)
-Then the decode step alone from a CUDA graph (CUDA events), shared positions against per-row positions spread over
-the last 60 positions before --context, at B = 8 (SIMT) and 40 (tensor cores).
+  uniform    one call of the same 40 rows with no prefix (90 steps)
+Then the decode step alone from a CUDA graph (CUDA events), per-row positions spread over the last 60 positions before
+--context, at B = 8 (SIMT) and 40 (tensor cores).  DESIGN section 6 keeps the comparison with the shared-position step
+this package no longer has.
 
     python tools/time_generate_ragged.py [--runs 5] [--context 1000] [--out DIR]
 """
@@ -76,7 +77,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("time_generate_ragged: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     torch.manual_seed(0)
@@ -113,27 +114,24 @@ def main():
     res = {k: dict(zip(("median_ms", "spread_ms"), stat(v)), runs_ms=v) for k, v in times.items()}
     for k, r in res.items():
         print(json.dumps(dict(call=k, **r)), flush=True)
-    # the decode step alone: shared position against per-row positions
+    # the decode step alone, per-row positions
     n = args.context
     steps = []
     for Bs in (8, 40):
-        for ragged_pos in (False, True):
-            pos = [n - (60 * b) // Bs for b in range(Bs)]
-            kw = dict(ragged=([p for p in pos], pos, [n + 8] * Bs), n_max=n + 8) if ragged_pos else {}
-            sess = DecodeSession(eng, Bs, n, 8, **kw)
-            gen = torch.Generator(device="cuda").manual_seed(Bs)
-            for c in sess.cache:
-                c.copy_(torch.randn(c.shape, device="cuda", generator=gen) * 0.3)
-            for c in sess.conv:
-                c.zero_()
-            ms = time_graph(lambda: sess.step(0), args.reps)
-            med, spread = stat(ms)
-            r = dict(B=Bs, positions="per-row" if ragged_pos else "shared", ms_per_step=med, spread_ms=spread, runs_ms=ms,
-                     path="tensor-core" if sess.batched else "simt")
-            steps.append(r)
-            print(json.dumps(r), flush=True)
-            del sess
-            torch.cuda.empty_cache()
+        pos = [n - (60 * b) // Bs for b in range(Bs)]
+        sess = DecodeSession(eng, Bs, n + 8, 8, row_arrays("cuda", Bs, pos=pos, pos_last=n + 8, pos_offset=0, top_k=1, temperature=1.0))
+        gen = torch.Generator(device="cuda").manual_seed(Bs)
+        for c in sess.cache:
+            c.copy_(torch.randn(c.shape, device="cuda", generator=gen) * 0.3)
+        for c in sess.conv:
+            c.zero_()
+        ms = time_graph(lambda: sess.step(0), args.reps)
+        med, spread = stat(ms)
+        r = dict(B=Bs, positions="per-row", ms_per_step=med, spread_ms=spread, runs_ms=ms, path="tensor-core" if sess.batched else "simt")
+        steps.append(r)
+        print(json.dumps(r), flush=True)
+        del sess
+        torch.cuda.empty_cache()
     print()
     print(f"{info}; musiclm_small coarse stage, B = {B}, prefixes 0..{P} steps, max_time_steps {T}; median of {args.runs} (spread)")
     for k, r in res.items():

@@ -54,7 +54,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("time_generate_seeded: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     torch.manual_seed(0)
@@ -65,7 +65,7 @@ def main():
     for B in [int(b) for b in args.batches.split(",")]:
         sess, graphs = {}, {}
         for mode in ("default", "seeded"):
-            s = DecodeSession(eng, B, n, 8, seeded=mode == "seeded")
+            s = DecodeSession(eng, B, n + 8, 8, row_arrays("cuda", B, pos=n, pos_last=n, pos_offset=0, top_k=1, temperature=1.0), seeded=mode == "seeded")
             g = torch.Generator(device="cuda").manual_seed(B)
             for c in s.cache:
                 c.copy_(torch.randn(c.shape, device="cuda", generator=g) * 0.3)

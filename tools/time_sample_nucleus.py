@@ -52,7 +52,7 @@ def main():
         raise SystemExit("time_sample_nucleus: needs a CUDA device (nothing is measured without one)")
     import open_musiclm_b200 as O
     from open_musiclm_b200 import lib
-    from open_musiclm_b200.decode import DecodeSession
+    from open_musiclm_b200.decode import DecodeSession, row_arrays
     info = card()
     print("card (name, power limit, max SM clock):", info, flush=True)
     dev = "cuda"
@@ -87,7 +87,8 @@ def main():
     n, C = args.context, 1025
     steps = []
     for B in [int(b) for b in args.step_batches.split(",")]:
-        s = DecodeSession(eng, B, n, 8)
+        s = DecodeSession(eng, B, n + 8, 8, row_arrays(dev, B, pos=n, pos_last=n, pos_offset=0, top_k=max(int(0.1 * C), 1), temperature=0.95))
+        top_p_rows = {tp: None if tp is None else torch.full((B,), tp, device=dev) for _, tp in VARIANTS}
         g = torch.Generator(device=dev).manual_seed(B)
         for c in s.cache:
             c.copy_(torch.randn(c.shape, device=dev, generator=g) * 0.3)
@@ -98,7 +99,8 @@ def main():
         def step(tp, s=s):
             s.step(0)
             s.counters.zero_()            # the token goes to column 0 on every replay
-            s.sample(0, max(int(0.1 * C), 1), 0.95, False, None, eng.seed, bump_pos=False, top_p=tp)
+            s.top_p = top_p_rows[tp]          # read when the graph is captured
+            s.sample(0, False, None, eng.seed, advance=False)
         graphs = {name: graph_of(lambda tp=tp: step(tp)) for name, tp in VARIANTS}
         res = alternate(graphs, 100, args.runs)
         r = dict(B=B, path="tensor-core" if s.batched else "simt",
