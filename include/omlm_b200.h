@@ -213,6 +213,16 @@ int omlm_attn_fwd(const void* qn, const void* kvn, const float* table, int table
 int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* table, int table_ld,
                      const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                      float scale, void* stream);
+/* omlm_attn_fwd_tc over sequences of their own lengths packed back to back without padding (a packed prefill): qn
+ * [M, heads*64], kvn [M, 128], out [M, heads*64], lse2 [M*heads] with M the packed rows.  Sequence b is rows
+ * seq_start[b] .. seq_start[b] + seq_len[b] - 1 (int32 device arrays), causal within itself, without key mask; rows past
+ * the last sequence are not written.  work (int32 device array [2 n_work]): one (sequence, 128-row query block of its
+ * seq_len[b]*heads folded rows) pair per CTA, every block of every sequence once, heaviest first.  table_ld >= max_len
+ * >= every seq_len[b].  Each CTA computes what omlm_attn_fwd_tc computes for that block with B = 1 and N = seq_len[b]:
+ * out and lse2 are bit-identical to running each sequence alone. */
+int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const float* table, int table_ld, const int* work, int n_work,
+                            const int* seq_start, const int* seq_len, int M, int max_len, void* out, float* lse2, int heads,
+                            float scale, void* stream);
 /* Accumulates (+=) into dqn fp32 [B,N,heads*64], dkvn fp32 [B,N,128], dtable fp32 [heads,table_ld]. */
 int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                   const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
@@ -243,6 +253,11 @@ int omlm_attn_bwd_tc(const void* qn, const void* kvn, const void* d_o, const voi
  * omlm_ffn_mid_bwd reads (omlm_ffn_norm_fwd's hn_copy_bf16 when act_f16) are always bf16. */
 int omlm_gemm_ffn_up(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
                      float* rowsum, int M, int Nseq, int K, int Fp, int act_f16, int max_ctas, void* stream);
+/* omlm_gemm_ffn_up over sequences of their own lengths packed back to back: row m's position within its sequence is
+ * row_pos[m] (int32 device array [M]: 0, 1, 2, ... from each sequence's first row), which starts the conv history
+ * afresh where M % Nseq did.  Every row's u, h and rowsum are bit-identical to omlm_gemm_ffn_up on its sequence alone. */
+int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
+                            float* rowsum, const int* row_pos, int M, int K, int Fp, int act_f16, int max_ctas, void* stream);
 /* hn = dropout(LayerNorm_F(h)) from the fused statistics; stats fp32 [M, 2] = (mean, rstd) for the backward pass.
  * With drop_p > 0 the Philox keep mask is also written to keep_bits (uint8 [M, Fp/8], bit i of byte j = channel 8j+i)
  * so the backward pass reads 1 bit per element instead of regenerating the random stream. */

@@ -46,11 +46,15 @@ __device__ __forceinline__ float ex2_fast(float x) {
   return y;
 }
 
+// kVarlen: sequences of their own lengths packed back to back.  CTA x takes the unit (sequence work[2x], row block
+// work[2x + 1]) of a host-built list (heaviest first); sequence b is rows seq_start[b] .. seq_start[b] + seq_len[b] - 1
+// of the packed Q and K/V buffers.  N, nbatch and key_mask are then unused (no key mask: visibility is j < seq_len[b]).
+template <bool kVarlen>
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
-                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N, int h, float scale, int nbatch,
-                   int win_ld) {
+                   __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N_fixed, int h, float scale, int nbatch,
+                   int win_ld, const int* __restrict__ work, const int* __restrict__ seq_start, const int* __restrict__ seq_len) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // pointer arithmetic (not an integer round trip) keeps the shared address space visible to the compiler: LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -60,11 +64,13 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* kv_empty = bars + 3;   // [2]
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  const int N = kVarlen ? seq_len[work[2 * blockIdx.x]] : N_fixed;
   const int R = N * h;
   const int nblk = (R + kTcBQ - 1) / kTcBQ;
   // longest-processing-time-first: all batch elements of the heaviest (latest) row block are scheduled first
-  const int b = blockIdx.x % nbatch;
-  const int rb = nblk - 1 - blockIdx.x / nbatch;
+  const int b = kVarlen ? work[2 * blockIdx.x] : blockIdx.x % nbatch;
+  const int rb = kVarlen ? work[2 * blockIdx.x + 1] : nblk - 1 - blockIdx.x / nbatch;
+  const int s0 = kVarlen ? seq_start[b] : 0;    // varlen: first packed row of the sequence
   const int r0 = rb * kTcBQ;
   const int i_max_cta = min(N - 1, (r0 + kTcBQ - 1) / h);
   const int T = i_max_cta / kTcBK + 1;
@@ -83,13 +89,13 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
       mbar_expect_tx(q_full, 16384);
-      tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, b * R + r0);
+      tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, kVarlen ? s0 * h + r0 : b * R + r0);
       for (int t = 0; t < T; ++t) {
         const int st = t & 1;
         mbar_wait(&kv_empty[st], ((t >> 1) & 1) ^ 1);
         mbar_expect_tx(&kv_full[st], 2 * 16384);
-        tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, b * N + t * kTcBK);
-        tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, b * N + t * kTcBK);
+        tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, (kVarlen ? s0 : b * N) + t * kTcBK);
+        tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, (kVarlen ? s0 : b * N) + t * kTcBK);
       }
     }
     return;
@@ -215,17 +221,18 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
     if (rr[hr] < R) {
       const float inv = l[hr] > 0.f ? 1.f / l[hr] : 0.f;
-      __nv_bfloat16* op = out + (static_cast<long long>(b) * R + rr[hr]) * 64 + 2 * qc;
+      __nv_bfloat16* op = out + ((kVarlen ? static_cast<long long>(s0) * h : static_cast<long long>(b) * R) + rr[hr]) * 64 + 2 * qc;
 #pragma unroll
       for (int c = 0; c < 8; ++c)
         *reinterpret_cast<uint32_t*>(op + 8 * c) = pack_bf16x2(o[4 * c + 2 * hr] * inv, o[4 * c + 2 * hr + 1] * inv);
-      if (qc == 0) lse2[static_cast<long long>(b) * R + rr[hr]] = m[hr] + log2f(l[hr]);
+      if (qc == 0) lse2[(kVarlen ? static_cast<long long>(s0) * h : static_cast<long long>(b) * R) + rr[hr]] = m[hr] + log2f(l[hr]);
     }
   }
 }
 
 }  // namespace omlm
 
+#ifndef OMLM_ATTN_FWD_TC_VARLEN
 extern "C" int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* table, int table_ld,
                                 const unsigned char* key_mask, void* out, float* lse2, int B, int N, int heads,
                                 float scale, void* stream) {
@@ -242,13 +249,40 @@ extern "C" int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* ta
   if (rc) return rc;
   static int configured = 0;
   if (configured < smem) {
-    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
   const unsigned grid = static_cast<unsigned>((R + kTcBQ - 1) / kTcBQ) * B;   // (row block, batch) in LPT order
-  OMLM_KLAUNCH((attn_fwd_tc_kernel), grid, kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
+  OMLM_KLAUNCH((attn_fwd_tc_kernel<false>), grid, kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
       tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, B,
-      fwd_win_ld(heads));
+      fwd_win_ld(heads), nullptr, nullptr, nullptr);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
+
+#else
+extern "C" int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const float* table, int table_ld, const int* work,
+                                       int n_work, const int* seq_start, const int* seq_len, int M, int max_len, void* out,
+                                       float* lse2, int heads, float scale, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && n_work > 0 && max_len > 0 && heads > 0, "attn_fwd_tc_varlen: bad shape");
+  OMLM_CHECK_ARG(table_ld >= max_len, "attn_fwd_tc_varlen: bias table shorter than the longest sequence");
+  const int smem = fwd_smem(heads);
+  OMLM_CHECK_ARG(smem <= kTcMaxSmem, "attn_fwd_tc_varlen: too many heads (%d) for the shared-memory bias windows", heads);
+  CUtensorMap tmQ, tmKV;
+  int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(M) * heads, 128, 64, kTcBQ);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(M), 256, 64, kTcBK);
+  if (rc) return rc;
+  static int configured = 0;
+  if (configured < smem) {
+    OMLM_CUDA(cudaFuncSetAttribute(attn_fwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    configured = smem;
+  }
+  OMLM_KLAUNCH((attn_fwd_tc_kernel<true>), static_cast<unsigned>(n_work), kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
+      tmQ, tmKV, table, table_ld, nullptr, reinterpret_cast<__nv_bfloat16*>(out), lse2, 0, heads, scale, 0, fwd_win_ld(heads),
+      work, seq_start, seq_len);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+#endif

@@ -28,11 +28,13 @@ constexpr int kFuThreads = 384;   // TMA warpgroup, two wgmma / epilogue warpgro
 
 // F16: xn, W1 arrive as fp16 and u, h leave as fp16 (all bounded by construction: LayerNorm output x weights);
 // otherwise everything is bf16.
-template <bool F16>
+// kVarlen: sequences of their own lengths packed back to back; row m's position within its sequence is row_pos[m]
+// (0 at each sequence start) instead of m % Nseq.
+template <bool F16, bool kVarlen = false>
 __global__ void __launch_bounds__(kFuThreads, 1)
 gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    __nv_bfloat16* __restrict__ u_out, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rowsum,
-                   const float* __restrict__ conv_w, int M, int Nseq, int K, int Fp) {
+                   const float* __restrict__ conv_w, int M, int Nseq, int K, int Fp, const int* __restrict__ row_pos) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kFuOffBar);
@@ -79,6 +81,12 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     bool first = true;
     for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
       const int n_blk = w % n_tiles, m_blk = w / n_tiles;
+      // varlen: lane r holds the position of row r of this warp's epilogue run (phase 2), loaded under the main loop
+      int lane_pos = 0;
+      if constexpr (kVarlen) {
+        const long g0 = static_cast<long>(m_blk) * kFuRowsOut + (et >> 5) * 16;
+        if (lane < min(16, kFuRowsOut - (et >> 5) * 16) && g0 + lane < M) lane_pos = row_pos[g0 + lane];
+      }
       float acc[kFuBN / 2];
 #pragma unroll
       for (int i = 0; i < kFuBN / 2; ++i) acc[i] = 0.f;
@@ -136,7 +144,9 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
         const int t0 = 2 + ew * 16;
         const long grow0 = static_cast<long>(m_blk) * kFuRowsOut - 2 + t0;
         const int nrows = min(min(16, kFuBM - t0), static_cast<int>(min(static_cast<long>(16), M - grow0)));
-        int pos = static_cast<int>(grow0 % Nseq);
+        int pos = kVarlen ? __shfl_sync(0xffffffffu, lane_pos, 0) : static_cast<int>(grow0 % Nseq);
+        // varlen: bit r set when row r starts a sequence (one ballot per run instead of a shuffle per row)
+        const unsigned starts = kVarlen ? __ballot_sync(0xffffffffu, lane < nrows && lane_pos == 0) : 0u;
         const uint8_t* rp = usm + t0 * kFuUPitch;
         float2 xv1[2], xg1[2], xv2[2], xg2[2];        // fp32x2 pairs: channels (0,1) and (2,3) of this lane
         {
@@ -162,7 +172,7 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             const uint2 a = *reinterpret_cast<const uint2*>(rr + lane * 8);
             const uint2 g = *reinterpret_cast<const uint2*>(rr + 256 + lane * 8);
             const float2 xv0[2] = {unpack16x2<F16>(a.x), unpack16x2<F16>(a.y)}, xg0[2] = {unpack16x2<F16>(g.x), unpack16x2<F16>(g.y)};
-            if (pos == 0) {   // sequence start: no history (the zeros then slide into the t-2 slot for the next row)
+            if (kVarlen ? ((starts >> r) & 1u) != 0 : pos == 0) {   // sequence start: no history (the zeros then slide into the t-2 slot for the next row)
               const float2 z = make_float2(0.f, 0.f);
               xv1[0] = xv1[1] = xg1[0] = xg1[1] = z;
               xv2[0] = xv2[1] = xg2[0] = xg2[1] = z;
@@ -180,7 +190,7 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             }
             s1 = sm.x + sm.y; s2 = sq.x + sq.y;
             *reinterpret_cast<uint2*>(hg + static_cast<long>(r) * Fp) = make_uint2(pack16x2<F16>(h[0].x, h[0].y), pack16x2<F16>(h[1].x, h[1].y));
-            if (++pos == Nseq) pos = 0;
+            if (!kVarlen && ++pos == Nseq) pos = 0;
           }
           st[2 * r] = s1;
           st[2 * r + 1] = s2;
@@ -207,6 +217,7 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
 
 }  // namespace omlm
 
+#ifndef OMLM_GEMM_FFN_UP_VARLEN
 extern "C" int omlm_gemm_ffn_up(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
                                 float* rowsum, int M, int Nseq, int K, int Fp, int act_f16, int max_ctas, void* stream) {
   using namespace omlm;
@@ -229,7 +240,37 @@ extern "C" int omlm_gemm_ffn_up(const void* xn, const void* w1_packed, const flo
   auto kern = act_f16 ? gemm_ffn_up_kernel<true> : gemm_ffn_up_kernel<false>;
   OMLM_KLAUNCH((kern), grid, kFuThreads, kFuSmem, reinterpret_cast<cudaStream_t>(stream), 
       tmA, tmB, reinterpret_cast<__nv_bfloat16*>(u_out), reinterpret_cast<__nv_bfloat16*>(h_out), rowsum, conv_w_packed, M,
-      Nseq, K, Fp);
+      Nseq, K, Fp, nullptr);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
+#else
+extern "C" int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out,
+                                       void* h_out, float* rowsum, const int* row_pos, int M, int K, int Fp, int act_f16,
+                                       int max_ctas, void* stream) {
+  using namespace omlm;
+  OMLM_CHECK_ARG(M > 0 && K > 0 && K % 8 == 0 && Fp > 0 && Fp % 128 == 0 && row_pos != nullptr,
+                 "gemm_ffn_up_varlen: bad shape M=%d K=%d Fp=%d", M, K, Fp);
+  CUtensorMap tmA, tmB;
+  int rc = make_tmap_bf16_2d(&tmA, xn, static_cast<uint64_t>(K), static_cast<uint64_t>(M), static_cast<uint64_t>(K) * 2, 64, kFuBM);
+  if (rc) return rc;
+  rc = make_tmap_bf16_2d(&tmB, w1_packed, static_cast<uint64_t>(K), static_cast<uint64_t>(2 * Fp), static_cast<uint64_t>(K) * 2, 64, kFuBN);
+  if (rc) return rc;
+  static bool configured = false;
+  if (!configured) {
+    OMLM_CUDA(cudaFuncSetAttribute(gemm_ffn_up_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFuSmem));
+    OMLM_CUDA(cudaFuncSetAttribute(gemm_ffn_up_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kFuSmem));
+    configured = true;
+  }
+  const int m_tiles = (M + kFuRowsOut - 1) / kFuRowsOut, n_tiles = (2 * Fp) / kFuBN;
+  int grid = num_sms();
+  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
+  if (m_tiles * n_tiles < grid) grid = m_tiles * n_tiles;
+  auto kern = act_f16 ? gemm_ffn_up_kernel<true, true> : gemm_ffn_up_kernel<false, true>;
+  OMLM_KLAUNCH((kern), grid, kFuThreads, kFuSmem, reinterpret_cast<cudaStream_t>(stream),
+      tmA, tmB, reinterpret_cast<__nv_bfloat16*>(u_out), reinterpret_cast<__nv_bfloat16*>(h_out), rowsum, conv_w_packed, M,
+      1, K, Fp, row_pos);
+  OMLM_LAUNCH_CHECK();
+  return 0;
+}
+#endif

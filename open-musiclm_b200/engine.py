@@ -502,11 +502,29 @@ class Engine:
         """Runs embeddings -> depth x (attention, conv-FFN) -> final LN -> logit heads.  Activations stay in `ws`.
         capture (decode.py): receives each layer's K/V rows and pre-conv FFN rows (the generation caches of the prompt)."""
         self.refresh_packed()
-        B, N, M, d, h, HD, F, Fp = pl.B, pl.N, pl.M, self.d, self.h, self.HD, self.F, self.Fp
+        B, N, h, Fp = pl.B, pl.N, self.h, self.Fp
+        pv = self.pview
+        lib.embed_gather(self.table, src_row, ws["x"][0], pl.src_row2)
+        self.build_bias_table(ws, N)
+        x_last = self._layers(ws, pl.M, train, drop, capture,
+                              lambda i: lib.attn_fwd_tc(ws["qn"][i], ws["kvn"][i], ws["table"], key_mask, ws["o"][i], ws["lse"][i], B, N, h),
+                              lambda xn2, i, pk: lib.gemm_ffn_up(xn2, pk["w1"], pk["conv"], ws["u"][i], ws["h"], ws["rowsum"], N, Fp))
+        f16 = self.a16 != torch.bfloat16
+        dup = f16 and train
+        xf = ws["xf16"] if f16 else ws["xf"]
+        lib.layernorm_fwd(x_last, pv["transformer.norm.gamma"], xf, None, ws["st_o"], pl.dest_row, ycopy=ws["xf"] if dup else None)
+        for gi, (s, qi, cnt, base) in enumerate(pl.groups):
+            if groups_wanted is not None and s not in groups_wanted:
+                continue
+            rows = B * cnt
+            lib.gemm(xf[base:base + rows], self.pk_logit[s][qi], ws["logits"][gi], block_n=128)
+
+    def _layers(self, ws, M: int, train: bool, drop: bool, capture, attn, ffn_up):
+        """The depth x (attention, conv-FFN) loop over the M rows of ws["x"][0]; attn(i) and ffn_up(xn2, i, pk) launch the
+        two kernels that depend on how the rows form sequences.  Returns the last residual stream."""
+        d, h, HD, F, Fp = self.d, self.h, self.HD, self.F, self.Fp
         pv = self.pview
         x = ws["x"]
-        lib.embed_gather(self.table, src_row, x[0], pl.src_row2)
-        self.build_bias_table(ws, N)
         drop_p = self.drop_p if drop else 0.0
         f16 = self.a16 != torch.bfloat16
         dup = f16 and train            # the backward pass needs bf16 duplicates of the fp16 forward operands
@@ -521,25 +539,58 @@ class Engine:
             lib.qk_l2norm_fwd(ws["q_raw"][i], ws["kv_raw"][i], pv[p + "0.q_scale"], pv[p + "0.k_scale"], ws["qn"][i], ws["kvn"][i], h)
             if capture is not None:
                 capture.after_kv(l, ws["kvn"][i])
-            lib.attn_fwd_tc(ws["qn"][i], ws["kvn"][i], ws["table"], key_mask, ws["o"][i], ws["lse"][i], B, N, h)
+            attn(i)
             lib.gemm(ws["o"][i], pk["wo_b"], xm, addend=xa, block_n=self._bn_for(M, d, HD))
             xn2 = ws["xn2_16"] if f16 else ws["xn2"][i]
             lib.layernorm_fwd(xm, pv[p + self.ffk["g1"]], xn2, None, ws["st_f"][i], ycopy=ws["xn2"][i] if dup else None)
-            lib.gemm_ffn_up(xn2, pk["w1"], pk["conv"], ws["u"][i], ws["h"], ws["rowsum"], N, Fp)   # conv + GEGLU in the epilogue
+            ffn_up(xn2, i, pk)                                                 # conv + GEGLU in the epilogue
             if capture is not None:
                 capture.after_u(l, ws["u"][i])
             hn = ws["hn16"] if f16 else ws["hn"][i]
             lib.ffn_norm_fwd(ws["h"], ws["rowsum"], pk["gin"], hn, ws["st_i"][i], F, Fp, drop_p, self.seed, l,
                              keep_bits=ws["keep"][i] if drop_p > 0 else None, hn_copy=ws["hn"][i] if dup else None)
             lib.gemm(hn, pk["w2"], xo, addend=xm, block_n=self._bn_for(M, d, Fp))
-        x_last = x[2 * self.L] if train else x[0]
-        xf = ws["xf16"] if f16 else ws["xf"]
-        lib.layernorm_fwd(x_last, pv["transformer.norm.gamma"], xf, None, ws["st_o"], pl.dest_row, ycopy=ws["xf"] if dup else None)
-        for gi, (s, qi, cnt, base) in enumerate(pl.groups):
-            if groups_wanted is not None and s not in groups_wanted:
-                continue
-            rows = B * cnt
-            lib.gemm(xf[base:base + rows], self.pk_logit[s][qi], ws["logits"][gi], block_n=128)
+        return x[2 * self.L] if train else x[0]
+
+    # ------------------------------------------------------------------------------------------ packed prefill
+    def packed_workspace(self, rows: int, head_rows: int):
+        """Inference activations for packed forwards of up to `rows` rows (forward_packed runs on views of the first M),
+        and up to `head_rows` rows of final-norm output and logits of the last sequence's heads."""
+        dev, bf, f32, a16 = self.dev, torch.bfloat16, torch.float32, self.a16
+        d, HD, Fp, h = self.d, self.HD, self.Fp, self.h
+        E = lambda *shape, dt=bf: torch.empty(*shape, device=dev, dtype=dt)
+        ws = dict(x=[E(rows, d, dt=f32) for _ in range(2)], xraw=[E(rows, d)], st_a=[E(rows, 2, dt=f32)], q_raw=[E(rows, HD)],
+                  kv_raw=[E(rows, 128)], qn=[E(rows, HD)], kvn=[E(rows, 128)], o=[E(rows, HD)], lse=[E(rows, h, dt=f32)],
+                  st_f=[E(rows, 2, dt=f32)], u=[E(rows, 2 * Fp, dt=a16)], st_i=[E(rows, 2, dt=f32)], h=E(rows, Fp, dt=a16),
+                  rowsum=E(rows, Fp // 128, 2, dt=f32), st_o=E(rows, 2, dt=f32),
+                  logits=E(head_rows, self.Cp[-1], dt=f32))
+        if a16 != bf:
+            ws.update(xn16=E(rows, d, dt=a16), xn2_16=E(rows, d, dt=a16), hn16=E(rows, Fp, dt=a16), xf16=E(head_rows, d, dt=a16))
+        else:
+            ws.update(xn=[E(rows, d)], xn2=[E(rows, d)], hn=[E(rows, Fp)], xf=E(head_rows, d))
+        return ws
+
+    def forward_packed(self, ws, pk_plan, table, capture=None):
+        """Inference forward of sequences of their own lengths packed back to back without padding (pk_plan: M rows,
+        src_row, src_row2, row_pos, seq_start, seq_len, the attention work list, dest_row and the head groups; see
+        session.PackedPrefill) in a packed_workspace.  The layer loop is forward_core's, with the varlen attention and
+        FFN-up kernels; table: a bias table at least as long as the longest sequence.  The final norm writes only the
+        rows dest_row names, and head group (qi, base, cnt) leaves the logits of head qi of the last sequence for its
+        cnt rows in ws["logits"][base:base + cnt].  Every row's values are those of forward_core on its sequence alone."""
+        self.refresh_packed()
+        pp, M, Fp = pk_plan, pk_plan.M, self.Fp
+        v = {k: [e[:M] for e in t] if isinstance(t, list) else t[:M] for k, t in ws.items() if k not in ("logits", "xf", "xf16")}
+        lib.embed_gather(self.table, pp.src_row, v["x"][0], pp.src_row2)
+        x_last = self._layers(v, M, False, False, capture,
+                              lambda i: lib.attn_fwd_tc_varlen(v["qn"][i], v["kvn"][i], table, pp.work, pp.seq_start, pp.seq_len,
+                                                               pp.max_len, v["o"][i], v["lse"][i], self.h),
+                              lambda xn2, i, pk: lib.gemm_ffn_up_varlen(xn2, pk["w1"], pk["conv"], v["u"][i], v["h"], v["rowsum"],
+                                                                        pp.row_pos, Fp))
+        xf = ws["xf16"] if self.a16 != torch.bfloat16 else ws["xf"]
+        lib.layernorm_fwd(x_last, self.pview["transformer.norm.gamma"], xf, None, v["st_o"], pp.dest_row)
+        S = len(self.seqs) - 1
+        for qi, base, cnt in pp.groups:
+            lib.gemm(xf[base:base + cnt], self.pk_logit[S][qi], ws["logits"][base:base + cnt], block_n=128)
 
     # ------------------------------------------------------------------------------------------ backward
     def _wgrad(self, dy, x, gout, m, n, det_part=None, **kw):

@@ -270,6 +270,15 @@ def attn_fwd_tc(qn, kvn, table, key_mask, out, lse2, B, N, heads, scale=8.0):
          _I(B), _I(N), _I(heads), _F(scale), _stream())
 
 
+def attn_fwd_tc_varlen(qn, kvn, table, work, seq_start, seq_len, max_len, out, lse2, heads, scale=8.0):
+    """attn_fwd_tc over packed sequences (omlm_attn_fwd_tc_varlen): qn [M, heads*64], kvn [M, 128]; work int32 [n_work, 2]
+    of (sequence, row block) pairs; seq_start, seq_len int32 [n_seq]; max_len >= every seq_len."""
+    for t in (work, seq_start, seq_len):
+        assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
+    call("omlm_attn_fwd_tc_varlen", _p(qn), _p(kvn), _p(table), _I(table.stride(0)), _p(work), _I(work.numel() // 2), _p(seq_start),
+         _p(seq_len), _I(qn.shape[0]), _I(max_len), _p(out), _p(lse2), _I(heads), _F(scale), _stream())
+
+
 def attn_bwd(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads, scale=8.0):
     call("omlm_attn_bwd", _p(qn), _p(kvn), _p(d_o), _p(o), _p(lse2), _p(table), _I(table.stride(0)), _p(key_mask),
          _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale), _stream())
@@ -309,6 +318,15 @@ def gemm_ffn_up(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, Nseq, Fp, ma
     M, K = xn.shape
     assert xn.dtype in _T16 and xn.dtype == w1_packed.dtype == u_out.dtype == h_out.dtype
     call("omlm_gemm_ffn_up", _p(xn), _p(w1_packed), _p(conv_w_packed), _p(u_out), _p(h_out), _p(rowsum), _I(M), _I(Nseq),
+         _I(K), _I(Fp), _I(int(xn.dtype == torch.float16)), _I(max_ctas), _stream())
+
+
+def gemm_ffn_up_varlen(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, row_pos, Fp, max_ctas=0):
+    """gemm_ffn_up over packed sequences (omlm_gemm_ffn_up_varlen): row_pos int32 [M], each row's position in its sequence."""
+    M, K = xn.shape
+    assert xn.dtype in _T16 and xn.dtype == w1_packed.dtype == u_out.dtype == h_out.dtype
+    assert row_pos.dtype == torch.int32 and row_pos.is_cuda and row_pos.is_contiguous() and row_pos.numel() >= M
+    call("omlm_gemm_ffn_up_varlen", _p(xn), _p(w1_packed), _p(conv_w_packed), _p(u_out), _p(h_out), _p(rowsum), _p(row_pos), _I(M),
          _I(K), _I(Fp), _I(int(xn.dtype == torch.float16)), _I(max_ctas), _stream())
 
 

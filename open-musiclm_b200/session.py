@@ -3,8 +3,9 @@ keep decoding.
 
 A `GenerationSession` holds one decode state of `slots` rows over one `TokenConditionedTransformerWrapper`.  `add`
 queues a request (conditioning, optional prefix, seed, sampling arguments); at the next time-step boundary it takes a
-free slot: its prompt is prefilled alone (the regular wgmma forward, as `generate` runs it for one row) and installed
-into that slot, and from then on it decodes with the others, one quantizer slot per step.  A row that has all its
+free slot: the prompts of every row that joins at that boundary are prefilled together, packed back to back in one
+forward (Engine.forward_packed: the regular layers with the varlen attention and FFN-up kernels), and installed into
+their slots, and from then on it decodes with the others, one quantizer slot per step.  A row that has all its
 tokens leaves at the end of that time step and its slot is refilled at the next boundary.  The tokens of a request,
 and the logits they were sampled from, are bit for bit those of `generate` with that row alone and its seed, whatever
 the slot, the join step and the other rows (DESIGN section 4, "Generation sessions").
@@ -14,13 +15,147 @@ and the per-slot CUDA graphs; the arrays those graphs read (positions, sample in
 arguments) change at a join, the graphs do not.  `SlotSchedule` is the host bookkeeping, without device work.
 """
 import numbers
+import types
 from collections import deque
 
+import numpy as np
 import torch
 
 from . import lib
 from .decode import (MAX_BATCH, DecodeSession, GraphCache, assemble_output, check_abs_positions, check_sampling_rows, plan_rows,
-                     prefill, prefix_logprobs, row_arrays, seeds_tensor)
+                     row_arrays, seeds_tensor)
+
+
+PACK_ROWS = 16384     # rows of a session's packed-prefill workspace: max(max_positions, this), at most slots * max_positions
+
+
+def split_joiners(prompt_lens, capacity: int):
+    """The joiners of one boundary (prompt lengths in admission order, each <= capacity) -> lists of their indices,
+    consecutive in admission order, each list's prompts together at most capacity rows: one packed prefill each."""
+    groups, total = [], capacity
+    for i, n in enumerate(prompt_lens):
+        if total + n > capacity:
+            groups.append([])
+            total = 0
+        groups[-1].append(i)
+        total += n
+    return groups
+
+
+def lpt_work(seq_lens, h: int):
+    """The attention work list of a packed forward: every (sequence, 128-row block of its len * h folded query rows)
+    once, as int32 [n, 2], heaviest first (the block's key tiles, min(len - 1, last row's position) // 128 + 1; ties by
+    sequence, then later blocks first), as omlm_attn_fwd_tc orders its fixed-length grid."""
+    b = np.concatenate([np.full((n * h + 127) // 128, i) for i, n in enumerate(seq_lens)]).astype(np.int64)
+    rb = np.concatenate([np.arange((n * h + 127) // 128) for n in seq_lens]).astype(np.int64)
+    lens = np.asarray(seq_lens, dtype=np.int64)[b]
+    tiles = np.minimum(lens - 1, (rb * 128 + 127) // h) // 128 + 1
+    order = np.lexsort((-rb, b, -tiles))
+    return np.stack([b[order], rb[order]], 1).astype(np.int32)
+
+
+class PackedPrefill:
+    """Host plan of one packed prefill: the prompts of k joiners back to back, without padding.  n_tok: per joiner the
+    token counts of its sequences (conditioning sequences with their eos, then its prefix of whole time steps), as
+    lib.token_plan returns them; its prompt is sum(n + 1) rows (each sequence after its start token).  slots: the
+    joiners' slots in a decode state of n_max positions per slot; q: quantizers of the last sequence; h: heads;
+    abs_row_base (absolute position embeddings): the first row of each sequence's position table.  logprob: also
+    plan the rows that score the prefix tokens.
+
+    Arrays (numpy): start, P (each joiner's first packed row and prompt length), row_pos [M] (position within its
+    prompt), src_row2 [M] (position-table rows, -1 for start tokens; None without absolute positions), work
+    (lpt_work), last_row [k] (each prompt's last row, whose head-0 logits predict the first sampled token: every prefix
+    is whole time steps, so the next token is at quantizer 0), prefix_rows[qi] (the rows whose head-qi logits score the
+    prefix tokens at quantizer qi, joiner by joiner), dest_row [M] (row -> final-norm output row, -1 when no head reads
+    it: last rows first, then prefix_rows[0], [1], ...), groups [(qi, base, cnt)] (head qi on output rows base ..
+    base + cnt - 1), prefix_off [k] and label_idx [head_rows] (each output row's prefix token in the joiners'
+    concatenated prefixes, -1 for the last rows), kv_dst [M] (flat cache row slot * n_max + row_pos), conv_src and
+    conv_dst [2k] (prompt rows P - 2, P - 1 -> flat conv-history rows slot * 2 + j) and conv_zero (flat conv rows
+    before a prompt's first row)."""
+
+    def __init__(self, n_tok, slots, n_max: int, q: int, h: int, abs_row_base=None, logprob: bool = False):
+        k = len(n_tok)
+        self.k = k
+        self.P = np.array([sum(n + 1 for n in t) for t in n_tok], dtype=np.int64)
+        self.start = np.concatenate([[0], np.cumsum(self.P)[:-1]]).astype(np.int64)
+        self.M = int(self.P.sum())
+        self.max_len = int(self.P.max())
+        self.row_pos = np.concatenate([np.arange(p) for p in self.P]).astype(np.int32)
+        self.src_row2 = None
+        if abs_row_base is not None:
+            r2 = np.full(self.M, -1, dtype=np.int32)
+            for s0, t in zip(self.start, n_tok):
+                pos0 = s0
+                for s, n in enumerate(t):
+                    r2[pos0 + 1:pos0 + 1 + n] = abs_row_base[s] + np.arange(n)
+                    pos0 += n + 1
+            self.src_row2 = r2
+        self.work = lpt_work(self.P.tolist(), h)
+        self.last_row = self.start + self.P - 1
+        n_pre = [t[-1] if logprob else 0 for t in n_tok]
+        pred0 = [s0 + sum(n + 1 for n in t[:-1]) for s0, t in zip(self.start, n_tok)]   # each predicted sequence's start token
+        self.prefix_off = np.concatenate([[0], np.cumsum(n_pre)[:-1]]).astype(np.int64)
+        self.prefix_rows = [np.concatenate([p0 + np.arange(qi, n, q) for p0, n in zip(pred0, n_pre)]).astype(np.int64) for qi in range(q)]
+        prefix_tok = [np.concatenate([o + np.arange(qi, n, q) for o, n in zip(self.prefix_off, n_pre)]).astype(np.int64) for qi in range(q)]
+        out_rows = [self.last_row] + self.prefix_rows
+        self.head_rows = sum(len(r) for r in out_rows)
+        self.dest_row = np.full(self.M, -1, dtype=np.int32)
+        self.dest_row[np.concatenate(out_rows)] = np.arange(self.head_rows)
+        self.groups, base = [], 0
+        for qi in range(q):
+            cnt = len(self.prefix_rows[qi]) + (k if qi == 0 else 0)
+            if cnt:
+                self.groups.append((qi, base, cnt))
+            base += cnt
+        self.label_idx = np.concatenate([np.full(k, -1, dtype=np.int64)] + prefix_tok)
+        slot = np.asarray(slots, dtype=np.int64)
+        self.slots = slot
+        self.kv_dst = np.repeat(slot * n_max, self.P) + self.row_pos
+        hist = self.P[:, None] + np.arange(-2, 0)[None]                               # prompt rows P - 2, P - 1
+        self.conv_dst = (slot[:, None] * 2 + np.arange(2)[None]).reshape(-1)
+        self.conv_src = (self.start[:, None] + np.maximum(hist, 0)).reshape(-1)
+        self.conv_zero = self.conv_dst[(hist < 0).reshape(-1)]
+
+    def to_device(self, dev):
+        """The device arrays, sent in one non-blocking copy (staged from pageable memory, as decode.row_arrays does, so
+        that it never waits for the device): a namespace of the arrays above that the forward and the install read."""
+        arrays = dict(row_pos=self.row_pos, work=self.work, seq_start=self.start.astype(np.int32), seq_len=self.P.astype(np.int32),
+                      dest_row=self.dest_row, kv_dst=self.kv_dst, conv_dst=self.conv_dst, conv_src=self.conv_src, slots=self.slots,
+                      label_idx=self.label_idx)
+        if self.src_row2 is not None:
+            arrays["src_row2"] = self.src_row2
+        if len(self.conv_zero):
+            arrays["conv_zero"] = self.conv_zero
+        parts, where, off = [], {}, 0
+        for name, a in arrays.items():
+            raw = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
+            where[name] = (off, a.dtype, a.shape)
+            parts += [raw, np.zeros(-len(raw) % 8, dtype=np.uint8)]
+            off += len(raw) + (-len(raw) % 8)
+        buf = torch.from_numpy(np.concatenate(parts)).to(dev, non_blocking=True)
+        dv = dict(M=self.M, max_len=self.max_len, groups=self.groups, src_row2=None, conv_zero=None)
+        for name, (o, dt, shape) in where.items():
+            tdt = torch.int32 if dt == np.int32 else torch.int64
+            dv[name] = buf[o:o + int(np.prod(shape)) * dt.itemsize].view(tdt).view(shape)
+        return types.SimpleNamespace(**dv)
+
+
+class _PackedCapture:
+    """Receives a packed prefill's per-layer K/V rows and pre-conv FFN rows (Engine.forward_packed) into the joiners'
+    slots of a DecodeSession: every prompt row's K/V at its position, and prompt rows P - 2, P - 1 as conv history
+    (zero before a prompt's first row), one gather or scatter per layer and kind, as _PromptCapture does per row."""
+
+    def __init__(self, dec, dv):
+        self.dec, self.dv = dec, dv
+
+    def after_kv(self, l, kvn):
+        self.dec.cache[l].view(-1, 128).index_copy_(0, self.dv.kv_dst, kvn)
+
+    def after_u(self, l, u):
+        conv = self.dec.conv[l].view(-1, u.shape[-1])
+        conv.index_copy_(0, self.dv.conv_dst, u.index_select(0, self.dv.conv_src))
+        if self.dv.conv_zero is not None:
+            conv.index_fill_(0, self.dv.conv_zero, 0)
 
 
 class _Row:
@@ -127,7 +262,7 @@ class GenerationSession:
     use and never again.  trace_logits (tests): run eagerly and keep the [n, codebook+1] logits each row's tokens were
     sampled from, returned by `traced_logits(handle)` once the row has finished.
     return_logprobs: `finished()` maps each handle to (tokens, logprobs, sample_logprobs), each [n, q], with the
-    definitions of `generate(..., return_logprobs=True)`; the prefix values come from the row's own prefill.
+    definitions of `generate(..., return_logprobs=True)`; the prefix values come from the row's rows of the packed prefill.
 
     The transformer's weights are packed when the session is created; train it between sessions, not during one.
     Every row gets exactly what `generate` gives that row alone with seeds=[seed] and the same arguments; free and
@@ -165,6 +300,7 @@ class GenerationSession:
         self._trace_base = 0
         self._graphs = GraphCache(self.use_graph)
         self.eng = self.dec = None     # the engine and the slots' device state, made by the first step that runs a row
+        self._pack_ws = None           # the packed prefill's workspace, made at the first join
 
     def _device_state(self):
         if self.dec is None:
@@ -233,8 +369,11 @@ class GenerationSession:
             if self.trace:
                 self._traced[handle] = torch.empty(0, self.C, device=dev)
             return handle
+        if self.append_eos:                                                                        # open_musiclm.py:288-290
+            cond = [torch.cat([t, torch.full((1, 1), e, device=dev, dtype=torch.int64)], 1) for t, e in zip(cond, self.w.eos_ids)]
         self.sched.submit(_Row(handle, P, n, pred_start, payload=dict(
-            cond=cond, prefix=prefix, seed=seed, top_k=top_k, temperature=float(temperature), top_p=top_p)))
+            ids=cond + [prefix], n_tok=cond_lens + [n_pre], prefix=prefix, seed=seed, top_k=top_k, temperature=float(temperature),
+            top_p=top_p)))
         return handle
 
     @property
@@ -265,17 +404,16 @@ class GenerationSession:
         return out[0] if lp is None else tuple(t[0] for t in out)
 
     def _install(self, rows):
-        """Prefills each joining row alone and writes its prompt's K/V rows, conv history and last logits into its
-        slot, then sets the slot's arrays.  Runs after the boundary step (which writes every slot's cache and conv
+        """Prefills the joining rows together, packed back to back (_prefill_packed; in consecutive groups when their
+        prompts exceed the packed workspace), writes each prompt's K/V rows, conv history and last logits into its
+        slot, then sets the slots' arrays.  Runs after the boundary step (which writes every slot's cache and conv
         history at the slot's old position) and before the boundary sample."""
         eng, dec, dev = self.eng, self.dec, self.eng.dev
-        for row in rows:
-            a = row.payload
-            pl, ws = prefill(self.w, a["cond"], a["prefix"], self.append_eos, dec, slice(row.slot, row.slot + 1),
-                             torch.full((1,), row.P, device=dev))
-            assert pl.N == row.P and pl.pos0[-1] == row.pred_start, (pl.N, row.P)
-            if self.logprob:
-                a["prefix_lp"] = prefix_logprobs(eng, pl, ws, a["prefix"], self.q, self.C)[0] if a["prefix"].shape[1] else None
+        if self._pack_ws is None:
+            self._pack_rows = min(max(self.max_positions, PACK_ROWS), self.slots * self.max_positions)
+            self._pack_ws = eng.packed_workspace(self._pack_rows, self._pack_rows if self.logprob else self.slots)
+        for group in split_joiners([r.P for r in rows], self._pack_rows):
+            self._prefill_packed([rows[i] for i in group])
         idx = torch.tensor([r.slot for r in rows], device=dev)
         states = [r.device_state() for r in rows]
         vals = row_arrays(dev, len(rows), pos=[s["pos"] for s in states], pos_last=[s["pos_last"] for s in states],
@@ -287,6 +425,37 @@ class GenerationSession:
             dst[idx] = vals[name]
         dec.top_p[idx] = vals["top_p"] if vals["top_p"] is not None else 1.0
         dec.seeds[idx] = seeds_tensor([r.payload["seed"] for r in rows], len(rows), dev)
+
+    def _prefill_packed(self, rows):
+        """One packed forward over the rows' prompts (Engine.forward_packed), installed by _PackedCapture; the last
+        rows' head-0 logits go to the slots' logits rows, and with return_logprobs each row's prefix log-probabilities
+        are scored from the same heads and rows as prefix_logprobs scores them in `generate`'s prefill."""
+        eng, dec, ws = self.eng, self.dec, self._pack_ws
+        plan = PackedPrefill([r.payload["n_tok"] for r in rows], [r.slot for r in rows], dec.n_max, self.q, eng.h,
+                             eng.abs_row_base if eng.abs_pos else None, self.logprob)
+        dv = plan.to_device(eng.dev)
+        src = []
+        for r in rows:                        # the token plan of each prompt, as decode.prefill makes it
+            _, src_row, _, _, _ = lib.token_plan(r.payload["ids"], [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs],
+                                                 eng.emb_row_base, eng.start_row, append_eos=False, drop_last=False, mask_cond=False,
+                                                 want_labels=False, err_flag=eng.err_flag)
+            src.append(src_row.view(-1))
+        dv.src_row = torch.cat(src) if len(src) > 1 else src[0]
+        eng.forward_packed(ws, dv, dec.table, capture=_PackedCapture(dec, dv))
+        k, Cp = len(rows), eng.Cp[-1]
+        dec.logits[:, :Cp].index_copy_(0, dv.slots, ws["logits"][:k])
+        if self.logprob:
+            pre = [r.payload["prefix"][0] for r in rows]
+            lp = torch.zeros(sum(p.shape[0] for p in pre), device=eng.dev, dtype=torch.float32)
+            if lp.numel():
+                ids = torch.cat(pre)
+                tok = torch.where((ids >= 0) & (ids < self.C), ids, -100)[dv.label_idx[k:]]
+                labels = torch.cat([tok.new_full((k,), -100), tok]).to(torch.int32)
+                out = torch.empty(plan.head_rows, device=eng.dev, dtype=torch.float32)
+                lib.token_logprob(ws["logits"][:plan.head_rows], labels, self.C, out)
+                lp.index_copy_(0, dv.label_idx[k:], out[k:])
+            for r, o, p in zip(rows, plan.prefix_off.tolist(), pre):
+                r.payload["prefix_lp"] = lp[o:o + p.shape[0]] if p.shape[0] else None
 
     def _sample_point(self):
         if self.trace:
