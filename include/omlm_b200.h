@@ -223,6 +223,15 @@ int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* table, int ta
 int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const float* table, int table_ld, const int* work, int n_work,
                             const int* seq_start, const int* seq_len, int M, int max_len, void* out, float* lse2, int heads,
                             float scale, void* stream);
+/* omlm_attn_fwd_tc_varlen over chunks of longer sequences (a chunked prefill): sequence b's seq_len[b] query rows are
+ * positions p0 = q_off[b] ... of its prompt (p0 * heads a multiple of 128) and its keys are rows kv_start[b] + j of kv
+ * (kv_rows rows of 128, e.g. a K/V cache that already holds positions 0 .. p0 + seq_len[b] - 1), visible for
+ * j < p0 + seq_len[b]; rows past that end may hold anything, NaN included.  work as above (row blocks counted from the
+ * chunk's first row); table_ld >= max_end >= every p0 + seq_len[b].  out and lse2 of each chunk row are bit-identical to
+ * omlm_attn_fwd_tc over the whole prompt. */
+int omlm_attn_fwd_tc_chunk(const void* qn, const void* kv, long kv_rows, const float* table, int table_ld, const int* work,
+                           int n_work, const int* seq_start, const int* seq_len, const int* q_off, const int* kv_start, int M,
+                           int max_end, void* out, float* lse2, int heads, float scale, void* stream);
 /* Accumulates (+=) into dqn fp32 [B,N,heads*64], dkvn fp32 [B,N,128], dtable fp32 [heads,table_ld]. */
 int omlm_attn_bwd(const void* qn, const void* kvn, const void* d_o, const void* o, const float* lse2,
                   const float* table, int table_ld, const unsigned char* key_mask, float* dsum_scratch,
@@ -258,6 +267,14 @@ int omlm_gemm_ffn_up(const void* xn, const void* w1_packed, const float* conv_w_
  * afresh where M % Nseq did.  Every row's u, h and rowsum are bit-identical to omlm_gemm_ffn_up on its sequence alone. */
 int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
                             float* rowsum, const int* row_pos, int M, int K, int Fp, int act_f16, int max_ctas, void* stream);
+/* omlm_gemm_ffn_up_varlen over chunks that continue longer sequences: a row m with c = hist_idx[m] >= 0 (int32 device
+ * array [M], -1 elsewhere) is the first row of a chunk at position p0 > 0, whose conv inputs t-2 and t-1 are rows 2c and
+ * 2c + 1 of hist (pre-conv u rows of the sequence's positions p0 - 2 and p0 - 1, [*, 2 Fp] in the activation format; a
+ * zero row for p0 - 2 < 0).  row_pos[m] is the row's position in its whole sequence.  Every row's u, h and rowsum are
+ * bit-identical to omlm_gemm_ffn_up on the whole sequence. */
+int omlm_gemm_ffn_up_chunk(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
+                           float* rowsum, const int* row_pos, const void* hist, const int* hist_idx, int M, int K, int Fp,
+                           int act_f16, int max_ctas, void* stream);
 /* hn = dropout(LayerNorm_F(h)) from the fused statistics; stats fp32 [M, 2] = (mean, rstd) for the backward pass.
  * With drop_p > 0 the Philox keep mask is also written to keep_bits (uint8 [M, Fp/8], bit i of byte j = channel 8j+i)
  * so the backward pass reads 1 bit per element instead of regenerating the random stream. */

@@ -49,12 +49,17 @@ __device__ __forceinline__ float ex2_fast(float x) {
 // kVarlen: sequences of their own lengths packed back to back.  CTA x takes the unit (sequence work[2x], row block
 // work[2x + 1]) of a host-built list (heaviest first); sequence b is rows seq_start[b] .. seq_start[b] + seq_len[b] - 1
 // of the packed Q and K/V buffers.  N, nbatch and key_mask are then unused (no key mask: visibility is j < seq_len[b]).
+// With q_off and kv_start (a chunk of a longer prompt): sequence b's query rows are positions p0 = q_off[b] ..
+// p0 + seq_len[b] - 1 (p0 * h a multiple of 128, so its row blocks are row blocks of the whole prompt), and its keys are
+// rows kv_start[b] + j of the K/V buffer, visible for j < p0 + seq_len[b].  Key rows past the visible end may hold
+// anything; their V rows are zeroed in shared memory, so P = 0 gives exact zero products as TMA zero fill does.
 template <bool kVarlen>
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                    const float* __restrict__ table, int table_ld, const unsigned char* __restrict__ key_mask,
                    __nv_bfloat16* __restrict__ out, float* __restrict__ lse2, int N_fixed, int h, float scale, int nbatch,
-                   int win_ld, const int* __restrict__ work, const int* __restrict__ seq_start, const int* __restrict__ seq_len) {
+                   int win_ld, const int* __restrict__ work, const int* __restrict__ seq_start, const int* __restrict__ seq_len,
+                   const int* __restrict__ q_off, const int* __restrict__ kv_start) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // pointer arithmetic (not an integer round trip) keeps the shared address space visible to the compiler: LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -64,13 +69,15 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
   uint64_t* kv_empty = bars + 3;   // [2]
 
   const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
-  const int N = kVarlen ? seq_len[work[2 * blockIdx.x]] : N_fixed;
+  const int p0 = kVarlen && q_off != nullptr ? q_off[work[2 * blockIdx.x]] : 0;   // varlen: first query row's position
+  const int N = kVarlen ? p0 + seq_len[work[2 * blockIdx.x]] : N_fixed;
   const int R = N * h;
   const int nblk = (R + kTcBQ - 1) / kTcBQ;
   // longest-processing-time-first: all batch elements of the heaviest (latest) row block are scheduled first
   const int b = kVarlen ? work[2 * blockIdx.x] : blockIdx.x % nbatch;
-  const int rb = kVarlen ? work[2 * blockIdx.x + 1] : nblk - 1 - blockIdx.x / nbatch;
+  const int rb = kVarlen ? p0 * h / kTcBQ + work[2 * blockIdx.x + 1] : nblk - 1 - blockIdx.x / nbatch;
   const int s0 = kVarlen ? seq_start[b] : 0;    // varlen: first packed row of the sequence
+  const int kv0 = kVarlen && kv_start != nullptr ? kv_start[b] : s0;   // varlen: K/V row of key 0
   const int r0 = rb * kTcBQ;
   const int i_max_cta = min(N - 1, (r0 + kTcBQ - 1) / h);
   const int T = i_max_cta / kTcBK + 1;
@@ -89,13 +96,13 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
       mbar_expect_tx(q_full, 16384);
-      tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, kVarlen ? s0 * h + r0 : b * R + r0);
+      tma_load_2d(smem + kOffQ, &tmQ, q_full, 0, kVarlen ? (s0 - p0) * h + r0 : b * R + r0);
       for (int t = 0; t < T; ++t) {
         const int st = t & 1;
         mbar_wait(&kv_empty[st], ((t >> 1) & 1) ^ 1);
         mbar_expect_tx(&kv_full[st], 2 * 16384);
-        tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, (kVarlen ? s0 : b * N) + t * kTcBK);
-        tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, (kVarlen ? s0 : b * N) + t * kTcBK);
+        tma_load_2d(smem + kOffK + st * 16384, &tmKV, &kv_full[st], 0, (kVarlen ? kv0 : b * N) + t * kTcBK);
+        tma_load_2d(smem + kOffV + st * 16384, &tmKV, &kv_full[st], 64, (kVarlen ? kv0 : b * N) + t * kTcBK);
       }
     }
     return;
@@ -153,6 +160,14 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     for (int k = 0; k < 4; ++k) {
       const int j = j0 + 32 * k + lane;
       visw[k] = __ballot_sync(0xffffffffu, j < N && (km == nullptr || km[j] != 0));
+    }
+    if constexpr (kVarlen) {
+      const int nz = j0 + kTcBK - N;    // key rows past the visible end in this tile: zero V (128 B per row)
+      if (nz > 0) {
+        uint4* vz = reinterpret_cast<uint4*>(smem + kOffV + st * 16384 + (kTcBK - nz) * 128);
+        for (int x = tid128; x < nz * 8; x += 128) vz[x] = make_uint4(0u, 0u, 0u, 0u);
+        fence_proxy_async();            // generic-proxy stores before the wgmma reads them (after the barrier below)
+      }
     }
     // the buffer written here was last read in tile t - 2, before every thread's barrier of tile t - 1
     asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
@@ -221,11 +236,11 @@ attn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     l[hr] += __shfl_xor_sync(0xffffffffu, l[hr], 2);
     if (rr[hr] < R) {
       const float inv = l[hr] > 0.f ? 1.f / l[hr] : 0.f;
-      __nv_bfloat16* op = out + ((kVarlen ? static_cast<long long>(s0) * h : static_cast<long long>(b) * R) + rr[hr]) * 64 + 2 * qc;
+      __nv_bfloat16* op = out + ((kVarlen ? static_cast<long long>(s0 - p0) * h : static_cast<long long>(b) * R) + rr[hr]) * 64 + 2 * qc;
 #pragma unroll
       for (int c = 0; c < 8; ++c)
         *reinterpret_cast<uint32_t*>(op + 8 * c) = pack_bf16x2(o[4 * c + 2 * hr] * inv, o[4 * c + 2 * hr + 1] * inv);
-      if (qc == 0) lse2[(kVarlen ? static_cast<long long>(s0) * h : static_cast<long long>(b) * R) + rr[hr]] = m[hr] + log2f(l[hr]);
+      if (qc == 0) lse2[(kVarlen ? static_cast<long long>(s0 - p0) * h : static_cast<long long>(b) * R) + rr[hr]] = m[hr] + log2f(l[hr]);
     }
   }
 }
@@ -255,24 +270,27 @@ extern "C" int omlm_attn_fwd_tc(const void* qn, const void* kvn, const float* ta
   const unsigned grid = static_cast<unsigned>((R + kTcBQ - 1) / kTcBQ) * B;   // (row block, batch) in LPT order
   OMLM_KLAUNCH((attn_fwd_tc_kernel<false>), grid, kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
       tmQ, tmKV, table, table_ld, key_mask, reinterpret_cast<__nv_bfloat16*>(out), lse2, N, heads, scale, B,
-      fwd_win_ld(heads), nullptr, nullptr, nullptr);
+      fwd_win_ld(heads), nullptr, nullptr, nullptr, nullptr, nullptr);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
 
 #else
-extern "C" int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const float* table, int table_ld, const int* work,
-                                       int n_work, const int* seq_start, const int* seq_len, int M, int max_len, void* out,
-                                       float* lse2, int heads, float scale, void* stream) {
+// Both varlen entry points: Q from the packed qn, K/V from kv (kv_rows rows of 128), sequence b's keys at kv_start[b]
+// (seq_start[b] when kv_start is null), its queries at positions q_off[b] ... (0 when q_off is null).
+static int attn_fwd_tc_varlen_launch(const void* qn, const void* kv, long kv_rows, const float* table, int table_ld,
+                                     const int* work, int n_work, const int* seq_start, const int* seq_len, const int* q_off,
+                                     const int* kv_start, int M, int max_end, void* out, float* lse2, int heads, float scale,
+                                     void* stream) {
   using namespace omlm;
-  OMLM_CHECK_ARG(M > 0 && n_work > 0 && max_len > 0 && heads > 0, "attn_fwd_tc_varlen: bad shape");
-  OMLM_CHECK_ARG(table_ld >= max_len, "attn_fwd_tc_varlen: bias table shorter than the longest sequence");
+  OMLM_CHECK_ARG(M > 0 && n_work > 0 && max_end > 0 && heads > 0 && kv_rows > 0, "attn_fwd_tc_varlen: bad shape");
+  OMLM_CHECK_ARG(table_ld >= max_end, "attn_fwd_tc_varlen: bias table shorter than the longest sequence");
   const int smem = fwd_smem(heads);
   OMLM_CHECK_ARG(smem <= kTcMaxSmem, "attn_fwd_tc_varlen: too many heads (%d) for the shared-memory bias windows", heads);
   CUtensorMap tmQ, tmKV;
   int rc = make_tmap_bf16_2d(&tmQ, qn, 64, static_cast<uint64_t>(M) * heads, 128, 64, kTcBQ);
   if (rc) return rc;
-  rc = make_tmap_bf16_2d(&tmKV, kvn, 128, static_cast<uint64_t>(M), 256, 64, kTcBK);
+  rc = make_tmap_bf16_2d(&tmKV, kv, 128, static_cast<uint64_t>(kv_rows), 256, 64, kTcBK);
   if (rc) return rc;
   static int configured = 0;
   if (configured < smem) {
@@ -281,8 +299,24 @@ extern "C" int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const fl
   }
   OMLM_KLAUNCH((attn_fwd_tc_kernel<true>), static_cast<unsigned>(n_work), kTcThreads, smem, reinterpret_cast<cudaStream_t>(stream),
       tmQ, tmKV, table, table_ld, nullptr, reinterpret_cast<__nv_bfloat16*>(out), lse2, 0, heads, scale, 0, fwd_win_ld(heads),
-      work, seq_start, seq_len);
+      work, seq_start, seq_len, q_off, kv_start);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int omlm_attn_fwd_tc_varlen(const void* qn, const void* kvn, const float* table, int table_ld, const int* work,
+                                       int n_work, const int* seq_start, const int* seq_len, int M, int max_len, void* out,
+                                       float* lse2, int heads, float scale, void* stream) {
+  return attn_fwd_tc_varlen_launch(qn, kvn, M, table, table_ld, work, n_work, seq_start, seq_len, nullptr, nullptr, M, max_len,
+                                   out, lse2, heads, scale, stream);
+}
+
+extern "C" int omlm_attn_fwd_tc_chunk(const void* qn, const void* kv, long kv_rows, const float* table, int table_ld,
+                                      const int* work, int n_work, const int* seq_start, const int* seq_len, const int* q_off,
+                                      const int* kv_start, int M, int max_end, void* out, float* lse2, int heads, float scale,
+                                      void* stream) {
+  OMLM_CHECK_ARG(q_off != nullptr && kv_start != nullptr, "attn_fwd_tc_chunk: q_off and kv_start are required");
+  return attn_fwd_tc_varlen_launch(qn, kv, kv_rows, table, table_ld, work, n_work, seq_start, seq_len, q_off, kv_start, M,
+                                   max_end, out, lse2, heads, scale, stream);
 }
 #endif

@@ -29,12 +29,15 @@ constexpr int kFuThreads = 384;   // TMA warpgroup, two wgmma / epilogue warpgro
 // F16: xn, W1 arrive as fp16 and u, h leave as fp16 (all bounded by construction: LayerNorm output x weights);
 // otherwise everything is bf16.
 // kVarlen: sequences of their own lengths packed back to back; row m's position within its sequence is row_pos[m]
-// (0 at each sequence start) instead of m % Nseq.
+// (0 at each sequence start) instead of m % Nseq.  With hist_idx: a row m with c = hist_idx[m] >= 0 is the first row
+// of a chunk that continues a sequence (position p0 > 0): its t-2 and t-1 conv inputs are rows 2c and 2c + 1 of hist
+// (pre-conv u rows in the activation format, [*, 2 Fp]), and the next row's t-2 input is row 2c + 1.
 template <bool F16, bool kVarlen = false>
 __global__ void __launch_bounds__(kFuThreads, 1)
 gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    __nv_bfloat16* __restrict__ u_out, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rowsum,
-                   const float* __restrict__ conv_w, int M, int Nseq, int K, int Fp, const int* __restrict__ row_pos) {
+                   const float* __restrict__ conv_w, int M, int Nseq, int K, int Fp, const int* __restrict__ row_pos,
+                   const __nv_bfloat16* __restrict__ hist, const int* __restrict__ hist_idx) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kFuOffBar);
@@ -82,10 +85,16 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
     for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
       const int n_blk = w % n_tiles, m_blk = w / n_tiles;
       // varlen: lane r holds the position of row r of this warp's epilogue run (phase 2), loaded under the main loop
-      int lane_pos = 0;
+      // and hist_idx of that row; lane 16 holds hist_idx of the row before the run
+      int lane_pos = 0, lane_hist = -1;
       if constexpr (kVarlen) {
         const long g0 = static_cast<long>(m_blk) * kFuRowsOut + (et >> 5) * 16;
-        if (lane < min(16, kFuRowsOut - (et >> 5) * 16) && g0 + lane < M) lane_pos = row_pos[g0 + lane];
+        if (lane < min(16, kFuRowsOut - (et >> 5) * 16) && g0 + lane < M) {
+          lane_pos = row_pos[g0 + lane];
+          if (hist_idx != nullptr) lane_hist = hist_idx[g0 + lane];
+        } else if (lane == 16 && hist_idx != nullptr && g0 >= 1 && g0 <= M) {
+          lane_hist = hist_idx[g0 - 1];
+        }
       }
       float acc[kFuBN / 2];
 #pragma unroll
@@ -160,6 +169,16 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
           xv2[0] = unpack16x2<F16>(a.x); xv2[1] = unpack16x2<F16>(a.y); xg2[0] = unpack16x2<F16>(g.x); xg2[1] = unpack16x2<F16>(g.y);
         }
         if (pos == 1) { xv2[0] = xv2[1] = xg2[0] = xg2[1] = make_float2(0.f, 0.f); }   // row t-2 belongs to the previous sequence
+        // varlen with history: bit r set when row r starts a chunk with history rows
+        const unsigned hstarts = kVarlen ? __ballot_sync(0xffffffffu, lane < nrows && lane_hist >= 0) : 0u;
+        if constexpr (kVarlen) {
+          const int prev_c = __shfl_sync(0xffffffffu, lane_hist, 16);
+          if (prev_c >= 0) {   // the run's first row is the second row of a chunk: its t-2 input is that chunk's t-1 history row
+            const uint8_t* hp = reinterpret_cast<const uint8_t*>(hist) + (2L * prev_c + 1) * (4L * Fp) + n_blk * 512 + lane * 8;
+            const uint2 a = *reinterpret_cast<const uint2*>(hp), g = *reinterpret_cast<const uint2*>(hp + 256);
+            xv2[0] = unpack16x2<F16>(a.x); xv2[1] = unpack16x2<F16>(a.y); xg2[0] = unpack16x2<F16>(g.x); xg2[1] = unpack16x2<F16>(g.y);
+          }
+        }
         float st[32];
         __nv_bfloat16* ug = u_out + grow0 * (2L * Fp) + n_blk * kFuBN + lane * 8;
         __nv_bfloat16* hg = h_out + grow0 * static_cast<long>(Fp) + n_blk * 128 + lane * 4;
@@ -172,10 +191,19 @@ gemm_ffn_up_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constan
             const uint2 a = *reinterpret_cast<const uint2*>(rr + lane * 8);
             const uint2 g = *reinterpret_cast<const uint2*>(rr + 256 + lane * 8);
             const float2 xv0[2] = {unpack16x2<F16>(a.x), unpack16x2<F16>(a.y)}, xg0[2] = {unpack16x2<F16>(g.x), unpack16x2<F16>(g.y)};
-            if (kVarlen ? ((starts >> r) & 1u) != 0 : pos == 0) {   // sequence start: no history (the zeros then slide into the t-2 slot for the next row)
-              const float2 z = make_float2(0.f, 0.f);
-              xv1[0] = xv1[1] = xg1[0] = xg1[1] = z;
-              xv2[0] = xv2[1] = xg2[0] = xg2[1] = z;
+            // one test per row on the common path: a sequence start or (varlen) a chunk start with history
+            if (kVarlen ? (((starts | hstarts) >> r) & 1u) != 0 : pos == 0) {
+              if (!kVarlen || ((starts >> r) & 1u) != 0) {   // sequence start: no history (the zeros then slide into the t-2 slot for the next row)
+                const float2 z = make_float2(0.f, 0.f);
+                xv1[0] = xv1[1] = xg1[0] = xg1[1] = z;
+                xv2[0] = xv2[1] = xg2[0] = xg2[1] = z;
+              } else {                                       // chunk start: history rows 2c (t-2), 2c + 1 (t-1)
+                const uint8_t* hp = reinterpret_cast<const uint8_t*>(hist) + 2L * hist_idx[grow0 + r] * (4L * Fp) + n_blk * 512 + lane * 8;
+                const uint2 a2 = *reinterpret_cast<const uint2*>(hp), g2 = *reinterpret_cast<const uint2*>(hp + 256);
+                const uint2 a1 = *reinterpret_cast<const uint2*>(hp + 4L * Fp), g1 = *reinterpret_cast<const uint2*>(hp + 4L * Fp + 256);
+                xv2[0] = unpack16x2<F16>(a2.x); xv2[1] = unpack16x2<F16>(a2.y); xg2[0] = unpack16x2<F16>(g2.x); xg2[1] = unpack16x2<F16>(g2.y);
+                xv1[0] = unpack16x2<F16>(a1.x); xv1[1] = unpack16x2<F16>(a1.y); xg1[0] = unpack16x2<F16>(g1.x); xg1[1] = unpack16x2<F16>(g1.y);
+              }
             }
             float2 h[2], sq = make_float2(0.f, 0.f), sm = sq;
 #pragma unroll
@@ -240,14 +268,14 @@ extern "C" int omlm_gemm_ffn_up(const void* xn, const void* w1_packed, const flo
   auto kern = act_f16 ? gemm_ffn_up_kernel<true> : gemm_ffn_up_kernel<false>;
   OMLM_KLAUNCH((kern), grid, kFuThreads, kFuSmem, reinterpret_cast<cudaStream_t>(stream), 
       tmA, tmB, reinterpret_cast<__nv_bfloat16*>(u_out), reinterpret_cast<__nv_bfloat16*>(h_out), rowsum, conv_w_packed, M,
-      Nseq, K, Fp, nullptr);
+      Nseq, K, Fp, nullptr, nullptr, nullptr);
   OMLM_LAUNCH_CHECK();
   return 0;
 }
 #else
-extern "C" int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out,
-                                       void* h_out, float* rowsum, const int* row_pos, int M, int K, int Fp, int act_f16,
-                                       int max_ctas, void* stream) {
+static int gemm_ffn_up_varlen_launch(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out, void* h_out,
+                                     float* rowsum, const int* row_pos, const void* hist, const int* hist_idx, int M, int K, int Fp,
+                                     int act_f16, int max_ctas, void* stream) {
   using namespace omlm;
   OMLM_CHECK_ARG(M > 0 && K > 0 && K % 8 == 0 && Fp > 0 && Fp % 128 == 0 && row_pos != nullptr,
                  "gemm_ffn_up_varlen: bad shape M=%d K=%d Fp=%d", M, K, Fp);
@@ -269,8 +297,23 @@ extern "C" int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, co
   auto kern = act_f16 ? gemm_ffn_up_kernel<true, true> : gemm_ffn_up_kernel<false, true>;
   OMLM_KLAUNCH((kern), grid, kFuThreads, kFuSmem, reinterpret_cast<cudaStream_t>(stream),
       tmA, tmB, reinterpret_cast<__nv_bfloat16*>(u_out), reinterpret_cast<__nv_bfloat16*>(h_out), rowsum, conv_w_packed, M,
-      1, K, Fp, row_pos);
+      1, K, Fp, row_pos, reinterpret_cast<const __nv_bfloat16*>(hist), hist_idx);
   OMLM_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int omlm_gemm_ffn_up_varlen(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out,
+                                       void* h_out, float* rowsum, const int* row_pos, int M, int K, int Fp, int act_f16,
+                                       int max_ctas, void* stream) {
+  return gemm_ffn_up_varlen_launch(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, row_pos, nullptr, nullptr, M, K, Fp,
+                                   act_f16, max_ctas, stream);
+}
+
+extern "C" int omlm_gemm_ffn_up_chunk(const void* xn, const void* w1_packed, const float* conv_w_packed, void* u_out,
+                                      void* h_out, float* rowsum, const int* row_pos, const void* hist, const int* hist_idx, int M,
+                                      int K, int Fp, int act_f16, int max_ctas, void* stream) {
+  OMLM_CHECK_ARG(hist != nullptr && hist_idx != nullptr, "gemm_ffn_up_chunk: hist and hist_idx are required");
+  return gemm_ffn_up_varlen_launch(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, row_pos, hist, hist_idx, M, K, Fp,
+                                   act_f16, max_ctas, stream);
 }
 #endif

@@ -507,8 +507,8 @@ class Engine:
         lib.embed_gather(self.table, src_row, ws["x"][0], pl.src_row2)
         self.build_bias_table(ws, N)
         x_last = self._layers(ws, pl.M, train, drop, capture,
-                              lambda i: lib.attn_fwd_tc(ws["qn"][i], ws["kvn"][i], ws["table"], key_mask, ws["o"][i], ws["lse"][i], B, N, h),
-                              lambda xn2, i, pk: lib.gemm_ffn_up(xn2, pk["w1"], pk["conv"], ws["u"][i], ws["h"], ws["rowsum"], N, Fp))
+                              lambda i, l: lib.attn_fwd_tc(ws["qn"][i], ws["kvn"][i], ws["table"], key_mask, ws["o"][i], ws["lse"][i], B, N, h),
+                              lambda xn2, i, l, pk: lib.gemm_ffn_up(xn2, pk["w1"], pk["conv"], ws["u"][i], ws["h"], ws["rowsum"], N, Fp))
         f16 = self.a16 != torch.bfloat16
         dup = f16 and train
         xf = ws["xf16"] if f16 else ws["xf"]
@@ -520,8 +520,8 @@ class Engine:
             lib.gemm(xf[base:base + rows], self.pk_logit[s][qi], ws["logits"][gi], block_n=128)
 
     def _layers(self, ws, M: int, train: bool, drop: bool, capture, attn, ffn_up):
-        """The depth x (attention, conv-FFN) loop over the M rows of ws["x"][0]; attn(i) and ffn_up(xn2, i, pk) launch the
-        two kernels that depend on how the rows form sequences.  Returns the last residual stream."""
+        """The depth x (attention, conv-FFN) loop over the M rows of ws["x"][0]; attn(i, l) and ffn_up(xn2, i, l, pk) launch
+        the two kernels that depend on how the rows form sequences (i: the workspace slot of layer l).  Returns the last residual stream."""
         d, h, HD, F, Fp = self.d, self.h, self.HD, self.F, self.Fp
         pv = self.pview
         x = ws["x"]
@@ -539,11 +539,11 @@ class Engine:
             lib.qk_l2norm_fwd(ws["q_raw"][i], ws["kv_raw"][i], pv[p + "0.q_scale"], pv[p + "0.k_scale"], ws["qn"][i], ws["kvn"][i], h)
             if capture is not None:
                 capture.after_kv(l, ws["kvn"][i])
-            attn(i)
+            attn(i, l)
             lib.gemm(ws["o"][i], pk["wo_b"], xm, addend=xa, block_n=self._bn_for(M, d, HD))
             xn2 = ws["xn2_16"] if f16 else ws["xn2"][i]
             lib.layernorm_fwd(xm, pv[p + self.ffk["g1"]], xn2, None, ws["st_f"][i], ycopy=ws["xn2"][i] if dup else None)
-            ffn_up(xn2, i, pk)                                                 # conv + GEGLU in the epilogue
+            ffn_up(xn2, i, l, pk)                                                 # conv + GEGLU in the epilogue
             if capture is not None:
                 capture.after_u(l, ws["u"][i])
             hn = ws["hn16"] if f16 else ws["hn"][i]
@@ -570,22 +570,35 @@ class Engine:
             ws.update(xn=[E(rows, d)], xn2=[E(rows, d)], hn=[E(rows, Fp)], xf=E(head_rows, d))
         return ws
 
-    def forward_packed(self, ws, pk_plan, table, capture=None):
+    def forward_packed(self, ws, pk_plan, table, capture=None, kv=None, hist=None):
         """Inference forward of sequences of their own lengths packed back to back without padding (pk_plan: M rows,
         src_row, src_row2, row_pos, seq_start, seq_len, the attention work list, dest_row and the head groups; see
         session.PackedPrefill) in a packed_workspace.  The layer loop is forward_core's, with the varlen attention and
         FFN-up kernels; table: a bias table at least as long as the longest sequence.  The final norm writes only the
         rows dest_row names, and head group (qi, base, cnt) leaves the logits of head qi of the last sequence for its
-        cnt rows in ws["logits"][base:base + cnt].  Every row's values are those of forward_core on its sequence alone."""
+        cnt rows in ws["logits"][base:base + cnt].  Every row's values are those of forward_core on its sequence alone.
+
+        Chunks (pk_plan also has q_off, kv_start, max_end and hist_idx): sequence b is positions q_off[b] ... of a longer
+        prompt.  With kv, layer l's attention reads its keys from kv[l] (viewed [rows, 128]) at rows kv_start[b] ...,
+        which capture.after_kv must have filled for positions 0 ... q_off[b] + seq_len[b] - 1; with hist, its FFN-up
+        takes the conv history of a chunk's first row from hist[l] (rows 2c, 2c + 1 for hist_idx = c; needed when some
+        q_off > 0).  Every row's values are then those of forward_core on its whole prompt."""
         self.refresh_packed()
         pp, M, Fp = pk_plan, pk_plan.M, self.Fp
         v = {k: [e[:M] for e in t] if isinstance(t, list) else t[:M] for k, t in ws.items() if k not in ("logits", "xf", "xf16")}
         lib.embed_gather(self.table, pp.src_row, v["x"][0], pp.src_row2)
-        x_last = self._layers(v, M, False, False, capture,
-                              lambda i: lib.attn_fwd_tc_varlen(v["qn"][i], v["kvn"][i], table, pp.work, pp.seq_start, pp.seq_len,
-                                                               pp.max_len, v["o"][i], v["lse"][i], self.h),
-                              lambda xn2, i, pk: lib.gemm_ffn_up_varlen(xn2, pk["w1"], pk["conv"], v["u"][i], v["h"], v["rowsum"],
-                                                                        pp.row_pos, Fp))
+        if kv is None:
+            attn = lambda i, l: lib.attn_fwd_tc_varlen(v["qn"][i], v["kvn"][i], table, pp.work, pp.seq_start, pp.seq_len, pp.max_len,
+                                                       v["o"][i], v["lse"][i], self.h)
+        else:
+            attn = lambda i, l: lib.attn_fwd_tc_chunk(v["qn"][i], kv[l].view(-1, 128), table, pp.work, pp.seq_start, pp.seq_len,
+                                                      pp.q_off, pp.kv_start, pp.max_end, v["o"][i], v["lse"][i], self.h)
+        if hist is None:
+            ffn_up = lambda xn2, i, l, pk: lib.gemm_ffn_up_varlen(xn2, pk["w1"], pk["conv"], v["u"][i], v["h"], v["rowsum"], pp.row_pos, Fp)
+        else:
+            ffn_up = lambda xn2, i, l, pk: lib.gemm_ffn_up_chunk(xn2, pk["w1"], pk["conv"], v["u"][i], v["h"], v["rowsum"], pp.row_pos,
+                                                                 hist[l], pp.hist_idx, Fp)
+        x_last = self._layers(v, M, False, False, capture, attn, ffn_up)
         xf = ws["xf16"] if self.a16 != torch.bfloat16 else ws["xf"]
         lib.layernorm_fwd(x_last, self.pview["transformer.norm.gamma"], xf, None, v["st_o"], pp.dest_row)
         S = len(self.seqs) - 1

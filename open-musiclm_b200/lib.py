@@ -279,6 +279,18 @@ def attn_fwd_tc_varlen(qn, kvn, table, work, seq_start, seq_len, max_len, out, l
          _p(seq_len), _I(qn.shape[0]), _I(max_len), _p(out), _p(lse2), _I(heads), _F(scale), _stream())
 
 
+def attn_fwd_tc_chunk(qn, kv, table, work, seq_start, seq_len, q_off, kv_start, max_end, out, lse2, heads, scale=8.0):
+    """attn_fwd_tc_varlen over chunks of longer sequences (omlm_attn_fwd_tc_chunk): qn [M, heads*64] packed chunk rows, kv
+    [rows, 128] (keys of sequence b at rows kv_start[b] ...); q_off int32 [n_seq] each chunk's first position; max_end >=
+    every q_off + seq_len."""
+    for t in (work, seq_start, seq_len, q_off, kv_start):
+        assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous()
+    assert kv.is_contiguous() and kv.shape[-1] == 128
+    call("omlm_attn_fwd_tc_chunk", _p(qn), _p(kv), _L(kv.numel() // 128), _p(table), _I(table.stride(0)), _p(work), _I(work.numel() // 2),
+         _p(seq_start), _p(seq_len), _p(q_off), _p(kv_start), _I(qn.shape[0]), _I(max_end), _p(out), _p(lse2), _I(heads), _F(scale),
+         _stream())
+
+
 def attn_bwd(qn, kvn, d_o, o, lse2, table, key_mask, dsum_scratch, dqn, dkvn, dtable, B, N, heads, scale=8.0):
     call("omlm_attn_bwd", _p(qn), _p(kvn), _p(d_o), _p(o), _p(lse2), _p(table), _I(table.stride(0)), _p(key_mask),
          _p(dsum_scratch), _p(dqn), _p(dkvn), _p(dtable), _I(B), _I(N), _I(heads), _F(scale), _stream())
@@ -328,6 +340,18 @@ def gemm_ffn_up_varlen(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, row_p
     assert row_pos.dtype == torch.int32 and row_pos.is_cuda and row_pos.is_contiguous() and row_pos.numel() >= M
     call("omlm_gemm_ffn_up_varlen", _p(xn), _p(w1_packed), _p(conv_w_packed), _p(u_out), _p(h_out), _p(rowsum), _p(row_pos), _I(M),
          _I(K), _I(Fp), _I(int(xn.dtype == torch.float16)), _I(max_ctas), _stream())
+
+
+def gemm_ffn_up_chunk(xn, w1_packed, conv_w_packed, u_out, h_out, rowsum, row_pos, hist, hist_idx, Fp, max_ctas=0):
+    """gemm_ffn_up_varlen over chunks that continue longer sequences (omlm_gemm_ffn_up_chunk): hist [*, 2Fp] the history
+    rows, hist_idx int32 [M] (c >= 0 at a chunk's first row: its t-2 and t-1 inputs are hist rows 2c and 2c + 1)."""
+    M, K = xn.shape
+    assert xn.dtype in _T16 and xn.dtype == w1_packed.dtype == u_out.dtype == h_out.dtype == hist.dtype
+    assert hist.is_contiguous() and hist.shape[-1] == 2 * Fp
+    for t in (row_pos, hist_idx):
+        assert t.dtype == torch.int32 and t.is_cuda and t.is_contiguous() and t.numel() >= M
+    call("omlm_gemm_ffn_up_chunk", _p(xn), _p(w1_packed), _p(conv_w_packed), _p(u_out), _p(h_out), _p(rowsum), _p(row_pos), _p(hist),
+         _p(hist_idx), _I(M), _I(K), _I(Fp), _I(int(xn.dtype == torch.float16)), _I(max_ctas), _stream())
 
 
 def ffn_norm_fwd(h, rowsum, gamma, hn, stats, F, Fp, drop_p=0.0, seed=None, layer=0, keep_bits=None, hn_copy=None):

@@ -14,6 +14,7 @@ Every prefix is whole time steps, so all rows sit at the same quantizer slot at 
 and the per-slot CUDA graphs; the arrays those graphs read (positions, sample indices, seeds, offsets, sampling
 arguments) change at a join, the graphs do not.  `SlotSchedule` is the host bookkeeping, without device work.
 """
+import math
 import numbers
 import types
 from collections import deque
@@ -42,14 +43,17 @@ def split_joiners(prompt_lens, capacity: int):
     return groups
 
 
-def lpt_work(seq_lens, h: int):
+def lpt_work(seq_lens, h: int, p0=None):
     """The attention work list of a packed forward: every (sequence, 128-row block of its len * h folded query rows)
     once, as int32 [n, 2], heaviest first (the block's key tiles, min(len - 1, last row's position) // 128 + 1; ties by
-    sequence, then later blocks first), as omlm_attn_fwd_tc orders its fixed-length grid."""
+    sequence, then later blocks first), as omlm_attn_fwd_tc orders its fixed-length grid.  p0: each sequence is a chunk
+    whose first row is position p0[b] of its prompt (p0[b] * h a multiple of 128); blocks are counted from the chunk's
+    first row and its key tiles from position 0, min(p0 + len - 1, last row's position) // 128 + 1."""
     b = np.concatenate([np.full((n * h + 127) // 128, i) for i, n in enumerate(seq_lens)]).astype(np.int64)
     rb = np.concatenate([np.arange((n * h + 127) // 128) for n in seq_lens]).astype(np.int64)
     lens = np.asarray(seq_lens, dtype=np.int64)[b]
-    tiles = np.minimum(lens - 1, (rb * 128 + 127) // h) // 128 + 1
+    p = np.zeros_like(lens) if p0 is None else np.asarray(p0, dtype=np.int64)[b]
+    tiles = np.minimum(p + lens - 1, (p * h + rb * 128 + 127) // h) // 128 + 1
     order = np.lexsort((-rb, b, -tiles))
     return np.stack([b[order], rb[order]], 1).astype(np.int32)
 
@@ -60,72 +64,104 @@ class PackedPrefill:
     lib.token_plan returns them; its prompt is sum(n + 1) rows (each sequence after its start token).  slots: the
     joiners' slots in a decode state of n_max positions per slot; q: quantizers of the last sequence; h: heads;
     abs_row_base (absolute position embeddings): the first row of each sequence's position table.  logprob: also
-    plan the rows that score the prefix tokens.
+    plan the rows that score the prefix tokens.  chunks: per joiner (p0, length), the positions p0 ... p0 + length - 1
+    of its prompt that this prefill runs (p0 a multiple of 128 / gcd(h, 128)); None: each whole prompt, (0, P).  A
+    chunk that ends its prompt is final: only final chunks have a next-token logits row and install conv history.
 
-    Arrays (numpy): start, P (each joiner's first packed row and prompt length), row_pos [M] (position within its
-    prompt), src_row2 [M] (position-table rows, -1 for start tokens; None without absolute positions), work
-    (lpt_work), last_row [k] (each prompt's last row, whose head-0 logits predict the first sampled token: every prefix
-    is whole time steps, so the next token is at quantizer 0), prefix_rows[qi] (the rows whose head-qi logits score the
-    prefix tokens at quantizer qi, joiner by joiner), dest_row [M] (row -> final-norm output row, -1 when no head reads
-    it: last rows first, then prefix_rows[0], [1], ...), groups [(qi, base, cnt)] (head qi on output rows base ..
-    base + cnt - 1), prefix_off [k] and label_idx [head_rows] (each output row's prefix token in the joiners'
-    concatenated prefixes, -1 for the last rows), kv_dst [M] (flat cache row slot * n_max + row_pos), conv_src and
-    conv_dst [2k] (prompt rows P - 2, P - 1 -> flat conv-history rows slot * 2 + j) and conv_zero (flat conv rows
-    before a prompt's first row)."""
+    Arrays (numpy): start, P, p0, end (each chunk's first packed row, length, first and one-past-last position), final
+    [k] (bool), row_pos [M] (position within its prompt), src_row2 [M] (position-table rows, -1 for start tokens; None
+    without absolute positions), work (lpt_work), last_row [k_final] (each final chunk's last row, whose head-0 logits
+    predict the first sampled token: every prefix is whole time steps, so the next token is at quantizer 0),
+    prefix_rows[qi] (the rows whose head-qi logits score the prefix tokens at quantizer qi, joiner by joiner),
+    dest_row [M] (row -> final-norm output row, -1 when no head reads it: last rows first, then prefix_rows[0], [1],
+    ...), groups [(qi, base, cnt)] (head qi on output rows base .. base + cnt - 1), prefix_off [k] and label_idx
+    [head_rows] (each output row's prefix token in the joiners' concatenated prefixes, -1 for the last rows),
+    prefix_span [k] (the range j_lo, j_hi of each joiner's prefix tokens scored here), kv_dst [M] (flat cache row
+    slot * n_max + row_pos), kv_start [k] (slot * n_max), hist_idx [M] (the slot at the first row of a chunk with p0 > 0,
+    whose conv history is rows 2 slot, 2 slot + 1 of the session's history buffer; -1 elsewhere), hist_src, hist_dst
+    (non-final chunks: rows end - 2, end - 1 -> history rows slot * 2 + j), and for final chunks conv_src and conv_dst
+    (prompt rows P - 2, P - 1 -> flat conv-history rows slot * 2 + j), conv_hsrc and conv_hdst (those of the two rows
+    that precede the chunk: from the history buffer) and conv_zero (flat conv rows before a prompt's first row)."""
 
-    def __init__(self, n_tok, slots, n_max: int, q: int, h: int, abs_row_base=None, logprob: bool = False):
+    def __init__(self, n_tok, slots, n_max: int, q: int, h: int, abs_row_base=None, logprob: bool = False, chunks=None):
         k = len(n_tok)
         self.k = k
-        self.P = np.array([sum(n + 1 for n in t) for t in n_tok], dtype=np.int64)
+        full = np.array([sum(n + 1 for n in t) for t in n_tok], dtype=np.int64)
+        if chunks is None:
+            chunks = [(0, int(n)) for n in full]
+        self.p0 = np.array([c[0] for c in chunks], dtype=np.int64)
+        self.P = np.array([c[1] for c in chunks], dtype=np.int64)
+        self.end = self.p0 + self.P
+        assert (self.P >= 1).all() and (self.end <= full).all()
+        self.final = self.end == full
         self.start = np.concatenate([[0], np.cumsum(self.P)[:-1]]).astype(np.int64)
         self.M = int(self.P.sum())
         self.max_len = int(self.P.max())
-        self.row_pos = np.concatenate([np.arange(p) for p in self.P]).astype(np.int32)
+        self.max_end = int(self.end.max())
+        self.row_pos = np.concatenate([np.arange(a, e) for a, e in zip(self.p0, self.end)]).astype(np.int32)
         self.src_row2 = None
         if abs_row_base is not None:
-            r2 = np.full(self.M, -1, dtype=np.int32)
-            for s0, t in zip(self.start, n_tok):
-                pos0 = s0
-                for s, n in enumerate(t):
-                    r2[pos0 + 1:pos0 + 1 + n] = abs_row_base[s] + np.arange(n)
-                    pos0 += n + 1
-            self.src_row2 = r2
-        self.work = lpt_work(self.P.tolist(), h)
-        self.last_row = self.start + self.P - 1
+            r2 = []
+            for t, a, e in zip(n_tok, self.p0, self.end):
+                whole = np.concatenate([np.concatenate([[-1], abs_row_base[s] + np.arange(n)]) for s, n in enumerate(t)])
+                r2.append(whole[a:e])
+            self.src_row2 = np.concatenate(r2).astype(np.int32)
+        self.work = lpt_work(self.P.tolist(), h, self.p0)
+        fin = np.flatnonzero(self.final)
+        self.k_final = len(fin)
+        self.last_row = (self.start + self.P - 1)[fin]
         n_pre = [t[-1] if logprob else 0 for t in n_tok]
-        pred0 = [s0 + sum(n + 1 for n in t[:-1]) for s0, t in zip(self.start, n_tok)]   # each predicted sequence's start token
+        pred0 = [sum(n + 1 for n in t[:-1]) for t in n_tok]         # each predicted sequence's start token (position)
+        # prefix token j is scored by the row at position pred0 + j: the tokens j_lo ... j_hi - 1 fall in this chunk
+        self.prefix_span = [(int(min(max(a - p, 0), n)), int(max(min(e - p, n), 0))) for a, e, p, n in zip(self.p0, self.end, pred0, n_pre)]
         self.prefix_off = np.concatenate([[0], np.cumsum(n_pre)[:-1]]).astype(np.int64)
-        self.prefix_rows = [np.concatenate([p0 + np.arange(qi, n, q) for p0, n in zip(pred0, n_pre)]).astype(np.int64) for qi in range(q)]
-        prefix_tok = [np.concatenate([o + np.arange(qi, n, q) for o, n in zip(self.prefix_off, n_pre)]).astype(np.int64) for qi in range(q)]
+        span = lambda i, qi: np.arange(self.prefix_span[i][0] + (qi - self.prefix_span[i][0]) % q, self.prefix_span[i][1], q)
+        self.prefix_rows = [np.concatenate([np.zeros(0)] + [self.start[i] + pred0[i] + span(i, qi) - self.p0[i] for i in range(k)]).astype(np.int64)
+                            for qi in range(q)]
+        prefix_tok = [np.concatenate([np.zeros(0)] + [self.prefix_off[i] + span(i, qi) for i in range(k)]).astype(np.int64) for qi in range(q)]
         out_rows = [self.last_row] + self.prefix_rows
         self.head_rows = sum(len(r) for r in out_rows)
         self.dest_row = np.full(self.M, -1, dtype=np.int32)
         self.dest_row[np.concatenate(out_rows)] = np.arange(self.head_rows)
         self.groups, base = [], 0
         for qi in range(q):
-            cnt = len(self.prefix_rows[qi]) + (k if qi == 0 else 0)
+            cnt = len(self.prefix_rows[qi]) + (self.k_final if qi == 0 else 0)
             if cnt:
                 self.groups.append((qi, base, cnt))
             base += cnt
-        self.label_idx = np.concatenate([np.full(k, -1, dtype=np.int64)] + prefix_tok)
+        self.label_idx = np.concatenate([np.full(self.k_final, -1, dtype=np.int64)] + prefix_tok)
         slot = np.asarray(slots, dtype=np.int64)
         self.slots = slot
         self.kv_dst = np.repeat(slot * n_max, self.P) + self.row_pos
-        hist = self.P[:, None] + np.arange(-2, 0)[None]                               # prompt rows P - 2, P - 1
-        self.conv_dst = (slot[:, None] * 2 + np.arange(2)[None]).reshape(-1)
-        self.conv_src = (self.start[:, None] + np.maximum(hist, 0)).reshape(-1)
+        self.kv_start = slot * n_max
+        self.hist_idx = np.full(self.M, -1, dtype=np.int32)
+        cont = self.p0 > 0
+        self.hist_idx[self.start[cont]] = slot[cont]
+        part = np.flatnonzero(~self.final)
+        assert (self.P[part] >= 2).all()                                             # non-final chunks are whole units
+        self.hist_dst = (slot[part, None] * 2 + np.arange(2)[None]).reshape(-1)
+        self.hist_src = (self.start[part, None] + self.P[part, None] + np.arange(-2, 0)[None]).reshape(-1)
+        hist = self.end[fin, None] + np.arange(-2, 0)[None]                           # prompt rows P - 2, P - 1
+        rel = hist - self.p0[fin, None]                                               # < 0: before the chunk
+        self.conv_dst = (slot[fin, None] * 2 + np.arange(2)[None]).reshape(-1)
+        self.conv_src = (self.start[fin, None] + np.maximum(rel, 0)).reshape(-1)
         self.conv_zero = self.conv_dst[(hist < 0).reshape(-1)]
+        before = ((hist >= 0) & (rel < 0)).reshape(-1)
+        self.conv_hdst = self.conv_dst[before]
+        self.conv_hsrc = (slot[fin, None] * 2 + rel + 2).reshape(-1)[before]          # history row of position p0 - 2 + j
+        self.fin_slots = slot[fin]
 
     def to_device(self, dev):
         """The device arrays, sent in one non-blocking copy (staged from pageable memory, as decode.row_arrays does, so
         that it never waits for the device): a namespace of the arrays above that the forward and the install read."""
         arrays = dict(row_pos=self.row_pos, work=self.work, seq_start=self.start.astype(np.int32), seq_len=self.P.astype(np.int32),
-                      dest_row=self.dest_row, kv_dst=self.kv_dst, conv_dst=self.conv_dst, conv_src=self.conv_src, slots=self.slots,
-                      label_idx=self.label_idx)
-        if self.src_row2 is not None:
-            arrays["src_row2"] = self.src_row2
-        if len(self.conv_zero):
-            arrays["conv_zero"] = self.conv_zero
+                      q_off=self.p0.astype(np.int32), kv_start=self.kv_start.astype(np.int32), hist_idx=self.hist_idx,
+                      dest_row=self.dest_row, kv_dst=self.kv_dst, label_idx=self.label_idx)
+        optional = ("src_row2", "conv_dst", "conv_src", "conv_zero", "conv_hdst", "conv_hsrc", "hist_dst", "hist_src", "fin_slots")
+        for name in optional:                   # None when absent or empty
+            a = getattr(self, name)
+            if a is not None and len(a):
+                arrays[name] = a
         parts, where, off = [], {}, 0
         for name, a in arrays.items():
             raw = np.ascontiguousarray(a).reshape(-1).view(np.uint8)
@@ -133,7 +169,8 @@ class PackedPrefill:
             parts += [raw, np.zeros(-len(raw) % 8, dtype=np.uint8)]
             off += len(raw) + (-len(raw) % 8)
         buf = torch.from_numpy(np.concatenate(parts)).to(dev, non_blocking=True)
-        dv = dict(M=self.M, max_len=self.max_len, groups=self.groups, src_row2=None, conv_zero=None)
+        dv = dict(M=self.M, max_len=self.max_len, max_end=self.max_end, k_final=self.k_final, groups=self.groups,
+                  **{name: None for name in optional})
         for name, (o, dt, shape) in where.items():
             tdt = torch.int32 if dt == np.int32 else torch.int64
             dv[name] = buf[o:o + int(np.prod(shape)) * dt.itemsize].view(tdt).view(shape)
@@ -142,31 +179,47 @@ class PackedPrefill:
 
 class _PackedCapture:
     """Receives a packed prefill's per-layer K/V rows and pre-conv FFN rows (Engine.forward_packed) into the joiners'
-    slots of a DecodeSession: every prompt row's K/V at its position, and prompt rows P - 2, P - 1 as conv history
-    (zero before a prompt's first row), one gather or scatter per layer and kind, as _PromptCapture does per row."""
+    slots of a DecodeSession: every chunk row's K/V at its position; for a final chunk, prompt rows P - 2, P - 1 as conv
+    history (zero before a prompt's first row, from the history buffer `hist` when they precede the chunk); for any
+    other chunk, its last two rows into `hist` (the decode step shifts every slot's conv history at every step, so a
+    prefilling slot's history lives outside it).  One gather or scatter per layer and kind, as _PromptCapture does per
+    row."""
 
-    def __init__(self, dec, dv):
-        self.dec, self.dv = dec, dv
+    def __init__(self, dec, dv, hist=None):
+        self.dec, self.dv, self.hist = dec, dv, hist
 
     def after_kv(self, l, kvn):
         self.dec.cache[l].view(-1, 128).index_copy_(0, self.dv.kv_dst, kvn)
 
     def after_u(self, l, u):
+        dv = self.dv
         conv = self.dec.conv[l].view(-1, u.shape[-1])
-        conv.index_copy_(0, self.dv.conv_dst, u.index_select(0, self.dv.conv_src))
-        if self.dv.conv_zero is not None:
-            conv.index_fill_(0, self.dv.conv_zero, 0)
+        if dv.conv_dst is not None:
+            conv.index_copy_(0, dv.conv_dst, u.index_select(0, dv.conv_src))
+        if dv.conv_hdst is not None:
+            conv.index_copy_(0, dv.conv_hdst, self.hist[l].index_select(0, dv.conv_hsrc))
+        if dv.conv_zero is not None:
+            conv.index_fill_(0, dv.conv_zero, 0)
+        if dv.hist_dst is not None:
+            self.hist[l].index_copy_(0, dv.hist_dst, u.index_select(0, dv.hist_src))
 
 
 class _Row:
     """One request: prompt length P (= the position its first decode step processes), n tokens to sample, its
-    predicted sequence's start position pred_start, and its progress t (tokens sampled so far)."""
+    predicted sequence's start position pred_start, and its progress: filled (prompt rows prefilled so far, counting
+    the chunk planned at this boundary), chunk ((p0, length) of that chunk) and t (tokens sampled so far)."""
 
     def __init__(self, handle, P, n, pred_start, payload=None):
         self.handle, self.P, self.n, self.pred_start, self.payload = handle, P, n, pred_start, payload
         self.t = 0
+        self.filled = 0
+        self.chunk = None
         self.slot = None
         self.join_step = None
+
+    @property
+    def prefilled(self) -> bool:
+        return self.filled == self.P
 
     def device_state(self):
         """The values the device arrays hold for this row after its t samples: sample index, position, last position,
@@ -178,13 +231,19 @@ class _Row:
 
 class SlotSchedule:
     """Slot allocation of a session: requests wait in a FIFO queue (at most `max_queue` beyond the free slots), take
-    the lowest free slot at a time-step boundary, sample q tokens per time step and leave when they have n."""
+    the lowest free slot at a time-step boundary, sample q tokens per time step and leave when they have n.
 
-    def __init__(self, slots: int, q: int, max_queue: int = 0):
+    prefill_rows: at most that many prompt rows are prefilled per boundary (None: no bound).  A prompt that does not
+    fit is prefilled in chunks over consecutive boundaries, each but the last a multiple of `unit` rows; its request
+    holds its slot meanwhile and samples from the boundary of its last chunk on."""
+
+    def __init__(self, slots: int, q: int, max_queue: int = 0, prefill_rows=None, unit: int = 1):
         self.slots, self.q, self.max_queue = slots, q, max_queue
+        self.prefill_rows, self.unit = prefill_rows, unit
         self.free = list(range(slots))
-        self.rows = {}                 # slot -> _Row
+        self.rows = {}                 # slot -> _Row (prefilling rows included)
         self.queue = deque()
+        self.prefilling = []           # rows part-way through their prompt, in admission order
         self.steps = 0                 # time steps run
 
     def check_room(self):
@@ -198,16 +257,39 @@ class SlotSchedule:
         self.queue.append(row)
 
     def admit(self):
-        """The boundary: queued rows take free slots (lowest first), in order.  Returns the rows that joined."""
-        joined = []
-        while self.queue and self.free:
-            row = self.queue.popleft()
-            row.slot = min(self.free)
-            self.free.remove(row.slot)
-            row.join_step = self.steps
-            self.rows[row.slot] = row
-            joined.append(row)
-        return joined
+        """The boundary: the budget of prompt rows goes in FIFO order, first to the rows part-way through their
+        prompt, then to queued rows, which take free slots (lowest first) while there are any.  A row gets a chunk
+        only if it can take min(unit, its remaining rows): its whole remainder if that fits, else the largest multiple
+        of unit that does; the first row that cannot ends the boundary, so no row overtakes an earlier one.  Returns
+        the rows with a chunk at this boundary (row.chunk = (p0, length)); without a budget, the rows that joined, each
+        with its whole prompt."""
+        left = float("inf") if self.prefill_rows is None else self.prefill_rows
+        out = []
+
+        def take(row):
+            nonlocal left
+            rem = row.P - row.filled
+            n = rem if rem <= left else int(left) // self.unit * self.unit
+            if n == 0:
+                return False
+            row.chunk = (row.filled, n)
+            row.filled += n
+            left -= n
+            out.append(row)
+            return True
+
+        for row in self.prefilling:
+            if not take(row):
+                break
+        else:
+            while self.queue and self.free and take(self.queue[0]):
+                row = self.queue.popleft()
+                row.slot = min(self.free)
+                self.free.remove(row.slot)
+                row.join_step = self.steps
+                self.rows[row.slot] = row
+        self.prefilling = [r for r in self.prefilling if not r.prefilled] + [r for r in out if r.chunk[0] == 0 and not r.prefilled]
+        return out
 
     def advance(self):
         """One time step: every active row samples q tokens.  Returns the rows that now have all theirs (their slots
@@ -215,6 +297,8 @@ class SlotSchedule:
         self.steps += 1
         done = []
         for slot, row in sorted(self.rows.items()):
+            if not row.prefilled:
+                continue
             row.t += self.q
             if row.t >= row.n:
                 done.append(row)
@@ -263,6 +347,12 @@ class GenerationSession:
     sampled from, returned by `traced_logits(handle)` once the row has finished.
     return_logprobs: `finished()` maps each handle to (tokens, logprobs, sample_logprobs), each [n, q], with the
     definitions of `generate(..., return_logprobs=True)`; the prefix values come from the row's rows of the packed prefill.
+    prefill_rows: None (every request's whole prompt is prefilled at the boundary where it joins), or the most prompt
+    rows prefilled at one boundary, across all requests, an int >= U = 128 / gcd(heads, 128).  A longer prompt is then
+    prefilled in chunks over consecutive boundaries (each but the last a multiple of U rows) while the other rows keep
+    decoding in between, so a mass join stalls the running rows for a bounded time.  The budget goes first to requests
+    part-way through their prompt, then to queued ones, in arrival order; a request takes its slot with its first
+    chunk and samples from the boundary of its last.  Time steps in which a request only prefills count for `step`.
 
     The transformer's weights are packed when the session is created; train it between sessions, not during one.
     Every row gets exactly what `generate` gives that row alone with seeds=[seed] and the same arguments; free and
@@ -270,7 +360,7 @@ class GenerationSession:
 
     def __init__(self, wrapper, slots: int, max_positions: int, allow_eos_in_output=False, include_eos_in_output=False,
                  append_eos_to_conditioning_tokens=True, max_queue: int = 0, use_cuda_graph=True, trace_logits=False,
-                 return_logprobs=False):
+                 return_logprobs=False, prefill_rows=None):
         if not isinstance(return_logprobs, bool):
             raise ValueError(f"open_musiclm_b200 GenerationSession: return_logprobs must be a bool, not {return_logprobs!r}")
         for name, v in (("slots", slots), ("max_positions", max_positions), ("max_queue", max_queue)):
@@ -284,6 +374,12 @@ class GenerationSession:
         m = wrapper.transformer
         if m.heads > 16:
             raise ValueError(f"open_musiclm_b200 GenerationSession: seeded generation supports at most 16 heads ({m.heads} given)")
+        unit = 128 // math.gcd(m.heads, 128)
+        if prefill_rows is not None and (isinstance(prefill_rows, bool) or not isinstance(prefill_rows, numbers.Integral)
+                                         or prefill_rows < unit):
+            raise ValueError(f"open_musiclm_b200 GenerationSession: prefill_rows must be None or an int >= {unit} "
+                             f"(128 / gcd(heads, 128)), not {prefill_rows!r}")
+        self.prefill_rows = None if prefill_rows is None else int(prefill_rows)
         self.w, self.m = wrapper, m
         info = wrapper.token_sequences[-1]
         self.q, self.C, self.eos = info.num_quantizers, info.codebook_size + 1, wrapper.eos_ids[-1]
@@ -292,7 +388,7 @@ class GenerationSession:
             bool(append_eos_to_conditioning_tokens)
         self.use_graph, self.trace = bool(use_cuda_graph) and not trace_logits, bool(trace_logits)
         self.logprob = return_logprobs
-        self.sched = SlotSchedule(self.slots, self.q, int(max_queue))
+        self.sched = SlotSchedule(self.slots, self.q, int(max_queue), self.prefill_rows, unit)
         self._next_handle = 0
         self._done = {}
         self._traced = {}
@@ -301,6 +397,7 @@ class GenerationSession:
         self._graphs = GraphCache(self.use_graph)
         self.eng = self.dec = None     # the engine and the slots' device state, made by the first step that runs a row
         self._pack_ws = None           # the packed prefill's workspace, made at the first join
+        self._hist = None              # with prefill_rows: per layer the conv history of prefilling slots, [2 slots, 2 Fp]
 
     def _device_state(self):
         if self.dec is None:
@@ -378,7 +475,7 @@ class GenerationSession:
 
     @property
     def idle(self) -> bool:
-        """No row is decoding or queued."""
+        """No row is decoding, prefilling or queued."""
         return not self.sched.rows and not self.sched.queue
 
     @property
@@ -404,20 +501,26 @@ class GenerationSession:
         return out[0] if lp is None else tuple(t[0] for t in out)
 
     def _install(self, rows):
-        """Prefills the joining rows together, packed back to back (_prefill_packed; in consecutive groups when their
-        prompts exceed the packed workspace), writes each prompt's K/V rows, conv history and last logits into its
-        slot, then sets the slots' arrays.  Runs after the boundary step (which writes every slot's cache and conv
-        history at the slot's old position) and before the boundary sample."""
+        """Prefills the chunks the schedule gave `rows` at this boundary, packed back to back (_prefill_packed; in
+        consecutive groups when they exceed the packed workspace), writes their K/V rows into the slots and, for each
+        row whose prompt is now complete, its conv history and last logits, then sets the slots' arrays.  Runs after the
+        boundary step (which writes every slot's cache and conv history at the slot's old position) and before the
+        boundary sample.  A row still prefilling is parked: it samples nothing (n = 0), and its position stays at its
+        first unfilled one, whose K/V the next chunk overwrites before anything reads it (pos_offset = -pos keeps the
+        absolute-position row of every step in range)."""
         eng, dec, dev = self.eng, self.dec, self.eng.dev
         if self._pack_ws is None:
             self._pack_rows = min(max(self.max_positions, PACK_ROWS), self.slots * self.max_positions)
+            if self.prefill_rows is not None:
+                self._pack_rows = min(self._pack_rows, self.prefill_rows)
+                self._hist = [torch.empty(2 * self.slots, 2 * eng.Fp, device=dev, dtype=eng.a16) for _ in range(eng.L)]
             self._pack_ws = eng.packed_workspace(self._pack_rows, self._pack_rows if self.logprob else self.slots)
-        for group in split_joiners([r.P for r in rows], self._pack_rows):
+        for group in split_joiners([r.chunk[1] for r in rows], self._pack_rows):
             self._prefill_packed([rows[i] for i in group])
         idx = torch.tensor([r.slot for r in rows], device=dev)
-        states = [r.device_state() for r in rows]
+        states = [r.device_state() if r.prefilled else dict(pos=r.filled, pos_last=r.filled, pos_offset=-r.filled) for r in rows]
         vals = row_arrays(dev, len(rows), pos=[s["pos"] for s in states], pos_last=[s["pos_last"] for s in states],
-                          pos_offset=[s["pos_offset"] for s in states], t=0, n=[r.n for r in rows],
+                          pos_offset=[s["pos_offset"] for s in states], t=0, n=[r.n if r.prefilled else 0 for r in rows],
                           top_k=[r.payload["top_k"] for r in rows], temperature=[r.payload["temperature"] for r in rows],
                           top_p=[r.payload["top_p"] for r in rows])
         for name, dst in (("pos", dec.pos), ("pos_last", dec.pos_last), ("pos_offset", dec.pos_offset), ("t", dec.t), ("n", dec.n_rows),
@@ -427,35 +530,50 @@ class GenerationSession:
         dec.seeds[idx] = seeds_tensor([r.payload["seed"] for r in rows], len(rows), dev)
 
     def _prefill_packed(self, rows):
-        """One packed forward over the rows' prompts (Engine.forward_packed), installed by _PackedCapture; the last
-        rows' head-0 logits go to the slots' logits rows, and with return_logprobs each row's prefix log-probabilities
-        are scored from the same heads and rows as prefix_logprobs scores them in `generate`'s prefill."""
+        """One packed forward over the rows' chunks (Engine.forward_packed, its attention reading each slot's K/V
+        cache), installed by _PackedCapture; the last rows' head-0 logits of the final chunks go to the slots' logits
+        rows, and with return_logprobs each row's prefix log-probabilities are scored from the same heads and rows as
+        prefix_logprobs scores them in `generate`'s prefill, chunk by chunk."""
         eng, dec, ws = self.eng, self.dec, self._pack_ws
         plan = PackedPrefill([r.payload["n_tok"] for r in rows], [r.slot for r in rows], dec.n_max, self.q, eng.h,
-                             eng.abs_row_base if eng.abs_pos else None, self.logprob)
+                             eng.abs_row_base if eng.abs_pos else None, self.logprob, [r.chunk for r in rows])
         dv = plan.to_device(eng.dev)
         src = []
         for r in rows:                        # the token plan of each prompt, as decode.prefill makes it
-            _, src_row, _, _, _ = lib.token_plan(r.payload["ids"], [s.codebook_size for s in eng.seqs], [s.num_quantizers for s in eng.seqs],
-                                                 eng.emb_row_base, eng.start_row, append_eos=False, drop_last=False, mask_cond=False,
-                                                 want_labels=False, err_flag=eng.err_flag)
-            src.append(src_row.view(-1))
+            if "src_row" not in r.payload:
+                _, src_row, _, _, _ = lib.token_plan(r.payload["ids"], [s.codebook_size for s in eng.seqs],
+                                                     [s.num_quantizers for s in eng.seqs], eng.emb_row_base, eng.start_row,
+                                                     append_eos=False, drop_last=False, mask_cond=False, want_labels=False,
+                                                     err_flag=eng.err_flag)
+                r.payload["src_row"] = src_row.view(-1)
+            p0, n = r.chunk
+            src.append(r.payload["src_row"][p0:p0 + n])
         dv.src_row = torch.cat(src) if len(src) > 1 else src[0]
-        eng.forward_packed(ws, dv, dec.table, capture=_PackedCapture(dec, dv))
-        k, Cp = len(rows), eng.Cp[-1]
-        dec.logits[:, :Cp].index_copy_(0, dv.slots, ws["logits"][:k])
+        eng.forward_packed(ws, dv, dec.table, capture=_PackedCapture(dec, dv, self._hist), kv=dec.cache, hist=self._hist)
+        k, Cp = plan.k_final, eng.Cp[-1]
+        if k:
+            dec.logits[:, :Cp].index_copy_(0, dv.fin_slots, ws["logits"][:k])
         if self.logprob:
             pre = [r.payload["prefix"][0] for r in rows]
             lp = torch.zeros(sum(p.shape[0] for p in pre), device=eng.dev, dtype=torch.float32)
-            if lp.numel():
+            if plan.head_rows > k:
                 ids = torch.cat(pre)
                 tok = torch.where((ids >= 0) & (ids < self.C), ids, -100)[dv.label_idx[k:]]
                 labels = torch.cat([tok.new_full((k,), -100), tok]).to(torch.int32)
                 out = torch.empty(plan.head_rows, device=eng.dev, dtype=torch.float32)
                 lib.token_logprob(ws["logits"][:plan.head_rows], labels, self.C, out)
                 lp.index_copy_(0, dv.label_idx[k:], out[k:])
-            for r, o, p in zip(rows, plan.prefix_off.tolist(), pre):
-                r.payload["prefix_lp"] = lp[o:o + p.shape[0]] if p.shape[0] else None
+            for r, o, p, (j0, j1) in zip(rows, plan.prefix_off.tolist(), pre, plan.prefix_span):
+                n = p.shape[0]
+                if n and (j0, j1) == (0, n):
+                    r.payload["prefix_lp"] = lp[o:o + n]
+                elif n:                               # the prefix spans chunks: gather it in a buffer of its own
+                    if r.payload.get("prefix_lp") is None:
+                        r.payload["prefix_lp"] = torch.zeros(n, device=eng.dev, dtype=torch.float32)
+                    if j1 > j0:
+                        r.payload["prefix_lp"][j0:j1].copy_(lp[o + j0:o + j1])
+                else:
+                    r.payload["prefix_lp"] = None
 
     def _sample_point(self):
         if self.trace:
@@ -464,8 +582,9 @@ class GenerationSession:
     @torch.no_grad()
     def step(self, n_time_steps: int = 1):
         """Runs n_time_steps time steps (q tokens per active row each).  Each starts at a boundary, where queued rows
-        take free slots: the running rows' step to quantizer slot 0, the joiners' prefill and install, then the
-        sample of slot 0 for every row; slots 1 ... q-1 follow as step and sample.  Rows with all their tokens leave
+        take free slots: the running rows' step to quantizer slot 0, the prefill of this boundary's chunks and the
+        install of the prompts they complete, then the sample of slot 0 for every row; slots 1 ... q-1 follow as step
+        and sample.  Rows with all their tokens leave
         at the end of the time step; `finished` returns them.  A time step with no row to run does nothing."""
         if isinstance(n_time_steps, bool) or not isinstance(n_time_steps, numbers.Integral) or n_time_steps < 0:
             raise ValueError(f"open_musiclm_b200 GenerationSession.step: n_time_steps must be an int >= 0, not {n_time_steps!r}")
@@ -473,20 +592,21 @@ class GenerationSession:
         allow = lambda qi: bool(self.allow_eos and qi == q - 1)                                   # open_musiclm.py:311-313
         for _ in range(n_time_steps):
             running = bool(sched.rows)
-            joined = sched.admit()
+            chunked = sched.admit()
             if not sched.rows:
                 break
             dec = self._device_state()
             if self.trace and not running:
                 self._trace, self._trace_base = [], self._trace_base + len(self._trace)
-            for row in joined:
-                row.trace_start = self._trace_base + len(self._trace)
+            for row in chunked:
+                if row.prefilled:
+                    row.trace_start = self._trace_base + len(self._trace)
             nucleus = any(r.payload["top_p"] is not None for r in sched.rows.values())
             for qi in range(q):
-                if qi == 0 and joined:
+                if qi == 0 and chunked:
                     if running:
                         self._graphs.run(("step", 0), lambda: dec.step(0))
-                    self._install(joined)
+                    self._install(chunked)
                     self._sample_point()
                     self._graphs.run(("sample", 0, nucleus), lambda: dec.sample_rows(0, allow(0), nucleus))
                 elif self.trace:
