@@ -9,6 +9,7 @@ Only what the TokenConditionedTransformer training path needs lives here:
   decode.py   `TokenConditionedTransformerWrapper.generate`: KV-cache autoregressive decoding
   session.py  `GenerationSession`: continuous batching, rows joining and leaving a running decode
   stages.py   `SemanticStage` / `CoarseStage` / `FineStage` and the windowed three-stage `MusicLM` generation
+  musiclm_session.py  `MusicLMSession`: continuous batching of whole songs through the three stages
 """
 __version__ = "0.1.0"
 
@@ -18,3 +19,4 @@ from .trainer import HotPathTrainer  # noqa: F401
 from .decode import TokenConditionedTransformerWrapper  # noqa: F401
 from .session import GenerationSession  # noqa: F401
 from .stages import CoarseStage, FineStage, MusicLM, NoiseStream, SemanticStage, prepare_audio  # noqa: F401
+from .musiclm_session import MusicLMSession  # noqa: F401

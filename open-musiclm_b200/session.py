@@ -58,6 +58,18 @@ def lpt_work(seq_lens, h: int, p0=None):
     return np.stack([b[order], rb[order]], 1).astype(np.int32)
 
 
+def check_seed(seed, where: str) -> int:
+    """A request's seed: one int or a one-element int64 tensor -> the int; anything else raises ValueError."""
+    if isinstance(seed, torch.Tensor):
+        if seed.dtype != torch.int64 or seed.numel() != 1:
+            raise ValueError(f"{where}: seed must be one int or a one-element int64 tensor, not a {seed.dtype} tensor of "
+                             f"{seed.numel()} elements")
+        seed = int(seed.reshape(-1)[0])
+    if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
+        raise ValueError(f"{where}: seed must be one int, not {seed!r}")
+    return seed
+
+
 class PackedPrefill:
     """Host plan of one packed prefill: the prompts of k joiners back to back, without padding.  n_tok: per joiner the
     token counts of its sequences (conditioning sequences with their eos, then its prefix of whole time steps), as
@@ -420,13 +432,7 @@ class GenerationSession:
         samples nothing finishes at once."""
         S = len(self.w.token_sequences)
         where = "open_musiclm_b200 GenerationSession.add"
-        if isinstance(seed, torch.Tensor):
-            if seed.dtype != torch.int64 or seed.numel() != 1:
-                raise ValueError(f"{where}: seed must be one int or a one-element int64 tensor, not a {seed.dtype} tensor of "
-                                 f"{seed.numel()} elements")
-            seed = int(seed.reshape(-1)[0])
-        if isinstance(seed, bool) or not isinstance(seed, numbers.Integral):
-            raise ValueError(f"{where}: seed must be one int, not {seed!r}")
+        seed = check_seed(seed, where)
         if not isinstance(conditioning_token_ids, (list, tuple)) or len(conditioning_token_ids) != S - 1:
             raise ValueError(f"{where}: conditioning_token_ids must be a list of {S - 1} tensors")
         for t in conditioning_token_ids:

@@ -13,7 +13,7 @@ continuation (MusicLM.forward(prime_wave=...)) and best-of-N sampling (MusicLM.g
 wav2vec, codec and CLAP objects for the prime tokens and the similarity scores; the generation itself is the same
 prefill + KV-cache decode, driven with the prime's tokens as the predicted sequence's prefix.
 """
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import torch
 import torch.nn.functional as F
@@ -184,6 +184,154 @@ def _windows(tokens: torch.Tensor, size: int, step: int):
     return [tokens[:, s:s + size] for s in range(0, T - size + 1, step)]
 
 
+# ---------------------------------------------------------------------------------------- the windowing of one song
+STREAMS = ("semantic", "coarse", "fine")     # the stream each stage's windows append to, by stage number
+
+
+class WindowJob(NamedTuple):
+    """One generate call of a song.  cond and prefix are (stream, start, stop): the tokens stream[:, start:stop] of a
+    generated stream (STREAMS) or of a prime ("prime_semantic", "prime_coarse", "prime_fine").  cond is what the
+    window is conditioned on after the clap ids (a coarse window: semantic tokens, a fine window: coarse tokens; None
+    for a semantic window); prefix is its pred_token_ids (None: none).  The call returns `steps` time steps (eos is
+    never allowed: max(max_time_steps, prefix length)); all but the first `drop` go to STREAMS[stage] at `dest`.
+    needs: {stream: length} that must exist before the call can run.  seed: window_seed(song seed, stage, window)."""
+    stage: int
+    window: int
+    cond: Optional[tuple]
+    prefix: Optional[tuple]
+    max_time_steps: int
+    temperature: float
+    top_p: Optional[float]
+    seed: Optional[int]
+    steps: int
+    drop: int
+    dest: int
+    needs: dict
+
+
+class SongPlan(NamedTuple):
+    """Every window job of one song in the order MusicLM.generate_tokens calls them, the final length of each
+    generated stream, and the output: semantic[:, sem_lo:] and, after the primes, coarse[:, coarse_lo:] and
+    fine[:, fine_lo:] (coarse_only: the whole coarse stream)."""
+    jobs: List[WindowJob]
+    length: dict
+    sem_lo: int
+    coarse_lo: int
+    fine_lo: int
+    primed: bool
+    coarse_only: bool
+
+
+def _tail(n: int, k: int) -> int:
+    """The start of x[:, -k:] for x of length n (k = 0: the whole of x)."""
+    return 0 if k == 0 else max(n - k, 0)
+
+
+def _start(n: int, lo: int) -> int:
+    """The start of x[:, lo:] for x of length n (lo may be negative)."""
+    return slice(lo, None).indices(n)[0]
+
+
+def plan_song(*, output_seconds, semantic_window_seconds=10, coarse_window_seconds=4, fine_window_seconds=2,
+              semantic_steps_per_second=50, acoustic_steps_per_second=75, semantic_sliding_window_step_percent=0.5,
+              coarse_sliding_window_step_percent=0.5, fine_sliding_window_step_percent=1, prime_lengths=None, coarse_only=False,
+              top_p=(None, None, None), seed=None) -> SongPlan:
+    """The sliding windows of MusicLM.forward (open_musiclm.py:913-1032) for one song, from shapes and arguments alone.
+    prime_lengths: None, or the time steps (semantic, coarse, fine) of the prime streams; top_p: one checked value per
+    stage (_stage_top_p); seed: the song's seed (None: the jobs carry no seed).  A song whose streams give no coarse
+    window, no fine window, or coarse and fine outputs of different lengths raises ValueError, as does a semantic
+    window that adds nothing to its stream."""
+    where = "open_musiclm_b200 MusicLM"
+    sps, aps = semantic_steps_per_second, acoustic_steps_per_second
+    sp, cp, fp = semantic_sliding_window_step_percent, coarse_sliding_window_step_percent, fine_sliding_window_step_percent
+    jobs, length = [], {name: 0 for name in STREAMS}
+    temperature = (1.0, 0.95, 0.4)
+
+    def job(stage, window, cond, prefix, max_time_steps, drop, needs):
+        steps = max(max_time_steps, 0 if prefix is None else prefix[2] - prefix[1])
+        name = STREAMS[stage]
+        jobs.append(WindowJob(stage, window, cond, prefix, max_time_steps, temperature[stage], top_p[stage],
+                              None if seed is None else window_seed(seed, stage, window), steps, drop, length[name],
+                              {k: v for k, v in needs.items() if v > 0}))
+        length[name] += max(steps - drop, 0)
+
+    # ---- audio continuation: condition lengths, the prime's tails and the crops that line the stages up (:913-926)
+    sem_prime = coarse_prime = fine_prime = None
+    sem_adj = coarse_adj = fine_adj = 0
+    tp = (0, 0, 0)
+    if prime_lengths is not None:
+        tp = tuple(int(n) for n in prime_lengths)
+        cond_sem = int(sps * semantic_window_seconds * (1 - sp))
+        cond_coarse = int(aps * coarse_window_seconds * (1 - cp))
+        cond_fine = int(aps * fine_window_seconds * (1 - fp))
+        sem_prime = ("prime_semantic", _tail(tp[0], cond_sem), tp[0])
+        coarse_prime = ("prime_coarse", _tail(tp[1], cond_coarse), tp[1])
+        fine_prime = ("prime_fine", _tail(tp[2], cond_fine), tp[2]) if cond_fine > 0 else None
+        sem_adj = cond_sem - int(sps * coarse_window_seconds * (1 - cp))
+        coarse_adj = cond_coarse - int(aps * fine_window_seconds * (1 - fp))
+        fine_adj = cond_fine
+    # ---- semantic stream: first window from the prime's tail (or scratch), then windows conditioned on the tail of
+    # the stream (:930-949); cropped to line up with the coarse windows (:952)
+    job(SEMANTIC, 0, None, sem_prime, int(min(output_seconds, semantic_window_seconds) * sps), 0, {})
+    keep = int(semantic_window_seconds * sps * (1 - sp))
+    w = 1
+    while length["semantic"] < int(output_seconds * sps):
+        n = length["semantic"]
+        job(SEMANTIC, w, None, ("semantic", _tail(n, keep), n), int(semantic_window_seconds * sps), keep, {"semantic": n})
+        w += 1
+        if length["semantic"] == n:
+            raise ValueError(f"{where}: a semantic window of these arguments adds no tokens to the stream")
+    sem_lo = _start(length["semantic"], sem_adj)
+    # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail, the first one
+    # on the prime's (:956-985)
+    win = int(coarse_window_seconds * sps - 1)
+    keep = int(coarse_window_seconds * aps * (1 - cp))
+    for w, s in enumerate(range(0, length["semantic"] - sem_lo - win + 1, int(win * cp))):
+        n = length["coarse"]
+        job(COARSE, w, ("semantic", sem_lo + s, sem_lo + s + win), coarse_prime if w == 0 else ("coarse", _tail(n, keep), n),
+            int(coarse_window_seconds * aps), 0 if w == 0 else keep, {"semantic": sem_lo + s + win, "coarse": n})
+    if length["coarse"] == 0:
+        raise ValueError(f"{where}: output_seconds = {output_seconds} gives {length['semantic'] - sem_lo} semantic steps, "
+                         f"fewer than one coarse window of {win}")
+    if coarse_only:                                                                                     # :986-989
+        return SongPlan(jobs, length, sem_lo, 0, 0, prime_lengths is not None, True)
+    coarse_lo = _start(length["coarse"], coarse_adj)                                                    # :992
+    # ---- fine stream: one window of coarse tokens per generate, the first one conditioned on the prime's tail (:995-1024)
+    fwin = int(fine_window_seconds * aps)
+    keep = int(fwin * (1 - fp))
+    for w, s in enumerate(range(0, length["coarse"] - coarse_lo - fwin + 1, int(fwin * fp))):
+        n = length["fine"]
+        prefix = fine_prime if w == 0 else (("fine", _tail(n, keep), n) if keep > 0 else None)
+        job(FINE, w, ("coarse", coarse_lo + s, coarse_lo + s + fwin), prefix, fwin, 0 if w == 0 else keep,
+            {"coarse": coarse_lo + s + fwin, "fine": n if w > 0 and keep > 0 else 0})
+    if length["fine"] == 0:
+        raise ValueError(f"{where}: output_seconds = {output_seconds} gives {length['coarse'] - coarse_lo} coarse steps, "
+                         f"fewer than one fine window of {fwin}")
+    fine_lo = _start(length["fine"], fine_adj)                                                          # :1026
+    # the coarse stream still starts with the fine_adj prime tokens the first fine window was conditioned on; the
+    # reference keeps them, so with a fine condition length > 0 its coarse and fine streams differ in length and
+    # cannot be joined.  Dropping them lines both up on the first token after the prime (no-op when fine_adj = 0).
+    coarse_lo += _start(length["coarse"] - coarse_lo, fine_adj)
+    n_coarse, n_fine = tp[1] + length["coarse"] - coarse_lo, tp[2] + length["fine"] - fine_lo
+    if n_coarse != n_fine:
+        raise ValueError(f"{where}: these window arguments give {n_coarse} coarse and {n_fine} fine output steps; "
+                         "they cannot be joined")
+    return SongPlan(jobs, length, sem_lo, coarse_lo, fine_lo, prime_lengths is not None, False)
+
+
+def song_output(plan: SongPlan, streams: dict, return_all: bool):
+    """MusicLM.generate_tokens' result from a song's streams (the generated ones whole, and the primes when primed),
+    [b, T, q] each: coarse_only, the coarse stream; else the acoustic tokens [b, T, coarse + fine quantizers], with
+    return_all (acoustic, semantic, coarse, fine)."""
+    if plan.coarse_only:
+        return streams["coarse"]
+    sem, coarse, fine = streams["semantic"][:, plan.sem_lo:], streams["coarse"][:, plan.coarse_lo:], streams["fine"][:, plan.fine_lo:]
+    if plan.primed:                                                                                     # :1028-1030
+        fine, coarse = torch.cat([streams["prime_fine"], fine], 1), torch.cat([streams["prime_coarse"], coarse], 1)
+    acoustic = torch.cat([coarse, fine], -1)                                                           # :1032
+    return (acoustic, sem, coarse, fine) if return_all else acoustic
+
+
 # ---------------------------------------------------------------------------------------- audio helpers (utils.py:147-166)
 def _resample(wave: torch.Tensor, orig_hz, new_hz) -> torch.Tensor:
     from torchaudio.functional import resample
@@ -215,9 +363,8 @@ def prepare_audio(data: torch.Tensor, sample_hz, target_sample_hz, normalize=Tru
     return int16_to_float32(float32_to_int16(_resample(data, sample_hz, target_sample_hz)))
 
 
-def _stage_top_p(top_p):
+def _stage_top_p(top_p, where="MusicLM.generate_tokens"):
     """MusicLM.generate_tokens' top_p -> one checked value (None or a float in (0, 1)) per stage, semantic, coarse, fine."""
-    where = "MusicLM.generate_tokens"
     if isinstance(top_p, (list, tuple)):
         if len(top_p) != 3:
             raise ValueError(f"open_musiclm_b200 {where}: top_p as a sequence needs 3 values (semantic, coarse, fine), got {len(top_p)}")
@@ -225,13 +372,19 @@ def _stage_top_p(top_p):
     return [check_top_p(top_p, where)] * 3
 
 
+def _check_prime(t: torch.Tensor, b: int, q: int, what: str, where="MusicLM.generate_tokens") -> torch.Tensor:
+    """Prime tokens [1 or b, T, q] ([1 or b, T] for the semantic stream) -> [1 or b, T, q], or ValueError."""
+    if isinstance(t, torch.Tensor) and t.dim() == 2 and q == 1:
+        t = t.unsqueeze(-1)
+    if not isinstance(t, torch.Tensor) or t.dim() != 3 or t.shape[-1] != q or t.shape[0] not in (1, b):
+        got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+        raise ValueError(f"open_musiclm_b200 {where}: {what} must be [1 or {b}, T, {q}], got {got}")
+    return t
+
+
 def _prime(t: torch.Tensor, b: int, q: int, device, what: str) -> torch.Tensor:
     """Prime tokens [1 or b, T, q] ([1 or b, T] for the semantic stream) -> [b, T, q] int64 on `device`."""
-    if t.dim() == 2 and q == 1:
-        t = t.unsqueeze(-1)
-    if t.dim() != 3 or t.shape[-1] != q or t.shape[0] not in (1, b):
-        raise ValueError(f"open_musiclm_b200 MusicLM.generate_tokens: {what} must be [1 or {b}, T, {q}], got {tuple(t.shape)}")
-    return t.to(device, torch.int64).expand(b, -1, -1).contiguous()
+    return _check_prime(t, b, q, what).to(device, torch.int64).expand(b, -1, -1).contiguous()
 
 
 class MusicLM(nn.Module):
@@ -275,7 +428,9 @@ class MusicLM(nn.Module):
         the crop that lines it up with the fine windows (forward's return_coarse_generated_wave).
         top_p (nucleus sampling, TokenConditionedTransformerWrapper.generate): None, one value for every stage, or a
         sequence of three values (semantic, coarse, fine), each None or a number in (0, 1]; every window's generate call
-        gets its stage's value.  A sequence of another length or a bad value raises ValueError before the first window."""
+        gets its stage's value.  A sequence of another length or a bad value raises ValueError before the first window.
+        The windows are those of plan_song, run in its order; arguments that give no coarse or no fine window, or
+        streams that cannot be joined, raise ValueError before the first window."""
         stage_top_p = _stage_top_p(top_p)
         if seeds is not None and noise is not None:
             raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: seeds and noise exclude each other")
@@ -283,84 +438,40 @@ class MusicLM(nn.Module):
             seeds = seeds.reshape(-1).tolist() if isinstance(seeds, torch.Tensor) else [int(s) for s in seeds]
             if len(seeds) != clap_token_ids.shape[0]:
                 raise ValueError(f"open_musiclm_b200 MusicLM.generate_tokens: {len(seeds)} seeds for {clap_token_ids.shape[0]} prompts")
-        counter = {}
-
-        def seeded(stage):             # the per-sequence seeds of this stage's next window (none when unseeded)
-            if seeds is None:
-                return {}
-            w = counter.get(stage, 0)
-            counter[stage] = w + 1
-            return dict(seeds=[window_seed(s, stage, w) for s in seeds])
-
-        def sampling(stage):           # this stage's seeds and nucleus mass (passed only when set)
-            kw = seeded(stage)
-            if stage_top_p[stage] is not None:
-                kw["top_p"] = stage_top_p[stage]
-            return kw
-
-        sps, aps = semantic_steps_per_second, acoustic_steps_per_second
         primes = (prime_semantic_token_ids, prime_coarse_token_ids, prime_fine_token_ids)
         primed = prime_semantic_token_ids is not None
         if any((p is not None) != primed for p in primes):
             raise ValueError("open_musiclm_b200 MusicLM.generate_tokens: pass all three prime token streams or none")
-        # ---- audio continuation: condition lengths, the prime's tails and the crops that line the stages up (:913-926)
-        sem_prime = coarse_prime = fine_prime = None
-        sem_adj = coarse_adj = fine_adj = 0
+        streams = {}
         if primed:
             B = clap_token_ids.shape[0]
             qc = self.coarse.num_coarse_quantizers
             qf = self.fine.transformer_wrapper.token_sequences[-1].num_quantizers
-            prime_sem = _prime(prime_semantic_token_ids, B, 1, self.semantic.device, "prime_semantic_token_ids")
-            prime_coarse = _prime(prime_coarse_token_ids, B, qc, self.coarse.device, "prime_coarse_token_ids")
-            prime_fine = _prime(prime_fine_token_ids, B, qf, self.fine.device, "prime_fine_token_ids")
-            cond_sem = int(sps * semantic_window_seconds * (1 - semantic_sliding_window_step_percent))
-            cond_coarse = int(aps * coarse_window_seconds * (1 - coarse_sliding_window_step_percent))
-            cond_fine = int(aps * fine_window_seconds * (1 - fine_sliding_window_step_percent))
-            sem_prime = prime_sem[:, -cond_sem:] if prime_sem.shape[1] >= cond_sem else prime_sem
-            coarse_prime = prime_coarse[:, -cond_coarse:]
-            fine_prime = prime_fine[:, -cond_fine:] if cond_fine > 0 else None
-            sem_adj = cond_sem - int(sps * coarse_window_seconds * (1 - coarse_sliding_window_step_percent))
-            coarse_adj = cond_coarse - int(aps * fine_window_seconds * (1 - fine_sliding_window_step_percent))
-            fine_adj = cond_fine
+            streams = dict(prime_semantic=_prime(prime_semantic_token_ids, B, 1, self.semantic.device, "prime_semantic_token_ids"),
+                           prime_coarse=_prime(prime_coarse_token_ids, B, qc, self.coarse.device, "prime_coarse_token_ids"),
+                           prime_fine=_prime(prime_fine_token_ids, B, qf, self.fine.device, "prime_fine_token_ids"))
+        plan = plan_song(output_seconds=output_seconds, semantic_window_seconds=semantic_window_seconds,
+                         coarse_window_seconds=coarse_window_seconds, fine_window_seconds=fine_window_seconds,
+                         semantic_steps_per_second=semantic_steps_per_second, acoustic_steps_per_second=acoustic_steps_per_second,
+                         semantic_sliding_window_step_percent=semantic_sliding_window_step_percent,
+                         coarse_sliding_window_step_percent=coarse_sliding_window_step_percent,
+                         fine_sliding_window_step_percent=fine_sliding_window_step_percent,
+                         prime_lengths=tuple(streams[k].shape[1] for k in ("prime_semantic", "prime_coarse", "prime_fine")) if primed else None,
+                         coarse_only=coarse_only, top_p=stage_top_p)
         common = dict(clap_token_ids=clap_token_ids, include_eos_in_output=False, append_eos_to_conditioning_tokens=True, noise=noise)
-        # ---- semantic stream: first window from the prime's tail (or scratch), then windows conditioned on the tail of
-        # the stream (:930-949); cropped to line up with the coarse windows (:952)
-        sem = self.semantic.generate(semantic_token_ids=sem_prime, max_time_steps=int(min(output_seconds, semantic_window_seconds) * sps),
-                                     **common, **sampling(SEMANTIC))
-        keep = int(semantic_window_seconds * sps * (1 - semantic_sliding_window_step_percent))
-        while sem.shape[1] < int(output_seconds * sps):
-            nxt = self.semantic.generate(semantic_token_ids=sem[:, -keep:], max_time_steps=int(semantic_window_seconds * sps), **common,
-                                         **sampling(SEMANTIC))
-            sem = torch.cat([sem, nxt[:, keep:]], 1)
-        sem = sem[:, sem_adj:]
-        # ---- coarse stream: one window of semantic tokens per generate, conditioned on the coarse tail, the first one
-        # on the prime's (:956-985)
-        win = int(coarse_window_seconds * sps - 1)
-        coarse, keep = None, int(coarse_window_seconds * aps * (1 - coarse_sliding_window_step_percent))
-        for sem_win in _windows(sem, win, int(win * coarse_sliding_window_step_percent)):
-            pred = self.coarse.generate(semantic_token_ids=sem_win, coarse_token_ids=coarse_prime if coarse is None else coarse[:, -keep:],
-                                        max_time_steps=int(coarse_window_seconds * aps), temperature=0.95, **common, **sampling(COARSE))
-            coarse = pred if coarse is None else torch.cat([coarse, pred[:, keep:]], 1)
-        if coarse_only:                                                                                 # :986-989
-            return coarse
-        coarse = coarse[:, coarse_adj:]                                                                 # :992
-        # ---- fine stream: one window of coarse tokens per generate, the first one conditioned on the prime's tail (:995-1024)
-        fwin = int(fine_window_seconds * aps)
-        fine, keep = None, int(fwin * (1 - fine_sliding_window_step_percent))
-        for coarse_win in _windows(coarse, fwin, int(fwin * fine_sliding_window_step_percent)):
-            cond = fine_prime if fine is None else (fine[:, -keep:] if keep > 0 else None)
-            pred = self.fine.generate(coarse_token_ids=coarse_win, fine_token_ids=cond, max_time_steps=fwin, temperature=0.4, **common,
-                                      **sampling(FINE))
-            fine = pred if fine is None else torch.cat([fine, pred[:, keep:]], 1)
-        fine = fine[:, fine_adj:]                                                                       # :1026
-        # the coarse stream still starts with the fine_adj prime tokens the first fine window was conditioned on; the
-        # reference keeps them, so with a fine condition length > 0 its coarse and fine streams differ in length and
-        # cannot be joined.  Dropping them lines both up on the first token after the prime (no-op when fine_adj = 0).
-        coarse = coarse[:, fine_adj:]
-        if primed:                                                                                      # :1028-1030
-            fine, coarse = torch.cat([prime_fine, fine], 1), torch.cat([prime_coarse, coarse], 1)
-        acoustic = torch.cat([coarse, fine], -1)                                                       # :1032
-        return (acoustic, sem, coarse, fine) if return_all else acoustic
+        part = lambda ref: None if ref is None else streams[ref[0]][:, ref[1]:ref[2]]
+        stages = (self.semantic, self.coarse, self.fine)
+        for job in plan.jobs:
+            kw = {} if seeds is None else dict(seeds=[window_seed(s, job.stage, job.window) for s in seeds])
+            if job.top_p is not None:                          # nucleus mass passed only when set
+                kw["top_p"] = job.top_p
+            cond, prefix = part(job.cond), part(job.prefix)
+            tokens = (dict(semantic_token_ids=prefix), dict(semantic_token_ids=cond, coarse_token_ids=prefix),
+                      dict(coarse_token_ids=cond, fine_token_ids=prefix))[job.stage]
+            out = stages[job.stage].generate(**tokens, max_time_steps=job.max_time_steps, temperature=job.temperature, **common, **kw)
+            name = STREAMS[job.stage]
+            streams[name] = out if name not in streams else torch.cat([streams[name], out[:, job.drop:]], 1)
+        return song_output(plan, streams, return_all)
 
     def prime_token_ids(self, prime_wave: torch.Tensor, prime_wave_sample_hz, semantic_window_seconds=10):
         """A [channels, n] prime wave -> the prime_{semantic,coarse,fine}_token_ids of generate_tokens (batch 1), through
