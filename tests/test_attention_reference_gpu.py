@@ -311,6 +311,52 @@ def test_training_attention_against_float64(lib, B, N, h, mask, bias, qk):
     assert not fails, "\n".join(fails)
 
 
+# The training workspace's forms: a bias table exactly N wide (table_ld = N), and the backward without the bias gradient
+# (a frozen or absent relative-position bias).  Shapes of the d = 72 / h = 3 and cfg2 / h = 8 training steps and prefills.
+EXACT_CASES = [
+    (4, 50, 3, "rand", "rand", "rand"),
+    (3, 33, 3, None, "diag", "rand"),
+    (20, 40, 3, "rand", "rand", "rand"),
+    (4, 1024, 8, "rand", "rand", "rand"),
+    (3, 230, 8, "rand", "diag", "rand"),
+    (2, 100, 16, None, "rand", "rand"),
+]
+
+
+@pytest.mark.parametrize("B,N,h,mask,bias,qk", EXACT_CASES,
+                         ids=[f"B{c[0]}-N{c[1]}-h{c[2]}-{c[3]}-{c[4]}-{c[5]}" for c in EXACT_CASES])
+def test_exact_table_width_and_no_bias_gradient(lib, B, N, h, mask, bias, qk):
+    """attn_fwd_tc and attn_bwd_tc (both modes) on a table exactly N wide against float64, and with dtable None: dqn / dkvn
+    against float64, in the fixed-order mode bit-identical to the call with a table gradient."""
+    qn, kvn, table, key_mask, d_o = make_inputs(B, N, h, mask, bias, qk, seed=3000 * h + N + B)
+    table = table[:, :N].contiguous()
+    inp = (qn, kvn, table, key_mask, d_o)
+    M = B * N
+    ref = reference(qn, kvn, table, key_mask, B, N, h, d_o)
+    tag = f"B={B} N={N} h={h} mask={mask} bias={bias} table_ld=N"
+    fails = []
+    out = torch.full((M, h * 64), float("nan"), device=DEV, dtype=torch.bfloat16)
+    lse = torch.full((B, N * h), float("nan"), device=DEV)
+    lib.attn_fwd_tc(qn, kvn, table, key_mask, out, lse, B, N, h)
+    torch.cuda.synchronize()
+    check(fails, "fwd_tc", "out", out, ref["out"].view(M, h * 64), B, N, h, tag)
+    check_lse2(fails, "fwd_tc", lse, ref["lse2"], tag)
+    ws = lib.AttnBwdDetWorkspace(DEV, B, N, h)
+    for kernel, det in (("bwd_tc", None), ("bwd_tc_det", ws)):
+        dq, dkv, dt = run_bwd_tc(lib, inp, out, lse, B, N, h, det, torch.zeros_like(table))
+        check_grads(fails, kernel, dq, dkv, dt, ref, B, N, h, tag)
+        dq0 = torch.full_like(dq, float("nan"))
+        dkv0 = torch.full_like(dkv, float("nan"))
+        lib.attn_bwd_tc(qn, kvn, d_o, out, lse, table, key_mask, torch.empty(M * h, device=DEV), dq0, dkv0, None, B, N, h, det=det)
+        torch.cuda.synchronize()
+        for name, x, r in (("dq", dq0, ref["dq"]), ("dk", dkv0, ref["dkv"]), ("dv", dkv0, ref["dkv"])):
+            check(fails, kernel, name, x, r, B, N, h, tag + " dtable=None")
+        if det is not None and not (torch.equal(dq0, dq) and torch.equal(dkv0, dkv)):
+            fails.append(f"{kernel} {tag}: dqn / dkvn without dtable differ from the call with it")
+    assert not ws.error()
+    assert not fails, "\n".join(fails)
+
+
 @pytest.mark.parametrize("B,N,h", [(2, 700, 3), (1, 1024, 8), (1, 260, 12)])
 def test_backward_at_forced_chunk_lengths(lib, monkeypatch, B, N, h):
     """OMLM_ATTN_BWD_T forces the backward's chunk length T (row tiles per work unit), which decides how dK|dV are

@@ -65,7 +65,8 @@ BOUNDS = {
 
 # (d, F, conv, B, N): a* d = 72 (K tail 8) with a sequence start at every offset of the 126-row tile and 16-row slab;
 # b* boundaries just before and on the tile seam; c an odd group count (no row-sum GEMM); d one real channel in the last
-# group; e the plain FeedForward; f cfg2 width (352 persistent work items); g 40 row-sum partials per row
+# group; e the plain FeedForward; f cfg2 width (352 persistent work items); g 40 row-sum partials per row; h cfg2 width with
+# sequence starts on 16-row slab edges (224, 448) away from the 126-row seams
 CASES = {
     "a1": (72, 192, True, 300, 1), "a2": (72, 192, True, 150, 2), "a3": (72, 192, True, 100, 3),
     "a127": (72, 192, True, 3, 127), "a129": (72, 192, True, 3, 129), "a252": (72, 192, True, 2, 252),
@@ -75,6 +76,7 @@ CASES = {
     "e": (72, 288, False, 3, 129),
     "f": (1024, 2730, True, 2, 1000),
     "g": (1280, 5120, False, 1, 300),
+    "h": (1024, 2730, True, 3, 224),
 }
 ADT = {"bf16": torch.bfloat16, "fp16": torch.float16}
 
@@ -152,7 +154,8 @@ def check(fails, name, got, ref, allow, keys, seams, tag, cb=128):
 
 # ------------------------------------------------------------------------------------------------ set-up
 def make_case(lib, key, adt, seed=0):
-    d, F, use_conv, B, N = CASES[key]
+    """key: a name of CASES or a (d, F, conv, B, N) tuple."""
+    d, F, use_conv, B, N = CASES[key] if isinstance(key, str) else key
     Fp, M = FR.padded(F), B * N
     g = torch.Generator(device=DEV).manual_seed(seed + F + N)
     xn = torch.randn(M, d, generator=g, device=DEV).to(adt)
@@ -201,12 +204,13 @@ def run_up(lib, c, max_ctas):
     return ub, hb, rb
 
 
-def run_norm(lib, c, h, rs, p):
-    """ffn_norm_fwd -> (hn, the bf16 hn the backward reads, stats, keep bits or None, their guarded buffers)."""
+def run_norm(lib, c, h, rs, p, copy=True):
+    """ffn_norm_fwd -> (hn, the bf16 hn the backward reads, stats, keep bits or None, their guarded buffers).  fp16
+    activations write the bf16 copy of hn (the training forward's form) unless copy is False (inference)."""
     M, F, Fp = c["M"], c["F"], c["Fp"]
     hnb, hn = guarded(M, Fp, c["adt"])
     sb, st = guarded(M, 2, torch.float32)
-    f16 = c["adt"] == torch.float16
+    f16 = c["adt"] == torch.float16 and copy
     hcb, hc = guarded(M, Fp, torch.bfloat16) if f16 else (hnb, hn)
     kb = torch.zeros(M + GUARD, Fp // 8, device=DEV, dtype=torch.uint8)
     kb[M:] = 0xA5
@@ -221,19 +225,31 @@ def pad_cols(x, C):
 
 
 # ------------------------------------------------------------------------------------------------ forward
+def norm_forms(adt):
+    """(dropout p, bf16 copy of hn) of the forward checks: the training forms, and fp16 inference without the copy."""
+    return [(p, True) for p in (0.0, 0.1, 0.5)] + ([(0.0, False)] if adt == torch.float16 else [])
+
+
 @pytest.mark.parametrize("adt", list(ADT))
 @pytest.mark.parametrize("key", list(CASES))
 def test_forward_against_float64(lib, key, adt):
     c = make_case(lib, key, ADT[adt])
-    F, Fp, B, N, M, unit = c["F"], c["Fp"], c["B"], c["N"], c["M"], UNIT[ADT[adt]]
+    fails = forward_checks(lib, c, f"{key} {adt}", (0, 1, 5), norm_forms(ADT[adt]))
+    assert not fails, "\n".join(fails)
+
+
+def forward_checks(lib, c, tag, max_ctas, norms):
+    """gemm_ffn_up at each max_ctas (bit-identical to the first) and ffn_norm_fwd at each (p, copy) of norms, against
+    float64 -> the list of failures."""
+    F, Fp, B, N, M, unit = c["F"], c["Fp"], c["B"], c["N"], c["M"], UNIT[c["adt"]]
     fails = []
-    runs = [run_up(lib, c, m) for m in (0, 1, 5)]
+    runs = [run_up(lib, c, m) for m in max_ctas]
     torch.cuda.synchronize()
     ub, hb, rb = runs[0]
     for i, (u2, h2, r2) in enumerate(runs[1:]):
         for name, a, b in (("u", ub, u2), ("h", hb, h2), ("rowsum", rb, r2)):
             if not torch.equal(a, b):
-                fails.append(f"{name}: max_ctas={(1, 5)[i]} differs from the default grid")
+                fails.append(f"{name}: max_ctas={max_ctas[i + 1]} differs from max_ctas={max_ctas[0]}")
     for name, buf in (("u", ub), ("h", hb), ("rowsum", rb)):
         guard_ok(fails, name, buf, M)
     u, h, rs = ub[:M], hb[:M], rb[:M].view(M, Fp // 128, 2)
@@ -241,9 +257,8 @@ def test_forward_against_float64(lib, key, adt):
         fails.append("h: padded columns are not zero")
     keys, seams = row_keys(B, N, True), seam_rows(B, N)
     kern = lambda x: FR.to_kernel(x, F)
-    tag = f"{key} {adt}"
     chain = FR.forward(c["xn"], c["W1"], c["cw"], c["gam"], N)
-    fl = FLOOR_S[ADT[adt]]
+    fl = FLOOR_S[c["adt"]]
     Sc = FR.magnitude(c["xn"], c["W1"], c["cw"], c["gam"], N, floor=fl)
     u_st = FR.from_kernel(u, F)
     iso = FR.forward(None, None, c["cw"], c["gam"], N, u=u_st)
@@ -259,9 +274,9 @@ def test_forward_against_float64(lib, key, adt):
     S_iso, S_chain = torch.stack([Si["s1"], Si["s2"]], 1), torch.stack([Sc["s1"], Sc["s2"]], 1)
     check(fails, "rowsum iso", rsum, s_iso, 2.0 ** -16 * S_iso, keys, seams, tag, cb=1)
     check(fails, "rowsum chain", rsum, s_chain, 2 * unit * S_chain, keys, seams, tag, cb=1)
-    for p in (0.0, 0.1, 0.5):
-        ptag = f"{tag} p={p}"
-        n = run_norm(lib, c, h, rs, p)
+    for p, copy in norms:
+        ptag = f"{tag} p={p}{'' if copy else ' no copy'}"
+        n = run_norm(lib, c, h, rs, p, copy)
         torch.cuda.synchronize()
         for name, buf in zip(("hn", "stats", "hn copy"), n["bufs"]):
             guard_ok(fails, name, buf, M)
@@ -289,7 +304,7 @@ def test_forward_against_float64(lib, key, adt):
         r_iso = FR.forward(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, h=h[:, :F], stats=(st[:, 0], st[:, 1]))
         S_hn_i = FR.magnitude(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, floor=fl)["hn"]
         check(fails, "hn iso", n["hn"], pad_cols(r_iso["hn"], Fp), pad_cols(2 * unit * S_hn_i, Fp), keys, seams, ptag)
-        if ADT[adt] == torch.float16:
+        if c["adt"] == torch.float16 and copy:
             check(fails, "hn iso", n["hn_b"], pad_cols(r_iso["hn"], Fp), pad_cols(2 * UNIT[torch.bfloat16] * S_hn_i, Fp),
                   keys, seams, ptag + " bf16 copy")
         r_ch = FR.forward(c["xn"], c["W1"], c["cw"], c["gam"], N, keep, p)
@@ -298,7 +313,7 @@ def test_forward_against_float64(lib, key, adt):
               keys, seams, ptag)
         if not bool((n["hn"][:, F:] == 0).all()):
             fails.append(f"hn {ptag}: padded columns are not zero")
-    assert not fails, "\n".join(fails)
+    return fails
 
 
 # ------------------------------------------------------------------------------------------------ backward
@@ -306,7 +321,7 @@ def run_mid_bwd(lib, c, dhn, n, u, p, rowstat, parts, det, dg0, dc0):
     """ffn_mid_bwd into a NaN-poisoned, guarded du and onto the start values dg0 / dc0 -> (du buffer, dgamma, dconv_w)."""
     M, F, Fp, B, N = c["M"], c["F"], c["Fp"], c["B"], c["N"]
     dub, du = guarded(M, 2 * Fp, torch.bfloat16)
-    dg = dg0.clone()
+    dg = None if dg0 is None else dg0.clone()
     dc = None if dc0 is None else dc0.clone()
     part = None
     if det:
@@ -331,9 +346,10 @@ def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag):
         fails.append(f"du {tag}: rel-L2 {e0:.3e} at the channels whose gamma is 0")
     one = torch.zeros(1, dtype=torch.long, device=DEV)
     no = torch.zeros(1, dtype=torch.bool, device=DEV)
-    got = (dg.double() - dg0.double())[None]
-    check(fails, "dgamma", got, ref["dgamma"][None], (2.0 ** -14 * S["dgamma"] + 2 * U32 * dg.double().abs())[None],
-          one, no, tag)
+    if dg is not None:
+        got = (dg.double() - dg0.double())[None]
+        check(fails, "dgamma", got, ref["dgamma"][None], (2.0 ** -14 * S["dgamma"] + 2 * U32 * dg.double().abs())[None],
+              one, no, tag)
     if dc0 is None:
         return
     taps = torch.arange(3, device=DEV)
@@ -348,17 +364,24 @@ def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag):
 def test_backward_against_float64(lib, key, adt):
     """ffn_mid_bwd against float64 autograd from the stored u, in its default and fixed-order modes, with the row sums
     from its own pass and (Fp % 256 == 0) from gemm_rowstat; gamma has exact zeros at channels 0, 127, F - 1 and one
-    more.  dgamma and dconv_w accumulate onto non-zero start values."""
+    more.  dgamma and dconv_w accumulate onto non-zero start values.  Without dgamma (a frozen gamma): du and dconv_w
+    against float64, in the fixed-order mode bit-identical to the call with it."""
     c = make_case(lib, key, ADT[adt])
+    fails = backward_checks(lib, c, f"{key} {adt}", (0.0, 0.1, 0.5))
+    assert not fails, "\n".join(fails)
+
+
+def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0):
+    """ffn_mid_bwd at each dropout p of ps and each mode of dets, with and without dgamma -> the list of failures."""
     F, Fp, B, N, M, d = c["F"], c["Fp"], c["B"], c["N"], c["M"], c["d"]
     fails = []
-    ub, hb, rb = run_up(lib, c, 0)
+    ub, hb, rb = run_up(lib, c, max_ctas)
     u, h, rs = ub[:M], hb[:M], rb[:M].view(M, Fp // 128, 2)
     u_st = FR.from_kernel(u, F)
     g = c["g"]
     dg0 = torch.randn(F, generator=g, device=DEV)
     dc0 = torch.randn(2 * F, 3, generator=g, device=DEV) if c["cw"] is not None else None
-    for p in (0.0, 0.1, 0.5):
+    for p in ps:
         n = run_norm(lib, c, h, rs, p)
         keep = None if p == 0 else FR.unpack_keep(n["kbits"], F)
         # d hn: a random bf16 gradient, and the product dx W2 of gemm_rowstat whose epilogue forms the row sums
@@ -382,18 +405,23 @@ def test_backward_against_float64(lib, key, adt):
             pv = part.view(M, Fp // 128, 2)
             keys, seams = row_keys(B, N, False), seam_rows(B, N)
             for j, (r, S) in enumerate(((s1, S1), (s2, S2))):
-                check(fails, "lnbwd sums", pv[..., j], r, 2.0 ** -16 * S, keys, seams, f"{key} {adt} p={p} s{j + 1}",
+                check(fails, "lnbwd sums", pv[..., j], r, 2.0 ** -16 * S, keys, seams, f"{tag} p={p} s{j + 1}",
                       cb=Fp // 128)
             variants.append(("gemm", dhn2, part))
         for src, dh, part in variants:
             ref = FR.grads(u_st, c["cw"], c["gam"], dh[:, :F], N, keep, p)
             S = FR.magnitude(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, dhn=dh[:, :F])
-            for det in (False, True):
+            for det in dets:
                 if part is None:
                     rowstat, parts = guarded(M, 2, torch.float32)[1], 0
                 else:
                     rowstat, parts = part, Fp // 128
                 dub, dg, dc = run_mid_bwd(lib, c, dh, n, u, p, rowstat, parts, det, dg0, dc0)
                 torch.cuda.synchronize()
-                check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, f"{key} {adt} p={p} {src} det={det}")
-    assert not fails, "\n".join(fails)
+                check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, f"{tag} p={p} {src} det={det}")
+                dub2, _, dc2 = run_mid_bwd(lib, c, dh, n, u, p, rowstat, parts, det, None, dc0)
+                torch.cuda.synchronize()
+                check_grads(fails, c, dub2, None, dc2, None, dc0, ref, S, f"{tag} p={p} {src} det={det} dgamma=None")
+                if det and not (torch.equal(dub2, dub) and (dc is None or torch.equal(dc2, dc))):
+                    fails.append(f"{tag} p={p} {src} det={det}: du / dconv_w without dgamma differ from the call with it")
+    return fails

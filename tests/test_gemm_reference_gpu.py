@@ -5,7 +5,7 @@ Every output is NaN-poisoned before the call; the rows past M (or past the remap
 and the pitch padding hold a sentinel that must survive.  A failure names the worst element in units of its bound and
 the worst 128 x 64 block.  The persistent grid (max_ctas 1, 2, 7) must give bit-identical results for every form
 without atomics, and the staged and direct epilogues bit-identical results at alpha = 1/3.  The engine's call forms
-are recorded over training steps and generation and replayed at their real shapes; a form whose coverage key the
+are recorded over the phases of tests/call_forms.py (training steps, generate and generation sessions) and replayed at their real shapes; a form whose coverage key the
 explicit matrix below lacks fails the coverage test."""
 
 import pytest
@@ -579,44 +579,17 @@ class _Recorder:
             setattr(self.lib, n, f)
 
 
-def _record(act16, small, monkeypatch):
-    """Forms of one training step in each mode and of generate at B <= 16 and B > 16."""
-    import open_musiclm_b200 as O
-    lib = _lib()
-    monkeypatch.setenv("OMLM_ACT16", act16)
-    torch.manual_seed(0)
-    if small:      # d = 72, codebooks whose C = 101 / 65 are not multiples of 64
-        kw = dict(dim=72, depth=1, heads=3, clap_codebook_size=100, semantic_codebook_size=100, acoustic_codebook_size=64,
-                  num_clap_quantizers=4, num_coarse_quantizers=3)
-        cond_n, pred_shape, vocab = [(4,), (11,)], (10, 3), 64
-    else:          # the cfg2 layer dims, one layer
-        kw = dict(dim=1024, depth=1, heads=8, num_coarse_quantizers=3)
-        cond_n, pred_shape, vocab = [(12,), (197,)], (270, 3), 1024
-    g = torch.Generator().manual_seed(1)
-    with _Recorder(lib) as rec:
-        for det in (False, True):
-            rec.phase = "deterministic step" if det else "default step"
-            m = O.create_coarse_transformer(attn_dropout=0.0, ff_dropout=0.1, **kw).cuda()
-            tr = O.HotPathTrainer(m, cross_entropy_loss_weights=[0.0, 1.0, 1.0], lr=3e-4, wd=1e-2, use_cuda_graph=False)
-            toks = [torch.randint(0, min(vocab, 64), (4,) + s, generator=g).cuda() for s in cond_n + [pred_shape]]
-            prev = torch.are_deterministic_algorithms_enabled()
-            torch.use_deterministic_algorithms(det)
-            try:
-                tr.train_step([toks])
-                torch.cuda.synchronize()
-            finally:
-                torch.use_deterministic_algorithms(prev)
-        m.eval()
-        w = O.TokenConditionedTransformerWrapper(transformer=m, unique_consecutive=False)
-        for B in (3, 20):
-            rec.phase = f"generate B={B}"
-            cond = [torch.randint(0, min(vocab, 64), (B,) + s, generator=g).cuda() for s in cond_n]
-            w.generate(conditioning_token_ids=cond, max_time_steps=3)
-        torch.cuda.synchronize()
+def _record(act16, model, monkeypatch):
+    """Forms of every phase of call_forms: training steps, eval_loss, generate at B <= 16 and B > 16, and sessions."""
+    import call_forms
+    with _Recorder(_lib()) as rec:
+        call_forms.run(rec, model, act16, monkeypatch)
     # the shim sees the engine only while it calls through lib's attributes: every path must have shown up
-    expected = {("default step", "gemm"), ("default step", "gemm_rowstat"), ("deterministic step", "gemm"),
-                ("deterministic step", "gemm_splitk_det"), ("generate B=3", "gemm"), ("generate B=3", "skinny_gemm"),
-                ("generate B=20", "decode_gemm")}
+    expected = {(p, "gemm") for p in call_forms.SESSION_PHASES} | {(p, "decode_gemm") for p in call_forms.SESSION_PHASES}
+    if model not in call_forms.SESSIONS_ONLY:
+        expected |= {("default step", "gemm"), ("default step", "gemm_rowstat"), ("deterministic step", "gemm"),
+                     ("deterministic step", "gemm_splitk_det"), ("generate B=3", "gemm"), ("generate B=3", "skinny_gemm"),
+                     ("generate B=20", "decode_gemm")}
     assert expected <= rec.seen, f"entry points the engine did not call through lib: {sorted(expected - rec.seen)}"
     return rec.forms
 
@@ -710,10 +683,10 @@ def _replay_splitk_det(f, gen):
     return ("gemm_splitk_det", str(dt), a_mn, b_mn, bn, (rs > 0) - (rs < 0), nv < N)
 
 
-@pytest.mark.parametrize("small", [True, False], ids=["d72", "cfg2_depth1"])
+@pytest.mark.parametrize("model", ["d72", "cfg2_depth1", "cfg2_h16"])
 @pytest.mark.parametrize("act16", ["fp16", "bf16"])
-def test_engine_call_forms_replayed_and_covered(act16, small, monkeypatch):
-    forms = _record(act16, small, monkeypatch)
+def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
+    forms = _record(act16, model, monkeypatch)
     gen = torch.Generator(device=DEV).manual_seed(17)
     covered, keys = explicit_gemm_keys(), set()
     for f in sorted(forms.get("gemm", ()), key=repr):
@@ -729,7 +702,7 @@ def test_engine_call_forms_replayed_and_covered(act16, small, monkeypatch):
         for f in sorted(forms.get(entry, ()), key=repr):
             keys.add(_replay_decode(entry, f, gen))
     covered |= explicit_decode_keys()
-    print(f"act16={act16} {'d72' if small else 'cfg2 depth 1'}: {len(keys)} keys issued by the engine")
+    print(f"act16={act16} {model}: {len(keys)} keys issued by the engine")
     for k in sorted(keys, key=repr):
         print("   ", k)
     missing = sorted((k for k in keys if k not in covered), key=repr)

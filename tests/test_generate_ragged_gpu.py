@@ -122,6 +122,20 @@ def _run_decode(lib, kernel, q_raw, kv_raw, q_scale, k_scale, cache, table, pos,
     return out
 
 
+def ragged_decode_reference(cache0, row, qn, table, pos):
+    """Float64 output [B, h*64] of one ragged decode step: row b at position n_b = pos[b] attends to its cached keys
+    0 .. n_b - 1 (cache0 [B, *, 128]) and its appended row n_b (row [B, 128]); qn [B, h, 64] the bf16 queries."""
+    B, h = qn.shape[0], qn.shape[1]
+    ref = torch.empty(B, h * 64, dtype=torch.float64, device=qn.device)
+    for b in range(B):
+        n = int(pos[b])
+        keys = torch.cat([cache0[b, :n], row[b:b + 1]], 0).double()
+        j = torch.arange(n + 1, device=qn.device)
+        sim = 8.0 * qn[b].double() @ keys[:, :64].t() + table[:, n - j].double()
+        ref[b] = (sim.softmax(-1) @ keys[:, 64:]).reshape(-1)
+    return ref
+
+
 KCASES = [(k, B, h) for k, Bs in (("decode", (1, 16)), ("decode_mqa", (1, 16, 17, 256))) for B in Bs for h in (1, 8, 16)]
 
 
@@ -136,16 +150,12 @@ def test_ragged_decode_attention_against_float64(kernel, B, h):
     out = _run_decode(lib, kernel, q_raw, kv_raw, q_scale, k_scale, cache, table, pos, h)
     row = torch.cat([(F.normalize(kv_raw[:, :64].float(), dim=-1) * k_scale).bfloat16(), kv_raw[:, 64:]], -1)
     qn = (F.normalize(q_raw.float().view(B, h, 64), dim=-1) * q_scale).bfloat16()
-    ref = torch.empty(B, h * 64, dtype=torch.float64, device=DEV)
     for b in range(B):
         n = int(pos[b])
         assert torch.equal(cache[b, :n], cache0[b, :n]) and torch.isnan(cache[b, n + 1:].float()).all(), b
         got = cache[b, n].float()
         assert ((got - row[b].float()).abs() <= row[b].float().abs() * 2.0 ** -7).all(), b
-        keys = torch.cat([cache0[b, :n], row[b:b + 1]], 0).double()
-        j = torch.arange(n + 1, device=DEV)
-        sim = 8.0 * qn[b].double() @ keys[:, :64].t() + table[:, n - j].double()
-        ref[b] = (sim.softmax(-1) @ keys[:, 64:]).reshape(-1)
+    ref = ragged_decode_reference(cache0, row, qn, table, pos)
     fails = []
     check(fails, kernel, "out", out, ref, B, 1, h, f"ragged B={B} h={h}")
     assert not fails, "\n".join(fails)

@@ -120,6 +120,29 @@ def test_token_logprob_against_ce_ref(lib, C):
     assert bool(((got + ref["loss"]).abs()[valid] <= ref["loss_bound"][valid]).all())
 
 
+@pytest.mark.parametrize("C", [65, 1025, 1281])
+def test_token_logprob_flat_labels_against_ce_ref(lib, C):
+    """omlm_token_logprob with one flat label per row, as a session's packed prefill scores its prefixes (rows of a
+    logits buffer wider than C, -100 on the next-token rows): the negated ce_ref row loss within its bound, 0 for
+    labels outside [0, C), and nothing written past the rows."""
+    g = torch.Generator().manual_seed(C + 1)
+    rows, ld = 37, (C + 63) // 64 * 64
+    x = torch.full((rows, ld), float("nan"))
+    x[:, :C] = torch.randn(rows, C, generator=g) * 3
+    lab = torch.randint(0, C, (rows,), generator=g, dtype=torch.int32)
+    lab[:3], lab[10] = -100, C
+    out = torch.full((rows + 2,), 7.0, device=DEV)
+    lib.token_logprob(x.to(DEV), lab.to(DEV), C, out, rows=rows)
+    torch.cuda.synchronize()
+    l = lab.long()
+    valid = (l >= 0) & (l < C)
+    ref = ce_ref(x, torch.where(valid, l, torch.full_like(l, -100)), C, C, grad_scale=0.0)
+    got = out.cpu().double()
+    assert bool((got[rows:] == 7.0).all())
+    assert bool((got[:rows][~valid] == 0).all())
+    assert bool(((got[:rows] + ref["loss"]).abs()[valid] <= ref["loss_bound"][valid]).all())
+
+
 # ------------------------------------------------------------------------------------------------ generate / session
 def _gen(w, cond, pred, **kw):
     return w.generate(conditioning_token_ids=cond, pred_token_ids=pred, **kw)

@@ -436,6 +436,40 @@ def ce_check(x, lab_arg, lab, C, Cp, has_dl, det, what, view=None):
     assert float(acc[1]) == 2.0 + ref["count"], f"{what}: row count {float(acc[1]) - 2} != {ref['count']}"
 
 
+def token_logprob_check(rows, C, ld, lstride, rpb, bstride, gen, what):
+    """token_logprob on logits [rows, ld] (NaN past C) with flat labels (rpb = 0) or the strided view, against the negated
+    ce_ref row loss within its bound; 0 for labels outside [0, C); the rows past `rows` of out keep their sentinel.
+    -> its coverage key ("token_logprob", strided)."""
+    lib = _lib()
+    x = torch.randn(rows, ld, device=DEV, generator=gen) * 3
+    x[:, C:] = NAN
+    if rpb:
+        plane = torch.randint(0, C, ((rows // rpb + 1) * bstride + rpb * lstride,), device=DEV, generator=gen, dtype=torch.int32)
+        plane[lstride] = -100
+        plane[0] = C
+        view = dict(label_stride=lstride, rows_per_batch=rpb, batch_stride=bstride)
+        lab = R.ce_labels(plane, rows, **view)
+    else:
+        plane = torch.randint(0, C, (rows,), device=DEV, generator=gen, dtype=torch.int32)
+        plane[::5] = -100
+        plane[1::7] = C
+        view, lab = dict(label_stride=lstride), plane.long()
+    out = torch.full((rows + 2,), 7.0, device=DEV)
+    lib.token_logprob(x, plane, C, out, rows=rows, **view)
+    torch.cuda.synchronize()
+    assert bool((out[rows:] == 7.0).all()), f"{what}: out written past its rows"
+    lab = lab.to(DEV).long()
+    valid = (lab >= 0) & (lab < C)
+    ref = R.ce_ref(x, torch.where(valid, lab, torch.full_like(lab, -100)), C, C, grad_scale=0.0)
+    got = out[:rows].double()
+    assert bool((got[~valid] == 0).all()), f"{what}: labels outside [0, C) must give 0"
+    err = (got + ref["loss"].to(DEV)).abs()[valid]
+    bnd = ref["loss_bound"].to(DEV)[valid]
+    assert bool((err <= bnd).all()), f"{what}: {int((err > bnd).sum())} rows beyond the bound, worst {float((err / bnd).max()):.3f}"
+    WORST["token_logprob"] = max(WORST.get("token_logprob", 0.0), float((err / bnd).max()) if err.numel() else 0.0)
+    return ("token_logprob", int(rpb > 0))
+
+
 @pytest.mark.parametrize("pad", CE_PAD)
 @pytest.mark.parametrize("C", CE_C)
 def test_cross_entropy_register_path_per_element(C, pad):
@@ -531,7 +565,8 @@ def test_embed_gather_exact(two):
 
 
 # ------------------------------------------------------------------------------------------------ the engine's call forms
-NAMES = ("layernorm_fwd", "layernorm_bwd", "qk_l2norm_fwd", "qk_l2norm_bwd", "cross_entropy", "embed_gather", "embed_scatter_add")
+NAMES = ("layernorm_fwd", "layernorm_bwd", "qk_l2norm_fwd", "qk_l2norm_bwd", "cross_entropy", "embed_gather", "embed_scatter_add",
+         "token_logprob")
 
 
 class _Recorder:
@@ -576,6 +611,12 @@ class _Recorder:
                                       label_stride=label_stride, rows=rows, rows_per_batch=rows_per_batch, batch_stride=batch_stride,
                                       loss_scale=loss_scale, part=part)
 
+        def token_logprob(logits, labels, C, out, *, label_stride=1, rows=None, rows_per_batch=0, batch_stride=0):
+            r = logits.shape[0] if rows is None else rows
+            self._add("token_logprob", (r, C, logits.stride(0), label_stride, rows_per_batch, batch_stride))
+            return o["token_logprob"](logits, labels, C, out, label_stride=label_stride, rows=rows, rows_per_batch=rows_per_batch,
+                                      batch_stride=batch_stride)
+
         def embed_gather(table, src_row, x, src_row2=None):
             self._add("embed_gather", (src_row2 is not None,))          # (no device read here: generate captures graphs)
             return o["embed_gather"](table, src_row, x, src_row2)
@@ -593,57 +634,23 @@ class _Recorder:
             setattr(self.lib, n, f)
 
 
-def _record(act16, small, monkeypatch):
-    """Forms of a default, a deterministic and a frozen-norm step, eval_loss and generate, with pad tokens."""
-    import open_musiclm_b200 as O
-    lib = _lib()
-    monkeypatch.setenv("OMLM_ACT16", act16)
-    torch.manual_seed(0)
-    if small:      # d = 72, codebooks whose C = 101 / 65 are not multiples of 64
-        kw = dict(dim=72, depth=1, heads=3, clap_codebook_size=100, semantic_codebook_size=100, acoustic_codebook_size=64,
-                  num_clap_quantizers=4, num_coarse_quantizers=3)
-        cond_n, pred_shape, vocab = [(4,), (11,)], (10, 3), 64
-    else:          # the cfg2 layer dims, one layer
-        kw = dict(dim=1024, depth=1, heads=8, num_coarse_quantizers=3)
-        cond_n, pred_shape, vocab = [(12,), (197,)], (270, 3), 1024
-    g = torch.Generator().manual_seed(1)
-
-    def batch():
-        toks = [torch.randint(0, min(vocab, 64), (4,) + s, generator=g) for s in cond_n + [pred_shape]]
-        toks[0][1, -2:] = -1                     # pad tokens: their embedding rows are zero
-        toks[1][2, -3:] = -1
-        return [t.cuda() for t in toks]
-
-    with _Recorder(lib) as rec:
-        for phase, det, frozen in (("default step", False, False), ("deterministic step", True, False),
-                                   ("frozen norms step", False, True), ("frozen norms deterministic step", True, True)):
-            rec.phase = phase
-            m = O.create_coarse_transformer(attn_dropout=0.0, ff_dropout=0.1, **kw).cuda()
-            if frozen:
-                for n, p in m.named_parameters():
-                    if n.endswith("gamma") or n.endswith("q_scale") or n.endswith("k_scale"):
-                        p.requires_grad_(False)
-            tr = O.HotPathTrainer(m, cross_entropy_loss_weights=[0.0, 1.0, 1.0], lr=3e-4, wd=1e-2, use_cuda_graph=False)
-            prev = torch.are_deterministic_algorithms_enabled()
-            torch.use_deterministic_algorithms(det)
-            try:
-                tr.train_step([batch()])
-                torch.cuda.synchronize()
-            finally:
-                torch.use_deterministic_algorithms(prev)
-        rec.phase = "eval_loss"
-        tr.eval_loss(batch())
-        m.eval()
-        w = O.TokenConditionedTransformerWrapper(transformer=m, unique_consecutive=False)
-        rec.phase = "generate"
-        cond = [torch.randint(0, min(vocab, 64), (3,) + s, generator=g).cuda() for s in cond_n]
-        w.generate(conditioning_token_ids=cond, max_time_steps=3)
-        torch.cuda.synchronize()
-    expected = {(p, n) for p in ("default step", "deterministic step") for n in NAMES if n != "embed_gather"} | \
-        {("default step", "embed_gather"), ("eval_loss", "cross_entropy"), ("eval_loss", "layernorm_fwd"),
-         ("generate", "layernorm_fwd"), ("generate", "embed_gather"), ("frozen norms step", "layernorm_bwd"),
-         ("frozen norms step", "qk_l2norm_bwd")}
+def _record(act16, model, monkeypatch):
+    """Forms of every phase of call_forms: default, deterministic, frozen-norm and frozen-relpos steps with pad tokens,
+    eval_loss, generate and sessions."""
+    import call_forms
+    with _Recorder(_lib()) as rec:
+        call_forms.run(rec, model, act16, monkeypatch)
+    # sessions: the packed prefill's final norm writes the rows dest_row names; return_logprobs scores the prefixes
+    expected = {(p, n) for p in call_forms.SESSION_PHASES for n in ("layernorm_fwd", "embed_gather")} | \
+        {("session logprobs", "token_logprob")}
+    if model not in call_forms.SESSIONS_ONLY:
+        expected |= {(p, n) for p in ("default step", "deterministic step") for n in NAMES if n not in ("embed_gather", "token_logprob")} | \
+            {("default step", "embed_gather"), ("eval_loss", "cross_entropy"), ("eval_loss", "layernorm_fwd"),
+             ("generate B=3", "layernorm_fwd"), ("generate B=3", "embed_gather"), ("frozen norms step", "layernorm_bwd"),
+             ("frozen norms step", "qk_l2norm_bwd")}
     assert expected <= rec.seen, f"entry points the engine did not call through lib: {sorted(expected - rec.seen)}"
+    dest = {f[6] for n, f in rec.forms if n == "layernorm_fwd"}
+    assert True in dest, "no layernorm_fwd call with dest_row was recorded"
     return rec.forms
 
 
@@ -690,6 +697,9 @@ def _replay(name, f, gen):
             view, lab_arg, lab = dict(label_stride=lstride), lab, lab.long()
         ce_check(x, lab_arg, lab, C, Cp, has_dl, int(det), f"engine form {name} {f}", view=view)
         return ce_key(C, Cp, has_dl, int(det), int(strided))
+    if name == "token_logprob":
+        rows, C, ld, lstride, rpb, bstride = f
+        return token_logprob_check(rows, C, ld, lstride, rpb, bstride, gen, f"engine form {name} {f}")
     if name == "embed_gather":
         return ("embed_gather", int(f[0]))
     if name == "embed_scatter_add":
@@ -697,18 +707,19 @@ def _replay(name, f, gen):
     raise AssertionError(name)
 
 
-@pytest.mark.parametrize("small", [True, False], ids=["d72", "cfg2_depth1"])
+@pytest.mark.parametrize("model", ["d72", "cfg2_depth1", "cfg2_h16"])
 @pytest.mark.parametrize("act16", ["fp16", "bf16"])
-def test_engine_call_forms_replayed_and_covered(act16, small, monkeypatch):
-    forms = _record(act16, small, monkeypatch)
+def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
+    forms = _record(act16, model, monkeypatch)
     gen = torch.Generator(device=DEV).manual_seed(23)
     covered = explicit_ln_keys() | explicit_qk_keys() | explicit_ce_keys()
     covered |= {("embed_gather", 0), ("embed_gather", 1)}               # test_embed_gather_exact
     covered |= {("embed_scatter_add", 0), ("embed_scatter_add", 1)}     # test_embed_scatter_add_per_element
+    covered |= {("token_logprob", 0), ("token_logprob", 1)}             # test_logprobs_gpu: flat and strided labels
     keys = set()
     for name, f in sorted(forms, key=repr):
         keys.add(_replay(name, f, gen))
-    print(f"act16={act16} {'d72' if small else 'cfg2 depth 1'}: {len(keys)} keys issued by the engine")
+    print(f"act16={act16} {model}: {len(keys)} keys issued by the engine")
     for k in sorted(keys, key=repr):
         print("   ", k)
     missing = sorted((k for k in keys if k not in covered), key=repr)

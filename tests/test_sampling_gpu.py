@@ -383,8 +383,12 @@ def test_decode_conv_geglu_equals_the_float64_sequence(lib, adt, F_, Fp):
     """Rows of u fed one at a time from a zero state: h equals the float64 causal conv (zero left padding) + exact-erf
     GEGLU over the whole sequence within one 16-bit ulp (fp16: saturated at +-65504), padded channels are exactly 0,
     the row sums match float64, and after each step the state holds the last two u rows bit for bit."""
-    B, T = 3, 7
-    g = torch.Generator().manual_seed(F_ + (adt == torch.float16))
+    conv_geglu_check(lib, adt, F_, Fp, 3, 7, F_ + (adt == torch.float16))
+
+
+def conv_geglu_check(lib, adt, F_, Fp, B, T, seed):
+    """decode_conv_geglu over T steps of B rows against the float64 sequence (the assertions of the test above)."""
+    g = torch.Generator().manual_seed(seed)
     u_nat = (torch.randn(T, B, 2 * F_, generator=g) * 1.5)
     u_nat[T - 3, :, [0, 1, F_, F_ + 1]] = torch.tensor([1000.0, -1000.0, 1000.0, 1000.0])  # |h| ~ 1e5: the fp16 clamp
     u_nat = u_nat.to(adt)

@@ -29,7 +29,25 @@ def _unit(h):
 
 
 # ------------------------------------------------------------------------------------------------ 1. attention
-@pytest.mark.parametrize("h,N", [(1, 1000), (2, 700), (6, 650), (8, 1000), (16, 700)])
+# (h, N); (3, 700): the d = 72 model's heads; (3, 100): a whole prompt shorter than U = 128; (8, 645), (16, 645): a final
+# chunk shorter than U at p0 = 640, on the 64-row grid
+CHUNK_ATTN = [(1, 1000), (2, 700), (6, 650), (8, 1000), (16, 700), (3, 700), (3, 100), (8, 645), (16, 645)]
+
+
+def chunk_attn_chunks(h, N):
+    """(p0, length) of the chunks of test_chunk_attention_is_the_whole_sequence: every U-aligned p0, every third chunk
+    to the end of the sequence, the others 1 ... 5 units long."""
+    U = _unit(h)
+    g = torch.Generator().manual_seed(h)
+    chunks = []
+    for i, p0 in enumerate(range(0, N, U)):
+        rem = N - p0
+        n = rem if i % 3 == 0 else min(rem, U * int(torch.randint(1, 6, (1,), generator=g)))
+        chunks.append((p0, n))
+    return chunks
+
+
+@pytest.mark.parametrize("h,N", CHUNK_ATTN)
 def test_chunk_attention_is_the_whole_sequence(lib, h, N):
     """Chunks at every U-aligned p0 < N (non-final ones of whole units, final ones to the end, p0 = 0 among them),
     all in one launch: each chunk's keys come from its own slot of a cache-shaped buffer that holds the sequence's K/V
@@ -40,12 +58,7 @@ def test_chunk_attention_is_the_whole_sequence(lib, h, N):
     o_ref = torch.empty(N, h * 64, device=DEV, dtype=torch.bfloat16)
     l_ref = torch.empty(N * h, device=DEV)
     lib.attn_fwd_tc(qn, kvn, table, None, o_ref, l_ref, 1, N, h)
-    g = torch.Generator().manual_seed(h)
-    chunks = []
-    for i, p0 in enumerate(range(0, N, U)):
-        rem = N - p0
-        n = rem if i % 3 == 0 else min(rem, U * int(torch.randint(1, 6, (1,), generator=g)))
-        chunks.append((p0, n))
+    chunks = chunk_attn_chunks(h, N)
     n_max = N + 8
     cache = torch.full((len(chunks), n_max, 128), float("nan"), device=DEV, dtype=torch.bfloat16)
     for s, (p0, n) in enumerate(chunks):
@@ -66,8 +79,17 @@ def test_chunk_attention_is_the_whole_sequence(lib, h, N):
 
 
 # ------------------------------------------------------------------------------------------------ 2. FFN up
+CHUNK_FFN = [(192, 384), (1024, 2816), (72, 256)]          # (K, Fp); K = 72: a K tail, as the d = 72 model's
+
+
+def chunk_ffn_chunks():
+    """(p0, length) of the chunks of test_chunk_ffn_up_is_the_whole_sequence, in packing order."""
+    return [(1, 1), (2, 1), (3, 2), (16, 3), (125, 1), (0, 130), (126, 7), (127, 126), (128, 127), (252, 148), (3, 300), (1, 2),
+            (0, 34), (0, 3)]          # the last starts at packed row 882 = 7 x 126, on a tile seam and a slab edge
+
+
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("K,Fp", [(192, 384), (1024, 2816)])
+@pytest.mark.parametrize("K,Fp", CHUNK_FFN)
 def test_chunk_ffn_up_is_the_whole_sequence(lib, dt, K, Fp):
     """Chunks of one sequence at p0 in {1, 2, 3, U, 125, 126, 127, 128, 252} (and a p0 = 0 chunk), packed in one
     launch, each first row's conv history from two supplied rows of the whole run's u (a zero row before position 0):
@@ -80,7 +102,7 @@ def test_chunk_ffn_up_is_the_whole_sequence(lib, dt, K, Fp):
     u_ref, h_ref = torch.empty(N, 2 * Fp, device=DEV, dtype=dt), torch.empty(N, Fp, device=DEV, dtype=dt)
     r_ref = torch.empty(N, Fp // 128, 2, device=DEV)
     lib.gemm_ffn_up(xn, w1, conv, u_ref, h_ref, r_ref, N, Fp)
-    chunks = [(1, 1), (2, 1), (3, 2), (16, 3), (125, 1), (0, 130), (126, 7), (127, 126), (128, 127), (252, 148), (3, 300), (1, 2)]
+    chunks = chunk_ffn_chunks()
     lens = [n for _, n in chunks]
     M = sum(lens)
     hist = torch.zeros(2 * len(chunks), 2 * Fp, device=DEV, dtype=dt)

@@ -85,8 +85,23 @@ def _ffn_lens():
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("max_ctas", [1, 2, 7])
 def test_varlen_ffn_up_is_each_sequence_alone(lib, dt, max_ctas):
+    _varlen_ffn_case(lib, dt, max_ctas, 192, 384)
+
+
+VARLEN_FFN = [(72, 256), (1024, 2816)]        # (K, Fp) of the d = 72 and cfg2 models: a K tail, and 22 channel groups
+
+
+@pytest.mark.parametrize("K,Fp", VARLEN_FFN)
+@pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
+def test_varlen_ffn_up_at_model_widths(lib, dt, K, Fp):
+    _varlen_ffn_case(lib, dt, 0, K, Fp)
+
+
+def _varlen_ffn_case(lib, dt, max_ctas, K, Fp):
+    """The sequences of _ffn_lens packed in one gemm_ffn_up_varlen launch: u, h and rowsum of each equal gemm_ffn_up on
+    that sequence alone."""
     lens = _ffn_lens()
-    M, K, Fp = sum(lens), 192, 384
+    M = sum(lens)
     g = torch.Generator(device=DEV).manual_seed(max_ctas + (dt == torch.float16))
     xn = torch.randn(M, K, device=DEV, generator=g).to(dt)
     w1 = (torch.randn(2 * Fp, K, device=DEV, generator=g) / K ** 0.5).to(dt)
