@@ -10,6 +10,7 @@ Only what the TokenConditionedTransformer training path needs lives here:
   session.py  `GenerationSession`: continuous batching, rows joining and leaving a running decode
   stages.py   `SemanticStage` / `CoarseStage` / `FineStage` and the windowed three-stage `MusicLM` generation
   musiclm_session.py  `MusicLMSession`: continuous batching of whole songs through the three stages
+  score.py    teacher-forced scoring in packed forwards: `wrapper.score`, `MusicLM.score_tokens`
 """
 __version__ = "0.1.0"
 

@@ -116,13 +116,13 @@ def check_top_p(top_p, where: str = "generate"):
     return p
 
 
-def check_pred_lengths(pred_lengths, pred_token_ids, B: int):
+def check_pred_lengths(pred_lengths, pred_token_ids, B: int, caller: str = "generate"):
     """generate's pred_lengths -> a list of B ints in [0, pred_token_ids.shape[1]], or None when it is None or every
     value equals pred_token_ids.shape[1] (every prefix whole).  A wrong count, a value out of
-    range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError."""
+    range, a non-integer or a bool, or pred_lengths without pred_token_ids raises ValueError (naming `caller`)."""
     if pred_lengths is None:
         return None
-    where = "open_musiclm_b200 generate: pred_lengths"
+    where = f"open_musiclm_b200 {caller}: pred_lengths"
     if pred_token_ids is None:
         raise ValueError(f"{where} needs pred_token_ids")
     if isinstance(pred_lengths, torch.Tensor):
@@ -233,6 +233,23 @@ def row_arrays(dev, B: int, **values):
     return out
 
 
+def bias_table(eng, N: int):
+    """The relative position bias of every distance 0 ... N - 1 (it depends on i - j only), as the scratch dict
+    Engine.build_bias_table fills: its "table" entry is [heads, N] float32 (zero with no bias)."""
+    dev, f32 = eng.dev, torch.float32
+    E = lambda *shape, dt=torch.bfloat16: torch.empty(*shape, device=dev, dtype=dt)
+    rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, eng.Hr, dt=f32) for _ in range(3)], rp_a=[E(N, eng.Hr, dt=f32) for _ in range(3)],
+              table=E(eng.h, N, dt=f32), rp_a3=[E(N, 3 * eng.Hr8) for _ in range(2)])
+    lib.arange_f32(rp["rp_in"])
+    eng.refresh_packed()
+    if eng.bias_type == "none":
+        rp["table"].zero_()
+    elif eng.bias_type == "t5":
+        rp["ones"] = torch.ones(N, device=dev, dtype=f32)
+    eng.build_bias_table(rp, N)
+    return rp
+
+
 class DecodeSession:
     """Caches and scratch of one decode: B sequences, caches of n_max positions, up to n_new new tokens per sequence.
     rows (row_arrays): the per-sequence state every step and sample reads, as device arrays [B]: pos (the position the
@@ -252,7 +269,7 @@ class DecodeSession:
             raise lib.OmlmError(f"open_musiclm_b200 generate: seeded generation supports at most 16 heads ({eng.h} given)")
         self.eng, self.B, self.n_max, self.n_new, self.seeded = eng, B, n_max, n_new, seeded
         dev, bf, f32, a16 = eng.dev, torch.bfloat16, torch.float32, eng.a16
-        d, HD, Fp, h, Hr = eng.d, eng.HD, eng.Fp, eng.h, eng.Hr
+        d, HD, Fp, h = eng.d, eng.HD, eng.Fp, eng.h
         E = lambda *shape, dt=bf: torch.empty(*shape, device=dev, dtype=dt)
         self.cache = [E(B, n_max, 128) for _ in range(eng.L)]
         self.conv = [E(B, 2, 2 * Fp, dt=a16) for _ in range(eng.L)]
@@ -273,16 +290,7 @@ class DecodeSession:
         self.pos, self.pos_last, self.pos_offset = rows["pos"], rows["pos_last"], rows["pos_offset"]
         self.top_k, self.temperature, self.top_p = rows["top_k"], rows["temperature"], rows["top_p"]
         # bias table for every distance the generation can reach (it depends on i - j only)
-        N = n_max
-        self.rp = dict(rp_in=E(N, 1, dt=f32), rp_z=[E(N, Hr, dt=f32) for _ in range(3)], rp_a=[E(N, Hr, dt=f32) for _ in range(3)],
-                       table=E(h, N, dt=f32), rp_a3=[E(N, 3 * eng.Hr8) for _ in range(2)])
-        lib.arange_f32(self.rp["rp_in"])
-        eng.refresh_packed()
-        if eng.bias_type == "none":
-            self.rp["table"].zero_()
-        elif eng.bias_type == "t5":
-            self.rp["ones"] = torch.ones(N, device=dev, dtype=f32)
-        eng.build_bias_table(self.rp, N)
+        self.rp = bias_table(eng, n_max)
         self.table = self.rp["table"]
         self.graphs = GraphCache(use_graph)
         # more than 16 sequences, or seeded mode: tensor-core GEMMs and the cache-sharing attention, with their scratch
@@ -651,6 +659,24 @@ class TokenConditionedTransformerWrapper(nn.Module):
             m.train()
         return assemble_output(prefix, new, rows["n_real"][:, None], rows["n_end"][:, None], max(state["n_end"]), eos,
                                include_eos_in_output, q, (pre_lp, lp_new, slp_new) if return_logprobs else None)
+
+    @torch.no_grad()
+    def score(self, *, conditioning_token_ids: List[torch.Tensor], pred_token_ids: torch.Tensor, pred_lengths=None,
+              max_rows: int = 16384):
+        """The model's log-probability of every given token, teacher-forced: [b, t, q] float32 on the device for
+        pred_token_ids [b, t, q] ([b, t] when q = 1).  Value [r, i, j] is log softmax of the fp32 logits row at that
+        token's position over all codebook+1 classes (no temperature, top-k or eos rule) at the token, exactly the value
+        generate(conditioning_token_ids=<row r>, pred_token_ids=x[r:r+1, :len_r], max_time_steps=len_r,
+        return_logprobs=True)[1] reports for that row alone, bit for bit.  pred_lengths: as in generate (len_r whole
+        time steps of row r are real, the rest is never read); positions past a row's length hold 0.
+        The rows' prompts are packed back to back without padding into forwards of at most max_rows rows each (a prompt
+        longer than that runs alone), on the varlen kernels of Engine.forward_packed (score.py).  There is no decode
+        state, so no row limit.  Eval semantics whatever the module's mode; no random draw, Engine.seed untouched.
+        Every id must lie in its sequence's codebook [0, codebook_size); a wrong count or shape, an id outside it, a
+        bad pred_lengths or a max_rows that is not an int >= 1 raises ValueError, and with absolute position
+        embeddings a sequence longer than max_absolute_position_embeddings raises IndexError, before any device work."""
+        from .score import score_batch
+        return score_batch(self, conditioning_token_ids, pred_token_ids, pred_lengths, max_rows)
 
     def forward(self, *, all_token_ids: List[torch.Tensor], return_loss: bool = False, **kwargs):
         """open_musiclm.py:328-411.  return_loss=True: (loss, None, None) with the loss computed by the fused path

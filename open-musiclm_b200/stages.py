@@ -119,6 +119,11 @@ class SemanticStage(_Stage):
             semantic_token_ids = self.wav2vec(raw_wave_for_semantic, flatten=False)
         return self.transformer_wrapper.forward(all_token_ids=[clap_token_ids, semantic_token_ids], return_loss=return_loss, **kwargs)
 
+    def score(self, *, clap_token_ids, semantic_token_ids, pred_lengths=None, max_rows=16384):
+        """TokenConditionedTransformerWrapper.score of semantic tokens [b, t] or [b, t, 1] given clap ids."""
+        return self.transformer_wrapper.score(conditioning_token_ids=[clap_token_ids], pred_token_ids=semantic_token_ids,
+                                              pred_lengths=pred_lengths, max_rows=max_rows)
+
 
 class CoarseStage(_Stage):
     """open_musiclm.py:606-716: clap + semantic tokens -> coarse acoustic tokens."""
@@ -148,6 +153,11 @@ class CoarseStage(_Stage):
         return self.transformer_wrapper.forward(all_token_ids=[clap_token_ids, semantic_token_ids, coarse_token_ids],
                                                 return_loss=return_loss, **kwargs)
 
+    def score(self, *, clap_token_ids, semantic_token_ids, coarse_token_ids, pred_lengths=None, max_rows=16384):
+        """TokenConditionedTransformerWrapper.score of coarse tokens [b, t, q] given clap ids and semantic tokens."""
+        return self.transformer_wrapper.score(conditioning_token_ids=[clap_token_ids, semantic_token_ids], pred_token_ids=coarse_token_ids,
+                                              pred_lengths=pred_lengths, max_rows=max_rows)
+
 
 class FineStage(_Stage):
     """open_musiclm.py:719-814: clap + coarse tokens -> fine acoustic tokens."""
@@ -176,6 +186,11 @@ class FineStage(_Stage):
     def forward(self, *, clap_token_ids, coarse_token_ids, fine_token_ids, return_loss=False, **kwargs):
         return self.transformer_wrapper.forward(all_token_ids=[clap_token_ids, coarse_token_ids, fine_token_ids],
                                                 return_loss=return_loss, **kwargs)
+
+    def score(self, *, clap_token_ids, coarse_token_ids, fine_token_ids, pred_lengths=None, max_rows=16384):
+        """TokenConditionedTransformerWrapper.score of fine tokens [b, t, q] given clap ids and coarse tokens."""
+        return self.transformer_wrapper.score(conditioning_token_ids=[clap_token_ids, coarse_token_ids], pred_token_ids=fine_token_ids,
+                                              pred_lengths=pred_lengths, max_rows=max_rows)
 
 
 def _windows(tokens: torch.Tensor, size: int, step: int):
@@ -472,6 +487,41 @@ class MusicLM(nn.Module):
             name = STREAMS[job.stage]
             streams[name] = out if name not in streams else torch.cat([streams[name], out[:, job.drop:]], 1)
         return song_output(plan, streams, return_all)
+
+    @torch.no_grad()
+    def score_tokens(self, *, clap_token_ids, semantic_token_ids, coarse_token_ids, fine_token_ids=None, output_seconds=8,
+                     semantic_window_seconds=10, coarse_window_seconds=4, fine_window_seconds=2, semantic_steps_per_second=50,
+                     acoustic_steps_per_second=75, semantic_sliding_window_step_percent=0.5, coarse_sliding_window_step_percent=0.5,
+                     fine_sliding_window_step_percent=1, prime_semantic_token_ids=None, prime_coarse_token_ids=None,
+                     prime_fine_token_ids=None, coarse_only=False, max_rows=16384):
+        """The model's log p of every generated token of given songs, each scored in the window of plan_song that
+        appended it to its stream: (semantic, coarse, fine) float32 scores shaped like the given streams (fine None
+        with coarse_only).  The streams are those generate_tokens(..., return_all=True) returns (semantic, coarse,
+        fine), with the window keywords and primes of that call; with coarse_only the coarse stream is the one
+        generate_tokens(coarse_only=True) returns (the semantic stream as above).  A batch of songs is tensors [b, ...]
+        of equal length (output_seconds one value), or lists of [1, ...] tensors, one per song (output_seconds one
+        value or one per song; primes a tensor [1 or b, ...] or a list with one tensor or None per song); lists of
+        songs come back as lists.
+        For window job j of a song, its scored tokens are those its generate call sampled, and their values are bit
+        for bit the logprobs of stage.generate(conditioning=<j's clap ids and cond slice>, pred_token_ids=<j's prefix,
+        then those tokens>, max_time_steps=<that length>, return_logprobs=True) for that song alone (score.song_rows).
+        Every generated token is scored once; prime tokens, including the prime steps a first window copies into its
+        stream, hold 0.  Each stage runs its windows of every song through packed forwards of at most max_rows rows
+        (TokenConditionedTransformerWrapper.score); no stage waits for another.  Temperature, top-k and top-p do not
+        enter (the model's log p).  Streams whose lengths differ from what the plan gives, a prime too short for the
+        crop generate_tokens applies to a stream, ids outside a codebook, or arguments plan_song refuses raise
+        ValueError before anything runs."""
+        from .score import score_songs
+        return score_songs(self, clap_token_ids=clap_token_ids, semantic_token_ids=semantic_token_ids, coarse_token_ids=coarse_token_ids,
+                           fine_token_ids=fine_token_ids, output_seconds=output_seconds,
+                           windowing=dict(semantic_window_seconds=semantic_window_seconds, coarse_window_seconds=coarse_window_seconds,
+                                          fine_window_seconds=fine_window_seconds, semantic_steps_per_second=semantic_steps_per_second,
+                                          acoustic_steps_per_second=acoustic_steps_per_second,
+                                          semantic_sliding_window_step_percent=semantic_sliding_window_step_percent,
+                                          coarse_sliding_window_step_percent=coarse_sliding_window_step_percent,
+                                          fine_sliding_window_step_percent=fine_sliding_window_step_percent),
+                           primes=(prime_semantic_token_ids, prime_coarse_token_ids, prime_fine_token_ids), coarse_only=coarse_only,
+                           max_rows=max_rows)
 
     def prime_token_ids(self, prime_wave: torch.Tensor, prime_wave_sample_hz, semantic_window_seconds=10):
         """A [channels, n] prime wave -> the prime_{semantic,coarse,fine}_token_ids of generate_tokens (batch 1), through
