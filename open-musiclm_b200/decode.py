@@ -88,7 +88,7 @@ class _PromptCapture:
 
 def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
     """B per-sequence seeds (ints, taken modulo 2^64, or an int64 tensor read as raw 64-bit patterns) as an int64
-    device tensor of those bit patterns."""
+    device tensor of those bit patterns, sent in a non-blocking copy as row_arrays sends its arrays."""
     if isinstance(seeds, torch.Tensor):
         if seeds.dtype != torch.int64:
             raise ValueError(f"open_musiclm_b200 generate: seeds must be an int64 tensor or a list of ints, not {seeds.dtype}")
@@ -98,7 +98,7 @@ def seeds_tensor(seeds, B: int, device) -> torch.Tensor:
     if len(vals) != B:
         raise ValueError(f"open_musiclm_b200 generate: {len(vals)} seeds for {B} sequences")
     vals = [v & 0xFFFFFFFFFFFFFFFF for v in vals]
-    return torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in vals], dtype=torch.int64, device=device)
+    return torch.tensor([v - (1 << 64) if v >= 1 << 63 else v for v in vals], dtype=torch.int64).to(device, non_blocking=True)
 
 
 def check_top_p(top_p, where: str = "generate"):

@@ -7,6 +7,10 @@ start while semantic windows remain, fine windows while coarse windows remain, a
 song run side by side.  A seeded session row is bit for bit `generate` with that row alone and its seed, and every
 job's seed is window_seed(song seed, stage, window), so each song is bit for bit `generate_tokens(seeds=[seed])` for
 that song alone, whatever else runs beside it (DESIGN section 4, "Song sessions").
+
+Each stage runs on a CUDA stream of its own, so the three stages' decode steps overlap on the GPU.  Within one time
+step they share no data: a window reads another stage's stream only after that window has finished, and events order
+those reads (DESIGN section 4, "Song sessions on three streams").
 """
 import numbers
 import sys
@@ -32,15 +36,16 @@ class _Song:
     how much of each generated stream is written from its start (`done`) and which written pieces lie beyond that,
     the next job of each stage to submit, the jobs not yet finished, and the output rows handed out so far."""
 
-    def __init__(self, handle, plan, clap, primes):
-        self.handle, self.plan, self.clap, self.primes = handle, plan, clap, primes
+    def __init__(self, handle, plan, clap, primes, given):
+        self.handle, self.plan, self.clap, self.primes, self.given = handle, plan, clap, primes, given
         self.streams = dict(primes)
         self.done = {name: 0 for name in STREAMS}
         self.pieces = {name: {} for name in STREAMS}
         self.by_stage = [[j for j in plan.jobs if j.stage == s] for s in (SEMANTIC, COARSE, FINE)]
         self.next = [0, 0, 0]
         self.left = len(plan.jobs)
-        self.sent = 0
+        self.sent = 0                  # output rows known to be final
+        self.handed = 0                # output rows handed out by ready()
 
     def write(self, job, tokens):
         """A finished job's tokens [steps, q] -> its stream."""
@@ -112,7 +117,15 @@ class MusicLMSession:
     windows that finished into their songs' streams and adds the jobs they unblock.  `ready` hands out, per song, the
     rows of its output tensor (the acoustic tokens [1, T, coarse + fine quantizers], or the coarse stream with
     coarse_only) that became final since the last call; the prime's rows are final at once.  Concatenated, a song's
-    rows are its `finished` output's first tensor.  Songs are seeded; there is no noise stream."""
+    rows are its `finished` output's first tensor.  Songs are seeded; there is no noise stream.
+
+    Streams: every stage's device work (its session's adds, steps, prefills and graph replays, and the writes of its
+    windows into the songs' streams) runs on `streams[stage]`, a CUDA stream the session owns on that stage's device.
+    Events order the rest, and `step` never waits for the device once the stage sessions have captured their graphs:
+    a stage stream waits on the caller's current stream before it reads what the caller passed to `add`, and on a
+    stage's `written` event (recorded after that stage's writes) before a window reads that stage's stream; `ready` and
+    `finished` make the caller's current stream wait on every stage's event, so what they return is usable on it as
+    is.  Tensors used on a stream other than the one they were allocated on are recorded on it (record_stream)."""
 
     def __init__(self, musiclm, slots=64, *, semantic_window_seconds=10, coarse_window_seconds=4, fine_window_seconds=2,
                  semantic_steps_per_second=50, acoustic_steps_per_second=75, semantic_sliding_window_step_percent=0.5,
@@ -153,12 +166,48 @@ class MusicLMSession:
                               _positions([self.clap_length, fwin * self.qc], fwin, self.qf))
         self.sessions = [GenerationSession(st.transformer_wrapper, slots=int(n), max_positions=p, max_queue=sys.maxsize)
                          for st, n, p in zip(stages, slots, self.max_positions)]
+        # one stream per stage (None on a CPU device); each starts after the caller's work so far, such as weight updates
+        self.streams = [torch.cuda.Stream(d) if torch.device(d).type == "cuda" else None for d in self.devices]
+        self.written = [torch.cuda.Event() if s is not None else None for s in self.streams]
+        for s in self.streams:
+            if s is not None:
+                s.wait_stream(torch.cuda.current_stream(s.device))
         self._next_handle = 0
         self._songs = {}               # handle -> _Song in flight, in admission order
-        self._queue = deque()          # (handle, plan, clap, primes) waiting for room
+        self._queue = deque()          # (handle, plan, claps, primes, given) waiting for room
         self._jobs = [{}, {}, {}]      # per stage: request handle -> (song, job)
-        self._ready = {}               # handle -> list of row tensors not handed out yet
-        self._done = {}
+        self._ready = {}               # handle -> _Song with final rows not handed out yet
+        self._done = {}                # handle -> finished _Song
+
+    # ------------------------------------------------------------------------------------------------ streams
+    def _caller_event(self):
+        """An event on the caller's current stream, after the work it enqueued so far (None without a GPU stage)."""
+        if not any(self.streams):
+            return None
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream())
+        return ev
+
+    def _wait_writes(self):
+        """The caller's current stream waits on every stage's writes so far; returns it (None without a GPU stage)."""
+        if not any(self.streams):
+            return None
+        cur = torch.cuda.current_stream()
+        for ev in self.written:
+            if ev is not None:
+                cur.wait_event(ev)
+        return cur
+
+    @staticmethod
+    def _record_on(cur, songs):
+        """`ready` and `finished` read the songs' streams on the caller's stream: as slices they hand out and as inputs
+        of the concatenations they make there.  Every stream buffer of those songs (generated ones, allocated on a
+        stage stream, and the primes) is recorded on it, so that no stage stream reuses a buffer before the caller's
+        reads are done, whether or not the caller keeps a view of it."""
+        if cur is not None:
+            for song in songs:
+                for t in song.streams.values():
+                    t.record_stream(cur)
 
     # ------------------------------------------------------------------------------------------------ songs
     def add(self, *, clap_token_ids, seed, output_seconds=8, top_p=None, prime_semantic_token_ids=None,
@@ -196,37 +245,65 @@ class MusicLMSession:
                              f"holds {len(self._queue)} of max_queue = {self.max_queue}")
         handle = self._next_handle
         self._next_handle += 1
+        # on the caller's stream: the clap ids on every stage's device and the primes on theirs, then an event that
+        # the stage streams wait on before they read them
+        claps = [clap_token_ids.to(d, torch.int64) for d in self.devices]
         primes = dict(zip(("prime_semantic", "prime_coarse", "prime_fine"),
                           (t.to(d, torch.int64) for t, d in zip(primes, self.devices)))) if primed else {}
-        self._queue.append((handle, plan, clap_token_ids, primes))
+        self._queue.append((handle, plan, claps, primes, self._caller_event()))
         self._admit()
         return handle
 
     def _admit(self):
         while self._queue and len(self._songs) < self.max_songs:
-            handle, plan, clap, primes = self._queue.popleft()
-            song = _Song(handle, plan, clap, primes)
+            handle, plan, claps, primes, given = self._queue.popleft()
+            song = _Song(handle, plan, claps, primes, given)
             q = (1, self.qc, self.qf)
             for s, name in enumerate(STREAMS):
                 if plan.length[name]:
-                    song.streams[name] = torch.empty(1, plan.length[name], q[s], device=self.devices[s], dtype=torch.int64)
+                    # allocated on the stage stream that writes it; recorded on every other stream that reads it
+                    with torch.cuda.stream(self.streams[s]):
+                        song.streams[name] = torch.empty(1, plan.length[name], q[s], device=self.devices[s], dtype=torch.int64)
             self._songs[handle] = song
             self._emit(song)
             self._submit(song)
 
     def _submit(self, song):
         for job in song.runnable():
-            cond = song.part(job.cond)
-            h = self.sessions[job.stage].add(conditioning_token_ids=[song.clap] + ([cond] if cond is not None else []),
-                                             pred_token_ids=song.part(job.prefix), seed=job.seed, max_time_steps=job.max_time_steps,
-                                             temperature=job.temperature, top_p=job.top_p)
-            self._jobs[job.stage][h] = (song, job)
+            s = job.stage
+            with torch.cuda.stream(self.streams[s]):
+                self._wait_inputs(song, job)
+                cond = song.part(job.cond)
+                h = self.sessions[s].add(conditioning_token_ids=[song.clap[s]] + ([cond] if cond is not None else []),
+                                         pred_token_ids=song.part(job.prefix), seed=job.seed, max_time_steps=job.max_time_steps,
+                                         temperature=job.temperature, top_p=job.top_p)
+            self._jobs[s][h] = (song, job)
+
+    def _wait_inputs(self, song, job):
+        """Orders a job's reads on its stage stream: after the caller's `add` (clap ids, primes) and after the writes of
+        the stage whose stream it reads; those tensors are recorded on the stage stream, whose reads may outlast the
+        caller's and the producer's references."""
+        st = self.streams[job.stage]
+        if st is None:
+            return
+        if song.given is not None:
+            st.wait_event(song.given)
+        song.clap[job.stage].record_stream(st)
+        for ref in (job.cond, job.prefix):
+            if ref is None:
+                continue
+            src = STREAMS.index(ref[0]) if ref[0] in STREAMS else None
+            if src != job.stage:
+                if src is not None:
+                    st.wait_event(self.written[src])
+                song.streams[ref[0]].record_stream(st)
 
     def _emit(self, song):
-        """Queues the song's output rows that became final since the last call for `ready`."""
+        """Marks the song's output rows that became final since the last call for `ready` (host bookkeeping: `ready`
+        slices them on the caller's stream)."""
         n = song.final_rows()
         if n > song.sent:
-            self._ready.setdefault(song.handle, []).append(song.rows(song.sent, n))
+            self._ready[song.handle] = song
             song.sent = n
 
     @property
@@ -237,32 +314,50 @@ class MusicLMSession:
     def step(self):
         """One time step of every stage session with work; then the windows that finished go into their songs'
         streams, the jobs they unblock are added, and finished songs make room for queued ones."""
-        for sess in self.sessions:
+        for stage, sess in enumerate(self.sessions):
             if not sess.idle:
-                sess.step()
+                with torch.cuda.stream(self.streams[stage]):
+                    sess.step()
         touched = {}
         for stage, sess in enumerate(self.sessions):
-            for h, tokens in sess.finished().items():
-                song, job = self._jobs[stage].pop(h)
-                song.write(job, tokens)
-                touched[song.handle] = song
+            done = sess.finished()
+            if not done:
+                continue
+            with torch.cuda.stream(self.streams[stage]):
+                for h, tokens in done.items():
+                    song, job = self._jobs[stage].pop(h)
+                    song.write(job, tokens)
+                    touched[song.handle] = song
+                if self.written[stage] is not None:
+                    self.written[stage].record(self.streams[stage])
         for song in sorted(touched.values(), key=lambda s: s.handle):
             self._emit(song)
             if song.left:
                 self._submit(song)
                 continue
             del self._songs[song.handle]
-            self._done[song.handle] = song_output(song.plan, song.streams, True)
+            self._done[song.handle] = song
         self._admit()
 
     def ready(self):
         """{handle: [1, t, q] rows} of each song's output tensor that became final since the last call, in order."""
-        out = {h: torch.cat(r, 1) if len(r) > 1 else r[0] for h, r in self._ready.items()}
+        if not self._ready:
+            return {}
+        cur = self._wait_writes()
+        out = {h: song.rows(song.handed, song.sent) for h, song in self._ready.items()}
+        for song in self._ready.values():
+            song.handed = song.sent
+        self._record_on(cur, self._ready.values())
         self._ready = {}
         return out
 
     def finished(self):
         """{handle: output} of the songs that finished since the last call: exactly
         generate_tokens(..., seeds=[seed], return_all=True) for that song alone."""
-        done, self._done = self._done, {}
-        return done
+        if not self._done:
+            return {}
+        cur = self._wait_writes()
+        out = {h: song_output(song.plan, song.streams, True) for h, song in self._done.items()}
+        self._record_on(cur, self._done.values())
+        self._done = {}
+        return out

@@ -523,16 +523,19 @@ class GenerationSession:
             self._pack_ws = eng.packed_workspace(self._pack_rows, self._pack_rows if self.logprob else self.slots)
         for group in split_joiners([r.chunk[1] for r in rows], self._pack_rows):
             self._prefill_packed([rows[i] for i in group])
-        idx = torch.tensor([r.slot for r in rows], device=dev)
         states = [r.device_state() if r.prefilled else dict(pos=r.filled, pos_last=r.filled, pos_offset=-r.filled) for r in rows]
-        vals = row_arrays(dev, len(rows), pos=[s["pos"] for s in states], pos_last=[s["pos_last"] for s in states],
-                          pos_offset=[s["pos_offset"] for s in states], t=0, n=[r.n if r.prefilled else 0 for r in rows],
-                          top_k=[r.payload["top_k"] for r in rows], temperature=[r.payload["temperature"] for r in rows],
-                          top_p=[r.payload["top_p"] for r in rows])
+        vals = row_arrays(dev, len(rows), slot=[r.slot for r in rows], pos=[s["pos"] for s in states],
+                          pos_last=[s["pos_last"] for s in states], pos_offset=[s["pos_offset"] for s in states], t=0,
+                          n=[r.n if r.prefilled else 0 for r in rows], top_k=[r.payload["top_k"] for r in rows],
+                          temperature=[r.payload["temperature"] for r in rows], top_p=[r.payload["top_p"] for r in rows])
+        idx = vals["slot"].long()
         for name, dst in (("pos", dec.pos), ("pos_last", dec.pos_last), ("pos_offset", dec.pos_offset), ("t", dec.t), ("n", dec.n_rows),
                           ("top_k", dec.top_k), ("temperature", dec.temperature)):
             dst[idx] = vals[name]
-        dec.top_p[idx] = vals["top_p"] if vals["top_p"] is not None else 1.0
+        if vals["top_p"] is not None:
+            dec.top_p[idx] = vals["top_p"]
+        else:                                   # not dec.top_p[idx] = 1.0: a Python scalar goes up in a blocking copy
+            dec.top_p.index_fill_(0, idx, 1.0)
         dec.seeds[idx] = seeds_tensor([r.payload["seed"] for r in rows], len(rows), dev)
 
     def _prefill_packed(self, rows):
