@@ -130,7 +130,8 @@ int omlm_attn_bwd_tc_det_workspace(int B, int N, int heads, long* ws_bytes, long
  * predicted sequence's last token (:356); mask_cond masks + zeroes conditioning pad/eos ids
  * (:358-367).  Per position: row of the concatenated embedding table (offset = codebook_size *
  * (t mod q) added BEFORE the pad test, open_musiclm.py:126-133, utils.py:133-138; -1 = zero row;
- * start tokens are extra rows) and the key mask (AND mask_in AND forget_keep when given, :373-376).
+ * start tokens are extra rows) and the key mask: the conditioning pad/eos mask of mask_cond (1 elsewhere), or mask_in
+ * instead when given (a self_attn_mask passed to the transformer itself, [B, N]), AND forget_keep when given (:373-376).
  *   ids[s]: int64 [B, len[s]] device pointers (host array of n_seqs pointers)
  *   ids_out int64 [B, sum n_tok]; src_row int32 [B, N]; key_mask u8 [B, N]; labels int32 [B, sum(len+eos)] or NULL.
  *   err_flag (device int, optional): bit s is set when sequence s holds an id outside its embedding table (where

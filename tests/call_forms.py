@@ -1,13 +1,16 @@
 """The engine's phases for the call-form inventories (test_gemm_reference_gpu.py, test_norm_loss_reference_gpu.py,
-test_attention_ffn_call_forms_gpu.py): one driver that runs training steps, eval_loss, generate and generation
-sessions inside a recorder, so that every inventory sees the same calls.
+test_attention_ffn_call_forms_gpu.py, test_sampler_token_call_forms_gpu.py) and the entry-point ledger
+(test_entry_points_gpu.py): one driver that runs training steps, eval_loss, generate, scoring, generation sessions and
+song sessions inside a recorder, so that every inventory sees the same calls.
 
 A recorder is any object with a `phase` attribute; run() sets it before each phase, and the recorder files every call
 it sees under the current phase.  Recorders read no device memory: generate and sessions capture CUDA graphs.
 
 Models (MODELS): "d72" (d = 72, h = 3, codebooks whose C = 101 / 65 are not multiples of 64), "cfg2_depth1" (the
-cfg2 layer dims at depth 1, h = 8) and "cfg2_h16" (d = 1024, h = 16, whose chunk unit U = 128 / gcd(h, 128) is 8; the
-session phases only)."""
+cfg2 layer dims at depth 1, h = 8), "d72_abspos" (d72 with absolute position embeddings: their rows in the
+embedding gathers and the decode step), "cfg2_h16" (d = 1024, h = 16, whose chunk unit U = 128 / gcd(h, 128) is 8; the
+session and score phases only) and "musiclm_prime" (the three stages of tests/golden/musiclm_prime.pt; song sessions
+and song scoring only)."""
 import math
 
 import torch
@@ -18,22 +21,33 @@ MODELS = {
                  num_clap_quantizers=4, num_coarse_quantizers=3), [(4,), (11,)], (10, 3), 64),
     "cfg2_depth1": (dict(dim=1024, depth=1, heads=8, num_coarse_quantizers=3), [(12,), (197,)], (270, 3), 1024),
     "cfg2_h16": (dict(dim=1024, depth=1, heads=16, num_coarse_quantizers=3), [(12,), (197,)], (270, 3), 1024),
+    "d72_abspos": (dict(dim=72, depth=1, heads=3, clap_codebook_size=100, semantic_codebook_size=100, acoustic_codebook_size=64,
+                        num_clap_quantizers=4, num_coarse_quantizers=3, use_absolute_position_embeddings=True,
+                        max_absolute_position_embeddings=320), [(4,), (11,)], (10, 3), 64),
 }
 SESSIONS_ONLY = {"cfg2_h16"}
+SONGS_ONLY = {"musiclm_prime"}
+MODEL_KEYS = list(MODELS) + sorted(SONGS_ONLY)
 
 # (phase, deterministic, frozen): "norms" freezes the LayerNorm gammas and the q/k scales, "relpos" the relative-position
 # MLP (the attention backward then forms no bias gradient)
 TRAIN_PHASES = [("default step", False, None), ("deterministic step", True, None), ("frozen norms step", False, "norms"),
                 ("frozen norms deterministic step", True, "norms"), ("frozen relpos step", False, "relpos"),
                 ("frozen relpos deterministic step", True, "relpos")]
-GENERATE_PHASES = ["generate B=3", "generate B=20"]
-SESSION_PHASES = ["session join", "session chunked", "session logprobs"]
+GENERATE_PHASES = ["generate B=3", "generate B=20", "generate sampling"]
+SCORE_PHASES = ["score"]
+SESSION_PHASES = ["session join", "session chunked", "session logprobs", "session sampling"]
+SONG_PHASES = ["song session", "score songs"]
+SCORE_MODELS = {"d72", "d72_abspos", "cfg2_h16"}
 
 
 def phases(model):
+    if model in SONGS_ONLY:
+        return list(SONG_PHASES)
+    score = SCORE_PHASES if model in SCORE_MODELS else []
     if model in SESSIONS_ONLY:
-        return list(SESSION_PHASES)
-    return [p for p, _, _ in TRAIN_PHASES] + ["eval_loss"] + GENERATE_PHASES + SESSION_PHASES
+        return score + SESSION_PHASES
+    return [p for p, _, _ in TRAIN_PHASES] + ["eval_loss"] + GENERATE_PHASES + score + SESSION_PHASES
 
 
 def unit(heads):
@@ -62,6 +76,57 @@ def _session_requests(g, cond_n, vocab, q, long_cond, n_req, prefixes):
     return reqs
 
 
+def _sampling_requests(g, cond_n, vocab, q, n_req):
+    """Requests with their own filter_thres, temperature and top_p (None, 1.0 and nuclei), some with prefixes."""
+    reqs = _session_requests(g, cond_n, vocab, q, cond_n[1][0], n_req, prefixes=True)
+    for i, r in enumerate(reqs):
+        r.update(filter_thres=(0.9, 0.5, 0.99, 0.0)[i % 4], temperature=(1.0, 0.7, 1.3)[i % 3], top_p=(None, 1.0, 0.9, 0.5, 0.75)[i % 5])
+    return reqs
+
+
+def _score(w, rec, g, cond_n, vocab, q):
+    """TokenConditionedTransformerWrapper.score twice: with max_rows small enough that first-fit decreasing makes several
+    forwards (the longest prompt, past max_rows, alone), and with the default max_rows (24 prompts in one forward).
+    The two calls have semantic conditioning of different lengths; prefixes from 0 to 40 time steps."""
+    rec.phase = "score"
+    T = 40
+    for B, n_sem, max_rows in ((7, cond_n[1][0], None), (24, max(2, cond_n[1][0] - 37), 16384)):
+        cond = [torch.randint(0, min(vocab, 64), (B,) + cond_n[0], generator=g).cuda(),
+                torch.randint(0, min(vocab, 64), (B, n_sem), generator=g).cuda()]
+        pred = torch.randint(0, min(vocab, 64), (B, T, q), generator=g).cuda()
+        lens = [(T, 0, 1, 13, 5, 22, 29)[b % 7] for b in range(B)]
+        rows = sum(c[0] + 2 for c in cond_n[:1]) + n_sem + 2 + 1
+        kw = dict(max_rows=rows + 17 * q + 1) if max_rows is None else dict(max_rows=max_rows)
+        w.score(conditioning_token_ids=cond, pred_token_ids=pred, pred_lengths=lens, **kw)
+    torch.cuda.synchronize()
+
+
+def _songs(rec):
+    """A MusicLMSession over a stream of songs (primes, per-stage top_p, coarse_only), then MusicLM.score_tokens on
+    the songs it finished with all three stages, with a small max_rows and with the default."""
+    import random
+    import open_musiclm_b200 as O
+    import test_musiclm_session_gpu as TM
+    mlm = TM.h100_musiclm(TM.load()[1])
+    rng, g = random.Random(3), torch.Generator().manual_seed(3)
+    songs = TM.song_args(rng, g, 8, 4, 64, 3, 5, [2, 3, 4.5], [(9, 7), (3, 2)])
+    for i, s in enumerate(songs):
+        s["coarse_only"] = i % 4 == 1
+    rec.phase = "song session"
+    sess = O.MusicLMSession(mlm, slots=6, max_songs=4, max_queue=len(songs), **TM.FIX_WIN)
+    res = TM.run_stream(sess, songs, rng)
+    torch.cuda.synchronize()
+    full = [r for r in res.values() if not r["args"]["coarse_only"]]
+    rec.phase = "score songs"
+    pk = ("prime_semantic_token_ids", "prime_coarse_token_ids", "prime_fine_token_ids")
+    args = dict(clap_token_ids=[r["args"]["clap_token_ids"] for r in full], semantic_token_ids=[r["out"][1] for r in full],
+                coarse_token_ids=[r["out"][2] for r in full], fine_token_ids=[r["out"][3] for r in full],
+                output_seconds=[r["args"]["output_seconds"] for r in full], **{k: [r["args"].get(k) for r in full] for k in pk})
+    for max_rows in (64, 16384):
+        mlm.score_tokens(max_rows=max_rows, **args, **TM.FIX_WIN)
+    torch.cuda.synchronize()
+
+
 def _run_session(w, rec, phase, reqs, **kw):
     import open_musiclm_b200 as O
     rec.phase = phase
@@ -79,6 +144,8 @@ def run(rec, model, act16, monkeypatch):
     import open_musiclm_b200 as O
     monkeypatch.setenv("OMLM_ACT16", act16)
     torch.manual_seed(0)
+    if model in SONGS_ONLY:
+        return _songs(rec)
     kw, cond_n, pred_shape, vocab = MODELS[model]
     g = torch.Generator().manual_seed(1)
 
@@ -121,7 +188,19 @@ def run(rec, model, act16, monkeypatch):
             pred = torch.randint(0, min(vocab, 64), (B, 4, q), generator=g).cuda()
             w.generate(conditioning_token_ids=cond, pred_token_ids=pred, pred_lengths=[1 + b % 4 for b in range(B)], max_time_steps=7)
             torch.cuda.synchronize()
+        # the sampler's noise sources and modes: supplied uniforms, a scalar top_p, the shared Philox stream, per-row seeds
+        # with log-probabilities
+        rec.phase = "generate sampling"
+        B, steps = 3, 4
+        C1 = w.token_sequences[-1].codebook_size + 1
+        cond = [torch.randint(0, min(vocab, 64), (B,) + s, generator=g).cuda() for s in cond_n]
+        uni = torch.rand(steps * q, B, C1, generator=g).clamp_(1e-6, 1 - 1e-6)
+        for extra in (dict(uniform_noise=uni), dict(top_p=0.8), dict(), dict(seeds=[5, 6, 7], return_logprobs=True, top_p=0.9)):
+            w.generate(conditioning_token_ids=cond, max_time_steps=steps, **extra)
+        torch.cuda.synchronize()
     U = unit(kw["heads"])
+    if model in SCORE_MODELS:
+        _score(w, rec, g, cond_n, vocab, q)
     long_cond = max(cond_n[1][0], 2 * U + 37)      # prompts of several units, so that the chunked sessions split them
     _run_session(w, rec, "session join", _session_requests(g, cond_n, vocab, q, long_cond, 5, prefixes=True))
     _run_session(w, rec, "session chunked", _session_requests(g, cond_n, vocab, q, long_cond, 5, prefixes=False), prefill_rows=U)
@@ -130,3 +209,6 @@ def run(rec, model, act16, monkeypatch):
     lp_cond = 2 * U - 30 if U >= 64 else long_cond
     _run_session(w, rec, "session logprobs", _session_requests(g, cond_n, vocab, q, lp_cond, 5, prefixes=True), prefill_rows=2 * U,
                  return_logprobs=True)
+    reqs = _sampling_requests(g, cond_n, vocab, q, 10)
+    _run_session(w, rec, "session sampling", reqs[:5])
+    _run_session(w, rec, "session sampling", reqs[5:], return_logprobs=True)

@@ -22,7 +22,9 @@ def test_attention_keys_on_hand_made_forms():
     assert T.attn_key(3, 50, True, 50) == ("attn_fwd_tc", 3, (True, False, False, False), True, False)
     assert T.attn_key(8, 1024, False, 1100, det=True, dtable_null=True) == \
         ("attn_bwd_tc", 8, (False, True, True, False), False, True, True, True)
-    assert T.varlen_keys(8, [1, 16, 300]) == {("attn_fwd_tc_varlen", 8, True), ("attn_fwd_tc_varlen", 8, False)}
+    assert T.varlen_keys(8, [1, 16, 300]) == {("attn_fwd_tc_varlen", 8, True), ("attn_fwd_tc_varlen", 8, False),
+                                              ("attn_fwd_tc_varlen", 8, "sequences > 16", False)}
+    assert ("attn_fwd_tc_varlen", 8, "sequences > 16", True) in T.varlen_keys(8, [20] * 17)
     # h = 3: U = 128; one chunk at p0 = 0, one short final chunk at p0 = 128 (on the 64 grid), the cache 512 rows a slot
     keys = T.chunk_keys(3, [(0, 128, 0), (128, 30, 512)], 1024)
     assert keys == {("attn_fwd_tc_chunk", 3, False, False, False, True), ("attn_fwd_tc_chunk", 3, True, True, False, True)}

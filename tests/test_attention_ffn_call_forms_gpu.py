@@ -53,8 +53,9 @@ def attn_key(h, N, mask, table_ld, det=None, dtable_null=None):
 
 
 def varlen_keys(h, lens):
-    """attn_fwd_tc_varlen: per sequence, whether it is shorter than one chunk unit U."""
-    return {("attn_fwd_tc_varlen", h, n < call_forms.unit(h)) for n in lens}
+    """attn_fwd_tc_varlen: per sequence, whether it is shorter than one chunk unit U; per launch, whether it packs more
+    than 16 sequences (as scoring does)."""
+    return {("attn_fwd_tc_varlen", h, n < call_forms.unit(h)) for n in lens} | {("attn_fwd_tc_varlen", h, "sequences > 16", len(lens) > 16)}
 
 
 def chunk_keys(h, seqs, kv_rows):
@@ -113,7 +114,7 @@ def covered_keys():
     for B, N, h, mask, _, _ in TA.EXACT_CASES:
         keys.add(attn_key(h, N, mask, N))
         keys |= {attn_key(h, N, mask, N, det, null) for det in (False, True) for null in (False, True)}
-    for h, lens in TP.ATTN_LENS.items():
+    for h, lens in list(TP.ATTN_LENS.items()) + list(TP.ATTN_LENS_MANY.items()):
         keys |= varlen_keys(h, lens)
     for h, N in TC.CHUNK_ATTN:
         chunks = TC.chunk_attn_chunks(h, N)
@@ -249,14 +250,22 @@ def _record(act16, model, monkeypatch):
     from open_musiclm_b200 import lib
     with _Recorder(lib) as rec:
         call_forms.run(rec, model, act16, monkeypatch)
-    expected = {(p, "attn_fwd_tc_chunk") for p in call_forms.SESSION_PHASES} | \
-        {(p, n) for p in call_forms.SESSION_PHASES for n in ("attn_decode_mqa", "decode_conv_geglu", "ffn_norm_fwd")} | \
-        {("session join", "gemm_ffn_up_varlen"), ("session chunked", "gemm_ffn_up_chunk"), ("session logprobs", "gemm_ffn_up_chunk")}
-    if model not in call_forms.SESSIONS_ONLY:
+    if model in call_forms.SONGS_ONLY:
+        expected = {("song session", n) for n in ("attn_decode_mqa", "decode_conv_geglu", "ffn_norm_fwd")} | \
+            {("score songs", n) for n in ("attn_fwd_tc_varlen", "gemm_ffn_up_varlen", "ffn_norm_fwd")}
+    else:
+        expected = {(p, "attn_fwd_tc_chunk") for p in call_forms.SESSION_PHASES} | \
+            {(p, n) for p in call_forms.SESSION_PHASES for n in ("attn_decode_mqa", "decode_conv_geglu", "ffn_norm_fwd")} | \
+            {("session join", "gemm_ffn_up_varlen"), ("session chunked", "gemm_ffn_up_chunk"), ("session logprobs", "gemm_ffn_up_chunk"),
+             ("session sampling", "gemm_ffn_up_varlen")}
+    if model in call_forms.SCORE_MODELS:
+        expected |= {("score", n) for n in ("attn_fwd_tc_varlen", "gemm_ffn_up_varlen", "ffn_norm_fwd")}
+    if model in call_forms.MODELS and model not in call_forms.SESSIONS_ONLY:
         expected |= {(p, n) for p, _, _ in call_forms.TRAIN_PHASES for n in ("attn_fwd_tc", "attn_bwd_tc", "gemm_ffn_up", "ffn_norm_fwd",
                                                                               "ffn_mid_bwd")} | \
             {("eval_loss", "attn_fwd_tc"), ("generate B=3", "attn_decode"), ("generate B=20", "attn_decode_mqa"),
-             ("generate B=3", "decode_conv_geglu"), ("generate B=3", "gemm_ffn_up")}
+             ("generate B=3", "decode_conv_geglu"), ("generate B=3", "gemm_ffn_up"), ("generate sampling", "attn_decode"),
+             ("generate sampling", "attn_decode_mqa")}
     assert expected <= rec.seen, f"entry points the engine did not call through lib: {sorted(expected - rec.seen)}"
     return rec.forms
 
@@ -519,7 +528,7 @@ def _one_per_key(items):
     return out
 
 
-@pytest.mark.parametrize("model", ["d72", "cfg2_depth1", "cfg2_h16"])
+@pytest.mark.parametrize("model", call_forms.MODEL_KEYS)
 @pytest.mark.parametrize("act16", ["fp16", "bf16"])
 def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
     forms = sorted(_record(act16, model, monkeypatch), key=repr)

@@ -1,4 +1,5 @@
-"""Device side of the token pipeline and the checkpoint files: batches gathered in HBM equal the host crops; a trainer
+"""Device side of the token pipeline and the checkpoint files: batches gathered in HBM (omlm_gather_windows) equal the
+host crops; a trainer
 saved in the reference's three-file format (trainer.py:359-391) loads into torch's own AdamW / LinearLR and back."""
 import os
 import random

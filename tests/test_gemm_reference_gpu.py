@@ -11,6 +11,7 @@ explicit matrix below lacks fails the coverage test."""
 import pytest
 import torch
 
+import call_forms
 import gemm_reference as G
 
 pytestmark = pytest.mark.gpu
@@ -581,15 +582,19 @@ class _Recorder:
 
 def _record(act16, model, monkeypatch):
     """Forms of every phase of call_forms: training steps, eval_loss, generate at B <= 16 and B > 16, and sessions."""
-    import call_forms
     with _Recorder(_lib()) as rec:
         call_forms.run(rec, model, act16, monkeypatch)
     # the shim sees the engine only while it calls through lib's attributes: every path must have shown up
-    expected = {(p, "gemm") for p in call_forms.SESSION_PHASES} | {(p, "decode_gemm") for p in call_forms.SESSION_PHASES}
-    if model not in call_forms.SESSIONS_ONLY:
+    if model in call_forms.SONGS_ONLY:
+        expected = {("song session", "gemm"), ("song session", "decode_gemm"), ("score songs", "gemm")}
+    else:
+        expected = {(p, "gemm") for p in call_forms.SESSION_PHASES} | {(p, "decode_gemm") for p in call_forms.SESSION_PHASES}
+    if model in call_forms.SCORE_MODELS:
+        expected.add(("score", "gemm"))
+    if model in call_forms.MODELS and model not in call_forms.SESSIONS_ONLY:
         expected |= {("default step", "gemm"), ("default step", "gemm_rowstat"), ("deterministic step", "gemm"),
                      ("deterministic step", "gemm_splitk_det"), ("generate B=3", "gemm"), ("generate B=3", "skinny_gemm"),
-                     ("generate B=20", "decode_gemm")}
+                     ("generate B=20", "decode_gemm"), ("generate sampling", "skinny_gemm"), ("generate sampling", "decode_gemm")}
     assert expected <= rec.seen, f"entry points the engine did not call through lib: {sorted(expected - rec.seen)}"
     return rec.forms
 
@@ -683,7 +688,7 @@ def _replay_splitk_det(f, gen):
     return ("gemm_splitk_det", str(dt), a_mn, b_mn, bn, (rs > 0) - (rs < 0), nv < N)
 
 
-@pytest.mark.parametrize("model", ["d72", "cfg2_depth1", "cfg2_h16"])
+@pytest.mark.parametrize("model", call_forms.MODEL_KEYS)
 @pytest.mark.parametrize("act16", ["fp16", "bf16"])
 def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
     forms = _record(act16, model, monkeypatch)

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(__file__))
+import call_forms  # noqa: E402
 import norm_loss_reference as R  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -637,13 +638,17 @@ class _Recorder:
 def _record(act16, model, monkeypatch):
     """Forms of every phase of call_forms: default, deterministic, frozen-norm and frozen-relpos steps with pad tokens,
     eval_loss, generate and sessions."""
-    import call_forms
     with _Recorder(_lib()) as rec:
         call_forms.run(rec, model, act16, monkeypatch)
     # sessions: the packed prefill's final norm writes the rows dest_row names; return_logprobs scores the prefixes
-    expected = {(p, n) for p in call_forms.SESSION_PHASES for n in ("layernorm_fwd", "embed_gather")} | \
-        {("session logprobs", "token_logprob")}
-    if model not in call_forms.SESSIONS_ONLY:
+    if model in call_forms.SONGS_ONLY:
+        expected = {(p, n) for p in call_forms.SONG_PHASES for n in ("layernorm_fwd", "embed_gather")} | {("score songs", "token_logprob")}
+    else:
+        expected = {(p, n) for p in call_forms.SESSION_PHASES for n in ("layernorm_fwd", "embed_gather")} | \
+            {("session logprobs", "token_logprob"), ("session sampling", "token_logprob")}
+    if model in call_forms.SCORE_MODELS:
+        expected |= {("score", "layernorm_fwd"), ("score", "embed_gather"), ("score", "token_logprob")}
+    if model in call_forms.MODELS and model not in call_forms.SESSIONS_ONLY:
         expected |= {(p, n) for p in ("default step", "deterministic step") for n in NAMES if n not in ("embed_gather", "token_logprob")} | \
             {("default step", "embed_gather"), ("eval_loss", "cross_entropy"), ("eval_loss", "layernorm_fwd"),
              ("generate B=3", "layernorm_fwd"), ("generate B=3", "embed_gather"), ("frozen norms step", "layernorm_bwd"),
@@ -707,7 +712,7 @@ def _replay(name, f, gen):
     raise AssertionError(name)
 
 
-@pytest.mark.parametrize("model", ["d72", "cfg2_depth1", "cfg2_h16"])
+@pytest.mark.parametrize("model", call_forms.MODEL_KEYS)
 @pytest.mark.parametrize("act16", ["fp16", "bf16"])
 def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
     forms = _record(act16, model, monkeypatch)

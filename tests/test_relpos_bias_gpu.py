@@ -16,6 +16,8 @@ w_hi + a_hi w_lo + a_lo w_hi, fp32 accumulation); forward and backward must be f
        dT: the colsum of dz cancels).  The mutation cases (dropping a_hi w_lo from the forward, a_lo from a weight
        gradient) must raise the error MUTATION_MARGIN times above the correct one (see d. below), so a lost cross term,
        swapped layout or plain-bf16 operand cannot pass.
+The bias MLP's thin layers (1 -> Hr in, Hr -> heads out, and their weight gradients) run on omlm_sgemm_small and, in
+deterministic mode, omlm_sgemm_small_det; the engine-level cases check them through the table and the gradients.
 The t5 and 'none' tables and their backward are exact, and the d = 72 model (Hr = 36, thirds padded to 40 columns) runs
 end to end against the CPU oracle."""
 import os

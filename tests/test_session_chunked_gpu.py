@@ -31,7 +31,7 @@ def _unit(h):
 # ------------------------------------------------------------------------------------------------ 1. attention
 # (h, N); (3, 700): the d = 72 model's heads; (3, 100): a whole prompt shorter than U = 128; (8, 645), (16, 645): a final
 # chunk shorter than U at p0 = 640, on the 64-row grid
-CHUNK_ATTN = [(1, 1000), (2, 700), (6, 650), (8, 1000), (16, 700), (3, 700), (3, 100), (8, 645), (16, 645)]
+CHUNK_ATTN = [(1, 1000), (2, 700), (6, 650), (8, 1000), (16, 700), (3, 700), (3, 100), (8, 645), (16, 645), (2, 40)]
 
 
 def chunk_attn_chunks(h, N):

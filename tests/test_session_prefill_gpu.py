@@ -35,9 +35,21 @@ def _packed_arrays(lens, h):
 # ------------------------------------------------------------------------------------------------ 1. attention
 ATTN_LENS = {
     1: [1, 2, 127, 128, 129, 300, 1, 2048, 3],
+    2: [1, 63, 64, 65, 2, 500, 3, 41],
+    3: [1, 2, 127, 128, 129, 300, 5, 1000, 43],
     8: [1, 2, 15, 17, 127, 128, 129, 1, 2, 700, 1000],
     12: [2, 1, 9, 11, 127, 128, 129, 64, 1500, 1],
     16: [1, 7, 9, 2, 127, 128, 129, 2048, 1, 33],
+}
+
+
+# launches of more than 16 sequences, as scoring packs them; at h = 1 also more than 2^14 rows in all (the varlen
+# kernels' row coordinates in their TMA maps)
+ATTN_LENS_MANY = {
+    1: [2048] * 8 + [1, 2, 127, 128, 129, 300, 3, 64, 65, 1000],
+    2: [1, 63, 64, 65, 2, 500, 3, 41] * 3,
+    3: [1, 2, 127, 128, 129, 300, 5, 1000, 43] * 2,
+    16: [1, 7, 9, 2, 127, 128, 129, 2048, 1, 33] * 2,
 }
 
 
@@ -46,9 +58,19 @@ def test_varlen_attention_is_each_sequence_alone(lib, h):
     """Sequences packed without gaps (lengths 1, 2, 128/h +- 1, 127, 128, 129 and up to 2048): out and lse2 equal
     attn_fwd_tc on each sequence alone (B = 1, N = its length), the rows after the last sequence keep their sentinel,
     and one sequence's values lie within the float64 bounds of the fixed-length kernel."""
-    lens = ATTN_LENS[h]
+    _varlen_check(lib, h, ATTN_LENS[h], 77 + h)
+
+
+@pytest.mark.parametrize("h", sorted(ATTN_LENS_MANY))
+def test_varlen_attention_many_sequences(lib, h):
+    """test_varlen_attention_is_each_sequence_alone's checks over 18 to 24 sequences in one launch, and past 2^14
+    packed rows."""
+    _varlen_check(lib, h, ATTN_LENS_MANY[h], 91 + h)
+
+
+def _varlen_check(lib, h, lens, seed):
     M = sum(lens)
-    qn, kvn, table, _, _ = make_inputs(1, M, h, None, "rand", "rand", seed=77 + h)
+    qn, kvn, table, _, _ = make_inputs(1, M, h, None, "rand", "rand", seed=seed)
     seq_start, seq_len, work, start = _packed_arrays(lens, h)
     out = torch.full((M + SENTINEL_ROWS, h * 64), 7.0, device=DEV, dtype=torch.bfloat16)
     lse = torch.full(((M + SENTINEL_ROWS) * h,), 7.0, device=DEV)
