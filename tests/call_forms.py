@@ -10,10 +10,23 @@ Models (MODELS): "d72" (d = 72, h = 3, codebooks whose C = 101 / 65 are not mult
 cfg2 layer dims at depth 1, h = 8), "d72_abspos" (d72 with absolute position embeddings: their rows in the
 embedding gathers and the decode step), "cfg2_h16" (d = 1024, h = 16, whose chunk unit U = 128 / gcd(h, 128) is 8; the
 session and score phases only) and "musiclm_prime" (the three stages of tests/golden/musiclm_prime.pt; song sessions
-and song scoring only)."""
+and song scoring only).
+
+The bench models (BENCH_MODELS) are the workloads bench.py times, taken from bench.py itself (WORKLOADS, COMMON, TRAIN,
+synth_batch), so that they follow it: "bench_cfg2" (the headline: coarse, B = 16, N = 1024), "bench_cfg3" (fine, B = 8,
+N = 2048, the fine ids flattened to 1269 = 253 x 5 + 4: the remainder heads), "bench_cfg4" (h = 16, B = 16) and
+"semantic" (the musiclm_small semantic stage, d = 1024, h = 8, N = 256, ce weights [0, 1], B = 16).  Each is built at
+depth 1: the per-layer forms repeat unchanged across layers, so bench.py's depth 6 and cfg4's depth 24 add no form.  They
+run bench.py's step (its batch, shapes, ce weights [0, 0, 1], FFN dropout 0.1 and the forgetful mask, eager: the
+captured graph replays the same launches), its deterministic variant and eval_loss.  "semantic" also runs "bench
+generation": MusicLM.generate_tokens with depth-1 musiclm_small semantic, coarse and fine stages at bench.py's batch 1
+and 10 seconds, as bench.measure_generation does."""
+import gc
 import math
 
 import torch
+
+import bench
 
 # model kwargs, conditioning shapes (clap, semantic), predicted shape (time steps, quantizers), token range
 MODELS = {
@@ -27,7 +40,26 @@ MODELS = {
 }
 SESSIONS_ONLY = {"cfg2_h16"}
 SONGS_ONLY = {"musiclm_prime"}
-MODEL_KEYS = list(MODELS) + sorted(SONGS_ONLY)
+
+
+def _bench_model(key):
+    wl = bench.WORKLOADS[key]
+    return dict(stage=wl["stage"], kw=dict(bench.COMMON, **dict(wl["model"], depth=1)), shapes=wl["shapes"], batch=wl["batch"],
+                ce=list(bench.TRAIN["ce_weights"]))
+
+
+# stage, model kwargs, token shapes per sequence, batch and ce weights of each bench model
+BENCH_MODELS = {
+    "bench_cfg2": _bench_model("cfg2"),
+    "bench_cfg3": _bench_model("cfg3"),
+    "bench_cfg4": _bench_model("cfg4"),
+    # bench.py has no semantic training workload: the musiclm_small semantic stage of its generation (bench.measure_generation:
+    # COMMON, h = 8) at the shapes of its cfg1 forward (bench.cpu_cfg1_forward: clap 12 + semantic 241, N = 256) and the
+    # per-GPU training batch of its headline workload
+    "semantic": dict(stage="semantic", kw=dict(bench.COMMON, depth=1, heads=8), shapes=[(12,), (241,)],
+                     batch=bench.WORKLOADS["cfg2"]["batch"], ce=[0.0, 1.0]),
+}
+MODEL_KEYS = list(MODELS) + sorted(SONGS_ONLY) + list(BENCH_MODELS)
 
 # (phase, deterministic, frozen): "norms" freezes the LayerNorm gammas and the q/k scales, "relpos" the relative-position
 # MLP (the attention backward then forms no bias gradient)
@@ -39,9 +71,21 @@ SCORE_PHASES = ["score"]
 SESSION_PHASES = ["session join", "session chunked", "session logprobs", "session sampling"]
 SONG_PHASES = ["song session", "score songs"]
 SCORE_MODELS = {"d72", "d72_abspos", "cfg2_h16"}
+BENCH_PHASES = ["bench step", "bench deterministic step", "eval_loss"]
+GENERATION_MODELS = {"semantic"}        # the bench models that also run "bench generation"
+
+
+def train_spec(model):
+    """Batch, token shapes per sequence and ce weights of a model's training phases."""
+    if model in BENCH_MODELS:
+        return {k: BENCH_MODELS[model][k] for k in ("batch", "shapes", "ce")}
+    _, cond_n, pred_shape, _ = MODELS[model]
+    return dict(batch=4, shapes=cond_n + [pred_shape], ce=[0.0, 1.0, 1.0])
 
 
 def phases(model):
+    if model in BENCH_MODELS:
+        return BENCH_PHASES + (["bench generation"] if model in GENERATION_MODELS else [])
     if model in SONGS_ONLY:
         return list(SONG_PHASES)
     score = SCORE_PHASES if model in SCORE_MODELS else []
@@ -127,6 +171,51 @@ def _songs(rec):
     torch.cuda.synchronize()
 
 
+def _bench(rec, model):
+    """bench.measure's step at depth 1: eager, then deterministic, then eval_loss, each on a batch of synth_batch."""
+    import open_musiclm_b200 as O
+    spec, ts = BENCH_MODELS[model], train_spec(model)
+    make = {"coarse": O.create_coarse_transformer, "fine": O.create_fine_transformer, "semantic": O.create_semantic_transformer}
+    m = make[spec["stage"]](**spec["kw"]).cuda()
+    tr = O.HotPathTrainer(m, cross_entropy_loss_weights=ts["ce"], lr=bench.TRAIN["lr"], lr_warmup=bench.TRAIN["lr_warmup"],
+                          wd=bench.TRAIN["wd"], max_grad_norm=bench.TRAIN["max_grad_norm"], grad_accum_every=1, use_cuda_graph=False)
+    gen = torch.Generator().manual_seed(1234)
+    batch = lambda: [t.cuda() for t in bench.synth_batch(ts["batch"], gen, ts["shapes"])]
+    for phase, det in (("bench step", False), ("bench deterministic step", True)):
+        rec.phase = phase
+        prev = torch.are_deterministic_algorithms_enabled()
+        torch.use_deterministic_algorithms(det)
+        try:
+            tr.train_step([batch()])
+            torch.cuda.synchronize()
+        finally:
+            torch.use_deterministic_algorithms(prev)
+    rec.phase = "eval_loss"
+    tr.eval_loss(batch())
+    torch.cuda.synchronize()
+    del m, tr
+    gc.collect()                # the d = 1024 workspaces at bench.py's batch: free them before the next phase or test
+    if model in GENERATION_MODELS:
+        rec.phase = "bench generation"
+        _bench_generation()
+        gc.collect()
+
+
+def _bench_generation(seconds=10, batch=1):
+    """bench.measure_generation's MusicLM.generate_tokens, with the three musiclm_small stages at depth 1 (its stage
+    construction restated, since bench.py builds them inside the timed function)."""
+    import open_musiclm_b200 as O
+    mk = dict(bench.COMMON, depth=1, heads=8)
+    sem = O.create_semantic_transformer(**mk).cuda().eval()
+    coa = O.create_coarse_transformer(**mk, num_coarse_quantizers=3).cuda().eval()
+    fin = O.create_fine_transformer(**mk, num_coarse_quantizers=3, num_fine_quantizers=5).cuda().eval()
+    mlm = O.MusicLM(semantic_transformer=sem, coarse_transformer=coa, fine_transformer=fin)
+    g = torch.Generator().manual_seed(1234)
+    clap = torch.randint(0, 1024, (batch, 12), generator=g).cuda()
+    mlm.generate_tokens(clap_token_ids=clap, output_seconds=seconds, return_all=True)
+    torch.cuda.synchronize()
+
+
 def _run_session(w, rec, phase, reqs, **kw):
     import open_musiclm_b200 as O
     rec.phase = phase
@@ -146,11 +235,14 @@ def run(rec, model, act16, monkeypatch):
     torch.manual_seed(0)
     if model in SONGS_ONLY:
         return _songs(rec)
+    if model in BENCH_MODELS:
+        return _bench(rec, model)
     kw, cond_n, pred_shape, vocab = MODELS[model]
+    ts = train_spec(model)
     g = torch.Generator().manual_seed(1)
 
     def batch():
-        toks = [torch.randint(0, min(vocab, 64), (4,) + s, generator=g) for s in cond_n + [pred_shape]]
+        toks = [torch.randint(0, min(vocab, 64), (ts["batch"],) + s, generator=g) for s in ts["shapes"]]
         toks[0][1, -2:] = -1                     # pad tokens: their embedding rows are zero
         toks[1][2, -3:] = -1
         return [t.cuda() for t in toks]
@@ -162,7 +254,7 @@ def run(rec, model, act16, monkeypatch):
             rec.phase = phase
             m = O.create_coarse_transformer(attn_dropout=0.0, ff_dropout=0.1, **kw).cuda()
             _freeze(m, frozen)
-            tr = O.HotPathTrainer(m, cross_entropy_loss_weights=[0.0, 1.0, 1.0], lr=3e-4, wd=1e-2, use_cuda_graph=False)
+            tr = O.HotPathTrainer(m, cross_entropy_loss_weights=ts["ce"], lr=3e-4, wd=1e-2, use_cuda_graph=False)
             prev = torch.are_deterministic_algorithms_enabled()
             torch.use_deterministic_algorithms(det)
             try:

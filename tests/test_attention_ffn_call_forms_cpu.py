@@ -57,6 +57,9 @@ def test_covered_set_holds_what_the_explicit_lists_cover():
         for null in (False, True):
             assert T.attn_key(3, 50, True, 50, det, null) in cov
             assert T.attn_key(8, 1024, True, 1024, det, null) in cov
+            assert T.attn_key(16, 1024, True, 1024, det, null) in cov      # bench.py's cfg4 training step
+    assert T.attn_key(16, 1024, True, 1024) in cov
+    assert T.attn_key(8, 15, True, 15) in cov                          # the semantic stage's prefill in bench generation
     assert T.attn_key(1, 1, False, 41) in cov                          # CASES[0]
     assert T.attn_key(3, 257, True, 257 + 40) in cov                    # CASES (2, 257, 3, ...)
     assert T.attn_key(3, 3000, True, 3040) not in cov                   # no case runs N > 2048

@@ -8,7 +8,8 @@ and chunked kernels, the host plan of the session's packed prefill (session.Pack
 sent to the device): sequence lengths, p0 per chunk, kv_start, max_len / max_end.  Nothing reads device memory.
 
 Each form is replayed at its shapes with fresh seeded inputs against the float64 references and bounds the families'
-own files use (test_attention_reference_gpu.py, test_generate_ragged_gpu.py, ffn_reference.py with the BOUNDS of
+own files use (a conv feed-forward form of more than test_ffn_reference_gpu.REF_ROWS rows, as at bench.py's batches, is
+launched whole and compared on its first, a middle and its last sequence, each alone) (test_attention_reference_gpu.py, test_generate_ragged_gpu.py, ffn_reference.py with the BOUNDS of
 test_ffn_reference_gpu.py, test_sampling_gpu.py's conv step); outputs are poisoned and the rows past them guarded.  A
 session issues a new plan at every boundary, so the packed and chunked kernels replay one form per coverage key.
 
@@ -253,6 +254,12 @@ def _record(act16, model, monkeypatch):
     if model in call_forms.SONGS_ONLY:
         expected = {("song session", n) for n in ("attn_decode_mqa", "decode_conv_geglu", "ffn_norm_fwd")} | \
             {("score songs", n) for n in ("attn_fwd_tc_varlen", "gemm_ffn_up_varlen", "ffn_norm_fwd")}
+    elif model in call_forms.BENCH_MODELS:
+        expected = {(p, n) for p in ("bench step", "bench deterministic step") for n in ("attn_fwd_tc", "attn_bwd_tc", "gemm_ffn_up",
+                                                                                      "ffn_norm_fwd", "ffn_mid_bwd")} | \
+            {("eval_loss", "attn_fwd_tc"), ("eval_loss", "gemm_ffn_up")}
+        if model in call_forms.GENERATION_MODELS:
+            expected |= {("bench generation", n) for n in ("attn_decode", "decode_conv_geglu", "gemm_ffn_up", "ffn_norm_fwd")}
     else:
         expected = {(p, "attn_fwd_tc_chunk") for p in call_forms.SESSION_PHASES} | \
             {(p, n) for p in call_forms.SESSION_PHASES for n in ("attn_decode_mqa", "decode_conv_geglu", "ffn_norm_fwd")} | \
@@ -575,7 +582,8 @@ def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
         mine = sorted({(n[4], n[6] or adt == BF16) for n in norms if (n[0], n[1], n[3]) == (adt, M, Fp)})
         done_norms |= {n for n in norms if (n[0], n[1], n[3]) == (adt, M, Fp)}
         c = TF.make_case(_lib(), (K, F, True, M // Nseq, Nseq), adt, seed=M)
-        fails += TF.forward_checks(_lib(), c, f"engine form gemm_ffn_up {f}", (mc,), mine or [(0.0, True)])
+        fails += TF.forward_checks(_lib(), c, f"engine form gemm_ffn_up {f}", (mc,), mine or [(0.0, True)],
+                                   seqs=TF.check_seqs(M // Nseq, Nseq))
         keys |= up_keys(adt, K, F, Fp, True, M // Nseq, Nseq)
     for n in norms:
         adt, M, F, Fp, p, kb, copy = n
@@ -586,7 +594,7 @@ def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
     for f in byname.get("ffn_mid_bwd", []):
         adt, B, N, F, Fp, p, parts, det, dg_null, dc_null = f
         c = TF.make_case(_lib(), (Kmap[Fp], F, True, B, N), adt, seed=B * N)
-        fails += TF.backward_checks(_lib(), c, f"engine form ffn_mid_bwd {f}", (p,), dets=(det,))
+        fails += TF.backward_checks(_lib(), c, f"engine form ffn_mid_bwd {f}", (p,), dets=(det,), seqs=TF.check_seqs(B, N))
         keys.add(mid_key(adt, F, Fp, True, p, parts, det, dg_null, dc_null))
     for name, chunk in (("gemm_ffn_up_varlen", False), ("gemm_ffn_up_chunk", True)):
         items = []

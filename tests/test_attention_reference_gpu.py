@@ -320,6 +320,8 @@ EXACT_CASES = [
     (4, 1024, 8, "rand", "rand", "rand"),
     (3, 230, 8, "rand", "diag", "rand"),
     (2, 100, 16, None, "rand", "rand"),
+    (2, 1024, 16, "rand", "rand", "rand"),         # bench.py's cfg4 (musiclm_large): h = 16 at N = 1024
+    (2, 15, 8, "rand", "rand", "rand"),            # bench.py's generation: the semantic stage's prefill of the clap ids
 ]
 
 

@@ -23,6 +23,36 @@ def _params(d, F, use_conv, seed, zero_gamma=()):
 
 
 @pytest.mark.parametrize("use_conv", [True, False])
+def test_per_sequence_references_equal_the_whole_batch(use_conv, monkeypatch):
+    """The rows test_ffn_reference_gpu compares a large form on: each sequence's forward, magnitude and du alone equal
+    those rows of the whole-batch reference, and dgamma / dconv_w and their scales accumulated over chunks of whole
+    sequences equal the whole-batch sums."""
+    import test_ffn_reference_gpu as TF
+    d, F, B, N, p = 16, 20, 5, 9, 0.25
+    W1, cw, gam = _params(d, F, use_conv, 11)
+    g = torch.Generator().manual_seed(12)
+    xn = torch.randn(B * N, d, generator=g, dtype=torch.float64)
+    keep = torch.rand(B * N, F, generator=g) > p
+    dh = torch.randn(B * N, F, generator=g, dtype=torch.float64)
+    u = xn @ W1.t()
+    whole = FR.forward(xn, W1, cw, gam, N, keep, p)
+    whole_g = FR.grads(u, cw, gam, dh, N, keep, p)
+    whole_S = FR.magnitude(None, None, cw, gam, N, keep, p, u=u, dhn=dh)
+    for rows in TF.row_groups(N, [0, 2, B - 1], device="cpu"):
+        part = FR.forward(xn[rows], W1, cw, gam, N, keep[rows], p)
+        for k in ("u", "h", "s1", "s2", "mean", "rstd", "hn"):
+            assert torch.allclose(part[k], whole[k][rows], rtol=1e-12, atol=1e-12), k
+        assert torch.allclose(FR.grads(u[rows], cw, gam, dh[rows], N, keep[rows], p)["du"], whole_g["du"][rows], rtol=1e-10, atol=1e-12)
+    assert TF.check_seqs(4, 1024) is None and TF.check_seqs(16, 1024) == [0, 8, 15] and TF.check_seqs(8, 2048) == [0, 4, 7]
+    monkeypatch.setattr(TF, "REF_ROWS", 2 * N)          # chunks of two sequences, the last one alone
+    c = dict(F=F, N=N, B=B, cw=cw, gam=gam)
+    ref, S = TF.weight_grad_refs(c, u, dh, keep, p)
+    for k in ("dgamma", "dconv_w") if use_conv else ("dgamma",):
+        assert torch.allclose(ref[k], whole_g[k], rtol=1e-10, atol=1e-12), k
+        assert torch.allclose(S[k], whole_S[k], rtol=1e-10, atol=1e-12), k
+
+
+@pytest.mark.parametrize("use_conv", [True, False])
 @pytest.mark.parametrize("with_drop", [False, True])
 def test_forward_matches_oracle(use_conv, with_drop):
     """forward() followed by the down projection is oracle/restatement.conv_feed_forward, in float64."""

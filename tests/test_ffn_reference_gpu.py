@@ -152,6 +152,36 @@ def check(fails, name, got, ref, allow, keys, seams, tag, cb=128):
         fails.append(f"{name} {tag}: rel-L2 {glob:.3e} >= {b_glob:.1e}")
 
 
+# ------------------------------------------------------------------------------------------------ reference rows
+# The float64 references of forward_checks / backward_checks take about 1.3 GB per 1024 rows of F = 2730.  A form of more
+# than REF_ROWS rows (bench.py's batches: 16384) is launched whole but compared sequence by sequence, on the first, a
+# middle and the last: conv, GEGLU and LayerNorm never cross a sequence, so those rows' references are exact.  The
+# weight gradients dgamma and dconv_w sum over every row; their references are accumulated over chunks of whole
+# sequences of at most REF_ROWS rows.
+REF_ROWS = 4096
+
+
+def check_seqs(B, N):
+    """The sequences a form is compared on: None (every row at once) up to REF_ROWS rows, else the first, a middle and
+    the last."""
+    return None if B * N <= REF_ROWS else sorted({0, B // 2, B - 1})
+
+
+def row_groups(N, seqs, device=DEV):
+    """Row indices of each reference group: [None] (every row) or one group per sequence of seqs."""
+    if seqs is None:
+        return [None]
+    return [torch.arange(b * N, (b + 1) * N, device=device) for b in seqs]
+
+
+def _sel(rows):
+    return lambda t: t if (rows is None or t is None) else t[rows]
+
+
+def _gtag(tag, rows, N):
+    return tag if rows is None else f"{tag} sequence {int(rows[0]) // N}"
+
+
 # ------------------------------------------------------------------------------------------------ set-up
 def make_case(lib, key, adt, seed=0):
     """key: a name of CASES or a (d, F, conv, B, N) tuple."""
@@ -238,9 +268,9 @@ def test_forward_against_float64(lib, key, adt):
     assert not fails, "\n".join(fails)
 
 
-def forward_checks(lib, c, tag, max_ctas, norms):
+def forward_checks(lib, c, tag, max_ctas, norms, seqs=None):
     """gemm_ffn_up at each max_ctas (bit-identical to the first) and ffn_norm_fwd at each (p, copy) of norms, against
-    float64 -> the list of failures."""
+    float64 -> the list of failures.  seqs: the sequences whose rows are compared (None: every row; see REF_ROWS)."""
     F, Fp, B, N, M, unit = c["F"], c["Fp"], c["B"], c["N"], c["M"], UNIT[c["adt"]]
     fails = []
     runs = [run_up(lib, c, m) for m in max_ctas]
@@ -250,69 +280,81 @@ def forward_checks(lib, c, tag, max_ctas, norms):
         for name, a, b in (("u", ub, u2), ("h", hb, h2), ("rowsum", rb, r2)):
             if not torch.equal(a, b):
                 fails.append(f"{name}: max_ctas={max_ctas[i + 1]} differs from max_ctas={max_ctas[0]}")
+    del runs[1:]
     for name, buf in (("u", ub), ("h", hb), ("rowsum", rb)):
         guard_ok(fails, name, buf, M)
     u, h, rs = ub[:M], hb[:M], rb[:M].view(M, Fp // 128, 2)
     if not bool((h[:, F:] == 0).all()):
         fails.append("h: padded columns are not zero")
-    keys, seams = row_keys(B, N, True), seam_rows(B, N)
-    kern = lambda x: FR.to_kernel(x, F)
-    chain = FR.forward(c["xn"], c["W1"], c["cw"], c["gam"], N)
-    fl = FLOOR_S[c["adt"]]
-    Sc = FR.magnitude(c["xn"], c["W1"], c["cw"], c["gam"], N, floor=fl)
-    u_st = FR.from_kernel(u, F)
-    iso = FR.forward(None, None, c["cw"], c["gam"], N, u=u_st)
-    Si = FR.magnitude(None, None, c["cw"], c["gam"], N, u=u_st, floor=fl)
-    # u: one rounding of an fp32 accumulation over d
-    check(fails, "u", u, kern(chain["u"]), kern(2 * unit * Sc["u"]), keys, seams, tag)
-    # h: from the stored u (fp32 conv and GEGLU, one rounding) and from xn (plus u's rounding, through S_h)
-    check(fails, "h iso", h, pad_cols(iso["h"], Fp), pad_cols(2 * unit * Si["h"], Fp), keys, seams, tag)
-    check(fails, "h chain", h, pad_cols(chain["h"], Fp), pad_cols(2 * unit * Sc["h"], Fp), keys, seams, tag)
-    # row sums of the unrounded fp32 h, added over the 128-channel tiles
-    rsum = rs.double().sum(1)
-    s_iso, s_chain = torch.stack([iso["s1"], iso["s2"]], 1), torch.stack([chain["s1"], chain["s2"]], 1)
-    S_iso, S_chain = torch.stack([Si["s1"], Si["s2"]], 1), torch.stack([Sc["s1"], Sc["s2"]], 1)
-    check(fails, "rowsum iso", rsum, s_iso, 2.0 ** -16 * S_iso, keys, seams, tag, cb=1)
-    check(fails, "rowsum chain", rsum, s_chain, 2 * unit * S_chain, keys, seams, tag, cb=1)
+    normed = []
     for p, copy in norms:
-        ptag = f"{tag} p={p}{'' if copy else ' no copy'}"
+        ptag = f"p={p}{'' if copy else ' no copy'}"
         n = run_norm(lib, c, h, rs, p, copy)
         torch.cuda.synchronize()
         for name, buf in zip(("hn", "stats", "hn copy"), n["bufs"]):
             guard_ok(fails, name, buf, M)
         if not bool((n["kb"][M:] == 0xA5).all()):
-            fails.append(f"keep bits {ptag}: a guard row past M was written")
+            fails.append(f"keep bits {tag} {ptag}: a guard row past M was written")
         keep = None
         if p > 0:
             keep = FR.unpack_keep(n["kbits"], F)
             frac = 1 - float(keep.double().mean())
             if abs(frac - p) > 0.02:
-                fails.append(f"dropout {ptag}: dropped fraction {frac:.4f}")
-        st = n["stats"]
-        # stats from the kernel's own row sums: fp32 E[h^2] - mean^2 and rsqrt
-        mean_i = rsum[:, 0] / F
-        var_i = (rsum[:, 1] / F - mean_i ** 2).clamp_min(0)
-        rstd_i = (var_i + FR.EPS).rsqrt()
-        a_abs = rs.double().abs().sum(1) / F
-        allow_i = torch.stack([64 * U32 * a_abs[:, 0],
-                               64 * U32 * rstd_i ** 3 / 2 * (a_abs[:, 1] + mean_i ** 2) + 4 * U32 * rstd_i], 1)
-        check(fails, "stats iso", st, torch.stack([mean_i, rstd_i], 1), allow_i, keys, seams, ptag, cb=1)
-        allow_c = torch.stack([2 * unit * Sc["mean"] + 64 * U32 * Sc["mean"],
-                               2 * unit * Sc["rstd"] + 64 * U32 * Sc["rstd32"]], 1)
-        check(fails, "stats chain", st, torch.stack([chain["mean"], chain["rstd"]], 1), allow_c, keys, seams, ptag, cb=1)
-        # hn from the stored h and the kernel's stats (one rounding), and from xn
-        r_iso = FR.forward(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, h=h[:, :F], stats=(st[:, 0], st[:, 1]))
-        S_hn_i = FR.magnitude(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, floor=fl)["hn"]
-        check(fails, "hn iso", n["hn"], pad_cols(r_iso["hn"], Fp), pad_cols(2 * unit * S_hn_i, Fp), keys, seams, ptag)
-        if c["adt"] == torch.float16 and copy:
-            check(fails, "hn iso", n["hn_b"], pad_cols(r_iso["hn"], Fp), pad_cols(2 * UNIT[torch.bfloat16] * S_hn_i, Fp),
-                  keys, seams, ptag + " bf16 copy")
-        r_ch = FR.forward(c["xn"], c["W1"], c["cw"], c["gam"], N, keep, p)
-        S_hn_c = FR.magnitude(c["xn"], c["W1"], c["cw"], c["gam"], N, keep, p, floor=fl)["hn"]
-        check(fails, "hn chain", n["hn"], pad_cols(r_ch["hn"], Fp), pad_cols((3 * unit + 64 * U32) * S_hn_c, Fp),
-              keys, seams, ptag)
+                fails.append(f"dropout {tag} {ptag}: dropped fraction {frac:.4f}")
         if not bool((n["hn"][:, F:] == 0).all()):
-            fails.append(f"hn {ptag}: padded columns are not zero")
+            fails.append(f"hn {tag} {ptag}: padded columns are not zero")
+        normed.append((p, copy, ptag, n, keep))
+    keys_all, seams_all = row_keys(B, N, True), seam_rows(B, N)
+    fl = FLOOR_S[c["adt"]]
+    kern = lambda x: FR.to_kernel(x, F)
+    for rows in row_groups(N, seqs):
+        sel, gtag = _sel(rows), _gtag(tag, rows, N)
+        keys, seams, xn, u_r, h_r, rs_r = sel(keys_all), sel(seams_all), sel(c["xn"]), sel(u), sel(h), sel(rs)
+        chain = FR.forward(xn, c["W1"], c["cw"], c["gam"], N)
+        Sc = FR.magnitude(xn, c["W1"], c["cw"], c["gam"], N, floor=fl)
+        u_st = FR.from_kernel(u_r, F)
+        iso = FR.forward(None, None, c["cw"], c["gam"], N, u=u_st)
+        Si = FR.magnitude(None, None, c["cw"], c["gam"], N, u=u_st, floor=fl)
+        # u: one rounding of an fp32 accumulation over d
+        check(fails, "u", u_r, kern(chain["u"]), kern(2 * unit * Sc["u"]), keys, seams, gtag)
+        # h: from the stored u (fp32 conv and GEGLU, one rounding) and from xn (plus u's rounding, through S_h)
+        check(fails, "h iso", h_r, pad_cols(iso["h"], Fp), pad_cols(2 * unit * Si["h"], Fp), keys, seams, gtag)
+        check(fails, "h chain", h_r, pad_cols(chain["h"], Fp), pad_cols(2 * unit * Sc["h"], Fp), keys, seams, gtag)
+        # row sums of the unrounded fp32 h, added over the 128-channel tiles
+        rsum = rs_r.double().sum(1)
+        s_iso, s_chain = torch.stack([iso["s1"], iso["s2"]], 1), torch.stack([chain["s1"], chain["s2"]], 1)
+        S_iso, S_chain = torch.stack([Si["s1"], Si["s2"]], 1), torch.stack([Sc["s1"], Sc["s2"]], 1)
+        check(fails, "rowsum iso", rsum, s_iso, 2.0 ** -16 * S_iso, keys, seams, gtag, cb=1)
+        check(fails, "rowsum chain", rsum, s_chain, 2 * unit * S_chain, keys, seams, gtag, cb=1)
+        del iso, Si, s_iso, S_iso
+        for p, copy, ptag, n, keep_all in normed:
+            ptag = f"{gtag} {ptag}"
+            keep, st = sel(keep_all), sel(n["stats"])
+            # stats from the kernel's own row sums: fp32 E[h^2] - mean^2 and rsqrt
+            mean_i = rsum[:, 0] / F
+            var_i = (rsum[:, 1] / F - mean_i ** 2).clamp_min(0)
+            rstd_i = (var_i + FR.EPS).rsqrt()
+            a_abs = rs_r.double().abs().sum(1) / F
+            allow_i = torch.stack([64 * U32 * a_abs[:, 0],
+                                   64 * U32 * rstd_i ** 3 / 2 * (a_abs[:, 1] + mean_i ** 2) + 4 * U32 * rstd_i], 1)
+            check(fails, "stats iso", st, torch.stack([mean_i, rstd_i], 1), allow_i, keys, seams, ptag, cb=1)
+            allow_c = torch.stack([2 * unit * Sc["mean"] + 64 * U32 * Sc["mean"],
+                                   2 * unit * Sc["rstd"] + 64 * U32 * Sc["rstd32"]], 1)
+            check(fails, "stats chain", st, torch.stack([chain["mean"], chain["rstd"]], 1), allow_c, keys, seams, ptag, cb=1)
+            # hn from the stored h and the kernel's stats (one rounding), and from xn
+            r_iso = FR.forward(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, h=h_r[:, :F], stats=(st[:, 0], st[:, 1]))
+            S_hn_i = FR.magnitude(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, floor=fl)["hn"]
+            check(fails, "hn iso", sel(n["hn"]), pad_cols(r_iso["hn"], Fp), pad_cols(2 * unit * S_hn_i, Fp), keys, seams, ptag)
+            if c["adt"] == torch.float16 and copy:
+                check(fails, "hn iso", sel(n["hn_b"]), pad_cols(r_iso["hn"], Fp), pad_cols(2 * UNIT[torch.bfloat16] * S_hn_i, Fp),
+                      keys, seams, ptag + " bf16 copy")
+            del r_iso, S_hn_i
+            r_ch = FR.forward(xn, c["W1"], c["cw"], c["gam"], N, keep, p)
+            S_hn_c = FR.magnitude(xn, c["W1"], c["cw"], c["gam"], N, keep, p, floor=fl)["hn"]
+            check(fails, "hn chain", sel(n["hn"]), pad_cols(r_ch["hn"], Fp), pad_cols((3 * unit + 64 * U32) * S_hn_c, Fp),
+                  keys, seams, ptag)
+            del r_ch, S_hn_c
+        del chain, Sc
     return fails
 
 
@@ -331,11 +373,14 @@ def run_mid_bwd(lib, c, dhn, n, u, p, rowstat, parts, det, dg0, dc0):
     return dub, dg, dc
 
 
-def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag):
+def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag, rows=None, weights=True):
+    """du on `rows` (None: every row) against ref["du"] of those rows; with weights, dgamma and dconv_w (sums over
+    every row) against ref's."""
     M, F, Fp, B, N = c["M"], c["F"], c["Fp"], c["B"], c["N"]
+    sel = _sel(rows)
     guard_ok(fails, f"du {tag}", dub, M)
-    du = dub[:M]
-    keys, seams = row_keys(B, N, False), seam_rows(B, N)
+    du = sel(dub[:M])
+    keys, seams = sel(row_keys(B, N, False)), sel(seam_rows(B, N))
     # du: one bf16 rounding; the row means m1, m2 inherit the bf16 hn (an error <= 2^-8 S_dh in dh)
     check(fails, "du", du, FR.to_kernel(ref["du"], F), FR.to_kernel(4 * 2.0 ** -8 * S["du"], F), keys, seams, tag)
     cols = FR.ileave_cols(F, DEV)[torch.tensor(c["zero"] + [F + z for z in c["zero"]], device=DEV)]
@@ -344,6 +389,8 @@ def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag):
     print(f"METRIC du at gamma = 0 {tag}: {e0:.3e}")
     if not e0 < BOUNDS["du"][0]:
         fails.append(f"du {tag}: rel-L2 {e0:.3e} at the channels whose gamma is 0")
+    if not weights:
+        return
     one = torch.zeros(1, dtype=torch.long, device=DEV)
     no = torch.zeros(1, dtype=torch.bool, device=DEV)
     if dg is not None:
@@ -359,6 +406,25 @@ def check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, tag):
     check(fails, "dconv_w", got, FR.to_kernel(ref["dconv_w"].t(), F), allow, taps, no3, tag)
 
 
+def weight_grad_refs(c, u_st, dh, keep, p):
+    """Float64 dgamma / dconv_w and their scales over every row, accumulated over chunks of whole sequences of at most
+    REF_ROWS rows -> (ref, S) dicts."""
+    F, N, B = c["F"], c["N"], c["B"]
+    per = max(1, REF_ROWS // N)
+    ref, S = {"dgamma": 0.0, "dconv_w": 0.0}, {"dgamma": 0.0, "dconv_w": 0.0}
+    for b0 in range(0, B, per):
+        rows = torch.arange(b0 * N, min(B, b0 + per) * N, device=u_st.device)
+        sel = _sel(rows)
+        r = FR.grads(sel(u_st), c["cw"], c["gam"], sel(dh)[:, :F], N, sel(keep), p)
+        m = FR.magnitude(None, None, c["cw"], c["gam"], N, sel(keep), p, u=sel(u_st), dhn=sel(dh)[:, :F])
+        for k in ("dgamma", "dconv_w"):
+            if r[k] is not None:
+                ref[k] = ref[k] + r[k]
+                S[k] = S[k] + m[k]
+        del r, m
+    return ref, S
+
+
 @pytest.mark.parametrize("adt", list(ADT))
 @pytest.mark.parametrize("key", list(CASES))
 def test_backward_against_float64(lib, key, adt):
@@ -371,8 +437,9 @@ def test_backward_against_float64(lib, key, adt):
     assert not fails, "\n".join(fails)
 
 
-def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0):
-    """ffn_mid_bwd at each dropout p of ps and each mode of dets, with and without dgamma -> the list of failures."""
+def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0, seqs=None):
+    """ffn_mid_bwd at each dropout p of ps and each mode of dets, with and without dgamma -> the list of failures.
+    seqs: the sequences whose rows are compared (None: every row; see REF_ROWS)."""
     F, Fp, B, N, M, d = c["F"], c["Fp"], c["B"], c["N"], c["M"], c["d"]
     fails = []
     ub, hb, rb = run_up(lib, c, max_ctas)
@@ -381,6 +448,7 @@ def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0):
     g = c["g"]
     dg0 = torch.randn(F, generator=g, device=DEV)
     dc0 = torch.randn(2 * F, 3, generator=g, device=DEV) if c["cw"] is not None else None
+    groups = row_groups(N, seqs)
     for p in ps:
         n = run_norm(lib, c, h, rs, p)
         keep = None if p == 0 else FR.unpack_keep(n["kbits"], F)
@@ -398,19 +466,20 @@ def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0):
             lib.gemm_rowstat(dx, w2, dhn2, n["hn_b"], c["gp"], part, b_mn=True, M=M, N=Fp, K=d, keep_bits=n["kbits"],
                              keep_scale=ks)
             guard_ok(fails, "gemm_rowstat partials", pb, M)
-            dref = dx.double() @ w2.double()
-            s1, s2 = FR.lnbwd_row_sums(dref, n["hn_b"], c["gam"], keep, p)
-            S1, S2 = FR.lnbwd_row_sums(dx.double().abs() @ w2.double().abs(), n["hn_b"].double().abs(), c["gam"].abs(),
-                                       keep, p)
             pv = part.view(M, Fp // 128, 2)
-            keys, seams = row_keys(B, N, False), seam_rows(B, N)
-            for j, (r, S) in enumerate(((s1, S1), (s2, S2))):
-                check(fails, "lnbwd sums", pv[..., j], r, 2.0 ** -16 * S, keys, seams, f"{tag} p={p} s{j + 1}",
-                      cb=Fp // 128)
+            for rows in groups:
+                sel = _sel(rows)
+                dxr, kr, hbr = sel(dx), sel(keep), sel(n["hn_b"])
+                s1, s2 = FR.lnbwd_row_sums(dxr.double() @ w2.double(), hbr, c["gam"], kr, p)
+                S1, S2 = FR.lnbwd_row_sums(dxr.double().abs() @ w2.double().abs(), hbr.double().abs(), c["gam"].abs(), kr, p)
+                keys, seams = sel(row_keys(B, N, False)), sel(seam_rows(B, N))
+                for j, (r, S) in enumerate(((s1, S1), (s2, S2))):
+                    check(fails, "lnbwd sums", sel(pv)[..., j], r, 2.0 ** -16 * S, keys, seams,
+                          f"{_gtag(tag, rows, N)} p={p} s{j + 1}", cb=Fp // 128)
+                del s1, s2, S1, S2
             variants.append(("gemm", dhn2, part))
         for src, dh, part in variants:
-            ref = FR.grads(u_st, c["cw"], c["gam"], dh[:, :F], N, keep, p)
-            S = FR.magnitude(None, None, c["cw"], c["gam"], N, keep, p, u=u_st, dhn=dh[:, :F])
+            outs = []
             for det in dets:
                 if part is None:
                     rowstat, parts = guarded(M, 2, torch.float32)[1], 0
@@ -418,10 +487,23 @@ def backward_checks(lib, c, tag, ps, dets=(False, True), max_ctas=0):
                     rowstat, parts = part, Fp // 128
                 dub, dg, dc = run_mid_bwd(lib, c, dh, n, u, p, rowstat, parts, det, dg0, dc0)
                 torch.cuda.synchronize()
-                check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, f"{tag} p={p} {src} det={det}")
                 dub2, _, dc2 = run_mid_bwd(lib, c, dh, n, u, p, rowstat, parts, det, None, dc0)
                 torch.cuda.synchronize()
-                check_grads(fails, c, dub2, None, dc2, None, dc0, ref, S, f"{tag} p={p} {src} det={det} dgamma=None")
                 if det and not (torch.equal(dub2, dub) and (dc is None or torch.equal(dc2, dc))):
                     fails.append(f"{tag} p={p} {src} det={det}: du / dconv_w without dgamma differ from the call with it")
+                outs.append((det, dub, dg, dc, dub2, dc2))
+            wref = weight_grad_refs(c, u_st, dh, keep, p) if seqs is not None else None
+            for i, rows in enumerate(groups):
+                sel = _sel(rows)
+                ref = FR.grads(sel(u_st), c["cw"], c["gam"], sel(dh)[:, :F], N, sel(keep), p)
+                S = FR.magnitude(None, None, c["cw"], c["gam"], N, sel(keep), p, u=sel(u_st), dhn=sel(dh)[:, :F])
+                if wref is not None:
+                    ref.update(wref[0])
+                    S.update(wref[1])
+                gtag = _gtag(tag, rows, N)
+                for det, dub, dg, dc, dub2, dc2 in outs:
+                    check_grads(fails, c, dub, dg, dc, dg0, dc0, ref, S, f"{gtag} p={p} {src} det={det}", rows, i == 0)
+                    check_grads(fails, c, dub2, None, dc2, None, dc0, ref, S, f"{gtag} p={p} {src} det={det} dgamma=None",
+                                rows, i == 0)
+                del ref, S
     return fails

@@ -587,6 +587,11 @@ def _record(act16, model, monkeypatch):
     # the shim sees the engine only while it calls through lib's attributes: every path must have shown up
     if model in call_forms.SONGS_ONLY:
         expected = {("song session", "gemm"), ("song session", "decode_gemm"), ("score songs", "gemm")}
+    elif model in call_forms.BENCH_MODELS:
+        expected = {(p, "gemm") for p in call_forms.BENCH_PHASES} | {("bench step", "gemm_rowstat"),
+                                                                     ("bench deterministic step", "gemm_splitk_det")}
+        if model in call_forms.GENERATION_MODELS:
+            expected |= {("bench generation", "gemm"), ("bench generation", "skinny_gemm")}
     else:
         expected = {(p, "gemm") for p in call_forms.SESSION_PHASES} | {(p, "decode_gemm") for p in call_forms.SESSION_PHASES}
     if model in call_forms.SCORE_MODELS:

@@ -643,6 +643,11 @@ def _record(act16, model, monkeypatch):
     # sessions: the packed prefill's final norm writes the rows dest_row names; return_logprobs scores the prefixes
     if model in call_forms.SONGS_ONLY:
         expected = {(p, n) for p in call_forms.SONG_PHASES for n in ("layernorm_fwd", "embed_gather")} | {("score songs", "token_logprob")}
+    elif model in call_forms.BENCH_MODELS:
+        expected = {(p, n) for p in ("bench step", "bench deterministic step") for n in NAMES if n not in ("embed_gather", "token_logprob")} | \
+            {("bench step", "embed_gather"), ("eval_loss", "cross_entropy"), ("eval_loss", "layernorm_fwd")}
+        if model in call_forms.GENERATION_MODELS:
+            expected |= {("bench generation", "layernorm_fwd"), ("bench generation", "embed_gather")}
     else:
         expected = {(p, n) for p in call_forms.SESSION_PHASES for n in ("layernorm_fwd", "embed_gather")} | \
             {("session logprobs", "token_logprob"), ("session sampling", "token_logprob")}
@@ -655,7 +660,7 @@ def _record(act16, model, monkeypatch):
              ("frozen norms step", "qk_l2norm_bwd")}
     assert expected <= rec.seen, f"entry points the engine did not call through lib: {sorted(expected - rec.seen)}"
     dest = {f[6] for n, f in rec.forms if n == "layernorm_fwd"}
-    assert True in dest, "no layernorm_fwd call with dest_row was recorded"
+    assert True in dest or model in call_forms.BENCH_MODELS, "no layernorm_fwd call with dest_row was recorded"
     return rec.forms
 
 

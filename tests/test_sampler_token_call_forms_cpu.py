@@ -50,6 +50,21 @@ def test_sample_symbol_follows_lib_sample():
     assert T.sample_symbol(1.0, (False, False, False), False) == (None, False)
 
 
+def test_plan_key_separates_a_last_sequence_that_ends_inside_a_time_step():
+    """bench.py's cfg3 flattens the fine ids to 1269 = 253 x 5 + 4: a key of its own, apart from 1270 ids at q = 5 and
+    from the coarse stage's whole steps; the explicit training plans cover it with and without forgetting and err_flag."""
+    form = lambda n, q, forget, err: ([12, 762, n], [12, 3, q], True, True, True, False, forget, True, err)
+    assert T.plan_key(*form(1269, 5, True, True)) != T.plan_key(*form(1270, 5, True, True))
+    assert T.plan_key(*form(1269, 5, True, True))[-1] and not T.plan_key(*form(1270, 5, True, True))[-1]
+    assert not T.plan_key([12, 197, 810], [12, 1, 3], True, True, True, False, True, True, True)[-1]
+    assert not T.plan_key([12, 241], [12, 1], True, True, True, False, True, True, True)[-1]
+    cov = T.covered_keys()
+    for forget in (False, True):
+        for err in (False, True):
+            assert T.plan_key(*form(1269, 5, forget, err)) in cov
+            assert T.plan_key([12, 241], [12, 1], True, True, True, False, forget, True, err) in cov
+
+
 def test_explicit_cases_are_covered_and_distinct():
     cov = T.covered_keys()
     assert all(T.sampler_key(*c) in cov for c in T.EXPLICIT_SAMPLER) and all(T.plan_key(*c) in cov for c in T.EXPLICIT_PLAN)

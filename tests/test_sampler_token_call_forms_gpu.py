@@ -14,7 +14,7 @@ Replays use fresh seeded inputs, outputs poisoned with a sentinel and rows past 
   near-tie exclusion) under the host replica of the form's noise source (supplied uniforms, the Philox stream of the
   shared seed, or per-row seeds); log-probability forms also against the float64 statements of logprob_reference.py
   under their bounds; indexed forms with rows at, past and before their last sample index;
-- token_plan: bit-exact against oracle.restatement for the training form and against plan_reference (below) for the
+- token_plan: at the recorded batch, bit-exact against oracle.restatement for the training form and against plan_reference (below) for the
   inference forms, with pads at quantizer positions other than 0, an empty sequence and ids outside a table (a -1
   row and the sequence's err_flag bit);
 - forgetful_mask against the replica ranking; embed_gather_pos_rows and decode_advance_pos against torch indexing,
@@ -71,8 +71,10 @@ def sampler_key(symbol, nucleus, row_step, logprob, rows, noise, C, ld):
 
 
 def plan_key(lens, nqs, append_eos, drop_last, mask_cond, mask_in, forget, labels, err):
+    """... and whether the last sequence ends inside a time step (ids not a multiple of its quantizer count: the fine
+    stage's flattened 1269 = 253 x 5 + 4, whose heads see one row fewer for the last quantizer)."""
     return ("token_plan", len(lens), bool(append_eos), bool(drop_last), bool(mask_cond), bool(mask_in), bool(forget), bool(labels),
-            bool(err), nqs[-1] > 1, max(lens) + 1 > 256, min(lens) == 0)
+            bool(err), nqs[-1] > 1, max(lens) + 1 > 256, min(lens) == 0, lens[-1] % nqs[-1] != 0)
 
 
 # explicit cases of the family files (their parametrizations, restated here; each runs with a contiguous C-wide pitch)
@@ -134,6 +136,15 @@ EXPLICIT_PLAN = [
     ([12, 300, 0], [12, 1, 3], True, True, True, False, True, True, True),
     ([12, 197, 810], [12, 1, 3], True, True, True, False, False, True, True),        # at the cfg2 shapes: past 256 ids a row
     ([12, 197, 810], [12, 1, 3], True, True, True, False, True, True, True),
+    ([12, 241], [12, 1], True, True, True, False, False, True, False),               # semantic training (bench.py's semantic
+    ([12, 241], [12, 1], True, True, True, False, False, True, True),                # stage): eval_loss and the step, with
+    ([12, 241], [12, 1], True, True, True, False, True, True, False),                # and without forgetting and err_flag
+    ([12, 241], [12, 1], True, True, True, False, True, True, True),
+    ([12, 762, 1269], [12, 3, 5], True, True, True, False, False, True, False),      # fine training at bench.py's cfg3: the
+    ([12, 762, 1269], [12, 3, 5], True, True, True, False, False, True, True),       # last sequence ends 4 ids into a step
+    ([12, 762, 1269], [12, 3, 5], True, True, True, False, True, True, False),
+    ([12, 762, 1269], [12, 3, 5], True, True, True, False, True, True, True),
+    ([12, 30, 40], [12, 3, 5], True, True, True, False, True, True, True),           # fine training on whole steps
     ([4, 11, 30], [4, 1, 3], False, False, False, False, False, False, True),       # inference: generate, score, sessions
     ([4, 11, 0], [4, 1, 3], False, False, False, False, False, False, True),        # a request with no prefix
     ([4, 11, 0], [4, 1, 3], True, False, True, False, False, False, True),
@@ -243,6 +254,11 @@ def _record(act16, model, monkeypatch):
     if model in call_forms.SONGS_ONLY:
         expected = {("song session", n) for n in ("omlm_sample_rows_indexed", "token_plan", "decode_advance_pos")} | \
             {("score songs", "token_plan")}
+    elif model in call_forms.BENCH_MODELS:
+        expected = {(p, "token_plan") for p in call_forms.BENCH_PHASES} | {("bench step", "forgetful_mask"),
+                                                                           ("bench deterministic step", "forgetful_mask")}
+        if model in call_forms.GENERATION_MODELS:
+            expected |= {("bench generation", "omlm_sample_rows"), ("bench generation", "token_plan")}
     else:
         expected = {(p, n) for p in call_forms.SESSION_PHASES for n in ("token_plan", "decode_advance_pos")} | \
             {("session logprobs", "omlm_sample_rows_indexed_logprob"), ("session join", "omlm_sample_rows_indexed"),
@@ -549,7 +565,7 @@ def test_engine_call_forms_replayed_and_covered(act16, model, monkeypatch):
             assert pad == -1, f
             k = plan_key(lens, nqs, ae, dl, mc, mi, fk, lab, err)
             if k not in keys:
-                fails += replay_plan(list(lens), list(nqs), ae, dl, mc, mi, fk, lab, err, B=min(B, 8), seed=len(keys))
+                fails += replay_plan(list(lens), list(nqs), ae, dl, mc, mi, fk, lab, err, B=B, seed=len(keys))
             keys.add(k)
         elif name == "forgetful_mask":
             fails += replay_forgetful(*f)
