@@ -46,6 +46,8 @@ class _Song:
         self.left = len(plan.jobs)
         self.sent = 0                  # output rows known to be final
         self.handed = 0                # output rows handed out by ready()
+        self.live = set()              # (stage, request handle) of its submitted jobs that have not finished
+        self.held = None               # suspended: the (stage, request handle) pairs suspend() suspended
 
     def write(self, job, tokens):
         """A finished job's tokens [steps, q] -> its stream."""
@@ -119,6 +121,9 @@ class MusicLMSession:
     coarse_only) that became final since the last call; the prime's rows are final at once.  Concatenated, a song's
     rows are its `finished` output's first tensor.  Songs are seeded; there is no noise stream.
 
+    Between steps, `status(h)` reports where a song is, `cancel(h)` drops it and frees its stage slots and its place
+    under max_songs, and `suspend(h)` / `resume(h)` stop a song's windows and later continue them bit for bit.
+
     Streams: every stage's device work (its session's adds, steps, prefills and graph replays, and the writes of its
     windows into the songs' streams) runs on `streams[stage]`, a CUDA stream the session owns on that stage's device.
     Events order the rest, and `step` never waits for the device once the stage sessions have captured their graphs:
@@ -178,6 +183,8 @@ class MusicLMSession:
         self._jobs = [{}, {}, {}]      # per stage: request handle -> (song, job)
         self._ready = {}               # handle -> _Song with final rows not handed out yet
         self._done = {}                # handle -> finished _Song
+        self._held = {}                # handle -> queue entry of a song suspended while queued
+        self._cancelled = set()
 
     # ------------------------------------------------------------------------------------------------ streams
     def _caller_event(self):
@@ -269,6 +276,8 @@ class MusicLMSession:
             self._submit(song)
 
     def _submit(self, song):
+        if song.held is not None:      # a suspended song submits nothing until it is resumed
+            return
         for job in song.runnable():
             s = job.stage
             with torch.cuda.stream(self.streams[s]):
@@ -278,6 +287,7 @@ class MusicLMSession:
                                          pred_token_ids=song.part(job.prefix), seed=job.seed, max_time_steps=job.max_time_steps,
                                          temperature=job.temperature, top_p=job.top_p)
             self._jobs[s][h] = (song, job)
+            song.live.add((s, h))
 
     def _wait_inputs(self, song, job):
         """Orders a job's reads on its stage stream: after the caller's `add` (clap ids, primes) and after the writes of
@@ -308,8 +318,100 @@ class MusicLMSession:
 
     @property
     def idle(self) -> bool:
-        """No song in flight or queued."""
-        return not self._songs and not self._queue
+        """No song in flight or queued, but suspended ones (they wait for `resume` and keep no session busy)."""
+        return not self._queue and all(song.held is not None for song in self._songs.values())
+
+    # ------------------------------------------------------------------------------------------------ cancel, suspend
+    def _state(self, handle, where: str) -> str:
+        if not isinstance(handle, bool) and isinstance(handle, numbers.Integral):
+            song = self._songs.get(handle)
+            if song is not None:
+                if song.held is not None:
+                    return "suspended"
+                running = any(self.sessions[s].status(h) in ("running", "prefilling") for s, h in song.live)
+                return "running" if running else "waiting"
+            if handle in self._held:
+                return "suspended"
+            if any(entry[0] == handle for entry in self._queue):
+                return "queued"
+            if handle in self._cancelled:
+                raise ValueError(f"{_WHERE}Session.{where}: song {handle} was cancelled")
+            if 0 <= handle < self._next_handle:
+                return "finished"
+        raise ValueError(f"{_WHERE}Session.{where}: {handle!r} is not a song handle of this session")
+
+    def status(self, handle) -> str:
+        """"queued" (waiting for room under max_songs), "running" (a window of it decodes), "waiting" (admitted, no
+        window decoding at the moment), "suspended" or "finished" (its output waits in `finished()` or was returned).
+        Host state only.  ValueError for a handle `add` never returned or a cancelled one."""
+        return self._state(handle, "status")
+
+    def cancel(self, handle) -> bool:
+        """Drops a queued, admitted or suspended song: its windows leave the three stage sessions (their slots are
+        free at the next step), its jobs are never submitted, its place under max_songs goes to the next queued song
+        at once, and it never appears in `ready()` or `finished()` again (rows `ready()` returned stay returned).  No
+        other song changes.  Returns False for a finished song, whose output stays where it is.  Called between steps;
+        ValueError for a handle `add` never returned or a cancelled one."""
+        state = self._state(handle, "cancel")
+        if state == "finished":
+            return False
+        if handle in self._held:
+            del self._held[handle]
+        elif state == "queued":
+            self._queue.remove(next(e for e in self._queue if e[0] == handle))
+        else:
+            song = self._songs.pop(handle)
+            for s, h in sorted(song.live):
+                self.sessions[s].cancel(h)
+                del self._jobs[s][h]
+            self._ready.pop(handle, None)
+        self._cancelled.add(handle)
+        self._admit()
+        return True
+
+    def suspend(self, handle):
+        """An admitted song stops: its windows' rows give up their stage slots (running ones keep a device snapshot
+        of their decode state, GenerationSession.suspend; the snapshots are taken on the stage streams after the
+        caller's current stream) and none of its jobs is submitted until `resume`.  It keeps its place under
+        max_songs (cancel it to free that).  A queued song leaves the queue.  Called between steps; ValueError for a
+        song that is suspended, finished, cancelled or unknown."""
+        state = self._state(handle, "suspend")
+        if state not in ("queued", "running", "waiting"):
+            raise ValueError(f"{_WHERE}Session.suspend: song {handle} is {state}; only queued and admitted songs can be suspended")
+        if state == "queued":
+            entry = next(e for e in self._queue if e[0] == handle)
+            self._queue.remove(entry)
+            self._held[handle] = entry
+            return
+        song = self._songs[handle]
+        ev = self._caller_event()
+        song.held = []
+        for s, h in sorted(song.live):
+            if self.sessions[s].status(h) not in ("queued", "running"):
+                continue
+            with torch.cuda.stream(self.streams[s]):
+                if ev is not None and self.streams[s] is not None:
+                    self.streams[s].wait_event(ev)
+                self.sessions[s].suspend(h)
+            song.held.append((s, h))
+
+    def resume(self, handle):
+        """A suspended song continues: its windows' rows go back to the head of their stage sessions' queues, in the
+        order they were submitted, and its jobs are submitted again as their inputs exist.  Its output and its
+        `ready()` rows are bit for bit those of the song never suspended.  A song suspended while queued goes back to
+        the head of the queue.  ValueError for a song that is not suspended."""
+        state = self._state(handle, "resume")
+        if state != "suspended":
+            raise ValueError(f"{_WHERE}Session.resume: song {handle} is {state}, not suspended")
+        if handle in self._held:
+            self._queue.appendleft(self._held.pop(handle))
+            self._admit()
+            return
+        song = self._songs[handle]
+        for s, h in song.held:
+            self.sessions[s].resume(h)
+        song.held = None
+        self._submit(song)
 
     def step(self):
         """One time step of every stage session with work; then the windows that finished go into their songs'
@@ -325,7 +427,10 @@ class MusicLMSession:
                 continue
             with torch.cuda.stream(self.streams[stage]):
                 for h, tokens in done.items():
+                    if h not in self._jobs[stage]:      # a window of a cancelled song that finished at its add
+                        continue
                     song, job = self._jobs[stage].pop(h)
+                    song.live.discard((stage, h))
                     song.write(job, tokens)
                     touched[song.handle] = song
                 if self.written[stage] is not None:

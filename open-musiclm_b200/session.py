@@ -228,6 +228,7 @@ class _Row:
         self.chunk = None
         self.slot = None
         self.join_step = None
+        self.snapshot = None           # a suspended running row's decode state (GenerationSession._snapshot)
 
     @property
     def prefilled(self) -> bool:
@@ -247,7 +248,12 @@ class SlotSchedule:
 
     prefill_rows: at most that many prompt rows are prefilled per boundary (None: no bound).  A prompt that does not
     fit is prefilled in chunks over consecutive boundaries, each but the last a multiple of `unit` rows; its request
-    holds its slot meanwhile and samples from the boundary of its last chunk on."""
+    holds its slot meanwhile and samples from the boundary of its last chunk on.
+
+    Between boundaries a row can be cancelled (it leaves wherever it is and its slot is free at once), suspended (a
+    queued row leaves the queue; a prefilled row leaves its slot, keeping its progress; a row part-way through its
+    prompt cannot be) and resumed.  A suspended row holds no slot and no queue place.  Resumed rows wait in `resumed`,
+    ahead of the queue, in the order they were resumed; a prefilled one takes a slot without prefill or budget."""
 
     def __init__(self, slots: int, q: int, max_queue: int = 0, prefill_rows=None, unit: int = 1):
         self.slots, self.q, self.max_queue = slots, q, max_queue
@@ -255,28 +261,70 @@ class SlotSchedule:
         self.free = list(range(slots))
         self.rows = {}                 # slot -> _Row (prefilling rows included)
         self.queue = deque()
+        self.resumed = deque()         # resumed rows, ahead of the queue
+        self.suspended = {}            # handle -> suspended _Row
+        self.live = {}                 # handle -> _Row of every queued, resumed, slotted or suspended row
         self.prefilling = []           # rows part-way through their prompt, in admission order
+        self.restored = []             # the prefilled rows the last admit put back into slots
         self.steps = 0                 # time steps run
 
     def check_room(self):
-        """Raises ValueError when every slot is taken or promised to a queued row and the queue is full."""
-        if len(self.rows) + len(self.queue) >= self.slots + self.max_queue:
+        """Raises ValueError when every slot is taken or promised to a waiting row and the queue is full."""
+        waiting = len(self.queue) + len(self.resumed)
+        if len(self.rows) + waiting >= self.slots + self.max_queue:
             raise ValueError(f"open_musiclm_b200 GenerationSession.add: all {self.slots} slots are taken and the queue holds "
-                             f"{len(self.queue)} of max_queue = {self.max_queue} requests")
+                             f"{waiting} of max_queue = {self.max_queue} requests")
 
     def submit(self, row: _Row):
         self.check_room()
         self.queue.append(row)
+        self.live[row.handle] = row
+
+    def status(self, row: _Row) -> str:
+        if row.handle in self.suspended:
+            return "suspended"
+        if row.slot is None:
+            return "queued"
+        return "running" if row.prefilled else "prefilling"
+
+    def _leave(self, row: _Row):
+        """Takes a row out of the queue, the resumed rows or its slot (freed at once)."""
+        if row.slot is not None:
+            del self.rows[row.slot]
+            self.free.append(row.slot)
+            row.slot = None
+            if row in self.prefilling:
+                self.prefilling.remove(row)
+        elif row in self.resumed:
+            self.resumed.remove(row)
+        else:
+            self.queue.remove(row)
+
+    def cancel(self, row: _Row):
+        if self.suspended.pop(row.handle, None) is None:
+            self._leave(row)
+        del self.live[row.handle]
+
+    def suspend(self, row: _Row):
+        assert row.handle not in self.suspended and (row.slot is None or row.prefilled)
+        self._leave(row)
+        self.suspended[row.handle] = row
+
+    def resume(self, row: _Row):
+        del self.suspended[row.handle]
+        self.resumed.append(row)
 
     def admit(self):
         """The boundary: the budget of prompt rows goes in FIFO order, first to the rows part-way through their
-        prompt, then to queued rows, which take free slots (lowest first) while there are any.  A row gets a chunk
-        only if it can take min(unit, its remaining rows): its whole remainder if that fits, else the largest multiple
-        of unit that does; the first row that cannot ends the boundary, so no row overtakes an earlier one.  Returns
-        the rows with a chunk at this boundary (row.chunk = (p0, length)); without a budget, the rows that joined, each
-        with its whole prompt."""
+        prompt, then to resumed rows and then queued rows, which take free slots (lowest first) while there are any.  A
+        row gets a chunk only if it can take min(unit, its remaining rows): its whole remainder if that fits, else the
+        largest multiple of unit that does; the first row that cannot ends the boundary's admissions, so no row
+        overtakes an earlier one.  A resumed row that was prefilled when it was suspended needs no chunk: it takes a slot
+        whatever is left of the budget and goes to `restored`.  Returns the rows with a chunk at this boundary
+        (row.chunk = (p0, length)); without a budget, the rows that joined, each with its whole prompt."""
         left = float("inf") if self.prefill_rows is None else self.prefill_rows
         out = []
+        self.restored = []
 
         def take(row):
             nonlocal left
@@ -290,16 +338,19 @@ class SlotSchedule:
             out.append(row)
             return True
 
-        for row in self.prefilling:
-            if not take(row):
+        blocked = not all(take(row) for row in self.prefilling)
+        while self.free and (self.resumed or self.queue):
+            line = self.resumed if self.resumed else self.queue
+            row = line[0]
+            if row.prefilled:
+                self.restored.append(row)
+            elif blocked or not take(row):
                 break
-        else:
-            while self.queue and self.free and take(self.queue[0]):
-                row = self.queue.popleft()
-                row.slot = min(self.free)
-                self.free.remove(row.slot)
-                row.join_step = self.steps
-                self.rows[row.slot] = row
+            line.popleft()
+            row.slot = min(self.free)
+            self.free.remove(row.slot)
+            row.join_step = self.steps
+            self.rows[row.slot] = row
         self.prefilling = [r for r in self.prefilling if not r.prefilled] + [r for r in out if r.chunk[0] == 0 and not r.prefilled]
         return out
 
@@ -316,6 +367,7 @@ class SlotSchedule:
                 done.append(row)
         for row in done:
             del self.rows[row.slot]
+            del self.live[row.handle]
             self.free.append(row.slot)
         return done
 
@@ -366,6 +418,11 @@ class GenerationSession:
     part-way through their prompt, then to queued ones, in arrival order; a request takes its slot with its first
     chunk and samples from the boundary of its last.  Time steps in which a request only prefills count for `step`.
 
+    Between steps, `status(h)` reports where a request is, `cancel(h)` drops it and frees its slot at once, and
+    `suspend(h)` / `resume(h)` take a running row out of its slot and later put it back into any free slot, restored
+    from a device snapshot of its decode state.  None of them changes another row's values, and a resumed row's values
+    are those of the row never suspended.  They add no CUDA graph and no host synchronisation.
+
     The transformer's weights are packed when the session is created; train it between sessions, not during one.
     Every row gets exactly what `generate` gives that row alone with seeds=[seed] and the same arguments; free and
     finished slots keep computing values nobody reads."""
@@ -402,6 +459,7 @@ class GenerationSession:
         self.logprob = return_logprobs
         self.sched = SlotSchedule(self.slots, self.q, int(max_queue), self.prefill_rows, unit)
         self._next_handle = 0
+        self._cancelled = set()
         self._done = {}
         self._traced = {}
         self._trace = []               # trace mode: the [slots, C] logits of every sample point since _trace_base
@@ -481,8 +539,97 @@ class GenerationSession:
 
     @property
     def idle(self) -> bool:
-        """No row is decoding, prefilling or queued."""
-        return not self.sched.rows and not self.sched.queue
+        """No row is decoding, prefilling or queued (suspended rows wait for `resume` and keep no session busy)."""
+        return not self.sched.rows and not self.sched.queue and not self.sched.resumed
+
+    # ------------------------------------------------------------------------------------------------ cancel, suspend
+    def _state(self, handle, where: str) -> str:
+        if not isinstance(handle, bool) and isinstance(handle, numbers.Integral):
+            row = self.sched.live.get(handle)
+            if row is not None:
+                return self.sched.status(row)
+            if 0 <= handle < self._next_handle and handle not in self._cancelled:
+                return "finished"
+            if handle in self._cancelled:
+                raise ValueError(f"open_musiclm_b200 GenerationSession.{where}: request {handle} was cancelled")
+        raise ValueError(f"open_musiclm_b200 GenerationSession.{where}: {handle!r} is not a handle of this session")
+
+    def status(self, handle) -> str:
+        """"queued", "prefilling" (part-way through a chunked prefill), "running", "suspended" or "finished" (its result
+        waits in `finished()` or was returned).  Host state only.  ValueError for a handle `add` never returned or a
+        cancelled one."""
+        return self._state(handle, "status")
+
+    def cancel(self, handle) -> bool:
+        """Removes a queued, prefilling, running or suspended request: its slot is free for the next boundary, it never
+        appears in `finished()`, and no other row changes.  Returns False, leaving the result where it is, for a
+        finished request.  Called between steps, like `add`; no device work.  ValueError for a handle `add` never
+        returned or a cancelled one."""
+        if self._state(handle, "cancel") == "finished":
+            return False
+        row = self.sched.live[handle]
+        self.sched.cancel(row)
+        row.snapshot = row.payload = None
+        self._cancelled.add(handle)
+        return True
+
+    def suspend(self, handle):
+        """A running row gives up its slot: its decode state is copied into a snapshot the session keeps on the row's
+        device (torch copies on the current stream), and `resume` later continues it bit for bit in whatever slot it
+        gets.  A queued request leaves the queue, keeping its arguments.  A suspended request holds no slot and no
+        queue place.  Called between steps.  ValueError, before any device work, under trace_logits and for a request
+        that is not queued or running: part-way through a chunked prefill (`status` says when it has finished),
+        suspended, finished, cancelled or unknown."""
+        state = self._state(handle, "suspend")
+        if self.trace:
+            raise ValueError("open_musiclm_b200 GenerationSession.suspend: not available with trace_logits=True")
+        if state not in ("queued", "running"):
+            raise ValueError(f"open_musiclm_b200 GenerationSession.suspend: request {handle} is {state}; only queued and running "
+                             f"requests can be suspended")
+        row = self.sched.live[handle]
+        if state == "running":
+            self._snapshot(row)
+        self.sched.suspend(row)
+
+    def resume(self, handle):
+        """Puts a suspended request at the head of the queue, behind the requests resumed before it and ahead of every
+        request `add` queued: it takes the lowest free slot at the next boundary with one.  A row that was running is
+        restored from its snapshot there and runs no prefill (it uses none of prefill_rows); a request suspended while
+        queued is prefilled as usual.  Never raises for lack of room.  ValueError for a request that is not suspended."""
+        state = self._state(handle, "resume")
+        if state != "suspended":
+            raise ValueError(f"open_musiclm_b200 GenerationSession.resume: request {handle} is {state}, not suspended")
+        self.sched.resume(self.sched.live[handle])
+
+    _ROW_STATE = ("next_row", "pos", "pos_last", "pos_offset", "t", "n_rows", "top_k", "temperature", "top_p", "seeds")
+
+    def _snapshot(self, row):
+        """Copies out what the next time step reads of the row's slot: the K/V of its live positions (those before
+        its current position P - 1 + t, which the next step writes), its conv history, its per-row arrays and its
+        samples so far."""
+        dec, s, t = self.dec, row.slot, row.t
+        pos = row.P - 1 + t
+        snap = dict(cache=[c[s, :pos].clone() for c in dec.cache], conv=[c[s].clone() for c in dec.conv],
+                    rows={name: getattr(dec, name)[s:s + 1].clone() for name in self._ROW_STATE},
+                    out=[o[s, :t].clone() for o in ((dec.tokens, dec.lp, dec.slp) if self.logprob else (dec.tokens,))])
+        row.snapshot = snap
+
+    def _restore(self, rows):
+        """Writes the snapshots of `rows` (restored by the schedule at this boundary) into their new slots, before the
+        boundary step reads them."""
+        dec = self.dec
+        for row in rows:
+            s, snap = row.slot, row.snapshot
+            pos = snap["cache"][0].shape[0]
+            for c, v in zip(dec.cache, snap["cache"]):
+                c[s, :pos].copy_(v)
+            for c, v in zip(dec.conv, snap["conv"]):
+                c[s].copy_(v)
+            for name, v in snap["rows"].items():
+                getattr(dec, name)[s:s + 1].copy_(v)
+            for o, v in zip((dec.tokens, dec.lp, dec.slp), snap["out"]):
+                o[s, :v.shape[0]].copy_(v)
+            row.snapshot = None
 
     @property
     def graph_count(self) -> int:
@@ -590,8 +737,9 @@ class GenerationSession:
 
     @torch.no_grad()
     def step(self, n_time_steps: int = 1):
-        """Runs n_time_steps time steps (q tokens per active row each).  Each starts at a boundary, where queued rows
-        take free slots: the running rows' step to quantizer slot 0, the prefill of this boundary's chunks and the
+        """Runs n_time_steps time steps (q tokens per active row each).  Each starts at a boundary, where resumed and
+        queued rows take free slots (resumed rows that were running are restored from their snapshots there):
+        the running rows' step to quantizer slot 0, the prefill of this boundary's chunks and the
         install of the prompts they complete, then the sample of slot 0 for every row; slots 1 ... q-1 follow as step
         and sample.  Rows with all their tokens leave
         at the end of the time step; `finished` returns them.  A time step with no row to run does nothing."""
@@ -605,6 +753,9 @@ class GenerationSession:
             if not sched.rows:
                 break
             dec = self._device_state()
+            if sched.restored:            # back in their slots before the boundary step, which runs them as it runs the others
+                self._restore(sched.restored)
+                running = True
             if self.trace and not running:
                 self._trace, self._trace_base = [], self._trace_base + len(self._trace)
             for row in chunked:
